@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - rows/sec of the batch-predict hot path on N B200s (BASELINE.json metric, configs[1] by default).
+"""bench.py - rows/sec of the batch-predict hot path on N H100s (BASELINE.json metric, configs[1] by default).
 
     python bench.py --gpus 1 --steps 20 --warmup 5                      # this repo's CUDA path, cfg 2 (10M x 64 -> 10)
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1      # the reference's CPU path, same metric
@@ -7,6 +7,7 @@
         bench.py --gpus N --steps K --warmup W                          # one rank per GPU
     ... --config cfg3 | cfg5        # 784 -> 10 logistic on 50M rows / 2-layer MLP 64 -> 32 -> 10 on 10M rows
     ... --scaling weak              # r01 mode: every GPU scores its own 10M rows (default: strong - ONE batch split)
+    ... --dump-outputs DIR          # also write the labels of the last timed step as DIR/labels.npy (float32)
 
 A "step" is one pass of the hot path over one batch.  At N > 1 the batch is split across the GPUs (north_star: "the
 batch is split across GPUs", SURVEY.md 8e partition [r*N/G, (r+1)*N/G)), every rank scores its shard in EXACT mode
@@ -15,7 +16,7 @@ and the uint8 label vector is exchanged so every rank holds all labels.
 `value`  : whole-job rows/s with the shard resident in HBM (CUDA events on the launching stream, barrier + synchronize
            on both sides, max over ranks).
 `e2e`    : the same metric through the reference-facing plugin with HOST buffers: a float64 feature-major pandas
-           DataFrame (what Dataset.get_features yields, /root/reference/unionml/dataset.py:506-520) ->
+           DataFrame (what Dataset.get_features yields, unionml/dataset.py:506-520) ->
            Model.predict(features=frame) -> List[float]  - the reference arm's own input and output types.  The
            pinned-fp32 -> int32-labels engine call of round 1 is reported beside it (`e2e.engine_pinned_f32`).
 `roofline`: algorithmic bytes (4 F per row) / CUDA-event duration of the scoring kernel, against MEASURED_PEAKS.json.
@@ -43,8 +44,7 @@ CONFIGS = {
         "metric": "rows/sec batch predict (64->10 logistic)", "kind": "linear", "F": 64, "C": 10, "rows": 10_000_000,
         "data": "digits", "kernel": "linear_argmax_tma_kernel<10, EXACT, QUEUE> (fp64 re-score by a tenth warp of the same launch)", "cpu_rows": 2_000_000,
         "what": "BASELINE.json configs[1]: digits predictor (golden LogisticRegression 64->10)",
-        # dram__bytes_read.sum + dram__bytes_write.sum of one launch on 10M rows (profiles/r02_linear_argmax_tma_queue.ncu_raw.csv)
-        "traffic_10m": 2_568_923_504, "traffic_src": "profiles/r02_linear_argmax_tma_queue.ncu_raw.csv (ncu --set full, per launch: dram read 2.560358 GB + write 8.565504 MB)",
+        "traffic_10m": None, "traffic_src": None,
     },
     "cfg3": {
         "metric": "rows/sec batch predict (784->10 logistic)", "kind": "linear", "F": 784, "C": 10, "rows": 50_000_000,
@@ -54,9 +54,9 @@ CONFIGS = {
     },
     "cfg5": {
         "metric": "rows/sec batch predict (2-layer MLP 64->32->10)", "kind": "mlp", "F": 64, "C": 10, "rows": 10_000_000,
-        "data": "digits", "kernel": "mlp_argmax_tc_kernel<32, 10, EXACT> (tcgen05 kind::tf32)", "cpu_rows": 200_000,
+        "data": "digits", "kernel": "mlp_argmax_tc_kernel<32, 10, EXACT> (wgmma tf32)", "cpu_rows": 200_000,
         "what": "BASELINE.json configs[4]: PyTorch 2-layer MLP predictor (torch.manual_seed(0) PytorchModel(64, 32, 10))",
-        "traffic_10m": 2_568_177_568, "traffic_src": "profiles/r02_mlp_argmax_tc.ncu_raw.csv (ncu --set full, per launch: dram read 2.560164 GB + write 8.013568 MB)",
+        "traffic_10m": None, "traffic_src": None,
     },
 }
 CHUNK = 1_000_000  # digits rows are generated in global 1M-row chunks: chunk k = default_rng(k)
@@ -110,7 +110,7 @@ def torch_module(arrs):
     import torch.nn as nn
     import torch.nn.functional as Fn
 
-    class PytorchModel(nn.Module):  # /root/reference/tests/integration/pytorch_app/quickstart.py:14-24
+    class PytorchModel(nn.Module):  # unionml tests/integration/pytorch_app/quickstart.py:14-24
         def __init__(self, in_dims, hidden_dims, out_dims):
             super().__init__()
             self.layers = nn.Sequential(nn.Linear(in_dims, hidden_dims), nn.ReLU(), nn.Linear(hidden_dims, out_dims))
@@ -142,7 +142,7 @@ def measured_peak_hbm():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 def usable_cores() -> int:
@@ -288,7 +288,7 @@ def cpu_reference_predict_rows_per_s(cfg, arrs, sample_rows: int, repeats: int):
         est = sklearn_estimator(arrs, cfg["F"])
         est.feature_names_in_ = np.asarray(frame.columns, dtype=object)
 
-        def predictor(estimator, features) -> list:  # /root/reference/README.md:87-92
+        def predictor(estimator, features) -> list:  # unionml README.md:87-92
             return [float(x) for x in estimator.predict(features)]
 
         model_object = est
@@ -348,7 +348,7 @@ def global_rows(args, cfg, n_gpus: int) -> int:
     if args.scaling_resolved == "weak":
         return cfg["rows"] * n_gpus if cfg["data"] != "mnist" else 6_250_000 * n_gpus
     if cfg["data"] == "mnist" and n_gpus < 4:
-        # 50M x 784 fp32 is 156.8 GB: it needs >= 4 GPUs; below that the bench scores the 8-GPU shard size per GPU
+        # 50M x 784 fp32 is 156.8 GB: it needs >= 4 80-GB GPUs; below that the bench scores the 8-GPU shard size per GPU
         return 6_250_000 * n_gpus
     return cfg["rows"]
 
@@ -364,7 +364,7 @@ def workload_config(args, cfg, n_gpus: int) -> dict:
         "labels": "uint8 class index per row",
         "parallelism": (f"row-sharded x{n_gpus} ({args.scaling_resolved} scaling), label exchange: " + getattr(args, "gather_used", args.gather))
         if n_gpus > 1 else "single GPU",
-        "l2_policy": f"inputs ({g // max(n_gpus, 1) * 4 * F / 1e9:.2f} GB/step/GPU) are larger than L2 (126 MB); no flush needed",
+        "l2_policy": f"inputs ({g // max(n_gpus, 1) * 4 * F / 1e9:.2f} GB/step/GPU) are larger than L2 (50 MB); no flush needed",
     }
 
 
@@ -533,8 +533,8 @@ def run_gpu_arm(args, cfg):
         "nccl": "ncclAllGather of uint8 labels", "none": "none"}[chosen]
 
     # warm-up: at least W steps, and keep going until the GPU has been under this load for ~0.25 s - the shard was just
-    # generated on the host for seconds, the clocks are at idle, and K x 0.4 ms of timed region would otherwise sit on
-    # the boost ramp (same-box A/B: 0.373 ms/step warm vs 0.40 right after idle)
+    # generated on the host for seconds, the clocks are at idle, and a short timed region would otherwise sit on the
+    # boost ramp
     n_warm = 0
     if world == 1:
         t_warm = time.perf_counter()
@@ -557,6 +557,8 @@ def run_gpu_arm(args, cfg):
     # ---- timed region: exactly K steps, CUDA events on the launching stream ----
     ms_per_step = timed_steps(step, args.steps)
     value = G / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        last_labels = labels_all.clone()  # the later legs write this vector again
 
     # ---- roofline of the dominant kernel: CUDA events around the scoring kernel inside the library, live ----
     k_ms, r_ms, flagged, launches_per_step, path = [], [], 0, 2, 0
@@ -680,6 +682,8 @@ def run_gpu_arm(args, cfg):
         cpu_baseline = {**extra, "value": rps, "unit": UNIT, "cores": cores, "kind": "port",
                         "sample": cpu_sample_note(cfg, sample, cores) + ", best of 3"}
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_labels.cpu().numpy())
     if rank == 0:
         line = {
             "metric": cfg["metric"], "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
@@ -695,6 +699,22 @@ def run_gpu_arm(args, cfg):
         dist.barrier()
         dist.destroy_process_group()
     return 0
+
+
+DUMP_MAX_ROWS = 16_000_000  # 64 MB of float32 labels
+DUMP_SAMPLE_ROWS = 4_000_000
+
+
+def dump_outputs(out_dir: str, labels: np.ndarray) -> None:
+    """The class index of every row (float32) as `out_dir`/labels.npy.  Past DUMP_MAX_ROWS rows, a seeded sample of
+    DUMP_SAMPLE_ROWS rows instead, with their row numbers in labels_rows.npy (float64)."""
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    if labels.shape[0] > DUMP_MAX_ROWS:
+        rows = np.sort(np.random.default_rng(0).choice(labels.shape[0], DUMP_SAMPLE_ROWS, replace=False))
+        np.save(out / "labels_rows.npy", rows.astype(np.float64))
+        labels = labels[rows]
+    np.save(out / "labels.npy", labels.astype(np.float32))
 
 
 def run_e2e_legs(args, cfg, arrs, eng, model, torch, dist, dev, rank, world, lo, hi, X_host, X_dev, labels_all, barrier, pd):
@@ -847,6 +867,8 @@ def main():
     ap.add_argument("--no-multicast", action="store_true", help="per-peer stores instead of the NVLS multicast alias")
     ap.add_argument("--no-graph", action="store_true", help="N > 1: launch every step eagerly instead of replaying a CUDA graph")
     ap.add_argument("--traffic", type=float, default=None, help="dram bytes/launch from a committed ncu capture")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the labels the last timed step computed to DIR/labels.npy (float32)")
     args = ap.parse_args()
     args.scaling_resolved = "strong" if args.scaling in ("auto", "strong") else "weak"
     cfg = CONFIGS[args.config]

@@ -1,5 +1,5 @@
 /*
- * uml_b200.h - C ABI of the B200-native batch-prediction engine for UnionML's predict hot path.
+ * uml_b200.h - C ABI of the H100-native (sm_90a) batch-prediction engine for UnionML's predict hot path.
  *
  * The reference (unionai-oss/unionml) is pure Python and has no FFI of its own; the single call this library stands
  * behind is the plugin boundary
@@ -74,7 +74,7 @@ typedef struct uml_stats {
   int64_t d2h_bytes;
   int32_t kernel_launches; /* kernels of this library launched by the call                                            */
   int32_t path;            /* 1 = TMA fp32 tile kernel, 2 = generic fp64 kernel, 3 = MLP CUDA-core kernel, 5 = MLP tensor-core
-                              (tcgen05) kernel, 4 = small-batch fp64
+                              (wgmma) kernel, 4 = small-batch fp64
                               kernel of the online path (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph)                 */
 } uml_stats;
 
@@ -206,7 +206,7 @@ UML_API int uml_mlp_predict_host_begin(uml_engine* e, const uml_mlp* m, const vo
                                int mode, int64_t chunk_rows);
 /* fused compute + collective for the MLP predictor: same contract as uml_linear_predict_peers (labels of this rank's
  * rows are stored into every entry of peer_labels at row_offset from the kernel epilogue; int32 or uint8 vectors).
- * Batches whose features are tf32 values (integer / pixel domains) run layer 1 on the tensor cores (tcgen05, stats
+ * Batches whose features are tf32 values (integer / pixel domains) run layer 1 on the tensor cores (wgmma, stats
  * path 5); other batches take the CUDA-core kernel (path 3) and a thin scatter kernel. */
 UML_API int uml_mlp_predict_peers(uml_engine* e, const uml_mlp* m, const uml_batch* b, void* const* peer_labels, int n_peers,
                           int64_t row_offset, int label_bytes, int mode, uml_stats* stats);

@@ -1,9 +1,9 @@
 """Oracle (test infrastructure only): numpy restatement of scikit-learn's linear-classifier predict.
 
 Follows ``sklearn/linear_model/_base.py`` (scikit-learn 1.9.0, the third-party dependency that holds
-the arithmetic of the reference's hot path; reference call sites: ``/root/reference/README.md:92``,
-``/root/reference/tests/integration/sklearn_app/quickstart.py:26``,
-``/root/reference/tests/unit/model_fixtures.py:71``):
+the arithmetic of the reference's hot path; reference call sites: ``unionml:README.md:92``,
+``unionml:tests/integration/sklearn_app/quickstart.py:26``,
+``unionml:tests/unit/model_fixtures.py:71``):
 
 * ``decision_function`` (``_base.py:366-396``): ``scores = X @ coef_.T + intercept_``; a single-row
   ``coef_`` (binary problem) is flattened to 1-D.
@@ -71,7 +71,7 @@ def predict(X, coef, intercept, classes) -> np.ndarray:
 
 
 def canonical_predictor(estimator, features) -> list:
-    """The reference's canonical user predictor (``/root/reference/README.md:87-92``):
+    """The reference's canonical user predictor (``unionml:README.md:87-92``):
     ``[float(x) for x in estimator.predict(features)]`` with ``estimator.predict`` restated above."""
     feats = features.to_numpy() if hasattr(features, "to_numpy") else np.asarray(features)
     labels = predict(feats, estimator.coef_, estimator.intercept_, estimator.classes_)

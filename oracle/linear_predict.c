@@ -2,7 +2,7 @@
  * Oracle (test infrastructure only): plain-C restatement of scikit-learn's linear-classifier predict,
  *     scores = X @ coef_.T + intercept_ ; idx = argmax(scores, axis=1)          (first maximum wins, like np.argmax)
  * following sklearn/linear_model/_base.py:366-427 (the arithmetic behind the reference's canonical predictor,
- * /root/reference/README.md:87-92).  float64 throughout, one sequential FMA-free dot product per (row, class) in
+ * unionml:README.md:87-92).  float64 throughout, one sequential FMA-free dot product per (row, class) in
  * feature order - the summation order differs from OpenBLAS' blocked dgemm, which only matters for gaps below ~1e-13
  * (tests/test_oracle_golden.py pins it against numpy and scikit-learn on seeded batches).
  *

@@ -1,6 +1,6 @@
 """Oracle (test infrastructure only): the PyTorch quickstart predictor, restated in numpy.
 
-Reference: ``/root/reference/tests/integration/pytorch_app/quickstart.py``
+Reference: ``unionml:tests/integration/pytorch_app/quickstart.py``
 
 * ``PytorchModel`` (14-24): ``Sequential(Linear(in, hidden), ReLU(), Linear(hidden, out))`` then ``softmax(dim=1)``;
 * ``process_features`` (31-32): ``torch.from_numpy(features.values).float()`` - features are cast to float32;

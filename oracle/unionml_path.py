@@ -4,15 +4,15 @@
 dispatch logic of the reference is restated as plain functions over a small spec object.  Each function cites the
 reference lines it follows; the code is written from the behaviour, not copied.
 
-* ``default_feature_loader``   - ``/root/reference/unionml/dataset.py:506-520``
+* ``default_feature_loader``   - ``unionml:unionml/dataset.py:506-520``
 * ``default_feature_transformer`` - ``dataset.py:522-527``
 * ``default_parser``           - ``dataset.py:489-504`` (including the 498-499 quirk: an explicit ``features`` list is
   *overridden* by "all non-target columns" whenever both are non-None)
 * ``get_features``             - ``dataset.py:350-359``
-* ``predict``                  - ``/root/reference/unionml/model.py:711-741`` dispatch,
+* ``predict``                  - ``unionml:unionml/model.py:711-741`` dispatch,
   ``model.py:603-614`` (reader path) and ``model.py:641-650`` (features path): predictor, then callbacks whose
   exceptions are logged and swallowed
-* ``serving_predict``          - ``/root/reference/unionml/fastapi.py:50-64`` (``get_features`` runs twice: 61 and
+* ``serving_predict``          - ``unionml:unionml/fastapi.py:50-64`` (``get_features`` runs twice: 61 and
   ``model.py:740``)
 """
 from __future__ import annotations

@@ -4,13 +4,13 @@ The reference (``unionml``) cannot be imported here (flytekit absent), so the fi
 reference's *arithmetic dependency* - scikit-learn, the library its canonical predictor calls - through a hand
 restatement of the default ``Dataset`` pipeline:
 
-* ``/root/reference/unionml/dataset.py:44-53``  defaults ``test_size=0.2, shuffle=True, random_state=12345``
+* ``unionml:unionml/dataset.py:44-53``  defaults ``test_size=0.2, shuffle=True, random_state=12345``
 * ``dataset.py:477-487``  default splitter = ``train_test_split(data, test_size, random_state, shuffle)``
 * ``dataset.py:489-504``  default parser   = all non-target columns / ``data[targets]``
-* trainer = ``estimator.fit(features, target.squeeze())`` (``/root/reference/README.md:80-85``)
+* trainer = ``estimator.fit(features, target.squeeze())`` (``unionml:README.md:80-85``)
 
-Known answers reproduced: ``[8.0, 8.0, 0.0]`` (``/root/reference/tests/unit/test_aws_lambda_handler.py:117-127``) and
-the quickstart sample (``/root/reference/tests/integration/sklearn_app/quickstart.py:34-40``).
+Known answers reproduced: ``[8.0, 8.0, 0.0]`` (``unionml:tests/unit/test_aws_lambda_handler.py:117-127``) and
+the quickstart sample (``unionml:tests/integration/sklearn_app/quickstart.py:34-40``).
 
     python tests/golden/make_golden.py
 """

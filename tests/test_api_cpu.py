@@ -1,7 +1,7 @@
 """Host-side logic on CPU: the decorator API mirror behaves like the reference's (no GPU, no flytekit).
 
-Modelled on /root/reference/tests/unit/{test_model.py,test_dataset.py,test_type_guards.py} and
-/root/reference/tests/integration/test_fastapi.py.  The predictors registered here are the reference's CPU
+Modelled on unionml:tests/unit/{test_model.py,test_dataset.py,test_type_guards.py} and
+unionml:tests/integration/test_fastapi.py.  The predictors registered here are the reference's CPU
 predictors (sklearn called directly) - the device predictor has its own `-m gpu` tests.
 """
 import io
@@ -20,7 +20,7 @@ from oracle import unionml_path as opath
 from unionml_b200 import Dataset, Model, ModelArtifact, type_guards
 
 
-# fixtures shaped like /root/reference/tests/unit/model_fixtures.py:12-82
+# fixtures shaped like unionml:tests/unit/model_fixtures.py:12-82
 @pytest.fixture
 def mock_data() -> pd.DataFrame:
     return pd.DataFrame({"x": [1, 2, 3, 4] * 25, "x2": [1, 2, 3, 4] * 25, "x3": [1, 2, 3, 4] * 25, "y": [0, 1, 0, 1] * 25})
@@ -259,7 +259,7 @@ def test_digits_app_known_answers(digits_app, digits_model):
     _, model = digits_app
     frame = load_digits(as_frame=True).frame
     feats = [c for c in frame if c != "target"]
-    # /root/reference/tests/unit/test_aws_lambda_handler.py:127 and quickstart sample
+    # unionml:tests/unit/test_aws_lambda_handler.py:127 and quickstart sample
     assert model.predict(features=frame[feats].sample(3, random_state=99)) == [8.0, 8.0, 0.0]
     assert model.predict(features=frame.sample(5, random_state=42)) == [6.0, 9.0, 3.0, 7.0, 2.0]
     # the app trains the very model stored in tests/golden/digits_lr.npz

@@ -5,8 +5,8 @@ dtypes and layouts the reference really feeds it.
   ``sklearn/linear_model/_base.py:366-396``): flagged rows are re-scored from the caller's own values;
 * the online shape (<= 64 rows): one float64 kernel replayed as a CUDA graph;
 * ``predict_proba`` against ``LogisticRegression.predict_proba`` with the tolerance stated;
-* the reader-kwargs route (``/root/reference/unionml/model.py:603-614``) and the BentoML runnable call site
-  (``/root/reference/unionml/services/bentoml.py:201-211``) on the device predictor.
+* the reader-kwargs route (``unionml:unionml/model.py:603-614``) and the BentoML runnable call site
+  (``unionml:unionml/services/bentoml.py:201-211``) on the device predictor.
 """
 from typing import List
 

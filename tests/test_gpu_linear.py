@@ -13,7 +13,7 @@ from oracle import linear as olin
 
 pytestmark = pytest.mark.gpu
 
-if not torch.cuda.is_available():  # collected on CPU boxes, skipped there (the -m gpu run happens on the B200)
+if not torch.cuda.is_available():  # collected on CPU boxes, skipped there (the -m gpu run happens on an H100)
     pytest.skip("needs a CUDA device", allow_module_level=True)
 
 
@@ -36,7 +36,7 @@ def oracle_idx(X, coef, intercept):
 # golden vectors
 # ---------------------------------------------------------------------------------------------------------------
 def test_known_answer_through_predictor(digits_model, known_answer):
-    """[8.0, 8.0, 0.0]: /root/reference/tests/unit/test_aws_lambda_handler.py:127,159 - now on the GPU."""
+    """[8.0, 8.0, 0.0]: unionml:tests/unit/test_aws_lambda_handler.py:127,159 - now on the GPU."""
     from sklearn.linear_model import LogisticRegression
 
     from unionml_b200.predictors import linear_argmax

@@ -95,7 +95,7 @@ def test_against_torch_cpu_module_and_predictor(mlp_golden):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# tensor-core (tcgen05, kind::tf32) kernel: stats path 5
+# tensor-core (wgmma, tf32) kernel: stats path 5
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("rows", [1, 127, 128, 129, 5000, 250_001])
 def test_tensor_core_path_parity_and_dispatch(engine, mlp_golden, rows, monkeypatch):
@@ -139,7 +139,7 @@ def test_tensor_core_kernel_is_safe_on_rows_that_are_not_tf32(engine, mlp_golden
 
 
 def test_tensor_core_queue_and_kernel_rescore_agree(mlp_golden):
-    """UML_B200_MLP_RESCORE_MODE=queue (four fp64 warps inside the scoring launch; lost the same-box A/B and is off by
+    """UML_B200_MLP_RESCORE_MODE=queue (four fp64 warps inside the scoring launch; loses to the separate kernel and is off by
     default) vs =kernel (flag list + mlp_rescore_f64_kernel): same labels and counters, also when every row is flagged
     and the queue backs up."""
     import os
@@ -201,7 +201,7 @@ def test_tensor_core_full_size_ten_million(engine, mlp_golden):
         np.testing.assert_array_equal(labels[sl], omlp.predict_indices_f64(X[sl], *w).astype(np.int32))
     fast, _ = engine.predict_mlp(m, b, exact=False)
     assert (fast != labels).sum() <= st["n_flagged"]
-    print(f"mlp tcgen05 10M x 64: kernel {st['kernel_ms']:.3f} ms, re-score {st['recheck_ms']:.3f} ms, flagged {st['n_flagged']}")
+    print(f"mlp tensor-core 10M x 64: kernel {st['kernel_ms']:.3f} ms, re-score {st['recheck_ms']:.3f} ms, flagged {st['n_flagged']}")
 
 
 def test_mlp_peer_label_vectors(engine, mlp_golden, monkeypatch):

@@ -18,7 +18,7 @@ def _estimator(m, dtype=np.float64):
 
 
 def test_known_answer_lambda_handler(digits_model, known_answer):
-    # /root/reference/tests/unit/test_aws_lambda_handler.py:127,159
+    # unionml:tests/unit/test_aws_lambda_handler.py:127,159
     ka = known_answer["sample3_random_state99"]
     frame = pd.DataFrame(ka["records"])[known_answer["feature_names"]]
     got = olin.canonical_predictor(_estimator(digits_model), frame)

@@ -1,12 +1,12 @@
-"""cfg 4 of BASELINE.json: FastAPI /predict online serving, batch = 32, p50 / p99 latency on 1 x B200 - with the
+"""cfg 4 of BASELINE.json: FastAPI /predict online serving, batch = 32, p50 / p99 latency on 1 x H100 - with the
 reference-shaped CPU predictor served through the SAME app beside it (one JSON line; not part of the driver contract).
 
     python tools/bench_online.py [--requests 1000]
 
-Both apps are `unionml_b200.Model.serve(FastAPI())` (mirror of /root/reference/unionml/fastapi.py:15-70) driven by the
+Both apps are `unionml_b200.Model.serve(FastAPI())` (mirror of unionml:unionml/fastapi.py:15-70) driven by the
 in-process ASGI TestClient with 1 000 POSTs of digits.frame[features].sample(32, random_state=i) records (SURVEY.md 8d):
   * device : @model.predictor = unionml_b200.predictors.linear_argmax  (small-batch float64 kernel, CUDA graph replay)
-  * cpu    : @model.predictor = [float(x) for x in estimator.predict(features)]  (/root/reference/README.md:87-92)
+  * cpu    : @model.predictor = [float(x) for x in estimator.predict(features)]  (unionml:README.md:87-92)
 and the predictor call alone is timed for both (what the device path changes inside a request).
 """
 import argparse

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Round-2 probes on one B200 (not a bench line): staging-kernel bandwidth, pageable-source H2D rate with and without
+"""Round-2 probes on one GPU (not a bench line): staging-kernel bandwidth, pageable-source H2D rate with and without
 the pinned bounce pool, online-path latency (<= 64 rows), and the step time of a 1.25M-row shard (the strong-scaling
 share of cfg 2 at 8 GPUs).  Writes gpurun_out/probe_r2.json."""
 from __future__ import annotations

@@ -1,7 +1,7 @@
-"""unionml_b200: a B200-native engine for UnionML's ``Model.predict`` / ``@model.predictor`` hot path.
+"""unionml_b200: an H100-native engine for UnionML's ``Model.predict`` / ``@model.predictor`` hot path.
 
 Keeps the reference's decorator surface for the predict slice (``Dataset``, ``Model``, ``@model.predictor``, callbacks,
-``serving_app``) and runs the canonical ``LogisticRegression`` predictor as hand-written sm_100a CUDA behind a C ABI
+``serving_app``) and runs the canonical ``LogisticRegression`` predictor as hand-written sm_90a CUDA behind a C ABI
 (``include/uml_b200.h``).  Importing this package never touches CUDA; the device is bound on first predict.
 """
 from unionml_b200.dataset import Dataset  # noqa: F401

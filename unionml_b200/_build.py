@@ -1,4 +1,4 @@
-"""Build the CUDA library in-tree: unionml_b200/_lib/libuml_b200.so (sm_100a only).
+"""Build the CUDA library in-tree: unionml_b200/_lib/libuml_b200.so (sm_90a only).
 
 nvcc cross-compiles without a GPU, so this runs in the build container and the resulting .so travels to the GPU
 box with the repo snapshot.  One object per .cu (compiled in parallel), then one link.
@@ -19,7 +19,7 @@ LIB = LIB_DIR / "libuml_b200.so"
 OBJ_DIR = PKG.parent / "build" / "obj"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
@@ -71,7 +71,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
                     print(log, file=sys.stderr)
     objs = [OBJ_DIR / (s.stem + ".o") for s in sources()]
     if force or jobs or _stale(LIB, objs):
-        cmd = [nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB), *map(str, objs)]
+        cmd = [nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB), *map(str, objs)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

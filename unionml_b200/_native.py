@@ -1,7 +1,7 @@
 """ctypes binding of ``include/uml_b200.h`` (the C ABI of the CUDA library).
 
 The library is built in-tree by :mod:`unionml_b200._build` (``unionml_b200/_lib/libuml_b200.so``).  There is no
-CPU fallback: if the library is missing, or no B200 is visible, the product path raises - loudly.
+CPU fallback: if the library is missing, or no H100 is visible, the product path raises - loudly.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """``serve`` launcher: ``python -m unionml_b200.cli serve app:app --model-path model.joblib [uvicorn options]``.
 
-The reference's ``unionml serve`` (``/root/reference/unionml/cli.py:285-320``) is uvicorn's own CLI with one extra option,
+The reference's ``unionml serve`` (``unionml:unionml/cli.py:285-320``) is uvicorn's own CLI with one extra option,
 ``--model-path``, exported to the app as ``UNIONML_MODEL_PATH`` before uvicorn starts (the FastAPI startup hook loads the
 model from it, ``unionml/fastapi.py:22-34``).  Same here; the other reference commands (``init / deploy / train /
 predict / list-* / fetch-*``) talk to a Flyte cluster and are out of scope.  The CUDA engine is bound lazily by the

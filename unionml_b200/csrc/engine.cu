@@ -310,9 +310,9 @@ int uml_engine_create(uml_engine** out, int device_id) {
   cudaDeviceGetAttribute(&e->info.sm_clock_khz, cudaDevAttrClockRate, device_id);
   cudaDeviceGetAttribute(&e->info.mem_clock_khz, cudaDevAttrMemoryClockRate, device_id);
   strncpy(e->info.name, prop.name, sizeof(e->info.name) - 1);
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     char buf[256];
-    snprintf(buf, sizeof(buf), "device %d (%s) is compute capability %d.%d; this library is built for sm_100a only",
+    snprintf(buf, sizeof(buf), "device %d (%s) is compute capability %d.%d; this library is built for sm_90a only",
              device_id, prop.name, prop.major, prop.minor);
     g_create_error = buf;
     delete e;
@@ -1918,7 +1918,7 @@ static int mlp_predict_common(uml_engine* e, const uml_mlp* m, const uml_batch* 
   int launches = 0, path = 3;
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
   if (use_tc) {
-    NvtxRange r_score("uml:mlp_score_tcgen05");
+    NvtxRange r_score("uml:mlp_score_tc");
     bool need_rescore = false;
     UML_CUDA(e, uml::launch_mlp_tc(b->map, m->dm, out, exact, fl, e->info.sm_count, e->stream, &need_rescore));
     launches += 1;

@@ -1,7 +1,7 @@
-// Scoring kernels for the linear predictor  X . W^T + b -> argmax   (sm_100a).
+// Scoring kernels for the linear predictor  X . W^T + b -> argmax   (sm_90a).
 //
 // Replaces the numeric body of sklearn's LinearClassifierMixin.predict (sklearn/linear_model/_base.py:366-427), which
-// is what the reference's canonical predictor runs (/root/reference/README.md:87-92).
+// is what the reference's canonical predictor runs (unionml:README.md:87-92).
 //
 //  * linear_argmax_tma_kernel<C, EXACT>: persistent, warp-specialised.  One producer warp streams 128-row x 32-feature
 //    boxes of X (16 KiB, 128B-swizzled) through a shared-memory ring with TMA + mbarriers; eight consumer warps each
@@ -21,7 +21,7 @@
 #include "rescore_util.cuh"
 
 #ifndef UML_RESCORE_QUEUE_DEFAULT
-#define UML_RESCORE_QUEUE_DEFAULT 1  // same-box A/B (profiles/r02_ab.json): 10M rows 0.366 vs 0.368-0.373 ms, 1.25M rows 59.0 vs 61.7 us
+#define UML_RESCORE_QUEUE_DEFAULT 1  // one launch per step; the few flagged rows (0.02 % on digits) cost the queue little
 #endif
 
 
@@ -49,8 +49,8 @@ struct RowScore {
 // scored sixteen at a time (32 independent fp64 chains per lane), the sixteen sums are reduced with warp_reduce16 and
 // the arg-max / runner-up found by a butterfly over the lanes.  LOAD(f) yields feature f of the row as double.
 // w64 is feature-major, w64[f * S + c]: a lane fetches the classes of its feature with 16-byte loads off ONE address
-// (immediate offsets) - the class-major table this replaces cost a 64-bit multiply-add per weight, 52 % of the kernel's
-// instructions at F = 784 (profiles/r02_rescore_f64_f784_before.*).
+// (immediate offsets) - the class-major table this replaces cost a 64-bit multiply-add per weight, half of the kernel's
+// instructions at F = 784.
 template <typename LOAD>
 __device__ __forceinline__ RowScore score_row_f64(LOAD load, const double* __restrict__ w64, int S,
                                                   const double* __restrict__ b64, int F, int C, int lane) {
@@ -195,7 +195,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr int CP = (C + 1 + 3) / 4 * 4;    // padded columns of wt in shared memory (layout shared by both modes)
   constexpr int NW4 = (NCOL + 3) / 4;        // float4 loads of W per feature
   constexpr int R = kRowsPerLane;
-  constexpr bool USE_F2 = EXACT;  // packed fp32x2 FMA where it measured faster (see the accumulator comment below)
+  constexpr bool USE_F2 = EXACT;  // fp32x2 accumulator pairs (see the accumulator comment below)
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // SWIZZLE_128B wants 1 KiB alignment
@@ -276,9 +276,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       const int nv = static_cast<int>(min(static_cast<long long>(kConsumerWarps), (num_tiles - first + G - 1) / G));
       if (warp < nv) {
         const long long tile = first + warp * G;
-        // USE_F2 (EXACT kernels): class accumulators as fp32x2 pairs (classes 2i, 2i+1 -> one FFMA2, SASS FFMA2); an odd
-        // last class and the error-bound column (|x| is a free operand modifier on scalar FFMA) stay scalar.  Same-box
-        // A/B on 10M x 64 -> 10: EXACT 0.459 -> 0.397 ms with FFMA2, FAST 0.387 -> 0.416 ms (so FAST keeps scalar FFMA).
+        // USE_F2 (EXACT kernels): class accumulators as fp32x2 pairs (classes 2i, 2i+1 -> one fma2); an odd last class
+        // and the error-bound column (|x| is a free operand modifier on scalar FFMA) stay scalar.
         constexpr int NPAIR = C / 2;
         constexpr bool ODD = (C & 1) != 0;
         uint64_t acc2[R][NPAIR > 0 ? NPAIR : 1];
@@ -826,7 +825,7 @@ static cudaError_t dispatch_classes(int C, const CUtensorMap& xmap, const TmaKer
 bool linear_queue_rescore() {
   // UML_B200_RESCORE_MODE=queue: flagged rows go through a shared-memory queue to a tenth warp of the tile kernel that
   // re-scores them in fp64 while the other warps keep streaming (one launch per step); =kernel: flag list in global
-  // memory + rescore_f64_kernel behind the tile kernel (two launches).  Default below, chosen by same-box A/B.
+  // memory + rescore_f64_kernel behind the tile kernel (two launches).  Default below.
   static const int mode = [] {
     const char* env = getenv("UML_B200_RESCORE_MODE");
     if (env && env[0] == 'q') return 1;

@@ -1,7 +1,7 @@
 // Scoring kernels for the 2-layer MLP predictor  argmax(softmax(W2 relu(W1 x + b1) + b2)) = argmax of the logits.
 //
 // Replaces PytorchModel.forward + .argmax(1) of the reference's torch quickstart
-// (/root/reference/tests/integration/pytorch_app/quickstart.py:14-24, 68-70; hyperparameters 64 -> 32 -> 10 at :80).
+// (unionml:tests/integration/pytorch_app/quickstart.py:14-24, 68-70; hyperparameters 64 -> 32 -> 10 at :80).
 //
 //  * mlp_argmax_tma_kernel<H, C, EXACT>: the same persistent TMA + mbarrier ring (128-row x 32-feature boxes) as the
 //    linear kernel; consumer warps work in pairs on a box (64 rows each, 2 rows x H hidden accumulators per lane).  Layer 1 runs per
@@ -22,7 +22,7 @@
 #include "mlp_rescore.cuh"
 
 #ifndef UML_MLP_UNROLL_Q
-#define UML_MLP_UNROLL_Q 8  // feature-quad unroll of the layer-1 loop (same-box A/B, EXACT: 1 -> 1.120, 2 -> 1.056, 4 -> 1.023, 8 -> 1.015 ms)
+#define UML_MLP_UNROLL_Q 8  // feature-quad unroll of the layer-1 loop
 #endif
 #define UML_PRAGMA_(x) _Pragma(#x)
 #define UML_UNROLL(n) UML_PRAGMA_(unroll n)

@@ -1,10 +1,11 @@
-// Tensor-core scoring kernel for the 2-layer MLP predictor (cfg 5): layer 1 on tcgen05 (kind::tf32), accumulators in TMEM.
+// Tensor-core scoring kernel for the 2-layer MLP predictor (cfg 5): layer 1 on Hopper wgmma (tf32), fp32 accumulators
+// in the registers of the consuming warpgroup.
 //
-// Replaces PytorchModel.forward + .argmax(1) of the reference's torch quickstart
-// (/root/reference/tests/integration/pytorch_app/quickstart.py:14-24, 68-70; hyperparameters 64 -> 32 -> 10 at :80).
+// Replaces PytorchModel.forward + .argmax(1) of UnionML's torch quickstart
+// (tests/integration/pytorch_app/quickstart.py:14-24, 68-70; hyperparameters 64 -> 32 -> 10 at :80).
 //
 // Why tensor cores here and not in the linear kernel: layer 1 is a real [rows x F] . [F x H] contraction (4 096 of the
-// 4 736 flop per row); on CUDA cores it needs 1 408 FFMA2 per row and caps the kernel at 0.37 of the HBM roofline.
+// 4 736 flop per row); on CUDA cores it is the bulk of the kernel's FMA issue.
 //
 // Exactness with 10-bit tf32 mantissas.  The MMA multiplies tf32 x tf32 exactly and accumulates in fp32, so the only
 // approximation is what the operands lose when they become tf32:
@@ -13,51 +14,48 @@
 //     re-checked here (scan warps OR the low bits): a row that is not tf32-exact gets A1 = +inf and is therefore
 //     flagged for the fp64 re-score, so the answer is right for any input - only slower.
 //   * W1: split on the host as w = hi + lo + r with hi, lo tf32 (round to nearest) and |r| <= 2^-22 |w|; B holds
-//     [hi | lo] as 2H columns, so ONE MMA per K step yields main = x.hi and small = x.lo in separate TMEM columns
-//     (the small terms never lose bits against the large accumulator), summed in fp32 in the epilogue.
+//     [hi | lo] as 2H columns, so ONE MMA per K step yields main = x.hi and small = x.lo in separate accumulator
+//     columns (the small terms never lose bits against the large accumulator), summed in fp32 in the epilogue.
 // EXACT mode bounds the error per row, |h_n - h_n_true| <= E1 = (32 n_mma + 12) 2^-24 A1 with
 // A1 = max|b1| + sum_f |x_f| max_n |w1_nf| (n_mma = F_pad / 8 accumulating MMA steps; the per-step term covers a
 // truncating 9-addend aligner with no guard bits, DESIGN.md 3.3), propagates it through layer 2 exactly like the
 // CUDA-core kernel, and re-scores rows whose logit margin is inside the bound in fp64 (mlp_rescore_f64_kernel).
 //
-// Roles (14 warps, one CTA per SM, persistent over 128-row tiles):
-//   warp 12 : TMA producer - 128 x 32 fp32 boxes of X (16 KiB, SWIZZLE_128B) into an S-stage ring
-//   warp 13 : MMA issuer   - one lane; per box 4 x tcgen05.mma (M128, N=2H, K8) from the box (A, K-major SW128) and
-//             the resident W1 tile (B); tcgen05.commit frees the ring stage / publishes the accumulator
-//   warps 0-3 : scan        - thread per row: A1 bound + tf32-exactness of the row from the same box (LDS.128)
-//   warps 4-11: epilogue    - two sets of four warps taking alternate tiles (the first ncu capture showed one set
-//             80 % busy and everything else waiting on it): tcgen05.ld the row's 2H accumulators, + b1, ReLU, layer 2
-//             from constant-bank operands, argmax (first maximum wins), margin guard, label store (+ peer stores)
+// Roles (13 warps, one CTA per SM, persistent over 128-row tiles):
+//   warp 12  : TMA producer - 128 x 32 fp32 boxes of X (16 KiB, SWIZZLE_128B) into an S-stage ring
+//   warps 0-3: scan         - thread per row: A1 bound + tf32-exactness of the row from the same box (LDS.128)
+//   warps 4-7, 8-11: two consumer warpgroups taking alternate tiles, so one runs its epilogue while the other's MMAs
+//             are in flight.  Per box 2 x 4 wgmma m64nNk8 (N = 2H; rows 0-63 and 64-127 of the box as A, K-major SW128,
+//             the resident W1 tile as B), then from the accumulator registers: + b1, ReLU, layer 2 over the lane's
+//             hidden units, a quad reduce-scatter that leaves each lane one row's logits, argmax (first maximum
+//             wins), margin guard, label store (+ peer stores)
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
 
 #include "uml_common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include "mlp_rescore.cuh"
 
 #ifndef UML_MLP_QUEUE_DEFAULT
-// 0: the queue variant lost the same-box A/B (profiles/r02_ab.json: 10M rows 0.640 vs 0.577 ms per step) - the scoring
-// kernel is issue-bound (68 % issue slots), so the 58 000 fp64 rows it takes in slow the pipeline by more than the
-// separate re-score kernel costs.  (The linear tile kernel, with 0.02 % flagged rows, wins with its queue.)
+// 0: flagged rows go to the separate fp64 re-score kernel.  The queue variant re-scores them inside the scoring launch,
+// where the fp64 work competes for issue slots with the epilogue warps that bound this kernel.
 #define UML_MLP_QUEUE_DEFAULT 0
 #endif
 
 namespace uml {
 
-constexpr int kTcThreads = 448;
+constexpr int kTcThreads = 416;
 constexpr int kTcProducerWarp = 12;
-constexpr int kTcMmaWarp = 13;
 // QUEUE kernels: rows flagged by the epilogue warps are re-scored in fp64 by four more warps of the same launch while
 // the tensor-core pipeline keeps streaming (fp64 units and these issue slots are otherwise idle)
 constexpr int kTcRescoreWarps = 4;
-constexpr int kTcFirstRescoreWarp = 14;
+constexpr int kTcFirstRescoreWarp = 13;
 constexpr int kTcThreadsQueue = kTcThreads + 32 * kTcRescoreWarps;
 constexpr int kTcEpilogueWarps = 8;
 constexpr int kTcQueueCap = 1024;       // power of two
 constexpr int kTcQueueHeadroom = 512;   // a warp publishes only while this many slots are free (8 warps x 32 rows at once)
-constexpr int kTcAccStages = 4;    // TMEM accumulator stages (tiles in flight between MMA and epilogue)
 constexpr int kTcSlots = 24;       // A1 hand-off slots (scan -> epilogue); > the scan warps' maximum lead over the epilogue
 constexpr int kTcMaxFpad = 128;    // features (padded to 32) the resident W1 tile is sized for
 
@@ -70,7 +68,7 @@ struct MlpTcParams {
   float w1max[kTcMaxFpad];  // max_n |w1_nf| per feature (zero padded)
   float b1max;
   float e1_scale, e2_scale;
-  const float* w1_tiles;    // [KC][2H rows][32 floats], rows 128-byte swizzled exactly as the UMMA descriptor reads them
+  const float* w1_tiles;    // [KC][2H rows][32 floats], rows 128-byte swizzled exactly as the wgmma descriptor reads them
   int32_t* labels;
   void* peers[8];
   int n_peers;
@@ -100,15 +98,16 @@ __device__ __forceinline__ void tc_store_final_label(const MlpTcParams<H, C>& p,
   }
 }
 
+// consumer lane l of warp wq (in its warpgroup) ends the epilogue owning one row of the 128-row tile: the quad
+// (l / 4) holds rows 16 wq + l / 4 (+ 8) of both 64-row halves, and lane l % 4 keeps the (half, +8) pair it names
+__device__ __forceinline__ int tc_row_of_lane(int wq, int l) { return 64 * ((l & 3) >> 1) + 16 * wq + (l >> 2) + 8 * (l & 1); }
+
 template <int H, int C, bool EXACT, bool QUEUE>
 __global__ void __launch_bounds__(kTcThreadsQueue, 1)
 mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ MlpTcParams<H, C> p) {
-  constexpr int N = 2 * H;  // accumulator columns per tile: [main | small]
-  constexpr int TMEM_COLS = kTcAccStages * N;
-  static_assert(TMEM_COLS == 128 || TMEM_COLS == 256 || TMEM_COLS == 512, "TMEM columns must be a power of two");
-  static_assert(N % 16 == 0 && N <= 256, "UMMA M=128 needs N % 16 == 0");
-  constexpr int CP = MlpTcParams<H, C>::CP;
-  constexpr uint32_t IDESC = umma_idesc_tf32(128, N);
+  constexpr int N = 2 * H;     // accumulator columns per row: [main | small]
+  constexpr int NACC = N / 2;  // fp32 accumulator registers per thread and 64-row half
+  static_assert(N == 32 || N == 64, "wgmma kind tf32 is instantiated for N in {32, 64}");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -119,13 +118,10 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
   float* a1_s = reinterpret_cast<float*>(btile + static_cast<size_t>(KC) * N * 128);  // [kTcSlots][128]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(a1_s + kTcSlots * kTileRows);
   uint64_t* empty_bar = full_bar + S;
-  uint64_t* dfull_bar = empty_bar + S;
-  uint64_t* dempty_bar = dfull_bar + kTcAccStages;
-  uint64_t* a1_bar = dempty_bar + kTcAccStages;
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(a1_bar + kTcSlots);
+  uint64_t* a1_bar = empty_bar + S;
   // QUEUE kernels: flagged-row queue (slot = row + 1, 0 = empty; ctl: 0 tail reserved, 1 head claimed, 2 epilogue
   // warps done, 3 slots consumed), then the fp64 weights and one strip per epilogue / re-score warp
-  int* q_slots = reinterpret_cast<int*>(tmem_base_s + 4);
+  int* q_slots = reinterpret_cast<int*>(a1_bar + kTcSlots);
   int* q_ctl = q_slots + kTcQueueCap;
   double* rs_area = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(q_ctl + 4) + 15u) & ~static_cast<uintptr_t>(15));  // 16-byte copies
 
@@ -150,21 +146,13 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1 + 4);  // tcgen05.commit + the four scan warps
-    }
-    for (int a = 0; a < kTcAccStages; ++a) {
-      mbar_init(&dfull_bar[a], 1);
-      mbar_init(&dempty_bar[a], 4);  // the four epilogue warps
+      mbar_init(&empty_bar[s], 1 + 4);  // the consuming warpgroup + the four scan warps
     }
     for (int s = 0; s < kTcSlots; ++s) mbar_init(&a1_bar[s], kTileRows);  // every scan thread arrives for its own row
     fence_barrier_init();
   }
-  if (warp == kTcMmaWarp) tmem_alloc<TMEM_COLS>(tmem_base_s);
-  fence_proxy_async_smem();  // the W1 tile was written with st.shared; UMMA reads it through the async proxy
-  tcgen05_fence_before();
+  fence_proxy_async_smem();  // the W1 tile was written with st.shared; wgmma reads it through the async proxy
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_s;
 
   pdl_launch_dependents();  // the fp64 re-score behind this launch may stage its weights while this grid runs
   const long long G = gridDim.x;
@@ -183,36 +171,6 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
           mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
           tma_load_2d(ring + static_cast<size_t>(stage) * kStageBytes, &xmap, &full_bar[stage], k * kChunkF,
                       static_cast<int>(tile * kTileRows), policy);
-          if (++stage == S) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (warp == kTcMmaWarp) {
-    // ===================== MMA issuer (one lane) =====================
-    if (elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t it = 0;
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += G, ++it) {
-        const uint32_t acc = it % kTcAccStages;
-        const uint32_t acc_phase = (it / kTcAccStages) & 1u;
-        const uint32_t d_tmem = tmem_base + acc * N;
-        for (int k = 0; k < KC; ++k) {
-          mbar_wait_relaxed(&full_bar[stage], phase);
-          if (k == 0) mbar_wait_relaxed(&dempty_bar[acc], acc_phase ^ 1u);  // epilogue has drained this accumulator
-          tcgen05_fence_after();
-          const uint32_t a_base = smem_u32(ring + static_cast<size_t>(stage) * kStageBytes);
-          const uint32_t b_base = smem_u32(btile + static_cast<size_t>(k) * N * 128);
-#pragma unroll
-          for (int j = 0; j < kChunkF / 8; ++j) {  // K = 8 tf32 (32 bytes) per MMA
-            umma_tf32_ss(d_tmem, umma_desc_k_sw128(a_base + j * 32), umma_desc_k_sw128(b_base + j * 32), IDESC,
-                         (k | j) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);               // ring stage free once these MMAs have read it
-          if (k == KC - 1) umma_commit(&dfull_bar[acc]);  // accumulator complete
           if (++stage == S) {
             stage = 0;
             phase ^= 1u;
@@ -259,45 +217,88 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
       mbar_arrive(&a1_bar[slot]);  // release: this thread's A1 is visible to whoever completes the wait
     }
   } else if (warp < 4 + kTcEpilogueWarps) {
-    // ===================== epilogue warps 4..11: TMEM lane = row; set 0 (warps 4-7) even tiles, set 1 odd tiles ====
-    const int wq = warp & 3;  // a warp may only touch TMEM lanes 32 * (warp % 4) .. + 31
+    // ===================== consumer warpgroups: warps 4-7 even tiles, warps 8-11 odd tiles =====================
+    // layer 1 as two m64 wgmma chains (rows 0-63, 64-127 of the tile) per K step, then the epilogue from the registers
+    const int wq = warp & 3;
     const int set = (warp - 4) >> 2;
-    const int row_in_tile = wq * 32 + lane;
+    const int q = lane & 3;
+    const int row_in_tile = tc_row_of_lane(wq, lane);
     uint32_t it = static_cast<uint32_t>(set);
     for (long long tile = blockIdx.x + set * G; tile < num_tiles; tile += 2 * G, it += 2) {
-      const uint32_t acc = it % kTcAccStages;
-      const uint32_t acc_phase = (it / kTcAccStages) & 1u;
-      const uint32_t slot = it % kTcSlots;
-      const uint32_t slot_phase = (it / kTcSlots) & 1u;
-      mbar_wait_bounded(&dfull_bar[acc], acc_phase);
-      mbar_wait_bounded(&a1_bar[slot], slot_phase);
-      tcgen05_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16) + acc * N;
-      uint32_t vmain[H], vsmall[H];
-      if constexpr (H == 32) {
-        tmem_ld_32x32b_x32(taddr, vmain);
-        tmem_ld_32x32b_x32(taddr + H, vsmall);
-      } else {
-        tmem_ld_32x32b_x16(taddr, vmain);
-        tmem_ld_32x32b_x16(taddr + H, vsmall);
+      // the ring carries this CTA's tiles in order, KC chunks each: chunk k of local tile `it` is number it * KC + k
+      const uint32_t first_chunk = it * static_cast<uint32_t>(KC);
+      float acc[2][NACC];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < NACC; ++r) {
+          acc[h][r] = 0.f;
+          wgmma_fence_operand(acc[h][r]);
+        }
+      wgmma_fence();
+      for (int k = 0; k < KC; ++k) {
+        const uint32_t chunk = first_chunk + static_cast<uint32_t>(k);
+        const uint32_t stage = chunk % static_cast<uint32_t>(S);
+        mbar_wait_bounded(&full_bar[stage], (chunk / static_cast<uint32_t>(S)) & 1u);
+        const uint32_t a_base = smem_u32(ring + static_cast<size_t>(stage) * kStageBytes);
+        const uint32_t b_base = smem_u32(btile + static_cast<size_t>(k) * N * 128);
+#pragma unroll
+        for (int j = 0; j < kChunkF / 8; ++j) {  // K = 8 tf32 (32 bytes) per MMA
+          const uint32_t scale_d = (k | j) != 0 ? 1u : 0u;
+          const uint64_t b_desc = wgmma_desc_k_sw128(b_base + j * 32);
+          WgmmaTf32<N>::mma(acc[0], wgmma_desc_k_sw128(a_base + j * 32), b_desc, scale_d);
+          WgmmaTf32<N>::mma(acc[1], wgmma_desc_k_sw128(a_base + 64 * 128 + j * 32), b_desc, scale_d);
+        }
       }
-      tmem_ld_wait();
+      wgmma_commit();
+      const uint32_t slot = it % kTcSlots;
+      mbar_wait_bounded(&a1_bar[slot], (it / kTcSlots) & 1u);
+      // read before the ring stages are released: the scan warps cannot reach this slot's next tile until they are
       const float a1 = a1_s[slot * kTileRows + row_in_tile];
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&dempty_bar[acc]);  // accumulator (and A1 slot) read: the MMA warp may reuse it
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < NACC; ++r) wgmma_fence_operand(acc[h][r]);
+      if (wq == 0 && lane == 0)
+        for (int k = 0; k < KC; ++k) mbar_arrive(&empty_bar[(first_chunk + static_cast<uint32_t>(k)) % static_cast<uint32_t>(S)]);
 
-      // ---- + b1, ReLU, layer 2 (weights are constant-bank operands of the FMAs), argmax ----
+      // ---- + b1, ReLU, layer 2 over this lane's hidden units for the quad's four rows ----
+      // row j of the quad: half j >> 1, + 8 for odd j; this lane's hidden units n = 8 i + 2 q + e (i < H / 8, e < 2):
+      // main term acc[j >> 1][4 i + 2 (j & 1) + e], small term the same entry of column group i + H / 8
       constexpr int NZ = C + (EXACT ? 1 : 0);
+      float part[4][NZ];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int c = 0; c < NZ; ++c) part[j][c] = 0.f;
+#pragma unroll
+        for (int i = 0; i < H / 8; ++i)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = 8 * i + 2 * q + e;
+            const int at = 4 * i + 2 * (j & 1) + e;
+            const float hv = fmaxf((acc[j >> 1][at + 4 * (H / 8)] + acc[j >> 1][at]) + p.b1[n], 0.f);
+#pragma unroll
+            for (int c = 0; c < NZ; ++c) part[j][c] = fmaf(hv, p.w2[n][c], part[j][c]);
+          }
+      }
+      // quad reduce-scatter: lane q ends with the complete logits of row j = q (xor 2 splits the rows by half, xor 1
+      // by the + 8 pair)
+      const bool hi2 = (q & 2) != 0, hi1 = (q & 1) != 0;
       float z[NZ];
 #pragma unroll
-      for (int c = 0; c < NZ; ++c) z[c] = p.b2[c];
+      for (int c = 0; c < NZ; ++c) {
+        float s[2];
 #pragma unroll
-      for (int n = 0; n < H; ++n) {
-        const float h = (__uint_as_float(vsmall[n]) + __uint_as_float(vmain[n])) + p.b1[n];
-        const float hv = fmaxf(h, 0.f);
-#pragma unroll
-        for (int c = 0; c < NZ; ++c) z[c] = fmaf(hv, p.w2[n][c], z[c]);
+        for (int r = 0; r < 2; ++r) {
+          const float keep = hi2 ? part[2 + r][c] : part[r][c];
+          const float send = hi2 ? part[r][c] : part[2 + r][c];
+          s[r] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+        }
+        const float keep = hi1 ? s[1] : s[0];
+        const float send = hi1 ? s[0] : s[1];
+        z[c] = (keep + __shfl_xor_sync(0xffffffffu, send, 1)) + p.b2[c];
       }
       const long long row = tile * kTileRows + row_in_tile;
       float best = z[0];
@@ -320,11 +321,18 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
           for (int i = 0; i < p.n_peers; ++i) static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idx;
       }
       if (p.wire_u8 && p.n_peers > 0) {
-        // byte labels: lanes 0..7 gather 4 consecutive rows each -> the warp's 32 labels leave as eight 4-byte words
+        // byte labels: the warp's rows are two runs of 16 (rows 16 wq + 0..15 of each half); lanes 0..7 gather 4
+        // consecutive rows each -> the warp's 32 labels leave as eight 4-byte words
+        const int run = (lane >> 2) & 1;
+        const int r0 = 4 * (lane & 3);
         uint32_t word = 0;
 #pragma unroll
-        for (int t = 0; t < 4; ++t) word |= (static_cast<uint32_t>(__shfl_sync(0xffffffffu, idx, (4 * lane + t) & 31)) & 0xffu) << (8 * t);
-        const long long row4 = tile * kTileRows + wq * 32 + 4 * lane;
+        for (int t = 0; t < 4; ++t) {
+          const int r = (r0 + t) & 15;
+          const int src = 4 * (r & 7) + 2 * run + (r >> 3);  // the lane that owns row r of the run
+          word |= (static_cast<uint32_t>(__shfl_sync(0xffffffffu, idx, src)) & 0xffu) << (8 * t);
+        }
+        const long long row4 = tile * kTileRows + 64 * run + 16 * wq + r0;
         const long long at = p.row_offset + row4;
         if (lane < 8) {
           if (row4 + 3 < p.n_rows && (at & 3) == 0) {
@@ -369,7 +377,7 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
               while (m2 != 0u) {
                 const int l = __ffs(static_cast<int>(m2)) - 1;
                 m2 &= m2 - 1u;
-                const long long frow = tile * kTileRows + wq * 32 + l;
+                const long long frow = tile * kTileRows + tc_row_of_lane(wq, l);
                 const MlpRowResult r = mlp_rs_row(rs_view, p.x + frow * p.ld, xs, xs + p.n_in, lane);
                 if (lane == 0) {
                   tc_store_final_label(p, frow, r.idx);
@@ -399,7 +407,7 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
       }
     }
   } else {
-    // ===================== re-score warps 14..17 (QUEUE kernels): fp64 rows from the queue =====================
+    // ===================== re-score warps 13..16 (QUEUE kernels): fp64 rows from the queue =====================
     if constexpr (EXACT && QUEUE) {
       double* xs = rs_strips + (kTcEpilogueWarps + (warp - kTcFirstRescoreWarp)) * mlp_rs_strip_doubles(p.n_in, H);
       int n_done = 0;
@@ -441,13 +449,6 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
       if (lane == 0 && n_done > 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n_done));
     }
   }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == kTcMmaWarp) {
-    tcgen05_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -464,7 +465,7 @@ static float tf32_round(float v) {  // round to nearest tf32 (10 mantissa bits),
 }
 
 // B operand of layer 1: per 32-feature chunk, 2H rows ([hi rows | lo rows]) of 32 floats, each row's 16-byte chunks
-// XOR-swizzled by (row & 7) - the SWIZZLE_128B K-major layout the UMMA descriptor (and TMA) use
+// XOR-swizzled by (row & 7) - the SWIZZLE_128B K-major layout the wgmma descriptor (and TMA) use
 std::vector<float> mlp_tc_build_w1_tiles(const float* w1 /*[H][F]*/, int H, int F, int f_pad) {
   const int KC = f_pad / kChunkF, N = 2 * H;
   std::vector<float> tiles(static_cast<size_t>(KC) * N * 32, 0.f);
@@ -487,7 +488,7 @@ std::vector<float> mlp_tc_build_w1_tiles(const float* w1 /*[H][F]*/, int H, int 
 static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool queue) {
   const size_t kc = m.f_pad / kChunkF;
   size_t bytes = 1024 + kc * (2 * m.n_hidden) * 128 + static_cast<size_t>(kTcSlots) * kTileRows * 4 +
-                 (2 * 64 + 2 * kTcAccStages + kTcSlots) * 8 + 16;
+                 (2 * 64 + kTcSlots) * 8 + 16;
   if (queue)  // flagged-row queue + fp64 weights + one strip per epilogue / re-score warp
     bytes += (kTcQueueCap + 4) * 4 + 16 +
              (mlp_rs_weight_doubles(m.n_in, m.n_hidden, m.n_classes) +
@@ -573,8 +574,9 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kStageBytes);
   stages = std::min(stages, 64);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(4, std::min(stages, atoi(env)));
-  // the A1 hand-off has kTcSlots slots: the scan warps lead the epilogue by at most S / KC + 1 + kTcAccStages tiles
-  stages = std::min(stages, (kTcSlots - 2 - kTcAccStages) * p.kc);
+  // the A1 hand-off has kTcSlots slots: a consumer reads its tile's A1 before it frees the tile's ring stages, so the
+  // scan warps lead it by at most S / KC tiles
+  stages = std::min(stages, (kTcSlots - 2) * p.kc);
   p.num_stages = stages;
   p.flag_count = flags.count;
   p.flag_rows = flags.rows;

@@ -1,7 +1,7 @@
 // Staging kernels: feature rows in the caller's dtype/order (already copied to a device scratch chunk) -> the
 // engine's resident layout: fp32 row-major [rows][ld] (optionally also an fp64 row-major copy for exact re-scoring).
 //
-// Replaces the host-side pandas/numpy copies of Dataset.get_features (/root/reference/unionml/dataset.py:350-359,
+// Replaces the host-side pandas/numpy copies of Dataset.get_features (unionml:unionml/dataset.py:350-359,
 // 506-520: pd.DataFrame(features)[cols]) and sklearn's check_array finiteness scan
 // (sklearn/utils/validation.py:107): the scan for NaN/Inf and the "is the fp32 copy lossless" test are fused into
 // the conversion pass, so each element is touched once.
@@ -210,7 +210,7 @@ static cudaError_t launch_typed(const void* src, bool feature_major, long long p
   if (sm_count == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0) sm_count = 148;
+    if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0) sm_count = 132;
   }
   const T* s = static_cast<const T*>(src);
   if (feature_major) {
@@ -367,7 +367,7 @@ cudaError_t launch_labels_take(const void* labels, int label_bytes, int64_t n, c
                                double* out, cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
   const long long want = (n + 255) / 256;
-  const int grid = static_cast<int>(want < 148 * 16 ? want : 148 * 16);
+  const int grid = static_cast<int>(want < 132 * 16 ? want : 132 * 16);
   labels_take_kernel<<<grid, 256, 0, stream>>>(labels, label_bytes, n, classes, n_classes, out);
   return cudaGetLastError();
 }
@@ -377,7 +377,7 @@ cudaError_t launch_labels_count_equal(const void* labels, int label_bytes, int64
                                       cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
   const long long want = (n + 255) / 256;
-  const int grid = static_cast<int>(want < 148 * 8 ? want : 148 * 8);
+  const int grid = static_cast<int>(want < 132 * 8 ? want : 132 * 8);
   labels_count_equal_kernel<<<grid, 256, 0, stream>>>(labels, label_bytes, n, classes, n_classes, targets, count);
   return cudaGetLastError();
 }
@@ -388,12 +388,12 @@ cudaError_t launch_finite_scan(const float* x, int64_t ld, int64_t rows, int n_f
   if (ld == n_features && (ld % 4) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
     const long long n4 = rows * ld / 4;
     const long long want4 = (n4 + 255) / 256;
-    const int grid4 = static_cast<int>(want4 < 148 * 32 ? (want4 < 1 ? 1 : want4) : 148 * 32);
+    const int grid4 = static_cast<int>(want4 < 132 * 32 ? (want4 < 1 ? 1 : want4) : 132 * 32);
     finite_scan_dense_kernel<<<grid4, 256, 0, stream>>>(reinterpret_cast<const float4*>(x), n4, result);
     return cudaGetLastError();
   }
   const long long want = (rows * ld + 255) / 256;
-  const int grid = static_cast<int>(want < 148 * 16 ? (want < 1 ? 1 : want) : 148 * 16);
+  const int grid = static_cast<int>(want < 132 * 16 ? (want < 1 ? 1 : want) : 132 * 16);
   finite_scan_kernel<<<grid, 256, 0, stream>>>(x, ld, rows, n_features, result);
   return cudaGetLastError();
 }

@@ -1,4 +1,4 @@
-// PTX building blocks of the TMA + mbarrier shared-memory ring used by the scoring kernels (sm_100a).
+// PTX building blocks of the TMA + mbarrier shared-memory ring used by the scoring kernels (sm_90a).
 #pragma once
 
 #include <cuda.h>
@@ -61,8 +61,8 @@ __device__ __forceinline__ bool elect_one_sync() {
   return pred != 0;
 }
 
-// packed fp32x2 FMA (sm_100 FFMA2): two independent IEEE fp32 FMAs per instruction - halves the issue slots of the
-// FMA-bound inner loops; a (x, x) pair folds into a scalar-broadcast operand in SASS
+// a pair of fp32 lanes as one 64-bit value: fma2 is two independent IEEE fp32 FMAs (sm_90 has no packed FFMA2, so it
+// issues two FFMA; the results are those of two fmaf calls)
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -72,9 +72,11 @@ __device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  unpack2(c, c0, c1);
+  return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
 // programmatic dependent launch (PDL): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may be

@@ -1,4 +1,4 @@
-// Shared declarations for the uml_b200 CUDA library (sm_100a only).
+// Shared declarations for the uml_b200 CUDA library (sm_90a only).
 #pragma once
 
 #include <cuda.h>

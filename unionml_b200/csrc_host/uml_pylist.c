@@ -1,4 +1,4 @@
-/* CPython glue for the predictor contract `-> List[float]` (/root/reference/README.md:87-92).
+/* CPython glue for the predictor contract `-> List[float]` (unionml:README.md:87-92).
  *
  * The canonical predictor returns `[float(x) for x in estimator.predict(features)]`: one Python float per row.
  * Creating 10M float objects costs ~0.25 s on the GPU box's host - more than the whole H2D + GPU pipeline (0.12 s).

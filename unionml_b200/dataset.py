@@ -1,6 +1,6 @@
 """``Dataset``: the data side of the decorator protocol, for the predict (and local train) slice.
 
-Mirrors the public surface of ``/root/reference/unionml/dataset.py`` that the hot path touches - ``reader``,
+Mirrors the public surface of ``unionml:unionml/dataset.py`` that the hot path touches - ``reader``,
 ``loader``, ``splitter``, ``parser``, ``feature_loader``, ``feature_transformer``, ``get_data``, ``get_features`` -
 with the same defaults and the same quirks, but without flytekit: functions are plain closures called in-process
 (the reference wraps each in a flytekit task and round-trips every DataFrame through a StructuredDataset).
@@ -31,7 +31,7 @@ class Dataset:
         shuffle: bool = True,
         random_state: int = 12345,
     ):
-        # same defaults as /root/reference/unionml/dataset.py:44-53
+        # same defaults as unionml:unionml/dataset.py:44-53
         self.name = name
         self._features: List[str] = [] if features is None else features
         self._targets = targets

@@ -2,7 +2,7 @@
 
 This is the device path that ``unionml_b200.model.Model.predict``, ``unionml_b200.fastapi.serving_app`` and
 ``unionml_b200.services`` all call (the reference reaches its CPU arithmetic through
-``self._predictor(model_object, features)``, ``/root/reference/unionml/model.py:606,642``).
+``self._predictor(model_object, features)``, ``unionml:unionml/model.py:606,642``).
 """
 from __future__ import annotations
 
@@ -160,7 +160,7 @@ class Engine:
         if st != N.UML_OK:
             msg = (lib.uml_last_error(None) or b"").decode()
             if st == N.UML_ERR_NO_DEVICE:
-                raise RuntimeError(f"unionml_b200 needs a B200 (sm_100a) and has no CPU fallback: {msg}")
+                raise RuntimeError(f"unionml_b200 needs an H100 (sm_90a) and has no CPU fallback: {msg}")
             _raise(st, msg)
         self._h = h.value
         self.device = int(device)

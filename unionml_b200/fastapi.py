@@ -1,6 +1,6 @@
 """FastAPI binding of the device predict path: ``POST /predict``, ``GET /health``, ``GET /``.
 
-Behaviour follows ``/root/reference/unionml/fastapi.py:15-70``:
+Behaviour follows ``unionml:unionml/fastapi.py:15-70``:
 
 * at startup the model object is loaded from ``UNIONML_MODEL_PATH`` unless the ``Model`` already carries an artifact
   (ref. 22-34).  The CUDA engine is *not* touched here: it is bound lazily by the first predict inside the worker
@@ -23,7 +23,7 @@ from unionml_b200.model import Model, ModelArtifact
 
 _INDEX_PAGE = (
     "<html><head><title>unionml</title></head>"
-    "<body><h1>unionml</h1><p>B200 batch-prediction engine behind the UnionML predictor API</p></body></html>"
+    "<body><h1>unionml</h1><p>H100 batch-prediction engine behind the UnionML predictor API</p></body></html>"
 )
 _NO_MODEL_PATH = (
     "Model artifact path not specified. Make sure to specify the unionml serve --model-path in "

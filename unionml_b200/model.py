@@ -1,6 +1,6 @@
 """``Model``: the model side of the decorator protocol with a local, in-process executor.
 
-Mirrors the surface of ``/root/reference/unionml/model.py`` that the predict hot path (and the local ``train`` of the
+Mirrors the surface of ``unionml:unionml/model.py`` that the predict hot path (and the local ``train`` of the
 README digits app) touches: ``init / trainer / predictor / evaluator / saver / loader`` decorators, prediction
 callbacks, ``train``, ``predict``, ``save``, ``load``, ``load_from_env``, ``serve``, ``resolve_model_artifact``.
 

@@ -1,8 +1,8 @@
-"""Drop-in predictors for ``@model.predictor`` backed by the B200 engine.
+"""Drop-in predictors for ``@model.predictor`` backed by the H100 engine.
 
-The reference's canonical predictor (``/root/reference/README.md:87-92``,
-``/root/reference/tests/integration/sklearn_app/quickstart.py:24-26``,
-``/root/reference/unionml/templates/basic/{{cookiecutter.app_name}}/app.py:26-28``) is::
+The reference's canonical predictor (``unionml:README.md:87-92``,
+``unionml:tests/integration/sklearn_app/quickstart.py:24-26``,
+``unionml:unionml/templates/basic/{{cookiecutter.app_name}}/app.py:26-28``) is::
 
     @model.predictor
     def predictor(estimator: LogisticRegression, features: pd.DataFrame) -> List[float]:
@@ -11,7 +11,7 @@ The reference's canonical predictor (``/root/reference/README.md:87-92``,
 ``linear_argmax`` has the same contract (one ``features`` argument, ``List[float]`` of class labels, inputs
 borrowed and left untouched, sklearn's ``ValueError`` / ``NotFittedError`` on bad input) but computes
 ``X @ coef_.T + intercept_ -> argmax -> classes_.take`` (``sklearn/linear_model/_base.py:366-427``) on the GPU.
-There is no CPU fallback: without the CUDA library or a B200 the call raises.
+There is no CPU fallback: without the CUDA library or an H100 the call raises.
 """
 
 import os

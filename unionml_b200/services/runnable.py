@@ -1,6 +1,6 @@
 """The runner entry point of the reference's BentoML binding, without BentoML.
 
-``/root/reference/unionml/services/bentoml.py:190-213`` defines ``UnionMLRunnable.predict`` as::
+``unionml:unionml/services/bentoml.py:190-213`` defines ``UnionMLRunnable.predict`` as::
 
     features = self.model.dataset.get_features(features)
     return self.model.predict(features=features)

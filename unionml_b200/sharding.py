@@ -1,6 +1,6 @@
 """Row sharding across GPUs: one process per GPU, W/b replicated, labels exchanged once.
 
-The reference has no distributed path (scale-out = independent Flyte pods, ``/root/reference/unionml/model.py:1160-1226``);
+The reference has no distributed path (scale-out = independent Flyte pods, ``unionml:unionml/model.py:1160-1226``);
 rows are independent, so rank r scores a contiguous row block ``[r*N/G, (r+1)*N/G)`` and every rank ends up with the
 full label vector (SURVEY.md 8e).  Exchange back-ends:
 

@@ -1,6 +1,6 @@
 """Registration-time signature checks for the decorator protocol.
 
-Same contract as the reference's guards (``/root/reference/unionml/type_guards.py``): a mismatch raises ``TypeError``
+Same contract as the reference's guards (``unionml:unionml/type_guards.py``): a mismatch raises ``TypeError``
 when the function is *registered*, never at predict time.  The rules that matter to the predict path:
 
 * ``guard_predictor`` (ref. 151-169): first parameter = model type, exactly one positional ``features`` parameter
