@@ -1,0 +1,259 @@
+// Where the time of the linear tile kernel goes, on 10M x 64 fp32 rows (2.56 GB, the cfg2 shape), against the card's
+// own read ceiling.  Built three times by tools/linear_probe.sh from linear_kernels.cu itself:
+//   plain                   read ceiling (streaming 16-byte non-allocating loads) + the tile kernel, both schedules
+//   -DUML_PROBE_FEED_ONLY   the same producer, ring, order and barriers with consumers that skip the math, under
+//                           L2_PROMOTION_256B (what the library encodes) and L2_PROMOTION_NONE
+//   -DUML_PROBE_WAIT_CLOCKS the tile kernel with clock64() totals around the producer's `empty` and the scoring
+//                           warps' `full` waits
+// Every figure is CUDA-event time over >= 0.5 s of back-to-back launches.  Prints one JSON object per line.
+#include "../unionml_b200/csrc/linear_kernels.cu"
+
+#include <cudaTypedefs.h>
+
+#include <cmath>
+#include <vector>
+
+using namespace uml;
+
+#define CK(x)                                                                               \
+  do {                                                                                      \
+    cudaError_t e_ = (x);                                                                   \
+    if (e_ != cudaSuccess) {                                                                \
+      fprintf(stderr, "%s:%d %s: %s\n", __FILE__, __LINE__, #x, cudaGetErrorString(e_));    \
+      exit(1);                                                                              \
+    }                                                                                       \
+  } while (0)
+
+static const long long kRows = 10000000;
+static const int kF = 64, kC = 10;
+
+__global__ void fill_kernel(float* x, long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    unsigned h = static_cast<unsigned>(i) * 2654435761u;
+    h ^= h >> 15;
+    x[i] = static_cast<float>(h % 17u);  // digits-like pixel values 0..16
+  }
+}
+
+// streaming read: 16-byte non-allocating loads, four in flight per thread, folded into one word per thread so no
+// load can be dropped; the block's clock64() span over its lifetime gives the SM clock under this load
+__global__ void __launch_bounds__(512) read_kernel(const uint4* __restrict__ x, long long n16, unsigned* sink,
+                                                   long long* cycles) {
+  const long long t0 = clock64();
+  unsigned acc = 0;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  for (; i + 3 * stride < n16; i += 4 * stride) {
+    uint4 v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+                   : "=r"(v[k].x), "=r"(v[k].y), "=r"(v[k].z), "=r"(v[k].w)
+                   : "l"(x + i + k * stride));
+#pragma unroll
+    for (int k = 0; k < 4; ++k) acc ^= v[k].x ^ v[k].y ^ v[k].z ^ v[k].w;
+  }
+  for (; i < n16; i += stride) {
+    const uint4 v = x[i];
+    acc ^= v.x ^ v.y ^ v.z ^ v.w;
+  }
+  if (acc == 0x9e3779b9u) sink[0] = acc;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *cycles = clock64() - t0;
+}
+
+static PFN_cuTensorMapEncodeTiled_v12000 encoder() {
+  void* fn = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  CK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
+  return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+}
+
+static CUtensorMap make_map(const float* x, int box_rows, CUtensorMapL2promotion promo) {
+  CUtensorMap map{};
+  cuuint64_t gdim[2] = {(cuuint64_t)kF, (cuuint64_t)kRows};
+  cuuint64_t gstride[1] = {(cuuint64_t)kF * 4};
+  cuuint32_t box[2] = {(cuuint32_t)kChunkF, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = encoder()(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)x, gdim, gstride, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    fprintf(stderr, "cuTensorMapEncodeTiled: %d\n", (int)r);
+    exit(1);
+  }
+  return map;
+}
+
+// mean ms per launch of fn() over >= 0.5 s (after a warm-up launch sized the count)
+template <typename FN>
+static double time_ms(FN fn) {
+  cudaEvent_t a, b;
+  CK(cudaEventCreate(&a));
+  CK(cudaEventCreate(&b));
+  for (int i = 0; i < 3; ++i) fn();
+  CK(cudaEventRecord(a));
+  fn();
+  CK(cudaEventRecord(b));
+  CK(cudaEventSynchronize(b));
+  float one = 0.f;
+  CK(cudaEventElapsedTime(&one, a, b));
+  const int n = std::max(100, static_cast<int>(std::ceil(600.0 / std::max(one, 0.01f))));
+  CK(cudaEventRecord(a));
+  for (int i = 0; i < n; ++i) fn();
+  CK(cudaEventRecord(b));
+  CK(cudaEventSynchronize(b));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, a, b));
+  CK(cudaGetLastError());
+  return ms / n;
+}
+
+int main() {
+  cudaDeviceProp prop;
+  CK(cudaGetDeviceProperties(&prop, 0));
+  const double bytes = static_cast<double>(kRows) * kF * 4;
+  float* x = nullptr;
+  CK(cudaMalloc(&x, static_cast<size_t>(bytes)));
+  fill_kernel<<<prop.multiProcessorCount * 8, 512>>>(x, kRows * kF);
+  CK(cudaDeviceSynchronize());
+
+#if defined(UML_PROBE_FEED_ONLY)
+  const char* build = "feed_only";
+#elif defined(UML_PROBE_WAIT_CLOCKS)
+  const char* build = "wait_clocks";
+#else
+  const char* build = "plain";
+  {
+    unsigned* sink = nullptr;
+    long long* cyc = nullptr;
+    CK(cudaMalloc(&sink, 4));
+    CK(cudaMalloc(&cyc, 8));
+    const int grid = prop.multiProcessorCount * 4;  // 2048 threads per SM resident, 64 KB of loads in flight per SM
+    const double ms = time_ms([&] { read_kernel<<<grid, 512>>>(reinterpret_cast<const uint4*>(x), kRows * kF / 4, sink, cyc); });
+    long long cycles = 0;
+    CK(cudaMemcpy(&cycles, cyc, 8, cudaMemcpyDeviceToHost));
+    printf("{\"probe\": \"read_ceiling\", \"device\": \"%s\", \"bytes\": %.0f, \"ms\": %.4f, \"hbm_gbs\": %.1f, "
+           "\"sm_clock_mhz_under_load\": %.0f}\n",
+           prop.name, bytes, ms, bytes / ms * 1e-6, cycles / (ms * 1e3));
+  }
+#endif
+
+  // the cfg2 model shape: 10 classes, wt [64][cp] with the wmax column, bias [cp] with max|b|
+  const int cp = (kC + 1 + 3) / 4 * 4;
+  std::vector<float> wt(static_cast<size_t>(kF) * cp, 0.f), bias(cp, 0.f);
+  std::vector<double> w64(static_cast<size_t>(kF) * linear_w64_stride(kC), 0.0), b64(kC, 0.0);
+  unsigned s = 12345u;
+  auto rnd = [&] {
+    s = s * 1664525u + 1013904223u;
+    return (static_cast<float>(s >> 8) / 16777216.f - 0.5f) * 0.1f;
+  };
+  for (int f = 0; f < kF; ++f) {
+    float wmax = 0.f;
+    for (int c = 0; c < kC; ++c) {
+      const float v = rnd();
+      wt[f * cp + c] = v;
+      w64[static_cast<size_t>(f) * linear_w64_stride(kC) + c] = v;
+      wmax = fmaxf(wmax, fabsf(v));
+    }
+    wt[f * cp + kC] = wmax;
+  }
+  float bmax = 0.f;
+  for (int c = 0; c < kC; ++c) {
+    bias[c] = rnd() * 10.f;
+    b64[c] = bias[c];
+    bmax = fmaxf(bmax, fabsf(bias[c]));
+  }
+  bias[kC] = bmax;
+  LinearDeviceModel m{};
+  float *d_wt, *d_bias;
+  double *d_w64, *d_b64;
+  CK(cudaMalloc(&d_wt, wt.size() * 4));
+  CK(cudaMalloc(&d_bias, bias.size() * 4));
+  CK(cudaMalloc(&d_w64, w64.size() * 8));
+  CK(cudaMalloc(&d_b64, b64.size() * 8));
+  CK(cudaMemcpy(d_wt, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(d_bias, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(d_w64, w64.data(), w64.size() * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(d_b64, b64.data(), b64.size() * 8, cudaMemcpyHostToDevice));
+  m.wt = d_wt;
+  m.bias = d_bias;
+  m.w64 = d_w64;
+  m.b64 = d_b64;
+  m.w64_stride = linear_w64_stride(kC);
+  m.n_classes = kC;
+  m.n_features = kF;
+  m.cp = cp;
+  m.f_pad = kF;
+  uint8_t* labels = nullptr;
+  unsigned long long* counters = nullptr;
+  CK(cudaMalloc(&labels, kRows));
+  CK(cudaMalloc(&counters, 8 * sizeof(unsigned long long)));
+  CK(cudaMemset(counters, 0, 8 * sizeof(unsigned long long)));
+
+  // the EXACT + QUEUE kernel bench.py runs (uint8 labels to one target), in either schedule
+  auto run = [&](bool whole, CUtensorMapL2promotion promo, const char* promo_name) {
+    const int tile = whole ? kWholeTileRows : kTileRows;
+    const CUtensorMap map = make_map(x, tile, promo);
+    TmaKernelParams p{};
+    p.wt = m.wt;
+    p.bias = m.bias;
+    p.peers[0] = labels;
+    p.n_peers = 1;
+    p.wire_u8 = 1;
+    p.n_rows = kRows;
+    p.num_tiles = (kRows + tile - 1) / tile;
+    p.f_pad = kF;
+    p.kc = kF / kChunkF;
+    const size_t fixed = tma_fixed_smem(m);
+    p.num_stages = std::min(64, static_cast<int>((kMaxSmemBytes - fixed) / kStageBytes));
+    p.thr = static_cast<float>(2.0 * (kF + 4.0) * 5.9604644775390625e-08 * (1.0 + kF * 4.76837158203125e-07) * 1.0001);
+    p.x = x;
+    p.ld = kF;
+    p.w64 = m.w64;
+    p.w64_stride = m.w64_stride;
+    p.b64 = m.b64;
+    p.n_classes = kC;
+    p.n_features = kF;
+    p.counters = counters;
+#ifdef UML_PROBE_WAIT_CLOCKS
+    p.probe_clocks = counters + 4;
+#endif
+    const size_t smem = fixed + static_cast<size_t>(p.num_stages) * kStageBytes;
+    const int grid = prop.multiProcessorCount;
+    auto launch = [&] {
+      const cudaError_t err = whole ? launch_one<kC, true, true, true>(map, p, grid, smem, 0)
+                                    : launch_one<kC, true, true, false>(map, p, grid, smem, 0);
+      CK(err);
+    };
+    const double ms = time_ms(launch);
+    printf("{\"probe\": \"tile_kernel\", \"build\": \"%s\", \"schedule\": \"%s\", \"l2_promotion\": \"%s\", \"stages\": %d, "
+           "\"ms\": %.4f, \"gbs\": %.1f",
+           build, whole ? "whole_rows_64" : "chunked_128x32", promo_name, p.num_stages, ms, bytes / ms * 1e-6);
+#ifdef UML_PROBE_WAIT_CLOCKS
+    // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time
+    CK(cudaMemset(counters + 4, 0, 4 * sizeof(unsigned long long)));
+    cudaEvent_t a, b;
+    CK(cudaEventCreate(&a));
+    CK(cudaEventCreate(&b));
+    CK(cudaEventRecord(a));
+    launch();
+    CK(cudaEventRecord(b));
+    CK(cudaEventSynchronize(b));
+    float one = 0.f;
+    CK(cudaEventElapsedTime(&one, a, b));
+    unsigned long long c[4];
+    CK(cudaMemcpy(c, counters + 4, sizeof(c), cudaMemcpyDeviceToHost));
+    printf(", \"producer_empty_wait_frac\": %.4f, \"consumer_full_wait_frac\": %.4f, \"sm_clock_mhz_under_load\": %.0f",
+           static_cast<double>(c[0]) / c[1], static_cast<double>(c[2]) / c[3],
+           static_cast<double>(c[1]) / grid / (one * 1e3));
+#endif
+    printf("}\n");
+    fflush(stdout);
+  };
+  run(false, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
+  run(true, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
+#ifdef UML_PROBE_FEED_ONLY
+  run(false, CU_TENSOR_MAP_L2_PROMOTION_NONE, "none");
+  run(true, CU_TENSOR_MAP_L2_PROMOTION_NONE, "none");
+#endif
+  return 0;
+}

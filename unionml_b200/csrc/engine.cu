@@ -230,7 +230,8 @@ struct uml_batch {
   bool lossless = true;
   int tf32_exact = -1;  // every fp32 feature is a tf32 value: 1 yes, 0 no, -1 not scanned yet (wrapped device rows)
   bool has_map = false;
-  CUtensorMap map{};  // boxes of 128 rows x 32 features
+  CUtensorMap map{};      // boxes of 128 rows x 32 features (MLP kernels)
+  CUtensorMap lin_map{};  // boxes of uml::linear_box_rows(f_pad) rows x 32 features (linear tile kernel)
 };
 
 struct uml_mlp {
@@ -559,6 +560,16 @@ static int encode_map(uml_engine* e, CUtensorMap* map, const float* x, int64_t n
   return UML_OK;
 }
 
+static int linear_box_rows_for(int F) { return uml::linear_box_rows((F + uml::kChunkF - 1) / uml::kChunkF * uml::kChunkF); }
+
+// both tensor maps of a batch: the MLP kernels' 128-row boxes and the linear tile kernel's
+static int encode_batch_maps(uml_engine* e, uml_batch* b) {
+  int rc = encode_map(e, &b->map, b->x, b->n_rows, b->n_features, b->ld);
+  if (rc == UML_OK) rc = encode_map(e, &b->lin_map, b->x, b->n_rows, b->n_features, b->ld, linear_box_rows_for(b->n_features));
+  b->has_map = rc == UML_OK;
+  return rc;
+}
+
 int uml_batch_from_device(uml_engine* e, uml_batch** out, const void* dev_ptr, int64_t n_rows, int n_features,
                           int64_t ld) {
   if (!e || !out || (!dev_ptr && n_rows > 0) || n_rows < 0 || n_features < 1 || ld < n_features) return UML_ERR_INVALID;
@@ -572,9 +583,8 @@ int uml_batch_from_device(uml_engine* e, uml_batch** out, const void* dev_ptr, i
   b->ld = ld;
   b->owns = false;
   if (n_rows > 0) {
-    int rc = encode_map(e, &b->map, b->x, n_rows, n_features, ld);
-    if (rc == UML_OK) b->has_map = true;
-    else if (rc != UML_ERR_UNSUPPORTED) {
+    int rc = encode_batch_maps(e, b);
+    if (rc != UML_OK && rc != UML_ERR_UNSUPPORTED) {
       delete b;
       return rc;
     }
@@ -860,9 +870,8 @@ int uml_stage_rows(uml_engine* e, uml_batch** out, const void* host_ptr, int64_t
     cudaFree(b->x64);
     b->x64 = nullptr;
   }
-  rc = encode_map(e, &b->map, b->x, n_rows, F, ld);
-  if (rc == UML_OK) b->has_map = true;
-  else if (rc != UML_ERR_UNSUPPORTED) return bail(rc);
+  rc = encode_batch_maps(e, b);
+  if (rc != UML_OK && rc != UML_ERR_UNSUPPORTED) return bail(rc);
   *out = b;
   return UML_OK;
 }
@@ -1028,7 +1037,7 @@ static int predict_common(uml_engine* e, const uml_model* m, const uml_batch* b,
   for (int i = 0; i < n_peers; ++i) l.peers[i] = peers[i];
   l.row_offset = row_offset;
   int launches = 0, path = 0;
-  rc = enqueue_predict(e, m, l, b->has_map ? &b->map : nullptr, mode, timed, &launches, &path);
+  rc = enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, mode, timed, &launches, &path);
   if (rc != UML_OK) return rc;
   int64_t d2h = 0;
   if (!labels_on_device && labels_out) {
@@ -1501,8 +1510,8 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       launches += 1;
     }
     // (3) score
-    CUtensorMap map;
-    bool has_map = encode_map(e, &map, xc, rows, F, ld) == UML_OK;
+    CUtensorMap map;  // the MLP kernels' boxes, or the linear tile kernel's
+    bool has_map = encode_map(e, &map, xc, rows, F, ld, mlp ? uml::kTileRows : linear_box_rows_for(F)) == UML_OK;
     LinearLaunch l{};
     l.x = xc;
     l.ld = ld;

@@ -3,9 +3,10 @@
 // Replaces the numeric body of sklearn's LinearClassifierMixin.predict (sklearn/linear_model/_base.py:366-427), which
 // is what the reference's canonical predictor runs (unionml:README.md:87-92).
 //
-//  * linear_argmax_tma_kernel<C, EXACT>: persistent, warp-specialised.  One producer warp streams 128-row x 32-feature
-//    boxes of X (16 KiB, 128B-swizzled) through a shared-memory ring with TMA + mbarriers; eight consumer warps each
-//    own one 128-row tile at a time (4 rows per lane), read X with conflict-free LDS.128, W as warp-uniform broadcast
+//  * linear_argmax_tma_kernel<C, EXACT, QUEUE, WHOLE>: persistent, warp-specialised.  One producer warp streams X
+//    through a 16 KiB-per-stage shared-memory ring with TMA + mbarriers: 128-row x 32-feature boxes (128B-swizzled), or
+//    at 33 <= F <= 64 (WHOLE) stages of 64 complete rows; eight consumer warps each own one tile at a time (4 or 2
+//    rows per lane), read X with conflict-free LDS.128, W as warp-uniform broadcast
 //    LDS.128 from a transposed copy in shared memory, keep C (+1) fp32 accumulators per row in registers, and fuse
 //    bias, argmax (first maximum wins, like np.argmax) and the label store.  In EXACT mode one extra accumulator
 //    carries A = max|b| + sum_f |x_f| * max_c |w_cf|; rows whose top-2 margin is not provably larger than the fp32
@@ -153,6 +154,9 @@ struct TmaKernelParams {
   int w64_stride;
   int n_classes, n_features;
   unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] re-scored rows
+#ifdef UML_PROBE_WAIT_CLOCKS
+  unsigned long long* probe_clocks;  // [4], see the diagnostic builds below
+#endif
 };
 
 // fp64 scores of one row by the whole warp (kept out of line so the hot loop's register allocation is untouched)
@@ -188,13 +192,39 @@ __device__ __forceinline__ void store_final_label(const TmaKernelParams& p, long
   }
 }
 
-template <int C, bool EXACT, bool QUEUE>
+// Diagnostic builds of this file (tools/linear_probe.cu defines these; the library defines neither):
+//  UML_PROBE_FEED_ONLY    the scoring warps hand each stage back as soon as it has landed, without the math: what the
+//                         ring (producer, order, barriers) delivers on its own
+//  UML_PROBE_WAIT_CLOCKS  clock64() totals added into p.probe_clocks: [0] the producer's `empty` waits, [1] its whole
+//                         loop, [2] the scoring warps' waits for their data, [3] their whole loops
+#ifdef UML_PROBE_FEED_ONLY
+constexpr bool kFeedOnly = true;
+#else
+constexpr bool kFeedOnly = false;
+#endif
+#ifdef UML_PROBE_WAIT_CLOCKS
+#define UML_PROBE_TIMED(total, ...)     \
+  do {                                  \
+    const long long t0_ = clock64();    \
+    __VA_ARGS__;                        \
+    (total) += clock64() - t0_;         \
+  } while (0)
+#else
+#define UML_PROBE_TIMED(total, ...) __VA_ARGS__
+#endif
+
+// WHOLE (f_pad == 64, linear_whole_rows): one ring stage is one 64-row tile with all its features, loaded as two
+// {32 features, 64 rows} boxes onto one barrier; warp w scores the CTA's tiles w, w + 8, ... (2 rows per lane).
+// Otherwise one stage is a 128-row x 32-feature box and a tile takes f_pad / 32 stages (4 rows per lane).
+template <int C, bool EXACT, bool QUEUE, bool WHOLE>
 __global__ void __launch_bounds__(kThreadsQueue, 1)
 linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ TmaKernelParams p) {
   constexpr int NCOL = C + (EXACT ? 1 : 0);  // accumulators per row (classes + error-bound column)
   constexpr int CP = (C + 1 + 3) / 4 * 4;    // padded columns of wt in shared memory (layout shared by both modes)
   constexpr int NW4 = (NCOL + 3) / 4;        // float4 loads of W per feature
-  constexpr int R = kRowsPerLane;
+  constexpr int TILE = WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = rows per TMA box
+  constexpr int R = TILE / 32;                               // rows per lane
+  constexpr int BOX_BYTES = TILE * kChunkF * 4;              // one {32, TILE} box: 8 KiB (two per stage) or 16 KiB
   constexpr bool USE_F2 = EXACT;  // fp32x2 accumulator pairs (see the accumulator comment below)
 
   extern __shared__ uint8_t smem_raw[];
@@ -238,9 +268,11 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   const long long G = gridDim.x;
   const long long num_tiles = p.num_tiles;
   const int KC = p.kc;
+#ifdef UML_PROBE_WAIT_CLOCKS
+  long long probe_wait = 0;
+  const long long probe_start = clock64();
+#endif
 
-  // Work items of this CTA, in ring order: for each round (kConsumerWarps tiles), for each 32-feature chunk k, for
-  // each active warp w: (tile = first + w*G, chunk k).  Producer and consumers derive the same sequence numbers.
   if (warp == kConsumerWarps) {
     // ===================== TMA producer (one elected lane) =====================
     if (elect_one_sync()) {
@@ -248,176 +280,185 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       const uint64_t policy = make_evict_first_policy();  // X is read exactly once
       int stage = 0;
       uint32_t phase = 0;
-      for (long long first = blockIdx.x; first < num_tiles; first += G * kConsumerWarps) {
-        const int nv = static_cast<int>(min(static_cast<long long>(kConsumerWarps), (num_tiles - first + G - 1) / G));
-        for (int k = 0; k < KC; ++k) {
-          for (int w = 0; w < nv; ++w) {
-            mbar_wait(&empty_bar[stage], phase ^ 1u);
-            mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-            tma_load_2d(smem + static_cast<size_t>(stage) * kStageBytes, &xmap, &full_bar[stage], k * kChunkF,
-                        static_cast<int>((first + w * G) * kTileRows), policy);
-            if (++stage == S) {
-              stage = 0;
-              phase ^= 1u;
+      auto next_stage = [&] {
+        if (++stage == S) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      };
+      if constexpr (WHOLE) {
+        // ring item n of this CTA = its n-th tile (tile blockIdx.x + n*G): both halves of its rows land together
+        for (long long tile = blockIdx.x; tile < num_tiles; tile += G) {
+          UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u));
+          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+          uint8_t* dst = smem + static_cast<size_t>(stage) * kStageBytes;
+          const int row = static_cast<int>(tile * TILE);
+          tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
+          tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], kChunkF, row, policy);
+          next_stage();
+        }
+      } else {
+        // Work items in ring order: for each round (kConsumerWarps tiles), for each 32-feature chunk k, for each
+        // active warp w: (tile = first + w*G, chunk k).  Producer and consumers derive the same sequence numbers.
+        for (long long first = blockIdx.x; first < num_tiles; first += G * kConsumerWarps) {
+          const int nv = static_cast<int>(min(static_cast<long long>(kConsumerWarps), (num_tiles - first + G - 1) / G));
+          for (int k = 0; k < KC; ++k) {
+            for (int w = 0; w < nv; ++w) {
+              UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u));
+              mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+              tma_load_2d(smem + static_cast<size_t>(stage) * kStageBytes, &xmap, &full_bar[stage], k * kChunkF,
+                          static_cast<int>((first + w * G) * TILE), policy);
+              next_stage();
             }
           }
         }
       }
+#ifdef UML_PROBE_WAIT_CLOCKS
+      atomicAdd(&p.probe_clocks[0], static_cast<unsigned long long>(probe_wait));
+      atomicAdd(&p.probe_clocks[1], static_cast<unsigned long long>(clock64() - probe_start));
+#endif
     }
   } else {
-    // ===================== consumers: one 128-row tile per warp at a time (warp 9 of the QUEUE kernels: re-score) ====
+    // ===================== consumers: one tile per warp at a time (warp 9 of the QUEUE kernels: re-score) ==========
     const bool scoring_warp = warp < kConsumerWarps;
-    // lane l owns rows l, l+32, l+64, l+96 of the tile.  Row r of a box sits at byte r*128 with its 16-byte chunks
-    // XOR-swizzled by (r & 7); r & 7 == l & 7 for all four rows, so one swizzle term serves them all and the eight
-    // lanes of every LDS.128 phase hit eight distinct bank groups.
+    // lane l owns rows l, l+32, ... of the tile.  In every box row r sits at byte r*128 with its 16-byte chunks
+    // XOR-swizzled by (r & 7); r & 7 == l & 7 for all of a lane's rows, so one swizzle term serves them all and the
+    // eight lanes of every LDS.128 phase (lanes 8i..8i+7: l & 7 = 0..7) hit eight distinct bank groups.  The whole-row
+    // stage is two such boxes (features 0-31, then 32-63 at +8 KiB), so the same holds in both halves.
     const uint32_t lanebase = static_cast<uint32_t>(lane) * 128u + static_cast<uint32_t>(lane & 7) * 16u;
-    uint32_t seq_base = 0;
-    for (long long first = blockIdx.x; scoring_warp && first < num_tiles; first += G * kConsumerWarps) {
-      const int nv = static_cast<int>(min(static_cast<long long>(kConsumerWarps), (num_tiles - first + G - 1) / G));
-      if (warp < nv) {
-        const long long tile = first + warp * G;
-        // USE_F2 (EXACT kernels): class accumulators as fp32x2 pairs (classes 2i, 2i+1 -> one fma2); an odd last class
-        // and the error-bound column (|x| is a free operand modifier on scalar FFMA) stay scalar.
-        constexpr int NPAIR = C / 2;
-        constexpr bool ODD = (C & 1) != 0;
-        uint64_t acc2[R][NPAIR > 0 ? NPAIR : 1];
-        float acc_last[R], acc_bound[R];
-        float acc[R][C + 1];
-#pragma unroll
-        for (int j = 0; j < R; ++j) {
-          if constexpr (USE_F2) {
-#pragma unroll
-            for (int i = 0; i < NPAIR; ++i) acc2[j][i] = pack2(bias_s[2 * i], bias_s[2 * i + 1]);
-            acc_last[j] = ODD ? bias_s[C - 1] : 0.f;
-            acc_bound[j] = EXACT ? bias_s[C] : 0.f;
-          } else {
-#pragma unroll
-            for (int c = 0; c < NCOL; ++c) acc[j][c] = bias_s[c];
-          }
-        }
 
-        for (int k = 0; k < KC; ++k) {
-          const uint32_t seq = seq_base + static_cast<uint32_t>(k * nv + warp);
-          const uint32_t stage = seq % static_cast<uint32_t>(S);
-          const uint32_t phase = (seq / static_cast<uint32_t>(S)) & 1u;
-          // A parity wait can only tell the current phase from the one before it.  Several warps share this ring and
-          // TMA completions are unordered, so the previous occupant of the stage (item seq - S, another warp's) may
-          // still be in flight or unread when this warp gets here; waiting on `full` right away would then match the
-          // *older* phase and read another tile's half-landed box.  First wait until that occupant has been released
-          // (empty phase seq/S - 1), then for our own data.  Both waits are at most one phase ahead of their barrier
-          // because a warp's next item is seq + nv <= seq + kConsumerWarps and the ring has S >= kConsumerWarps stages:
-          // the producer could only issue item seq after item seq - S was released, so item seq + nv - 2S was too.
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_wait(&full_bar[stage], phase);
-
-          const uint8_t* xs = smem + static_cast<size_t>(stage) * kStageBytes;
-          const float* wk = wt_s + k * kChunkF * CP;
+    // USE_F2 (EXACT kernels): class accumulators as fp32x2 pairs (classes 2i, 2i+1 -> one fma2); an odd last class
+    // and the error-bound column (|x| is a free operand modifier on scalar FFMA) stay scalar.
+    constexpr int NPAIR = C / 2;
+    constexpr bool ODD = (C & 1) != 0;
+    uint64_t acc2[R][NPAIR > 0 ? NPAIR : 1];
+    float acc_last[R], acc_bound[R];
+    float acc[R][C + 1];
+    auto init_acc = [&] {
 #pragma unroll
-          for (int q = 0; q < kChunkF / 4; ++q) {
-            float4 xv[R];
-            const uint32_t off = lanebase ^ static_cast<uint32_t>(q * 16);
-#pragma unroll
-            for (int j = 0; j < R; ++j) xv[j] = *reinterpret_cast<const float4*>(xs + off + j * 32 * 128);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float wv[NW4 * 4];
-#pragma unroll
-              for (int m = 0; m < NW4; ++m) {
-                const float4 t = *reinterpret_cast<const float4*>(wk + (q * 4 + e) * CP + m * 4);
-                wv[m * 4 + 0] = t.x;
-                wv[m * 4 + 1] = t.y;
-                wv[m * 4 + 2] = t.z;
-                wv[m * 4 + 3] = t.w;
-              }
-#pragma unroll
-              for (int j = 0; j < R; ++j) {
-                const float x = e == 0 ? xv[j].x : e == 1 ? xv[j].y : e == 2 ? xv[j].z : xv[j].w;
-                if constexpr (USE_F2) {
-                  const uint64_t xx = pack2(x, x);
-#pragma unroll
-                  for (int i = 0; i < NPAIR; ++i) acc2[j][i] = fma2(xx, pack2(wv[2 * i], wv[2 * i + 1]), acc2[j][i]);
-                  if (ODD) acc_last[j] = fmaf(x, wv[C - 1], acc_last[j]);
-                  if (EXACT) acc_bound[j] = fmaf(fabsf(x), wv[C], acc_bound[j]);
-                } else {
-#pragma unroll
-                  for (int c = 0; c < C; ++c) acc[j][c] = fmaf(x, wv[c], acc[j][c]);
-                  if (EXACT) acc[j][C] = fmaf(fabsf(x), wv[C], acc[j][C]);
-                }
-              }
-            }
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[stage]);  // hand the stage back to the producer
-        }
-
+      for (int j = 0; j < R; ++j) {
         if constexpr (USE_F2) {
 #pragma unroll
+          for (int i = 0; i < NPAIR; ++i) acc2[j][i] = pack2(bias_s[2 * i], bias_s[2 * i + 1]);
+          acc_last[j] = ODD ? bias_s[C - 1] : 0.f;
+          acc_bound[j] = EXACT ? bias_s[C] : 0.f;
+        } else {
+#pragma unroll
+          for (int c = 0; c < NCOL; ++c) acc[j][c] = bias_s[c];
+        }
+      }
+    };
+    // features kChunkF*k .. +31 of the lane's rows from box xs, with wk = the W^T rows of those features; every row's
+    // FMAs run in feature order, so scores do not depend on the schedule
+    auto fma_box = [&](const uint8_t* xs, const float* wk) {
+      if constexpr (kFeedOnly) return;
+#pragma unroll
+      for (int q = 0; q < kChunkF / 4; ++q) {
+        float4 xv[R];
+        const uint32_t off = lanebase ^ static_cast<uint32_t>(q * 16);
+#pragma unroll
+        for (int j = 0; j < R; ++j) xv[j] = *reinterpret_cast<const float4*>(xs + off + j * 32 * 128);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float wv[NW4 * 4];
+#pragma unroll
+          for (int m = 0; m < NW4; ++m) {
+            const float4 t = *reinterpret_cast<const float4*>(wk + (q * 4 + e) * CP + m * 4);
+            wv[m * 4 + 0] = t.x;
+            wv[m * 4 + 1] = t.y;
+            wv[m * 4 + 2] = t.z;
+            wv[m * 4 + 3] = t.w;
+          }
+#pragma unroll
           for (int j = 0; j < R; ++j) {
+            const float x = e == 0 ? xv[j].x : e == 1 ? xv[j].y : e == 2 ? xv[j].z : xv[j].w;
+            if constexpr (USE_F2) {
+              const uint64_t xx = pack2(x, x);
 #pragma unroll
-            for (int i = 0; i < NPAIR; ++i) unpack2(acc2[j][i], acc[j][2 * i], acc[j][2 * i + 1]);
-            if (ODD) acc[j][C - 1] = acc_last[j];
-            acc[j][C] = acc_bound[j];
-          }
-        }
-        // ---- fused epilogue: argmax (first maximum wins), margin guard, label store (+ peer stores) ----
-        const long long row0 = tile * kTileRows;
-        int idxs[R];
-        bool flag[R];
-#pragma unroll
-        for (int j = 0; j < R; ++j) {
-          const long long row = row0 + lane + 32 * j;
-          float best = acc[j][0];
-          float second = -INFINITY;
-          int idx = 0;
-#pragma unroll
-          for (int c = 1; c < C; ++c) {
-            const float v = acc[j][c];
-            if (v > best) {
-              second = best;
-              best = v;
-              idx = c;
+              for (int i = 0; i < NPAIR; ++i) acc2[j][i] = fma2(xx, pack2(wv[2 * i], wv[2 * i + 1]), acc2[j][i]);
+              if (ODD) acc_last[j] = fmaf(x, wv[C - 1], acc_last[j]);
+              if (EXACT) acc_bound[j] = fmaf(fabsf(x), wv[C], acc_bound[j]);
             } else {
-              second = fmaxf(second, v);
+#pragma unroll
+              for (int c = 0; c < C; ++c) acc[j][c] = fmaf(x, wv[c], acc[j][c]);
+              if (EXACT) acc[j][C] = fmaf(fabsf(x), wv[C], acc[j][C]);
             }
           }
-          idxs[j] = idx;
-          // certain iff margin > 2 * err, err <= (F+4) 2^-24 A; NaN/Inf anywhere makes the comparison false
-          flag[j] = EXACT && row < p.n_rows && !((best - second) > p.thr * acc[j][C]);
         }
+      }
+    };
+
+    // ---- fused epilogue: argmax (first maximum wins), margin guard, label store (+ peer stores) ----
+    auto finish_tile = [&](long long tile) {
+      if constexpr (USE_F2) {
 #pragma unroll
         for (int j = 0; j < R; ++j) {
-          const long long row = row0 + lane + 32 * j;
-          if (row < p.n_rows) {
-            if (p.labels) p.labels[row] = idxs[j];
-            if (!p.wire_u8)
-              for (int i = 0; i < p.n_peers; ++i) static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idxs[j];
+#pragma unroll
+          for (int i = 0; i < NPAIR; ++i) unpack2(acc2[j][i], acc[j][2 * i], acc[j][2 * i + 1]);
+          if (ODD) acc[j][C - 1] = acc_last[j];
+          acc[j][C] = acc_bound[j];
+        }
+      }
+      const long long row0 = tile * TILE;
+      int idxs[R];
+      bool flag[R];
+#pragma unroll
+      for (int j = 0; j < R; ++j) {
+        const long long row = row0 + lane + 32 * j;
+        float best = acc[j][0];
+        float second = -INFINITY;
+        int idx = 0;
+#pragma unroll
+        for (int c = 1; c < C; ++c) {
+          const float v = acc[j][c];
+          if (v > best) {
+            second = best;
+            best = v;
+            idx = c;
+          } else {
+            second = fmaxf(second, v);
           }
-          if constexpr (EXACT && !QUEUE) {
-            const unsigned mask = __ballot_sync(0xffffffffu, flag[j]);
-            if (mask != 0u) {
-              int base = 0;
-              if (lane == 0) base = atomicAdd(p.flag_count, __popc(mask));
-              base = __shfl_sync(0xffffffffu, base, 0);
-              if (flag[j]) {
-                const int pos = base + __popc(mask & ((1u << lane) - 1u));
-                if (pos < p.flag_cap) p.flag_rows[pos] = static_cast<int32_t>(row);
-              }
+        }
+        idxs[j] = idx;
+        // certain iff margin > 2 * err, err <= (F+4) 2^-24 A; NaN/Inf anywhere makes the comparison false
+        flag[j] = EXACT && row < p.n_rows && !((best - second) > p.thr * acc[j][C]);
+      }
+#pragma unroll
+      for (int j = 0; j < R; ++j) {
+        const long long row = row0 + lane + 32 * j;
+        if (row < p.n_rows) {
+          if (p.labels) p.labels[row] = idxs[j];
+          if (!p.wire_u8)
+            for (int i = 0; i < p.n_peers; ++i) static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idxs[j];
+        }
+        if constexpr (EXACT && !QUEUE) {
+          const unsigned mask = __ballot_sync(0xffffffffu, flag[j]);
+          if (mask != 0u) {
+            int base = 0;
+            if (lane == 0) base = atomicAdd(p.flag_count, __popc(mask));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (flag[j]) {
+              const int pos = base + __popc(mask & ((1u << lane) - 1u));
+              if (pos < p.flag_cap) p.flag_rows[pos] = static_cast<int32_t>(row);
             }
           }
         }
-        if (p.wire_u8 && p.n_peers > 0) {
-          uint32_t word = 0;
-          // byte labels: transpose through shuffles so lane l holds rows 4l..4l+3 of the tile and the whole 128-row
-          // tile leaves as ONE coalesced 128-byte store per target (instead of four int32 stores)
-          const uint32_t packed = static_cast<uint32_t>(idxs[0]) | (static_cast<uint32_t>(idxs[1]) << 8) |
-                                  (static_cast<uint32_t>(idxs[2]) << 16) | (static_cast<uint32_t>(idxs[3]) << 24);
+      }
+      if (p.wire_u8 && p.n_peers > 0) {
+        // byte labels: transpose through shuffles so lane l < TILE/4 holds rows 4l..4l+3 of the tile and the whole
+        // tile leaves as ONE coalesced TILE-byte store per target (instead of R int32 stores).  Row 4l+t sits in byte
+        // (4l+t)/32 = l/8 of lane (4l+t) % 32's packed word.
+        uint32_t packed = 0, word = 0;
 #pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
-            word |= ((w >> (8 * (lane >> 3))) & 0xffu) << (8 * t);
-          }
-          const long long row4 = row0 + 4 * lane;
-          const long long at = p.row_offset + row4;
+        for (int j = 0; j < R; ++j) packed |= static_cast<uint32_t>(idxs[j]) << (8 * j);
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
+          word |= ((w >> (8 * (lane >> 3))) & 0xffu) << (8 * t);
+        }
+        const long long row4 = row0 + 4 * lane;
+        const long long at = p.row_offset + row4;
+        if (4 * lane < TILE) {
           if (row4 + 3 < p.n_rows && (at & 3) == 0) {
             for (int i = 0; i < p.n_peers; ++i)
               *reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(p.peers[i]) + at) = word;
@@ -428,59 +469,113 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
                   static_cast<uint8_t*>(p.peers[i])[at + t] = static_cast<uint8_t>((word >> (8 * t)) & 0xffu);
           }
         }
-        if constexpr (EXACT && QUEUE) {
-          // hand the (rare) flagged rows to the re-score warp: the labels above are provisional for them
-          unsigned masks[R];
-          int total = 0;
+      }
+      if constexpr (EXACT && QUEUE) {
+        // hand the (rare) flagged rows to the re-score warp: the labels above are provisional for them
+        unsigned masks[R];
+        int total = 0;
 #pragma unroll
-          for (int j = 0; j < R; ++j) {
-            masks[j] = __ballot_sync(0xffffffffu, flag[j]);
-            total += __popc(masks[j]);
+        for (int j = 0; j < R; ++j) {
+          masks[j] = __ballot_sync(0xffffffffu, flag[j]);
+          total += __popc(masks[j]);
+        }
+        if (total > 0) {
+          __threadfence();  // the provisional labels are visible before the re-score warp may overwrite them
+          int base = -1;
+          if (lane == 0) {
+            const int tail = atomicAdd(&q_ctl[0], 0);
+            const int consumed = atomicAdd(&q_ctl[3], 0);
+            if (tail - consumed <= kQueueCap - kQueueHeadroom) base = atomicAdd(&q_ctl[0], total);
           }
-          if (total > 0) {
-            __threadfence();  // the provisional labels are visible before the re-score warp may overwrite them
-            int base = -1;
-            if (lane == 0) {
-              const int tail = atomicAdd(&q_ctl[0], 0);
-              const int consumed = atomicAdd(&q_ctl[3], 0);
-              if (tail - consumed <= kQueueCap - kQueueHeadroom) base = atomicAdd(&q_ctl[0], total);
-            }
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (base >= 0) {
-              int off = base;
+          base = __shfl_sync(0xffffffffu, base, 0);
+          if (base >= 0) {
+            int off = base;
 #pragma unroll
-              for (int j = 0; j < R; ++j) {
-                if (flag[j]) {
-                  const int slot = (off + __popc(masks[j] & ((1u << lane) - 1u))) & (kQueueCap - 1);
-                  // (atomics, not plain volatile accesses: the queue is a lock-free hand-off between warps and the
-                  // race checker should see it as one)
-                  while (atomicAdd(&q_slots[slot], 0) != 0) {  // only if the slot's previous ticket is claimed but not read yet
-                  }
-                  atomicExch(&q_slots[slot], static_cast<int>(row0 + lane + 32 * j) + 1);
+            for (int j = 0; j < R; ++j) {
+              if (flag[j]) {
+                const int slot = (off + __popc(masks[j] & ((1u << lane) - 1u))) & (kQueueCap - 1);
+                // (atomics, not plain volatile accesses: the queue is a lock-free hand-off between warps and the
+                // race checker should see it as one)
+                while (atomicAdd(&q_slots[slot], 0) != 0) {  // only if the slot's previous ticket is claimed but not read yet
                 }
-                off += __popc(masks[j]);
+                atomicExch(&q_slots[slot], static_cast<int>(row0 + lane + 32 * j) + 1);
               }
-            } else {
-              // the queue is backed up (most rows of the batch are near-ties): this warp re-scores its own rows, which
-              // keeps the worst case at "every warp does fp64" instead of "every warp waits for one"
-#pragma unroll
-              for (int j = 0; j < R; ++j) {
-                unsigned mask = masks[j];
-                while (mask != 0u) {
-                  const int l = __ffs(static_cast<int>(mask)) - 1;
-                  mask &= mask - 1u;
-                  const long long row = row0 + l + 32 * j;
-                  const int idx64 = rescore_row_inline(p, row, lane);
-                  if (lane == 0) store_final_label(p, row, idx64);
-                }
-              }
-              if (lane == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(total));
+              off += __popc(masks[j]);
             }
+          } else {
+            // the queue is backed up (most rows of the batch are near-ties): this warp re-scores its own rows, which
+            // keeps the worst case at "every warp does fp64" instead of "every warp waits for one"
+#pragma unroll
+            for (int j = 0; j < R; ++j) {
+              unsigned mask = masks[j];
+              while (mask != 0u) {
+                const int l = __ffs(static_cast<int>(mask)) - 1;
+                mask &= mask - 1u;
+                const long long row = row0 + l + 32 * j;
+                const int idx64 = rescore_row_inline(p, row, lane);
+                if (lane == 0) store_final_label(p, row, idx64);
+              }
+            }
+            if (lane == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(total));
           }
         }
       }
-      seq_base += static_cast<uint32_t>(KC * nv);
+    };
+
+    if constexpr (WHOLE) {
+      // this warp's ring items are n = warp, warp + 8, ... (stage n % S, phase (n / S) & 1); S >= 8 lets stage and
+      // phase advance without a division.  Both waits keep the invariant argued below: the next item is n + 8 <= n + S.
+      uint32_t stage = static_cast<uint32_t>(warp), phase = 0;
+      for (long long tile = blockIdx.x + warp * G; scoring_warp && tile < num_tiles; tile += G * kConsumerWarps) {
+        init_acc();
+        UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
+        const uint8_t* xs = smem + static_cast<size_t>(stage) * kStageBytes;
+        fma_box(xs, wt_s);
+        fma_box(xs + BOX_BYTES, wt_s + kChunkF * CP);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);  // hand the stage back to the producer
+        stage += kConsumerWarps;
+        if (stage >= static_cast<uint32_t>(S)) {
+          stage -= S;
+          phase ^= 1u;
+        }
+        finish_tile(tile);
+      }
+    } else {
+      uint32_t seq_base = 0;
+      for (long long first = blockIdx.x; scoring_warp && first < num_tiles; first += G * kConsumerWarps) {
+        const int nv = static_cast<int>(min(static_cast<long long>(kConsumerWarps), (num_tiles - first + G - 1) / G));
+        if (warp < nv) {
+          const long long tile = first + warp * G;
+          init_acc();
+          for (int k = 0; k < KC; ++k) {
+            const uint32_t seq = seq_base + static_cast<uint32_t>(k * nv + warp);
+            const uint32_t stage = seq % static_cast<uint32_t>(S);
+            const uint32_t phase = (seq / static_cast<uint32_t>(S)) & 1u;
+            // A parity wait can only tell the current phase from the one before it.  Several warps share this ring
+            // and TMA completions are unordered, so the previous occupant of the stage (item seq - S, another warp's)
+            // may still be in flight or unread when this warp gets here; waiting on `full` right away would then
+            // match the *older* phase and read another tile's half-landed box.  First wait until that occupant has
+            // been released (empty phase seq/S - 1), then for our own data.  Both waits are at most one phase ahead
+            // of their barrier because a warp's next item is seq + nv <= seq + kConsumerWarps and the ring has
+            // S >= kConsumerWarps stages: the producer could only issue item seq after item seq - S was released, so
+            // item seq + nv - 2S was too.
+            UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
+            fma_box(smem + static_cast<size_t>(stage) * kStageBytes, wt_s + k * kChunkF * CP);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);  // hand the stage back to the producer
+          }
+          finish_tile(tile);
+        }
+        seq_base += static_cast<uint32_t>(KC * nv);
+      }
     }
+#ifdef UML_PROBE_WAIT_CLOCKS
+    if (scoring_warp && lane == 0) {
+      atomicAdd(&p.probe_clocks[2], static_cast<unsigned long long>(probe_wait));
+      atomicAdd(&p.probe_clocks[3], static_cast<unsigned long long>(clock64() - probe_start));
+    }
+#endif
     if constexpr (EXACT && QUEUE) {
       if (warp < kConsumerWarps) {
         __syncwarp();
@@ -793,10 +888,10 @@ bool linear_tma_supported(const LinearDeviceModel& m, std::string* why) {
   return true;
 }
 
-template <int C, bool EXACT, bool QUEUE>
+template <int C, bool EXACT, bool QUEUE, bool WHOLE>
 static cudaError_t launch_one(const CUtensorMap& xmap, const TmaKernelParams& p, int grid, size_t smem,
                               cudaStream_t stream) {
-  auto kern = linear_argmax_tma_kernel<C, EXACT, QUEUE>;
+  auto kern = linear_argmax_tma_kernel<C, EXACT, QUEUE, WHOLE>;
   static size_t configured = 0;  // per instantiation (one device per process): set the attribute once, not per launch
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -807,13 +902,13 @@ static cudaError_t launch_one(const CUtensorMap& xmap, const TmaKernelParams& p,
   return cudaGetLastError();
 }
 
-template <bool EXACT, bool QUEUE>
+template <bool EXACT, bool QUEUE, bool WHOLE>
 static cudaError_t dispatch_classes(int C, const CUtensorMap& xmap, const TmaKernelParams& p, int grid, size_t smem,
                                     cudaStream_t stream) {
   switch (C) {
 #define UML_CASE(N) \
   case N:           \
-    return launch_one<N, EXACT, QUEUE>(xmap, p, grid, smem, stream);
+    return launch_one<N, EXACT, QUEUE, WHOLE>(xmap, p, grid, smem, stream);
     UML_CASE(2) UML_CASE(3) UML_CASE(4) UML_CASE(5) UML_CASE(6) UML_CASE(7) UML_CASE(8) UML_CASE(9) UML_CASE(10)
     UML_CASE(11) UML_CASE(12) UML_CASE(13) UML_CASE(14) UML_CASE(15) UML_CASE(16)
 #undef UML_CASE
@@ -854,7 +949,9 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& 
   for (int i = 0; i < 8; ++i) p.peers[i] = i < l.n_peers ? l.peers[i] : nullptr;
   p.row_offset = l.row_offset;
   p.n_rows = l.n_rows;
-  p.num_tiles = (l.n_rows + kTileRows - 1) / kTileRows;
+  const bool whole = linear_whole_rows(m.f_pad);
+  const int tile_rows = linear_box_rows(m.f_pad);
+  p.num_tiles = (l.n_rows + tile_rows - 1) / tile_rows;
   p.f_pad = m.f_pad;
   p.kc = m.f_pad / kChunkF;
   const size_t fixed = tma_fixed_smem(m);
@@ -883,9 +980,14 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& 
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
   const long long slots = (p.num_tiles + kConsumerWarps - 1) / kConsumerWarps;
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
-  if (!exact) return dispatch_classes<false, false>(m.n_classes, xmap, p, grid, smem, stream);
-  return inline_rescore ? dispatch_classes<true, true>(m.n_classes, xmap, p, grid, smem, stream)
-                        : dispatch_classes<true, false>(m.n_classes, xmap, p, grid, smem, stream);
+  if (whole) {
+    if (!exact) return dispatch_classes<false, false, true>(m.n_classes, xmap, p, grid, smem, stream);
+    return inline_rescore ? dispatch_classes<true, true, true>(m.n_classes, xmap, p, grid, smem, stream)
+                          : dispatch_classes<true, false, true>(m.n_classes, xmap, p, grid, smem, stream);
+  }
+  if (!exact) return dispatch_classes<false, false, false>(m.n_classes, xmap, p, grid, smem, stream);
+  return inline_rescore ? dispatch_classes<true, true, false>(m.n_classes, xmap, p, grid, smem, stream)
+                        : dispatch_classes<true, false, false>(m.n_classes, xmap, p, grid, smem, stream);
 }
 
 cudaError_t launch_rescore_f64(const LinearDeviceModel& m, const LinearLaunch& l, const FlagList& flags, bool all_rows,

@@ -24,6 +24,13 @@ constexpr int kThreads = (kConsumerWarps + 1) * 32;       // + 1 TMA producer wa
 constexpr int kRowsPerLane = kTileRows / 32;              // R = 4 rows per thread
 constexpr int kMaxClassesTma = 16;                        // classes handled in registers by the TMA kernel
 constexpr int kMaxSmemBytes = 227 * 1024;
+// Whole-row schedule of the linear tile kernel (33 <= F <= 64, f_pad = 64): one stage holds complete rows, 64 rows x
+// 64 features = kStageBytes, loaded as two {32, 64} boxes onto one barrier.  Other widths keep 128-row boxes: at
+// F <= 32 one box already holds whole rows, and wider rows do not fit eight stages.
+constexpr int kWholeTileRows = kStageBytes / (2 * kChunkF * 4);  // 64
+__host__ __device__ inline bool linear_whole_rows(int f_pad) { return f_pad == 2 * kChunkF; }
+// rows per box of the tensor map the linear tile kernel reads (its feature width is always kChunkF)
+__host__ __device__ inline int linear_box_rows(int f_pad) { return linear_whole_rows(f_pad) ? kWholeTileRows : kTileRows; }
 
 struct LinearDeviceModel {
   // fp32 operands of the tile kernel: wt[f][cp] (feature-major, classes padded to cp = 4*ceil((C+1)/4), column C holds
@@ -103,6 +110,7 @@ inline cudaError_t launch_dependent(void (*kern)(Params), int grid, int block, s
 
 // scoring kernels (linear_kernels.cu)
 // *rescore_kernel_needed: exact mode with the inline re-score switched off -> the caller launches launch_rescore_f64
+// xmap: the rows as a 2-D map {F, n_rows} with {kChunkF, linear_box_rows(m.f_pad)} boxes, SWIZZLE_128B
 cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& m, const LinearLaunch& l, bool exact,
                               const FlagList& flags, int sm_count, cudaStream_t stream, std::string* err,
                               bool* rescore_kernel_needed);
