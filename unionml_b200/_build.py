@@ -99,6 +99,22 @@ def build_pylist(force: bool = False) -> Path:
     return PYLIST_LIB
 
 
+PROBE_SRC = PKG.parent / "tests" / "cuda" / "wgmma_accum_probe.cu"
+PROBE_LIB = PKG.parent / "build" / "tests" / "libwgmma_accum_probe.so"
+
+
+def build_test_probes(force: bool = False) -> Path:
+    """Test-only library of tests/test_gpu_wgmma_accum.py (the product never loads it): the wgmma accumulation probe,
+    compiled against the product's own wgmma.cuh."""
+    PROBE_LIB.parent.mkdir(parents=True, exist_ok=True)
+    if force or _stale(PROBE_LIB, [PROBE_SRC, *CSRC.glob("*.cuh")]):
+        cmd = [nvcc(), *NVCC_FLAGS, "-shared", str(PROBE_SRC), "-o", str(PROBE_LIB)]
+        r = subprocess.run(cmd, capture_output=True, text=True)
+        if r.returncode != 0:
+            raise RuntimeError(f"nvcc failed for {PROBE_SRC.name}:\n{r.stdout}\n{r.stderr}")
+    return PROBE_LIB
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
     print(build_pylist(force="--force" in sys.argv))

@@ -438,7 +438,12 @@ static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& 
     bias[c] = (float)b[c];
     bmax = fmaxf(bmax, fabsf(bias[c]));
   }
-  bias[C] = bmax;
+  // bound column (DESIGN.md 3.2).  A weight that rounds into the subnormals errs by up to 2^-150 = u FLT_MIN, so
+  // wmax_f is floored at FLT_MIN.  Every FMA of a class chain, the bias rounding and every float64 -> fp32 feature
+  // cast add up to 2^-150 |w| absolute: (F + 2 + sum_f wmax_f) 2^-150 per score.  The guard compares the margin of
+  // two scores, each of which may carry that error with opposite signs, so the constant added to max|b| makes
+  // thr * K cover twice it; its FLT_MIN / thr part keeps thr * A a normal number.
+  double wsum = 0.0;
   for (int f = 0; f < F; ++f) {
     float wmax = 0.f;
     for (int c = 0; c < C; ++c) {
@@ -446,8 +451,12 @@ static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& 
       wt[(size_t)f * cp + c] = v;
       wmax = fmaxf(wmax, fabsf(v));
     }
+    wmax = fmaxf(wmax, (float)uml::kFltMin);
     wt[(size_t)f * cp + C] = wmax;
+    wsum += wmax;
   }
+  const double abs_err = (F + 2.0 + wsum) * uml::kHalfSubnormal;
+  bias[C] = (float)(bmax + (uml::kFltMin + 2.0 * abs_err) / uml::linear_margin_thr(F) * (1.0 + 1.0 / 1024));
   auto ensure = [&](void** p, size_t bytes) -> cudaError_t {
     if (*p) cudaFree(*p);
     *p = nullptr;
@@ -1787,7 +1796,9 @@ int uml_mlp_load(uml_engine* e, uml_mlp** out, const float* w1, const float* b1,
     b2p[c] = b2[c];
     bmax = fmaxf(bmax, fabsf(b2[c]));
   }
-  b2p[C] = bmax;
+  // CUDA-core kernel (DESIGN.md 3.4): the weights and features are the caller's fp32 values, so a hidden unit's only
+  // absolute error is its F FMAs' roundings into the subnormals, plus one for the fp32 A1 chain it is bounded with
+  b2p[C] = uml::mlp_a2_bias_entry(bmax, (F + 2.0) * uml::kHalfSubnormal, row_sum_max, H);
   // fp64 operands of the re-score, laid out as the kernels keep them in shared memory
   const std::vector<double> w64 = uml::mlp_rs_build_pack(w1, b1, w2, b2, F, H, C);
 

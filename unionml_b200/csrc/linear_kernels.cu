@@ -961,8 +961,7 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& 
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(kConsumerWarps, std::min(stages, atoi(env)));
   p.num_stages = stages;
   // margin > 2 err guarantees the fp32 argmax is the exact argmax; err <= (F+4) 2^-24 A (1 + F 2^-21), see DESIGN.md
-  const double F = static_cast<double>(m.n_features);
-  p.thr = static_cast<float>(2.0 * (F + 4.0) * 5.9604644775390625e-08 * (1.0 + F * 4.76837158203125e-07) * 1.0001);
+  p.thr = linear_margin_thr(m.n_features);
   p.flag_count = flags.count;
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;

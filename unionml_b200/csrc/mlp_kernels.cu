@@ -415,10 +415,10 @@ cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, con
   stages = std::min(stages, 64);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(kMlpPairs, std::min(stages, atoi(env)));
   p.num_stages = stages;
-  const double u = 5.9604644775390625e-08;
-  const double F = m.n_in, H = m.n_hidden;
-  p.e1_scale = static_cast<float>((F + 4.0) * u * (1.0 + F * 4.76837158203125e-07) * 1.0001 * m.w2_abs_row_sum_max);
-  p.e2_scale = static_cast<float>((H + 4.0) * u * 1.0001);
+  // the absolute (underflow) part of the bound is in entry C of b2 (uml_mlp_load)
+  const double F = m.n_in;
+  p.e1_scale = static_cast<float>((F + 4.0) * kU * (1.0 + F * 4.76837158203125e-07) * 1.0001 * m.w2_abs_row_sum_max);
+  p.e2_scale = mlp_e2_scale(m.n_hidden);
   p.flag_count = flags.count;
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;

@@ -541,21 +541,27 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
     p.b2[c] = hm.b2[c];
     b2max = fmaxf(b2max, fabsf(hm.b2[c]));
   }
-  p.b2[C] = b2max;
   for (int n = 0; n < H; ++n) b1max = fmaxf(b1max, fabsf(hm.b1[n]));
   p.b1max = b1max;
+  // Below FLT_MIN (DESIGN.md 3.3): the hi / lo split leaves |r| <= 2^-22 |w| only while w - hi is normal; for
+  // |w| < 2^-115 the remainder, or a lo / hi operand the tensor cores flush, is up to FLT_MIN = 4 u 2^-104.  Flooring
+  // w1max_f at 2^-104 puts that inside the split term of e1.
+  double w1max_sum = 0.0;
   for (int f = 0; f < m.n_in; ++f) {
     float wmax = 0.f;
     for (int n = 0; n < H; ++n) wmax = fmaxf(wmax, fabsf(hm.w1[static_cast<size_t>(n) * m.n_in + f]));
-    p.w1max[f] = wmax;
+    p.w1max[f] = fmaxf(wmax, 0x1p-104f);
+    w1max_sum += p.w1max[f];
   }
-  const double u = 5.9604644775390625e-08;  // 2^-24
   const double F = m.n_in, n_mma = m.f_pad / 8.0;
   // layer-1 error as it reaches a logit: per accumulating MMA step <= 32 u (running |.| sum) - a truncating 9-addend
   // aligner without guard bits gives (9 * 2 + 2) u = 20 u -, + 4 u for the W1 split remainder, + 8 u for the small
   // accumulator and the two fp32 adds of the epilogue; A1 itself is an fp32 sum of F terms (factor 1 + F 2^-21)
-  p.e1_scale = static_cast<float>((32.0 * n_mma + 12.0) * u * (1.0 + F * 4.76837158203125e-07) * 1.0001 * m.w2_abs_row_sum_max);
-  p.e2_scale = static_cast<float>((H + 4.0) * u * 1.0001);
+  p.e1_scale = static_cast<float>((32.0 * n_mma + 12.0) * kU * (1.0 + F * 4.76837158203125e-07) * 1.0001 * m.w2_abs_row_sum_max);
+  p.e2_scale = mlp_e2_scale(H);
+  // absolute error of a hidden unit if the tensor cores flush what falls below FLT_MIN: per step and accumulator
+  // (main, small) 8 products and the sum, a subnormal feature |x_f| w1max_f, and 3 for the bias and epilogue adds
+  p.b2[C] = mlp_a2_bias_entry(b2max, (18.0 * n_mma + 3.0 + w1max_sum) * kFltMin, m.w2_abs_row_sum_max, H);
   p.w1_tiles = m.w1_tiles;
   p.labels = l.labels;
   p.n_peers = l.n_peers;

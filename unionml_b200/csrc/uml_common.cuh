@@ -57,6 +57,31 @@ __host__ __device__ inline int linear_w64_stride(int n_classes) {
   return 2 * pairs;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Exactness bounds below FLT_MIN (DESIGN.md 3.2-3.4).  The margin guards compare fp32 margins with a RELATIVE bound
+// (a multiple of u = 2^-24 times an accumulated |.| sum); an fp32 rounding whose result is subnormal errs by up to
+// 2^-150 absolute instead, and a tensor-core flush by up to FLT_MIN.  These host-side constants make the bound columns
+// cover that: they are ~1e-37 of A on ordinary data, so they round away there and change no flag decision.  The bound
+// entries are rounded to nearest; that relative error (u) is inside the 1.0001 slack of every threshold.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr double kU = 5.9604644775390625e-08;            // 2^-24
+constexpr double kFltMin = 1.1754943508222875e-38;       // 2^-126
+constexpr double kHalfSubnormal = 7.006492321624085e-46;  // 2^-150: largest error of a rounding into the subnormals
+// linear tile kernel: a row is certain iff margin > thr * A, thr = 2 err / A, err <= (F+4) u A (1 + F 2^-21)
+inline float linear_margin_thr(int F) {
+  return static_cast<float>(2.0 * (F + 4.0) * kU * (1.0 + F * 4.76837158203125e-07) * 1.0001);
+}
+// MLP kernels: the layer-2 term of err = e1 A1 + e2 A2
+inline float mlp_e2_scale(int H) { return static_cast<float>((H + 4.0) * kU * 1.0001); }
+// entry C of the A2 bias column: max_c |b2_c| plus K2 with e2 K2 >= FLT_MIN + (absolute error of a logit), where a
+// hidden unit carries at most `hidden_abs` absolute error into layer 2 (weighted by max_c sum_n |w2_cn|) and the H
+// fp32 FMAs of layer 2, the two bias adds and the two products of err add 2^-150 each.  The FLT_MIN keeps e2 A2
+// (and so err) a normal number, where the comparison with the margin is relative again.
+inline float mlp_a2_bias_entry(float b2max, double hidden_abs, double w2_abs_row_sum_max, int H) {
+  const double babs = hidden_abs * w2_abs_row_sum_max + (H + 4.0) * kHalfSubnormal;
+  return static_cast<float>(static_cast<double>(b2max) + (kFltMin + babs) / mlp_e2_scale(H) * (1.0 + 1.0 / 1024));
+}
+
 struct FlagList {
   int* count;        // number of flagged rows appended so far; the re-score kernel's last block resets it to 0
   int32_t* rows;     // flagged row indices
