@@ -140,7 +140,8 @@ int main() {
   // the cfg2 model shape: 10 classes, wt [64][cp] with the wmax column, bias [cp] with max|b|
   const int cp = (kC + 1 + 3) / 4 * 4;
   std::vector<float> wt(static_cast<size_t>(kF) * cp, 0.f), bias(cp, 0.f);
-  std::vector<double> w64(static_cast<size_t>(kF) * linear_w64_stride(kC), 0.0), b64(kC, 0.0);
+  // b64 holds 2C doubles as in upload_model: the biases, then the bias magnitudes score_row_f64's bound reads
+  std::vector<double> w64(static_cast<size_t>(kF) * linear_w64_stride(kC), 0.0), b64(2 * kC, 0.0);
   unsigned s = 12345u;
   auto rnd = [&] {
     s = s * 1664525u + 1013904223u;
@@ -160,6 +161,7 @@ int main() {
   for (int c = 0; c < kC; ++c) {
     bias[c] = rnd() * 10.f;
     b64[c] = bias[c];
+    b64[kC + c] = fabs(static_cast<double>(bias[c]));
     bmax = fmaxf(bmax, fabsf(bias[c]));
   }
   bias[kC] = bmax;
@@ -213,6 +215,8 @@ int main() {
     p.b64 = m.b64;
     p.n_classes = kC;
     p.n_features = kF;
+    p.fold_rel = m.fold_rel;  // 0: no affine fold
+    p.binary = m.binary;      // 0: ten classes
     p.counters = counters;
 #ifdef UML_PROBE_WAIT_CLOCKS
     p.probe_clocks = counters + 4;

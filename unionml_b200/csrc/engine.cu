@@ -428,7 +428,10 @@ int uml_host_free(uml_engine* e, void* p) {
 // ---------------------------------------------------------------------------------------------------------------
 // model
 // ---------------------------------------------------------------------------------------------------------------
-static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& w, const std::vector<double>& b) {
+// bmag[c] >= |b_c| is the bias magnitude both bounds use (|b_c| + sum_f |shift_f w'_cf| for a folded affine map) and
+// fold_rel the fp64 bound's extra relative term of such a map (DESIGN.md 3.2)
+static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& w, const std::vector<double>& b,
+                        const std::vector<double>& bmag, double fold_rel) {
   const int C = m->dm.n_classes, F = m->dm.n_features;
   const int cp = (C + 1 + 3) / 4 * 4;
   const int f_pad = (F + uml::kChunkF - 1) / uml::kChunkF * uml::kChunkF;
@@ -436,7 +439,7 @@ static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& 
   float bmax = 0.f;
   for (int c = 0; c < C; ++c) {
     bias[c] = (float)b[c];
-    bmax = fmaxf(bmax, fabsf(bias[c]));
+    bmax = fmaxf(bmax, fmaxf(fabsf(bias[c]), (float)bmag[c]));
   }
   // bound column (DESIGN.md 3.2).  A weight that rounds into the subnormals errs by up to 2^-150 = u FLT_MIN, so
   // wmax_f is floored at FLT_MIN.  Every FMA of a class chain, the bias rounding and every float64 -> fp32 feature
@@ -470,16 +473,20 @@ static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& 
   for (int c = 0; c < C; ++c)
     for (int f = 0; f < F; ++f) w64t[(size_t)f * stride + c] = w[(size_t)c * F + f];
   UML_CUDA(e, ensure((void**)&m->d_w64, w64t.size() * 8));
-  UML_CUDA(e, ensure((void**)&m->d_b64, b.size() * 8));
+  std::vector<double> b64(b);
+  b64.insert(b64.end(), bmag.begin(), bmag.end());
+  UML_CUDA(e, ensure((void**)&m->d_b64, b64.size() * 8));
   UML_CUDA(e, cudaMemcpy(m->d_wt, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice));
   UML_CUDA(e, cudaMemcpy(m->d_bias, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice));
   UML_CUDA(e, cudaMemcpy(m->d_w64, w64t.data(), w64t.size() * 8, cudaMemcpyHostToDevice));
-  UML_CUDA(e, cudaMemcpy(m->d_b64, b.data(), b.size() * 8, cudaMemcpyHostToDevice));
+  UML_CUDA(e, cudaMemcpy(m->d_b64, b64.data(), b64.size() * 8, cudaMemcpyHostToDevice));
   m->dm.wt = m->d_wt;
   m->dm.bias = m->d_bias;
   m->dm.w64 = m->d_w64;
   m->dm.b64 = m->d_b64;
   m->dm.w64_stride = stride;
+  m->dm.fold_rel = fold_rel;
+  m->dm.binary = m->n_classes_in == 1 ? 1 : 0;
   m->dm.cp = cp;
   m->dm.f_pad = f_pad;
   m->uid = g_model_uid.fetch_add(1);
@@ -511,7 +518,9 @@ int uml_linear_load(uml_engine* e, uml_model** out, const void* coef, const void
   }
   m->dm.n_classes = C;
   m->dm.n_features = F;
-  int rc = upload_model(e, m, m->coef64, m->intercept64);
+  std::vector<double> bmag(C);
+  for (int c = 0; c < C; ++c) bmag[c] = fabs(m->intercept64[c]);
+  int rc = upload_model(e, m, m->coef64, m->intercept64, bmag, 0.0);
   if (rc != UML_OK) {
     uml_model_free(m);
     return rc;
@@ -524,20 +533,36 @@ int uml_linear_set_affine(uml_engine* e, uml_model* m, const double* shift, cons
   if (!e || !m) return UML_ERR_INVALID;
   UML_CUDA(e, cudaSetDevice(e->device));
   const int C = m->dm.n_classes, F = m->dm.n_features;
-  std::vector<double> w = m->coef64, b = m->intercept64;
-  // s_c = sum_f ((x_f - shift_f) * scale_f) w_cf + b_c = sum_f x_f (scale_f w_cf) + (b_c - sum_f shift_f scale_f w_cf)
+  std::vector<double> w = m->coef64, b = m->intercept64, bmag(C);
+  // s_c = sum_f ((x_f - shift_f) * scale_f) w_cf + b_c = sum_f x_f w'_cf + b'_c,  w'_cf = scale_f w_cf,
+  // b'_c = b_c - sum_f shift_f w'_cf.  With shift >> the spread of x (a StandardScaler's mean_), the terms of b'_c are
+  // large, of one sign, and cancel against sum_f x_f w'_cf: a plain running sum would round every step the same way
+  // and move the score by up to (F/2) u sum_f |shift_f w'_cf|, outside both bounds.  So b'_c is summed exactly up to
+  // one final rounding plus O(F u^2): each product is split by fma into p + pe (TwoProduct) and the sum carries its
+  // rounding errors in a Neumaier compensation term.  bmag_c = |b_c| + sum_f |shift_f w'_cf| bounds every term.
   for (int c = 0; c < C; ++c) {
-    double acc = b[c];
+    double s = b[c], comp = 0.0, mag = fabs(b[c]);
     for (int f = 0; f < F; ++f) {
       const double sc = scale ? scale[f] : 1.0;
       const double sh = shift ? shift[f] : 0.0;
       const double wf = w[(size_t)c * F + f] * sc;
       w[(size_t)c * F + f] = wf;
-      acc -= sh * wf;
+      const double p = -(sh * wf);
+      const double pe = -std::fma(sh, wf, p);  // sh * wf + p exactly, negated: p + pe = -sh * wf
+      const double t = s + p;
+      comp += fabs(s) >= fabs(p) ? (s - t) + p : (p - t) + s;
+      comp += pe;
+      s = t;
+      mag += fabs(p);
     }
-    b[c] = acc;
+    b[c] = s + comp;
+    bmag[c] = mag;
   }
-  return upload_model(e, m, w, b);
+  // the fold's own rounding (DESIGN.md 3.2): w'_cf and scikit-learn's z_f = (x_f - mean_f) / scale_f each round
+  // relatively (2u both), which moves a score by <= 4.01 u sum_f |z_f w_cf| <= 4.01 u (a + bmag); b'_c errs by <= u |b'_c|
+  // + O(F u^2) bmag.  fold_rel = 8u covers both against the bound's a = max_c (sum_f |x_f w'_cf| + bmag_c).
+  const double fold_rel = (shift || scale) ? 8.0 * 1.1102230246251565e-16 : 0.0;
+  return upload_model(e, m, w, b, bmag, fold_rel);
 }
 
 void uml_model_free(uml_model* m) {

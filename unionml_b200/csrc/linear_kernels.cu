@@ -51,11 +51,15 @@ struct RowScore {
 // the arg-max / runner-up found by a butterfly over the lanes.  LOAD(f) yields feature f of the row as double.
 // w64 is feature-major, w64[f * S + c]: a lane fetches the classes of its feature with 16-byte loads off ONE address
 // (immediate offsets) - the class-major table this replaces cost a 64-bit multiply-add per weight, half of the kernel's
-// instructions at F = 784.
+// instructions at F = 784.  b64 holds 2C doubles: the biases, then each class's bias magnitude for the bound (|b_c|, or
+// |b_c| + sum_f |shift_f w'_cf| for a folded affine map); fold_rel is the bound's extra relative term of a folded map
+// (0 otherwise) and `binary` selects sklearn's `score > 0` rule for the expanded binary layout [0, s] (DESIGN.md 3.2).
 template <typename LOAD>
 __device__ __forceinline__ RowScore score_row_f64(LOAD load, const double* __restrict__ w64, int S,
-                                                  const double* __restrict__ b64, int F, int C, int lane) {
+                                                  const double* __restrict__ b64, int F, int C, double fold_rel,
+                                                  bool binary, int lane) {
   const double u = 1.1102230246251565e-16;  // 2^-53
+  const double q64 = 4.9406564584124654e-324;  // 2^-1074: the spacing of float64 subnormals
   bool bad = false;
   double best = 0.0, second = -INFINITY, amax = 0.0;
   int idx = 0;
@@ -100,25 +104,28 @@ __device__ __forceinline__ RowScore score_row_f64(LOAD load, const double* __res
     t.second = -INFINITY;
     t.idx = cl;
     top2_butterfly(t, 2);
-    amax = fmax(amax, warp_max(valid ? av + fabs(b64[cl]) : 0.0, 2));
+    amax = fmax(amax, warp_max(valid ? av + b64[C + cl] : 0.0, 2));
     if (c0 == 0) {
       best = t.best;
       second = t.second;
       idx = t.idx;
-    } else if (t.best > best) {  // strict: a tie keeps the earlier (lower) class
-      second = fmax(best, t.second);
+    } else if (isnan(t.best) ? !isnan(best) : t.best > best) {  // strict: a tie keeps the earlier (lower) class; the
+      second = fmax(best, t.second);                             // first NaN wins, as in np.argmax
       best = t.best;
       idx = t.idx;
     } else {
       second = fmax(second, t.best);
     }
   }
-  if (idx >= C) idx = 0;  // only reachable with NaN scores, which are reported through `bad`
+  if (idx >= C) idx = 0;  // padding classes score -inf and lose every tie, so this is a guard only
+  if (binary && isnan(best)) idx = 0;  // sklearn's binary rule: `NaN > 0` is False
   RowScore r;
   r.idx = idx;
   r.bad = __any_sync(0xffffffffu, bad);
-  // fp64 error of each score <= (F/32 + 7) u a  (<= 32-way split FMA chains + 5 shuffle adds + bias add)
-  const double err = (static_cast<double>(F) / 32.0 + 8.0) * u * amax;
+  // fp64 error of each score: at most F/32 + 7 roundings (<= 32-way split FMA chains + 5 shuffle adds + bias add),
+  // each <= u |result| or, in the subnormals, <= 2^-1075 absolute.  A folded affine map adds fold_rel a.
+  const double n_ops = static_cast<double>(F) / 32.0 + 8.0;
+  const double err = (n_ops * u + fold_rel) * amax + n_ops * q64;
   r.ambiguous = !((best - second) > 2.0 * err);
   return r;
 }
@@ -153,6 +160,8 @@ struct TmaKernelParams {
   const double* b64;
   int w64_stride;
   int n_classes, n_features;
+  double fold_rel;  // score_row_f64's extra relative bound term (LinearDeviceModel)
+  int binary;
   unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] re-scored rows
 #ifdef UML_PROBE_WAIT_CLOCKS
   unsigned long long* probe_clocks;  // [4], see the diagnostic builds below
@@ -164,13 +173,13 @@ __device__ __noinline__ int rescore_row_inline(const TmaKernelParams& p, long lo
   RowScore r;
   if (p.src.base) {
     const SrcView v = p.src;
-    r = score_row_f64([&](int f) { return load_src(v, row, f); }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, lane);
+    r = score_row_f64([&](int f) { return load_src(v, row, f); }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, p.fold_rel, p.binary != 0, lane);
   } else if (p.x64) {
     const double* xr64 = p.x64 + row * p.ld64;
-    r = score_row_f64([&](int f) { return xr64[f]; }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, lane);
+    r = score_row_f64([&](int f) { return xr64[f]; }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, p.fold_rel, p.binary != 0, lane);
   } else {
     const float* xr = p.x + row * p.ld;
-    r = score_row_f64([&](int f) { return static_cast<double>(xr[f]); }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, lane);
+    r = score_row_f64([&](int f) { return static_cast<double>(xr[f]); }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, p.fold_rel, p.binary != 0, lane);
   }
   if (lane == 0) {
     if (r.bad) atomicAdd(&p.counters[1], 1ull);
@@ -647,7 +656,9 @@ struct RescoreParams {
   int wire_u8;
   long long row_offset;
   unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] flagged (re-scored) rows
-  int smem_weights;              // W, b staged in dynamic shared memory ((C F + C) doubles)
+  int smem_weights;              // W, b staged in dynamic shared memory ((C F + 2 C) doubles)
+  double fold_rel;
+  int binary;
 };
 
 
@@ -661,13 +672,13 @@ __device__ __forceinline__ void rescore_rows(const RescoreParams& p, WPTR w64, W
     RowScore r;
     if (p.src.base) {
       const SrcView v = p.src;
-      r = score_row_f64([&](int f) { return load_src(v, row, f); }, w64, S, b64, F, C, lane);
+      r = score_row_f64([&](int f) { return load_src(v, row, f); }, w64, S, b64, F, C, p.fold_rel, p.binary != 0, lane);
     } else if (p.x64) {
       const double* xr64 = p.x64 + row * p.ld64;
-      r = score_row_f64([&](int f) { return xr64[f]; }, w64, S, b64, F, C, lane);
+      r = score_row_f64([&](int f) { return xr64[f]; }, w64, S, b64, F, C, p.fold_rel, p.binary != 0, lane);
     } else {
       const float* xr = p.x + row * p.ld;
-      r = score_row_f64([&](int f) { return static_cast<double>(xr[f]); }, w64, S, b64, F, C, lane);
+      r = score_row_f64([&](int f) { return static_cast<double>(xr[f]); }, w64, S, b64, F, C, p.fold_rel, p.binary != 0, lane);
     }
     if (lane == 0) {
       if (p.labels) p.labels[row] = r.idx;
@@ -691,7 +702,7 @@ __global__ void __launch_bounds__(256) rescore_f64_kernel(const RescoreParams p)
     const double2* src = reinterpret_cast<const double2*>(p.w64);
     double2* dst = reinterpret_cast<double2*>(rs_w);
     for (int i = threadIdx.x; i < nw / 2; i += blockDim.x) dst[i] = src[i];
-    for (int i = threadIdx.x; i < p.n_classes; i += blockDim.x) rs_w[nw + i] = p.b64[i];
+    for (int i = threadIdx.x; i < 2 * p.n_classes; i += blockDim.x) rs_w[nw + i] = p.b64[i];  // biases + magnitudes
     __syncthreads();
   }
   pdl_wait_for_predecessor();  // the flag list is written by the scoring kernel this launch depends on
@@ -730,6 +741,8 @@ struct SmallParams {
   const double* b64;
   int w64_stride;
   int n_classes, n_features, n_rows;
+  double fold_rel;
+  int binary;
   SmallResult* out;
 };
 
@@ -738,7 +751,7 @@ __global__ void __launch_bounds__(256) linear_small_kernel(const SmallParams p) 
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (row >= p.n_rows) return;
   const SrcView v = p.src;
-  const RowScore r = score_row_f64([&](int f) { return load_src(v, row, f); }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, lane);
+  const RowScore r = score_row_f64([&](int f) { return load_src(v, row, f); }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, p.fold_rel, p.binary != 0, lane);
   if (lane == 0) {
     p.out[row].label = r.idx;
     p.out[row].status = (r.bad ? 1 : 0) | (r.ambiguous ? 2 : 0);
@@ -756,6 +769,8 @@ cudaError_t launch_linear_small(const LinearDeviceModel& m, const SrcView& src, 
   p.n_classes = m.n_classes;
   p.n_features = m.n_features;
   p.n_rows = n_rows;
+  p.fold_rel = m.fold_rel;
+  p.binary = m.binary;
   p.out = out;
   linear_small_kernel<<<(n_rows + 7) / 8, 256, 0, stream>>>(p);
   return cudaGetLastError();
@@ -975,6 +990,8 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& 
   p.b64 = m.b64;
   p.n_classes = m.n_classes;
   p.n_features = m.n_features;
+  p.fold_rel = m.fold_rel;
+  p.binary = m.binary;
   p.counters = flags.counters;
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
   const long long slots = (p.num_tiles + kConsumerWarps - 1) / kConsumerWarps;
@@ -1014,8 +1031,10 @@ cudaError_t launch_rescore_f64(const LinearDeviceModel& m, const LinearLaunch& l
   for (int i = 0; i < 8; ++i) p.peers[i] = i < l.n_peers ? l.peers[i] : nullptr;
   p.row_offset = l.row_offset;
   p.counters = flags.counters;
-  // shared-memory copy of W, b when it fits next to nothing else (<= 200 KB)
-  size_t smem = (static_cast<size_t>(m.n_features) * m.w64_stride + m.n_classes) * sizeof(double);
+  p.fold_rel = m.fold_rel;
+  p.binary = m.binary;
+  // shared-memory copy of W, b (with the bias magnitudes) when it fits next to nothing else (<= 200 KB)
+  size_t smem = (static_cast<size_t>(m.n_features) * m.w64_stride + 2 * m.n_classes) * sizeof(double);
   if (smem > 200 * 1024) smem = 0;
   p.smem_weights = smem > 0 ? 1 : 0;
   static size_t configured = 0;

@@ -219,7 +219,7 @@ __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* con
       t.best = c < C ? s[r] + b : -INFINITY;
       t.second = -INFINITY;
       t.idx = c;
-      top2_butterfly(t, 1);
+      top2_butterfly<false>(t, 1);  // finite logits: no NaN rule needed
       if (c0 == 0) {
         top[r] = t;
       } else if (t.best > top[r].best) {

@@ -26,14 +26,24 @@ __device__ __forceinline__ double warp_reduce16(double (&v)[16], int lane) {
 }
 
 // Running (best, second, argmax) with numpy's first-maximum rule; `second` is the largest of the OTHER scores, so an
-// exact tie gives second == best (margin 0 -> "ambiguous").
+// exact tie gives second == best (margin 0 -> "ambiguous").  NaN follows np.argmax too: a NaN score is the maximum, and
+// the first NaN wins among several (finite features can overflow to inf - inf in float64).  best = NaN then makes the
+// margin test fail, so such a row is counted as ambiguous.
 struct Top2 {
   double best, second;
   int idx;
 };
 
+// does candidate (ob, oi) beat the current best (b, bi) under np.argmax's rule?
+__device__ __forceinline__ bool argmax_takes(double ob, int oi, double b, int bi) {
+  if (isnan(ob)) return !isnan(b) || oi < bi;
+  return !isnan(b) && (ob > b || (ob == b && oi < bi));
+}
+
+// NAN_RULE = false: the caller's scores cannot be NaN (the MLP stage's logits of finite fp32 inputs, DESIGN.md 3.3)
+template <bool NAN_RULE = true>
 __device__ __forceinline__ void top2_merge(Top2& t, double ob, double os, int oi) {
-  const bool take = ob > t.best || (ob == t.best && oi < t.idx);
+  const bool take = NAN_RULE ? argmax_takes(ob, oi, t.best, t.idx) : (ob > t.best || (ob == t.best && oi < t.idx));
   const double loser = take ? t.best : ob;
   t.second = fmax(fmax(t.second, os), loser);
   if (take) {
@@ -43,6 +53,7 @@ __device__ __forceinline__ void top2_merge(Top2& t, double ob, double os, int oi
 }
 
 // all-lanes top-2 over per-lane candidates; first_offset = 2 when lane pairs hold the same class (after warp_reduce16)
+template <bool NAN_RULE = true>
 __device__ __forceinline__ void top2_butterfly(Top2& t, int first_offset) {
 #pragma unroll
   for (int o = 16; o >= 1; o >>= 1) {
@@ -50,7 +61,7 @@ __device__ __forceinline__ void top2_butterfly(Top2& t, int first_offset) {
     const double ob = __shfl_xor_sync(0xffffffffu, t.best, o);
     const double os = __shfl_xor_sync(0xffffffffu, t.second, o);
     const int oi = __shfl_xor_sync(0xffffffffu, t.idx, o);
-    top2_merge(t, ob, os, oi);
+    top2_merge<NAN_RULE>(t, ob, os, oi);
   }
 }
 

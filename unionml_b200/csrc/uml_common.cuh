@@ -38,10 +38,12 @@ struct LinearDeviceModel {
   const float* wt;
   const float* bias;
   // fp64 operands of the re-score / generic kernel: w64[F][w64_stride] (feature-major, classes contiguous and zero
-  // padded; see linear_w64_stride), b64[C]
+  // padded; see linear_w64_stride), b64[2C] = the biases, then each class's bias magnitude for the error bound
   const double* w64;
   const double* b64;
   int w64_stride;
+  double fold_rel;  // extra relative term of the fp64 bound for a folded affine map (DESIGN.md 3.2), else 0
+  int binary;       // the caller's model has one coef_ row: sklearn's `score > 0` rule, NaN gives class 0
   int n_classes;   // C after binary expansion (>= 2)
   int n_features;  // F
   int cp;          // padded class columns in wt
