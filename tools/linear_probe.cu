@@ -1,10 +1,12 @@
 // Where the time of the linear tile kernel goes, on 10M x 64 fp32 rows (2.56 GB, the cfg2 shape), against the card's
-// own read ceiling.  Built three times by tools/linear_probe.sh from linear_kernels.cu itself:
+// own read ceiling.  Built four times by tools/linear_probe.sh from linear_kernels.cu itself:
 //   plain                   read ceiling (streaming 16-byte non-allocating loads) + the tile kernel, both schedules
 //   -DUML_PROBE_FEED_ONLY   the same producer, ring, order and barriers with consumers that skip the math, under
 //                           L2_PROMOTION_256B (what the library encodes) and L2_PROMOTION_NONE
 //   -DUML_PROBE_WAIT_CLOCKS the tile kernel with clock64() totals around the producer's `empty` and the scoring
-//                           warps' `full` waits
+//                           warps' `full` waits, and over the time the scoring warps hold a landed stage
+//   -DUML_PROBE_TIMELINE    the tile kernel with %globaltimer stamps per CTA (entry, first issue, first landing, last
+//                           release, exit) over two back-to-back launches: ramp, exit spread, launch gap
 // Every figure is CUDA-event time over >= 0.5 s of back-to-back launches.  Prints one JSON object per line.
 #include "../unionml_b200/csrc/linear_kernels.cu"
 
@@ -120,6 +122,8 @@ int main() {
   const char* build = "feed_only";
 #elif defined(UML_PROBE_WAIT_CLOCKS)
   const char* build = "wait_clocks";
+#elif defined(UML_PROBE_TIMELINE)
+  const char* build = "timeline";
 #else
   const char* build = "plain";
   {
@@ -188,8 +192,14 @@ int main() {
   uint8_t* labels = nullptr;
   unsigned long long* counters = nullptr;
   CK(cudaMalloc(&labels, kRows));
-  CK(cudaMalloc(&counters, 8 * sizeof(unsigned long long)));
-  CK(cudaMemset(counters, 0, 8 * sizeof(unsigned long long)));
+  CK(cudaMalloc(&counters, 16 * sizeof(unsigned long long)));
+  CK(cudaMemset(counters, 0, 16 * sizeof(unsigned long long)));
+#ifdef UML_PROBE_TIMELINE
+  unsigned long long* timeline = nullptr;  // [2 launches][grid][5]
+  const size_t timeline_words = 2 * static_cast<size_t>(prop.multiProcessorCount) * 5;
+  CK(cudaMalloc(&timeline, timeline_words * sizeof(unsigned long long)));
+  CK(cudaMemset(timeline, 0, timeline_words * sizeof(unsigned long long)));
+#endif
 
   // the EXACT + QUEUE kernel bench.py runs (uint8 labels to one target), in either schedule
   auto run = [&](bool whole, CUtensorMapL2promotion promo, const char* promo_name) {
@@ -219,7 +229,10 @@ int main() {
     p.binary = m.binary;      // 0: ten classes
     p.counters = counters;
 #ifdef UML_PROBE_WAIT_CLOCKS
-    p.probe_clocks = counters + 4;
+    p.probe_clocks = counters + 8;
+#endif
+#ifdef UML_PROBE_TIMELINE
+    p.probe_timeline = timeline;
 #endif
     const size_t smem = fixed + static_cast<size_t>(p.num_stages) * kStageBytes;
     const int grid = prop.multiProcessorCount;
@@ -234,7 +247,7 @@ int main() {
            build, whole ? "whole_rows_64" : "chunked_128x32", promo_name, p.num_stages, ms, bytes / ms * 1e-6);
 #ifdef UML_PROBE_WAIT_CLOCKS
     // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time
-    CK(cudaMemset(counters + 4, 0, 4 * sizeof(unsigned long long)));
+    CK(cudaMemset(counters + 8, 0, 5 * sizeof(unsigned long long)));
     cudaEvent_t a, b;
     CK(cudaEventCreate(&a));
     CK(cudaEventCreate(&b));
@@ -244,11 +257,68 @@ int main() {
     CK(cudaEventSynchronize(b));
     float one = 0.f;
     CK(cudaEventElapsedTime(&one, a, b));
-    unsigned long long c[4];
-    CK(cudaMemcpy(c, counters + 4, sizeof(c), cudaMemcpyDeviceToHost));
-    printf(", \"producer_empty_wait_frac\": %.4f, \"consumer_full_wait_frac\": %.4f, \"sm_clock_mhz_under_load\": %.0f",
-           static_cast<double>(c[0]) / c[1], static_cast<double>(c[2]) / c[3],
-           static_cast<double>(c[1]) / grid / (one * 1e3));
+    unsigned long long c[5];
+    CK(cudaMemcpy(c, counters + 8, sizeof(c), cudaMemcpyDeviceToHost));
+    // mean stages per CTA landed and not yet released (one scoring warp per stage): the scoring warps' summed hold time
+    // over one warp's loop time, per CTA
+    const int scoring_warps = grid * kConsumerWarps;
+    const double held_stages = static_cast<double>(c[4]) / (static_cast<double>(c[3]) / scoring_warps) / grid;
+    printf(", \"producer_empty_wait_frac\": %.4f, \"consumer_full_wait_frac\": %.4f, \"held_stages\": %.3f, "
+           "\"ring_stages\": %d, \"sm_clock_mhz_under_load\": %.0f",
+           static_cast<double>(c[0]) / c[1], static_cast<double>(c[2]) / c[3], held_stages,
+           p.num_stages, static_cast<double>(c[1]) / grid / (one * 1e3));
+#endif
+#ifdef UML_PROBE_TIMELINE
+    // two launches back to back, each stamping its own [grid][5] block
+    CK(cudaMemset(timeline, 0, timeline_words * sizeof(unsigned long long)));
+    CK(cudaDeviceSynchronize());
+    launch();
+    p.probe_timeline = timeline + static_cast<size_t>(grid) * 5;
+    launch();
+    p.probe_timeline = timeline;
+    CK(cudaDeviceSynchronize());
+    std::vector<unsigned long long> t(timeline_words);
+    CK(cudaMemcpy(t.data(), timeline, timeline_words * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    auto col = [&](int launch_k, int slot) {
+      std::vector<double> v(grid);
+      for (int b = 0; b < grid; ++b) v[b] = static_cast<double>(t[(static_cast<size_t>(launch_k) * grid + b) * 5 + slot]);
+      return v;
+    };
+    auto median = [](std::vector<double> v) {
+      std::sort(v.begin(), v.end());
+      return v[v.size() / 2];
+    };
+    for (int k = 0; k < 2; ++k) {
+      const std::vector<double> entry = col(k, 0), issue = col(k, 1), land = col(k, 2), rel = col(k, 3), ex = col(k, 4);
+      std::vector<double> ramp(grid), first_issue(grid), tail(grid);
+      for (int b = 0; b < grid; ++b) {
+        ramp[b] = land[b] - entry[b];
+        first_issue[b] = issue[b] - entry[b];
+        tail[b] = ex[b] - rel[b];
+      }
+      const double e0 = *std::min_element(entry.begin(), entry.end());
+      const double x0 = *std::min_element(ex.begin(), ex.end()), x1 = *std::max_element(ex.begin(), ex.end());
+      printf(", \"launch%d\": {\"span_us\": %.2f, \"entry_spread_us\": %.2f, \"first_issue_us_median\": %.2f, "
+             "\"ramp_us_median\": %.2f, \"ramp_us_max\": %.2f, \"exit_spread_us_max\": %.2f, "
+             "\"exit_spread_us_median\": %.2f, \"last_release_to_exit_us_max\": %.2f}",
+             k, (x1 - e0) * 1e-3, (*std::max_element(entry.begin(), entry.end()) - e0) * 1e-3,
+             median(first_issue) * 1e-3, median(ramp) * 1e-3, *std::max_element(ramp.begin(), ramp.end()) * 1e-3,
+             (x1 - x0) * 1e-3, (median(ex) - x0) * 1e-3, *std::max_element(tail.begin(), tail.end()) * 1e-3);
+    }
+    {
+      const std::vector<double> ex0 = col(0, 4), entry1 = col(1, 0);
+      std::vector<double> all;
+      for (int k = 0; k < 2; ++k)
+        for (int s = 0; s < 5; ++s)
+          for (double v : col(k, s)) all.push_back(v);
+      std::sort(all.begin(), all.end());
+      double quantum = 0.0;  // the smallest step between distinct stamps: the timer's resolution, or finer
+      for (size_t i = 1; i < all.size(); ++i)
+        if (all[i] > all[i - 1] && (quantum == 0.0 || all[i] - all[i - 1] < quantum)) quantum = all[i] - all[i - 1];
+      printf(", \"launch_gap_us\": %.2f, \"timer_step_ns_min\": %.0f",
+             (*std::min_element(entry1.begin(), entry1.end()) - *std::max_element(ex0.begin(), ex0.end())) * 1e-3,
+             quantum);
+    }
 #endif
     printf("}\n");
     fflush(stdout);

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Read ceiling + feed-only + wait-clock breakdown of the linear tile kernel (tools/linear_probe.cu), on GPU 0.
+# Read ceiling + feed-only + wait-clock + timeline breakdown of the linear tile kernel (tools/linear_probe.cu), on GPU 0.
 # Writes MEASURED_PEAKS.json (the read ceiling bench.py's roofline divides by) and the probe's JSON lines to
 # ${1:-build/probe}/linear_probe.jsonl.  Binaries go to build/probe/.
 set -euo pipefail
@@ -8,8 +8,8 @@ out=${1:-build/probe}
 mkdir -p build/probe "$out"
 nvcc=${NVCC:-$(command -v nvcc || echo /usr/local/cuda/bin/nvcc)}
 flags=(-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo)
-declare -A defs=([plain]="" [feed_only]="-DUML_PROBE_FEED_ONLY" [wait_clocks]="-DUML_PROBE_WAIT_CLOCKS")
-for v in plain feed_only wait_clocks; do
+declare -A defs=([plain]="" [feed_only]="-DUML_PROBE_FEED_ONLY" [wait_clocks]="-DUML_PROBE_WAIT_CLOCKS" [timeline]="-DUML_PROBE_TIMELINE")
+for v in plain feed_only wait_clocks timeline; do
   bin=build/probe/linear_probe_$v
   if [ ! -x "$bin" ] || [ tools/linear_probe.cu -nt "$bin" ] || [ unionml_b200/csrc/linear_kernels.cu -nt "$bin" ]; then
     "$nvcc" "${flags[@]}" ${defs[$v]} tools/linear_probe.cu -o "$bin" &
@@ -17,7 +17,7 @@ for v in plain feed_only wait_clocks; do
 done
 wait
 nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noheader | sed 's/^/# before: /' | tee -a "$out/linear_probe.jsonl"
-for v in plain feed_only wait_clocks; do
+for v in plain feed_only wait_clocks timeline; do
   build/probe/linear_probe_$v | tee -a "$out/linear_probe.jsonl"
 done
 nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noheader | sed 's/^/# after: /' | tee -a "$out/linear_probe.jsonl"

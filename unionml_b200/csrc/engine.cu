@@ -329,14 +329,14 @@ int uml_engine_create(uml_engine** out, int device_id) {
   for (auto& ev : e->chunk_ev)
     if ((err = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", err);
   if ((err = cudaMalloc(&e->d_flag_count, sizeof(int))) != cudaSuccess) return fail("cudaMalloc", err);
-  if ((err = cudaMalloc(&e->d_counters, 4 * sizeof(unsigned long long))) != cudaSuccess) return fail("cudaMalloc", err);
+  if ((err = cudaMalloc(&e->d_counters, 6 * sizeof(unsigned long long))) != cudaSuccess) return fail("cudaMalloc", err);
   if ((err = cudaMalloc(&e->d_stage, sizeof(StageResult))) != cudaSuccess) return fail("cudaMalloc", err);
   if ((err = cudaHostAlloc((void**)&e->h, sizeof(HostMirror), cudaHostAllocMapped)) != cudaSuccess)
     return fail("cudaHostAlloc", err);
   memset(e->h, 0, sizeof(HostMirror));
   // the scoring steps do not memset these: the re-score kernel hands the flag list back empty (linear_kernels.cu)
   if ((err = cudaMemset(e->d_flag_count, 0, sizeof(int))) != cudaSuccess) return fail("cudaMemset", err);
-  if ((err = cudaMemset(e->d_counters, 0, 4 * sizeof(unsigned long long))) != cudaSuccess) return fail("cudaMemset", err);
+  if ((err = cudaMemset(e->d_counters, 0, 6 * sizeof(unsigned long long))) != cudaSuccess) return fail("cudaMemset", err);
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   err = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);

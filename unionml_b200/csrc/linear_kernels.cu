@@ -164,7 +164,10 @@ struct TmaKernelParams {
   int binary;
   unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] re-scored rows
 #ifdef UML_PROBE_WAIT_CLOCKS
-  unsigned long long* probe_clocks;  // [4], see the diagnostic builds below
+  unsigned long long* probe_clocks;  // [5], see the diagnostic builds below
+#endif
+#ifdef UML_PROBE_TIMELINE
+  unsigned long long* probe_timeline;  // [gridDim.x][5], see the diagnostic builds below
 #endif
 };
 
@@ -188,6 +191,7 @@ __device__ __noinline__ int rescore_row_inline(const TmaKernelParams& p, long lo
   return r.idx;
 }
 
+constexpr int kTileSentinel = -1;        // WHOLE: ring item that ends a scoring warp's loop
 constexpr int kQueueCap = 2048;           // flagged-row queue of the QUEUE kernels (power of two)
 constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this many slots are free (8 warps x 128 rows)
 constexpr int kThreadsQueue = kThreads + 32;  // + 1 fp64 re-score warp
@@ -205,7 +209,10 @@ __device__ __forceinline__ void store_final_label(const TmaKernelParams& p, long
 //  UML_PROBE_FEED_ONLY    the scoring warps hand each stage back as soon as it has landed, without the math: what the
 //                         ring (producer, order, barriers) delivers on its own
 //  UML_PROBE_WAIT_CLOCKS  clock64() totals added into p.probe_clocks: [0] the producer's `empty` waits, [1] its whole
-//                         loop, [2] the scoring warps' waits for their data, [3] their whole loops
+//                         loop, [2] the scoring warps' waits for their data, [3] their whole loops, [4] the time they
+//                         hold a landed stage (from the return of the `full` wait to the `empty` arrive)
+//  UML_PROBE_TIMELINE     %globaltimer per CTA into p.probe_timeline[blockIdx.x][5]: [0] entry, [1] the producer's first
+//                         issue, [2] the first stage landed (warp 0), [3] the last `empty` arrive, [4] exit
 #ifdef UML_PROBE_FEED_ONLY
 constexpr bool kFeedOnly = true;
 #else
@@ -218,13 +225,33 @@ constexpr bool kFeedOnly = false;
     __VA_ARGS__;                        \
     (total) += clock64() - t0_;         \
   } while (0)
+#define UML_PROBE_CLOCK(t) const long long t = clock64()
+#define UML_PROBE_SINCE(total, t) (total) += clock64() - (t)
 #else
 #define UML_PROBE_TIMED(total, ...) __VA_ARGS__
+#define UML_PROBE_CLOCK(t)
+#define UML_PROBE_SINCE(total, t)
+#endif
+#ifdef UML_PROBE_TIMELINE
+__device__ __forceinline__ unsigned long long probe_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#define UML_PROBE_STAMP(slot) (p.probe_timeline[blockIdx.x * 5 + (slot)] = probe_globaltimer())
+#define UML_PROBE_LANDED(first) \
+  if ((first) && warp == 0 && lane == 0) UML_PROBE_STAMP(2)
+#define UML_PROBE_RELEASED() probe_last_release = probe_globaltimer()
+#else
+#define UML_PROBE_STAMP(slot)
+#define UML_PROBE_LANDED(first)
+#define UML_PROBE_RELEASED()
 #endif
 
 // WHOLE (f_pad == 64, linear_whole_rows): one ring stage is one 64-row tile with all its features, loaded as two
-// {32 features, 64 rows} boxes onto one barrier; warp w scores the CTA's tiles w, w + 8, ... (2 rows per lane).
-// Otherwise one stage is a 128-row x 32-feature box and a tile takes f_pad / 32 stages (4 rows per lane).
+// {32 features, 64 rows} boxes onto one barrier; the producer claims the tiles in groups of 8 from a global counter
+// and ring item n goes to warp n % 8 (2 rows per lane).  Otherwise one stage is a 128-row x 32-feature box, a tile
+// takes f_pad / 32 stages (4 rows per lane) and the CTA scores tiles blockIdx.x, blockIdx.x + gridDim.x, ...
 template <int C, bool EXACT, bool QUEUE, bool WHOLE>
 __global__ void __launch_bounds__(kThreadsQueue, 1)
 linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ TmaKernelParams p) {
@@ -249,9 +276,13 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   // warps done, ctl[3] = slots consumed
   int* q_slots = reinterpret_cast<int*>(empty_bar + S);
   int* q_ctl = q_slots + kQueueCap;
+  // WHOLE: the tile each stage holds, written by the producer before the stage's `full` arrive (whose release makes it
+  // visible to the waiters); kTileSentinel ends a scoring warp's loop
+  int* tile_slot = q_ctl + 4;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) UML_PROBE_STAMP(0);
 
   // stage W^T (with its wmax column) and the bias once per CTA; they stay resident for every tile this CTA scores
   {
@@ -286,6 +317,9 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     // ===================== TMA producer (one elected lane) =====================
     if (elect_one_sync()) {
       tma_prefetch_desc(&xmap);
+#ifdef UML_PROBE_TIMELINE
+      bool probe_first_issue = true;
+#endif
       const uint64_t policy = make_evict_first_policy();  // X is read exactly once
       int stage = 0;
       uint32_t phase = 0;
@@ -296,15 +330,46 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         }
       };
       if constexpr (WHOLE) {
-        // ring item n of this CTA = its n-th tile (tile blockIdx.x + n*G): both halves of its rows land together
-        for (long long tile = blockIdx.x; tile < num_tiles; tile += G) {
-          UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u));
-          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-          uint8_t* dst = smem + static_cast<size_t>(stage) * kStageBytes;
-          const int row = static_cast<int>(tile * TILE);
-          tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
-          tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], kChunkF, row, policy);
-          next_stage();
+        // Tiles are claimed, kConsumerWarps at a time, from a counter shared by the grid: with a static split, CTAs
+        // with equal tile counts finished up to ~0.24 ms apart (SMs draw unequal shares of HBM bandwidth), and the
+        // launch lasted as long as the slowest one.  Ring item n is one tile with both halves of its rows and goes to
+        // warp n % kConsumerWarps; a group claimed past the end hands every warp kTileSentinel.  The next group is
+        // claimed while this one is issued, so the atomic's round trip stays off the ring.
+        unsigned long long* claim = p.counters + 4;  // [0] next unclaimed tile, [1] CTAs done claiming
+        long long base = static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(kConsumerWarps)));
+        for (;;) {
+          const long long next =
+              base < num_tiles ? static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(kConsumerWarps)))
+                               : base;
+          for (int w = 0; w < kConsumerWarps; ++w) {
+            const long long tile = base + w;
+            UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u));
+            tile_slot[stage] = base < num_tiles ? static_cast<int>(tile) : kTileSentinel;
+            if (tile < num_tiles) {
+              mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+              uint8_t* dst = smem + static_cast<size_t>(stage) * kStageBytes;
+              const int row = static_cast<int>(tile * TILE);
+              tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
+              tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], kChunkF, row, policy);
+#ifdef UML_PROBE_TIMELINE
+              if (probe_first_issue) UML_PROBE_STAMP(1);
+              probe_first_issue = false;
+#endif
+            } else {
+              mbar_arrive(&full_bar[stage]);  // past the last tile: nothing to load, the warp skips or stops
+            }
+            next_stage();
+          }
+          if (base >= num_tiles) break;
+          base = next;
+        }
+        // this CTA claims no more; the last CTA to get here hands the counter back at 0 for the next launch on the
+        // stream (no memset between steps, and correct under CUDA-graph replay)
+        __threadfence();
+        if (atomicAdd(claim + 1, 1ull) == static_cast<unsigned long long>(gridDim.x) - 1ull) {
+          claim[0] = 0ull;
+          claim[1] = 0ull;
+          __threadfence();
         }
       } else {
         // Work items in ring order: for each round (kConsumerWarps tiles), for each 32-feature chunk k, for each
@@ -317,6 +382,9 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
               mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
               tma_load_2d(smem + static_cast<size_t>(stage) * kStageBytes, &xmap, &full_bar[stage], k * kChunkF,
                           static_cast<int>((first + w * G) * TILE), policy);
+#ifdef UML_PROBE_TIMELINE
+              if (first == blockIdx.x && k == 0 && w == 0) UML_PROBE_STAMP(1);
+#endif
               next_stage();
             }
           }
@@ -335,6 +403,12 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     // eight lanes of every LDS.128 phase (lanes 8i..8i+7: l & 7 = 0..7) hit eight distinct bank groups.  The whole-row
     // stage is two such boxes (features 0-31, then 32-63 at +8 KiB), so the same holds in both halves.
     const uint32_t lanebase = static_cast<uint32_t>(lane) * 128u + static_cast<uint32_t>(lane & 7) * 16u;
+#ifdef UML_PROBE_WAIT_CLOCKS
+    long long probe_hold = 0;
+#endif
+#ifdef UML_PROBE_TIMELINE
+    unsigned long long probe_last_release = 0;
+#endif
 
     // USE_F2 (EXACT kernels): class accumulators as fp32x2 pairs (classes 2i, 2i+1 -> one fma2); an odd last class
     // and the error-bound column (|x| is a free operand modifier on scalar FFMA) stay scalar.
@@ -535,20 +609,29 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       // this warp's ring items are n = warp, warp + 8, ... (stage n % S, phase (n / S) & 1); S >= 8 lets stage and
       // phase advance without a division.  Both waits keep the invariant argued below: the next item is n + 8 <= n + S.
       uint32_t stage = static_cast<uint32_t>(warp), phase = 0;
-      for (long long tile = blockIdx.x + warp * G; scoring_warp && tile < num_tiles; tile += G * kConsumerWarps) {
+      for (bool first = true; scoring_warp; first = false) {
         init_acc();
         UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
-        const uint8_t* xs = smem + static_cast<size_t>(stage) * kStageBytes;
-        fma_box(xs, wt_s);
-        fma_box(xs + BOX_BYTES, wt_s + kChunkF * CP);
+        UML_PROBE_CLOCK(probe_landed);
+        UML_PROBE_LANDED(first);
+        const int tile = tile_slot[stage];
+        const bool scored = tile >= 0 && tile < num_tiles;
+        if (scored) {
+          const uint8_t* xs = smem + static_cast<size_t>(stage) * kStageBytes;
+          fma_box(xs, wt_s);
+          fma_box(xs + BOX_BYTES, wt_s + kChunkF * CP);
+        }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[stage]);  // hand the stage back to the producer
+        UML_PROBE_SINCE(probe_hold, probe_landed);
+        UML_PROBE_RELEASED();
+        if (tile == kTileSentinel) break;
         stage += kConsumerWarps;
         if (stage >= static_cast<uint32_t>(S)) {
           stage -= S;
           phase ^= 1u;
         }
-        finish_tile(tile);
+        if (scored) finish_tile(tile);
       }
     } else {
       uint32_t seq_base = 0;
@@ -570,19 +653,27 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             // S >= kConsumerWarps stages: the producer could only issue item seq after item seq - S was released, so
             // item seq + nv - 2S was too.
             UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
+            UML_PROBE_CLOCK(probe_landed);
+            UML_PROBE_LANDED(seq == 0);
             fma_box(smem + static_cast<size_t>(stage) * kStageBytes, wt_s + k * kChunkF * CP);
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[stage]);  // hand the stage back to the producer
+            UML_PROBE_SINCE(probe_hold, probe_landed);
+            UML_PROBE_RELEASED();
           }
           finish_tile(tile);
         }
         seq_base += static_cast<uint32_t>(KC * nv);
       }
     }
+#ifdef UML_PROBE_TIMELINE
+    if (scoring_warp && lane == 0 && probe_last_release != 0) atomicMax(&p.probe_timeline[blockIdx.x * 5 + 3], probe_last_release);
+#endif
 #ifdef UML_PROBE_WAIT_CLOCKS
     if (scoring_warp && lane == 0) {
       atomicAdd(&p.probe_clocks[2], static_cast<unsigned long long>(probe_wait));
       atomicAdd(&p.probe_clocks[3], static_cast<unsigned long long>(clock64() - probe_start));
+      atomicAdd(&p.probe_clocks[4], static_cast<unsigned long long>(probe_hold));
     }
 #endif
     if constexpr (EXACT && QUEUE) {
@@ -631,6 +722,9 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       if (lane == 0 && n_done > 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n_done));
     }
   }
+#ifdef UML_PROBE_TIMELINE
+  if (lane == 0) atomicMax(&p.probe_timeline[blockIdx.x * 5 + 4], probe_globaltimer());
+#endif
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -886,8 +980,10 @@ cudaError_t launch_linear_proba(const LinearDeviceModel& m, const float* x, int6
 // host side
 // ---------------------------------------------------------------------------------------------------------------
 static size_t tma_fixed_smem(const LinearDeviceModel& m) {
-  // alignment slack + W^T + bias + barriers (64 stages max) + the flagged-row queue of the QUEUE kernels
-  return 1024 + static_cast<size_t>(m.f_pad) * m.cp * 4 + static_cast<size_t>(m.cp) * 4 + 2 * 64 * 8 + (kQueueCap + 4) * 4;
+  // alignment slack + W^T + bias + barriers (64 stages max) + the flagged-row queue of the QUEUE kernels (+ the tile
+  // index of each stage, whole-row schedule)
+  return 1024 + static_cast<size_t>(m.f_pad) * m.cp * 4 + static_cast<size_t>(m.cp) * 4 + 2 * 64 * 8 + (kQueueCap + 4) * 4 +
+         (linear_whole_rows(m.f_pad) ? 64 * 4 : 0);
 }
 
 bool linear_tma_supported(const LinearDeviceModel& m, std::string* why) {

@@ -88,7 +88,8 @@ struct FlagList {
   int* count;        // number of flagged rows appended so far; the re-score kernel's last block resets it to 0
   int32_t* rows;     // flagged row indices
   int capacity;
-  unsigned long long* counters;  // [0] = n_ambiguous, [1] = n_nonfinite, [2] = n_flagged, [3] = re-score blocks done
+  unsigned long long* counters;  // [0] = n_ambiguous, [1] = n_nonfinite, [2] = n_flagged, [3] = re-score blocks done,
+                                 // [4], [5] = the whole-row tile kernel's tile claim (handed back at 0 by every launch)
 };
 
 // The caller's own values for the rows of a launch: the raw source chunk as it was copied to the device (any dtype,
