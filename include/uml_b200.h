@@ -193,6 +193,11 @@ UML_API int uml_mlp_load(uml_engine* e, uml_mlp** out, const float* w1, const fl
 UML_API void uml_mlp_free(uml_mlp* m);
 UML_API int uml_mlp_predict(uml_engine* e, const uml_mlp* m, const uml_batch* b, int32_t* labels_out, int labels_on_device,
                     int mode, uml_stats* stats);
+/* class probabilities of the MLP predictor: softmax(W2 relu(W1 x + b1) + b2) per row, i.e. PytorchModel.forward of
+ * tests/integration/pytorch_app/quickstart.py:23-24.  fp32; proba_out: n_rows x n_out row-major, host or device memory.
+ * stats (optional): path 5 / 3 / 2 as for uml_mlp_predict, kernel_ms, kernel_launches. */
+UML_API int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, float* proba_out,
+                                  int proba_on_device, uml_stats* stats);
 
 /* the MLP predictor from HOST rows through the same chunk pipeline as uml_linear_predict_host (pinned bounce buffers,
  * GPU transpose / down-cast to fp32 - the reference predictor casts features to float32 -, scoring kernel, fp64

@@ -175,6 +175,8 @@ struct uml_engine {
   int64_t flag_cap = 0;
   int32_t* d_labels = nullptr;
   int64_t labels_cap = 0;
+  float* d_proba = nullptr;  // class probabilities bound for host memory (uml_mlp_predict_proba)
+  int64_t proba_cap = 0;     // floats
   void* d_chunk[3] = {nullptr, nullptr, nullptr};  // raw source chunks (staging / predict_host)
   int64_t chunk_cap = 0;
   float* d_xchunk[3] = {nullptr, nullptr, nullptr};  // converted fp32 chunks (predict_host)
@@ -356,6 +358,7 @@ void uml_engine_destroy(uml_engine* e) {
   cudaFree(e->d_stage);
   cudaFree(e->d_flag_rows);
   cudaFree(e->d_labels);
+  cudaFree(e->d_proba);
   for (auto p : e->d_chunk) cudaFree(p);
   for (auto p : e->d_xchunk) cudaFree(p);
   for (auto p : e->d_vchunk) cudaFree(p);
@@ -949,6 +952,16 @@ static int ensure_labels(uml_engine* e, int64_t rows) {
   e->labels_cap = 0;
   UML_CUDA(e, cudaMalloc((void**)&e->d_labels, (size_t)rows * 4));
   e->labels_cap = rows;
+  return UML_OK;
+}
+
+static int ensure_proba(uml_engine* e, int64_t n_floats) {
+  if (e->proba_cap >= n_floats) return UML_OK;
+  cudaFree(e->d_proba);
+  e->d_proba = nullptr;
+  e->proba_cap = 0;
+  UML_CUDA(e, cudaMalloc((void**)&e->d_proba, (size_t)n_floats * 4));
+  e->proba_cap = n_floats;
   return UML_OK;
 }
 
@@ -2019,6 +2032,69 @@ int uml_mlp_predict_peers(uml_engine* e, const uml_mlp* m, const uml_batch* b, v
                           int64_t row_offset, int label_bytes, int mode, uml_stats* stats) {
   if (!peer_labels || n_peers < 1) return UML_ERR_INVALID;
   return mlp_predict_common(e, m, b, nullptr, 1, peer_labels, n_peers, row_offset, label_bytes, mode, stats);
+}
+
+int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, float* proba_out, int proba_on_device,
+                          uml_stats* stats) {
+  if (!e || !m || !b || (!proba_out && b->n_rows > 0)) return UML_ERR_INVALID;
+  if (b->n_features != m->dm.n_in)
+    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the module is expecting %d features as input.", b->n_features,
+             m->dm.n_in);
+  UML_CUDA(e, cudaSetDevice(e->device));
+  (void)cudaGetLastError();
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (b->n_rows == 0) return UML_OK;
+  NvtxRange r_all("uml:mlp_proba");
+  // the labels' kernel choice, except that UML_B200_MLP_TC=1 does not send rows that are not tf32 values to the
+  // tensor cores: the probability kernels have no fp64 re-score behind them
+  std::string why;
+  bool use_tc = b->has_map && uml::mlp_tc_supported(m->dm, &why);
+  if (use_tc) {
+    const char* env = getenv("UML_B200_MLP_TC");
+    use_tc = !(env && env[0] == '0') && batch_tf32_exact(e, b) == 1;
+  }
+  const bool use_ffma = !use_tc && b->has_map && uml::mlp_tma_supported(m->dm, &why, true);
+  const int64_t n_floats = b->n_rows * m->dm.n_classes;
+  float* d_out = proba_out;
+  int rc;
+  if (!proba_on_device) {
+    if ((rc = ensure_proba(e, n_floats)) != UML_OK) return rc;
+    d_out = e->d_proba;
+  }
+  const bool timed = stats != nullptr;
+  if (timed) {
+    UML_CUDA(e, cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), e->stream));
+    UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
+    UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
+  }
+  int path;
+  if (use_tc) {
+    uml::MlpTcLaunch out{};
+    out.n_rows = b->n_rows;
+    out.proba = d_out;
+    UML_CUDA(e, uml::launch_mlp_tc_proba(b->map, m->dm, out, e->info.sm_count, e->stream));
+    path = 5;
+  } else if (use_ffma) {
+    UML_CUDA(e, uml::launch_mlp_tma(b->map, m->dm, b->x, b->n_rows, nullptr, false, FlagList{}, e->info.sm_count, e->stream,
+                                    d_out));
+    path = 3;
+  } else {
+    UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, b->x, b->ld, b->n_rows, d_out, e->info.sm_count, e->stream));
+    path = 2;
+  }
+  if (timed) {
+    UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
+    UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
+  }
+  if (!proba_on_device)
+    UML_CUDA(e, cudaMemcpyAsync(proba_out, d_out, (size_t)n_floats * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (timed) {
+    rc = finish_stats(e, stats, b->n_rows, 1, path, true);
+    stats->d2h_bytes = proba_on_device ? 0 : n_floats * 4;
+    return rc;
+  }
+  if (!proba_on_device) UML_CUDA(e, cudaStreamSynchronize(e->stream));
+  return UML_OK;
 }
 
 }  // extern "C"

@@ -8,8 +8,11 @@
 //    landed box (W1^T rows are warp-uniform broadcast LDS.128 from shared memory), then ReLU, layer 2 and the argmax are
 //    fused in registers.  EXACT mode carries two bound accumulators (A1 over layer 1, A2 over layer 2) and re-scores
 //    rows whose logit margin is inside the propagated fp32 error bound in fp64.
+//    PROBA instantiations store softmax(logits) instead of the label: each warp's 32 consecutive rows per j leave as one
+//    coalesced run through shared memory (mlp_proba.cuh).
 //  * mlp_rescore_f64_kernel: warp per row, lane per hidden unit, fp64; flagged rows of EXACT mode, or every row for
 //    shapes the tile kernel is not instantiated for.
+//  * mlp_proba_f64_kernel: class probabilities for those shapes - the same fp64 scorer, then a float64 softmax.
 //
 // This is CUDA-core fp32 (FFMA): 4 736 flop/row puts the HBM roofline (25 G rows/s) above the FFMA peak, so this kernel
 // is FMA-pipe bound (~0.66 ms per 10M rows at 1.9 GHz).  It serves batches whose features are NOT tf32 values (general
@@ -20,6 +23,7 @@
 #include "uml_common.cuh"
 #include "tma_ring.cuh"
 #include "mlp_rescore.cuh"
+#include "mlp_proba.cuh"
 
 #ifndef UML_MLP_UNROLL_Q
 #define UML_MLP_UNROLL_Q 8  // feature-quad unroll of the layer-1 loop
@@ -55,9 +59,10 @@ struct MlpKernelParams {
   int* flag_count;
   int32_t* flag_rows;
   int flag_cap;
+  float* proba;  // PROBA kernels: [n_rows][C] row-major
 };
 
-template <int H, int C, bool EXACT>
+template <int H, int C, bool EXACT, bool PROBA>
 __global__ void __launch_bounds__(kMlpThreads, 1)
 mlp_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const MlpKernelParams p) {
   constexpr int HP = H + 4;
@@ -224,6 +229,18 @@ mlp_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const MlpKernelP
 #pragma unroll
         for (int j = 0; j < R; ++j) {
           const long long row = tile * kMlpTileRows + half * 64 + lane + 32 * j;
+          if constexpr (PROBA) {
+            // the warp's rows 32 j .. 32 j + 31 of its half: lane l's C probabilities at l C of the warp's strip
+            float* strip = reinterpret_cast<float*>(empty_bar + S) + warp * 32 * C;
+            float pr[C];
+            mlp_softmax_f32<C>(z[j], pr);
+#pragma unroll
+            for (int c = 0; c < C; ++c) strip[lane * C + c] = pr[c];
+            __syncwarp();
+            mlp_proba_store_run<C, 32>(strip, p.proba, row - lane, p.n_rows, lane);
+            __syncwarp();  // the strip is rewritten for the next run
+            continue;
+          }
           float best = z[j][0];
           float second = -INFINITY;
           int idx = 0;
@@ -351,31 +368,76 @@ __global__ void __launch_bounds__(256) mlp_rescore_f64_kernel(const MlpRescorePa
   }
 }
 
+// class probabilities for shapes no tile kernel takes: the logits of the fp64 scorer above (mlp_rs_rows), a float64
+// softmax, each probability rounded once to fp32.  A warp scores kMlpRsRows consecutive rows per pass; lane per class,
+// so each row's C floats leave as consecutive stores.
+struct MlpProbaF64Params {
+  const float* x;
+  long long ld;
+  long long n_rows;
+  const double* pack;
+  int F, H, C;
+  float* proba;
+};
+
+__global__ void __launch_bounds__(256) mlp_proba_f64_kernel(const MlpProbaF64Params p) {
+  extern __shared__ __align__(16) double rs_smem[];
+  constexpr int R = kMlpRsRows;
+  MlpRsView view = mlp_rs_stage(rs_smem, p.pack, p.F, p.H, p.C);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double* xs = rs_smem + mlp_rs_weight_doubles(p.F, p.H, p.C) + warp * (mlp_rs_strip_doubles(p.F, p.H, R) + p.C * R);
+  double* hv = xs + p.F * R;
+  double* zs = hv + p.H * R;  // the pass's logits, [c][R]
+  __syncthreads();
+  mlp_rs_finish_stage(view);
+
+  const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const long long warps_total = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  for (long long i = warp_global * R; i < p.n_rows; i += warps_total * R) {
+    const float* xr[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) xr[r] = p.x + (i + r < p.n_rows ? i + r : i) * p.ld;  // unused slots repeat row i
+    MlpRowResult res[R];
+    mlp_rs_rows<R, true>(view, xr, xs, hv, lane, res, zs);
+    for (int r = 0; r < R && i + r < p.n_rows; ++r) {
+      double m = -INFINITY;
+      for (int c = lane; c < p.C; c += 32) m = fmax(m, zs[c * R + r]);
+      m = warp_max(m, 1);
+      double s = 0.0;
+      for (int c = lane; c < p.C; c += 32) s += exp(zs[c * R + r] - m);
+      s = warp_sum(s);
+      float* out = p.proba + (i + r) * p.C;
+      for (int c = lane; c < p.C; c += 32) out[c] = static_cast<float>(exp(zs[c * R + r] - m) / s);
+    }
+    __syncwarp();  // the strip is rewritten by the next pass
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-static size_t mlp_fixed_smem(const MlpDeviceModel& m) {
+static size_t mlp_fixed_smem(const MlpDeviceModel& m, bool proba = false) {
   return 1024 + (static_cast<size_t>(m.f_pad) * (m.n_hidden + 4) + (m.n_hidden + 4) + static_cast<size_t>(m.n_hidden) * m.cp + m.cp) * 4 +
-         2 * 64 * 8;
+         2 * 64 * 8 + (proba ? static_cast<size_t>(kMlpConsumerWarps) * 32 * m.n_classes * 4 : 0);  // + a staging strip per warp
 }
 
-bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why) {
+bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why, bool proba) {
   const bool shape_ok = (m.n_hidden == 32 || m.n_hidden == 16) && (m.n_classes == 10 || m.n_classes == 2 || m.n_classes == 3);
   if (!shape_ok) {
     if (why) *why = "tile kernel instantiated for hidden in {16, 32} and classes in {2, 3, 10}";
     return false;
   }
-  if (mlp_fixed_smem(m) + kMlpPairs * static_cast<size_t>(kMlpStageBytes) > static_cast<size_t>(kMaxSmemBytes)) {
+  if (mlp_fixed_smem(m, proba) + kMlpPairs * static_cast<size_t>(kMlpStageBytes) > static_cast<size_t>(kMaxSmemBytes)) {
     if (why) *why = "W1^T does not fit in shared memory next to a 4-stage ring";
     return false;
   }
   return true;
 }
 
-template <int H, int C, bool EXACT>
+template <int H, int C, bool EXACT, bool PROBA = false>
 static cudaError_t mlp_launch_one(const CUtensorMap& xmap, const MlpKernelParams& p, int grid, size_t smem,
                                   cudaStream_t stream) {
-  auto kern = mlp_argmax_tma_kernel<H, C, EXACT>;
+  auto kern = mlp_argmax_tma_kernel<H, C, EXACT, PROBA>;
   static size_t configured = 0;
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -386,20 +448,22 @@ static cudaError_t mlp_launch_one(const CUtensorMap& xmap, const MlpKernelParams
   return cudaGetLastError();
 }
 
-template <bool EXACT>
+template <bool EXACT, bool PROBA = false>
 static cudaError_t mlp_dispatch(int H, int C, const CUtensorMap& xmap, const MlpKernelParams& p, int grid, size_t smem,
                                 cudaStream_t stream) {
 #define UML_MLP_CASE(HH, CC) \
-  if (H == HH && C == CC) return mlp_launch_one<HH, CC, EXACT>(xmap, p, grid, smem, stream);
+  if (H == HH && C == CC) return mlp_launch_one<HH, CC, EXACT, PROBA>(xmap, p, grid, smem, stream);
   UML_MLP_CASE(32, 10) UML_MLP_CASE(32, 2) UML_MLP_CASE(32, 3) UML_MLP_CASE(16, 10) UML_MLP_CASE(16, 2) UML_MLP_CASE(16, 3)
 #undef UML_MLP_CASE
   return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, const float* x, int64_t n_rows,
-                           int32_t* labels, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream) {
+                           int32_t* labels, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream,
+                           float* proba) {
   (void)x;
   if (n_rows <= 0) return cudaSuccess;
+  const bool want_proba = proba != nullptr;
   MlpKernelParams p{};
   p.w1t = m.w1t;
   p.b1 = m.b1;
@@ -410,7 +474,7 @@ cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, con
   p.num_tiles = (n_rows + kMlpTileRows - 1) / kMlpTileRows;
   p.f_pad = m.f_pad;
   p.kc = m.f_pad / kChunkF;
-  const size_t fixed = mlp_fixed_smem(m);
+  const size_t fixed = mlp_fixed_smem(m, want_proba);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kMlpStageBytes);
   stages = std::min(stages, 64);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(kMlpPairs, std::min(stages, atoi(env)));
@@ -422,9 +486,11 @@ cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, con
   p.flag_count = flags.count;
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
+  p.proba = proba;
   const size_t smem = fixed + static_cast<size_t>(stages) * kMlpStageBytes;
   const long long slots = (p.num_tiles + kMlpPairs - 1) / kMlpPairs;
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
+  if (want_proba) return mlp_dispatch<false, true>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream);
   return exact ? mlp_dispatch<true>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream)
                : mlp_dispatch<false>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream);
 }
@@ -466,6 +532,35 @@ cudaError_t launch_mlp_rescore_f64(const MlpDeviceModel& m, const float* x, int6
   if (all_rows) blocks = std::min<long long>(blocks, (n_rows + 8 * kMlpRsRows - 1) / (8 * kMlpRsRows));
   cudaError_t lerr = launch_dependent(mlp_rescore_f64_kernel, static_cast<int>(std::max<long long>(1, blocks)), 256, smem, stream, p);
   if (lerr != cudaSuccess) return lerr;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, float* proba,
+                                 int sm_count, cudaStream_t stream) {
+  if (n_rows <= 0) return cudaSuccess;
+  MlpProbaF64Params p{};
+  p.x = x;
+  p.ld = ld;
+  p.n_rows = n_rows;
+  p.pack = m.rs_pack;
+  p.F = m.n_in;
+  p.H = m.n_hidden;
+  p.C = m.n_classes;
+  p.proba = proba;
+  // the re-score kernel's shared memory plus C x kMlpRsRows logits per warp
+  const size_t strip = mlp_rs_strip_doubles(m.n_in, m.n_hidden, kMlpRsRows) + static_cast<size_t>(m.n_classes) * kMlpRsRows;
+  const size_t smem = (mlp_rs_weight_doubles(m.n_in, m.n_hidden, m.n_classes) + 8 * strip) * sizeof(double);
+  if (smem > static_cast<size_t>(kMaxSmemBytes)) return cudaErrorInvalidValue;
+  static size_t configured = 0;
+  if (smem > configured) {
+    cudaError_t err = cudaFuncSetAttribute(mlp_proba_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (err != cudaSuccess) return err;
+    configured = smem;
+  }
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mlp_proba_f64_kernel, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  const long long blocks = std::min<long long>(static_cast<long long>(sm_count) * per_sm, (n_rows + 8 * kMlpRsRows - 1) / (8 * kMlpRsRows));
+  mlp_proba_f64_kernel<<<static_cast<int>(std::max<long long>(1, blocks)), 256, smem, stream>>>(p);
   return cudaGetLastError();
 }
 

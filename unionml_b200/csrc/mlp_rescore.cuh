@@ -118,10 +118,11 @@ struct MlpRowResult {
 };
 
 // One warp, R rows per pass.  xr[r] = row r's fp32 features in global memory (callers pass a valid row for unused
-// slots and ignore that result); xs / hv = the warp's strip, F x R and H x R doubles, 16-byte aligned.
-template <int R>
+// slots and ignore that result); xs / hv = the warp's strip, F x R and H x R doubles, 16-byte aligned.  KEEP_Z: the
+// logits are also left in zs[c R + r] (C x R doubles, visible to the whole warp on return).
+template <int R, bool KEEP_Z = false>
 __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* const (&xr)[R], double* xs, double* hv, int lane,
-                                            MlpRowResult (&out)[R]) {
+                                            MlpRowResult (&out)[R], double* zs = nullptr) {
   static_assert(R == 1 || R == 2 || R == 4, "rows per pass");
   const double u = 1.1102230246251565e-16;  // 2^-53
   const int F = v.F, H = v.H, C = v.C, HP = v.H + 1;
@@ -215,6 +216,8 @@ __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* con
     const double b = c < C ? v.b2s[c] : 0.0;
 #pragma unroll
     for (int r = 0; r < R; ++r) {
+      if constexpr (KEEP_Z)
+        if (c < C) zs[c * R + r] = s[r] + b;
       Top2 t;
       t.best = c < C ? s[r] + b : -INFINITY;
       t.second = -INFINITY;

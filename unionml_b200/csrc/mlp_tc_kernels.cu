@@ -28,7 +28,8 @@
 //             are in flight.  Per box 2 x 4 wgmma m64nNk8 (N = 2H; rows 0-63 and 64-127 of the box as A, K-major SW128,
 //             the resident W1 tile as B), then from the accumulator registers: + b1, ReLU, layer 2 over the lane's
 //             hidden units, a quad reduce-scatter that leaves each lane one row's logits, argmax (first maximum
-//             wins), margin guard, label store (+ peer stores)
+//             wins), margin guard, label store (+ peer stores); PROBA kernels instead take the softmax of the logits
+//             and store each warp's two 16-row runs of probabilities through shared memory (mlp_proba.cuh)
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -37,6 +38,7 @@
 #include "uml_common.cuh"
 #include "wgmma.cuh"
 #include "mlp_rescore.cuh"
+#include "mlp_proba.cuh"
 
 #ifndef UML_MLP_QUEUE_DEFAULT
 // 0: flagged rows go to the separate fp64 re-score kernel.  The queue variant re-scores them inside the scoring launch,
@@ -87,6 +89,7 @@ struct MlpTcParams {
   int n_in;
   const double* rs_pack;  // shared-memory image of the fp64 operands (mlp_rs_build_pack)
   unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] re-scored rows
+  float* proba;  // PROBA kernels: [n_rows][C] row-major
 };
 
 template <int H, int C>
@@ -102,7 +105,7 @@ __device__ __forceinline__ void tc_store_final_label(const MlpTcParams<H, C>& p,
 // (l / 4) holds rows 16 wq + l / 4 (+ 8) of both 64-row halves, and lane l % 4 keeps the (half, +8) pair it names
 __device__ __forceinline__ int tc_row_of_lane(int wq, int l) { return 64 * ((l & 3) >> 1) + 16 * wq + (l >> 2) + 8 * (l & 1); }
 
-template <int H, int C, bool EXACT, bool QUEUE>
+template <int H, int C, bool EXACT, bool QUEUE, bool PROBA>
 __global__ void __launch_bounds__(kTcThreadsQueue, 1)
 mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ MlpTcParams<H, C> p) {
   constexpr int N = 2 * H;     // accumulator columns per row: [main | small]
@@ -300,6 +303,23 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
         const float send = hi1 ? s[0] : s[1];
         z[c] = (keep + __shfl_xor_sync(0xffffffffu, send, 1)) + p.b2[c];
       }
+      if constexpr (PROBA) {
+        // this warp's staging strip (32 rows x C floats behind the A1 hand-off barriers): row r of run h at
+        // (16 h + r) C, so each run is 64 C contiguous bytes, as it is in the output
+        float* strip = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(a1_bar + kTcSlots) + 15u) & ~static_cast<uintptr_t>(15)) +
+                       (warp - 4) * 32 * C;
+        float pr[C];
+        mlp_softmax_f32<C>(z, pr);
+        float* mine = strip + (16 * ((lane & 3) >> 1) + (lane >> 2) + 8 * (lane & 1)) * C;
+#pragma unroll
+        for (int c = 0; c < C; ++c) mine[c] = pr[c];
+        __syncwarp();
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          mlp_proba_store_run<C, 16>(strip + 16 * h * C, p.proba, tile * kTileRows + 64 * h + 16 * wq, p.n_rows, lane);
+        __syncwarp();  // the strip is rewritten by this warp's next tile
+        continue;
+      }
       const long long row = tile * kTileRows + row_in_tile;
       float best = z[0];
       float second = -INFINITY;
@@ -485,7 +505,7 @@ std::vector<float> mlp_tc_build_w1_tiles(const float* w1 /*[H][F]*/, int H, int 
   return tiles;
 }
 
-static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool queue) {
+static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool queue, bool proba = false) {
   const size_t kc = m.f_pad / kChunkF;
   size_t bytes = 1024 + kc * (2 * m.n_hidden) * 128 + static_cast<size_t>(kTcSlots) * kTileRows * 4 +
                  (2 * 64 + kTcSlots) * 8 + 16;
@@ -493,6 +513,7 @@ static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool queue) {
     bytes += (kTcQueueCap + 4) * 4 + 16 +
              (mlp_rs_weight_doubles(m.n_in, m.n_hidden, m.n_classes) +
               (kTcEpilogueWarps + kTcRescoreWarps) * mlp_rs_strip_doubles(m.n_in, m.n_hidden)) * 8;
+  if (proba) bytes += 16 + static_cast<size_t>(kTcEpilogueWarps) * 32 * m.n_classes * 4;  // one staging strip per epilogue warp
   return bytes;
 }
 
@@ -521,7 +542,7 @@ bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why) {
   return mlp_tc_fixed_smem(m, true) + 6 * static_cast<size_t>(kStageBytes) <= static_cast<size_t>(kMaxSmemBytes);
 }
 
-template <int H, int C, bool EXACT, bool QUEUE>
+template <int H, int C, bool EXACT, bool QUEUE, bool PROBA = false>
 static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l,
                                      const FlagList& flags, int sm_count, cudaStream_t stream) {
   using Params = MlpTcParams<H, C>;
@@ -576,7 +597,8 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   p.n_in = m.n_in;
   p.rs_pack = m.rs_pack;
   p.counters = flags.counters;
-  const size_t fixed = mlp_tc_fixed_smem(m, QUEUE);
+  p.proba = l.proba;
+  const size_t fixed = mlp_tc_fixed_smem(m, QUEUE, PROBA);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kStageBytes);
   stages = std::min(stages, 64);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(4, std::min(stages, atoi(env)));
@@ -588,7 +610,7 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
-  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, QUEUE>;
+  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, QUEUE, PROBA>;
   static size_t configured = 0;
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -611,6 +633,17 @@ cudaError_t launch_mlp_tc(const CUtensorMap& xmap, const MlpDeviceModel& m, cons
     return queue ? mlp_tc_launch_one<HH, CC, true, true>(xmap, m, l, flags, sm_count, stream)                    \
                  : mlp_tc_launch_one<HH, CC, true, false>(xmap, m, l, flags, sm_count, stream);                  \
   }
+  UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
+#undef UML_TC_CASE
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, int sm_count,
+                                cudaStream_t stream) {
+  if (l.n_rows <= 0) return cudaSuccess;
+  const FlagList none{};
+#define UML_TC_CASE(HH, CC) \
+  if (m.n_hidden == HH && m.n_classes == CC) return mlp_tc_launch_one<HH, CC, false, false, true>(xmap, m, l, none, sm_count, stream);
   UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
 #undef UML_TC_CASE
   return cudaErrorInvalidValue;

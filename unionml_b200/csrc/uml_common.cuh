@@ -184,10 +184,13 @@ struct MlpTcLaunch {
   long long n_rows;
   const float* x;  // the batch rows (the in-kernel fp64 re-score of the tensor-core kernel reads flagged rows again)
   long long ld;
+  float* proba;    // launch_mlp_tc_proba: class probabilities [n_rows][n_classes] (device)
 };
-bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why);
+// proba: the tile kernel's probability form (n_rows x n_classes fp32 instead of labels; exact and flags unused)
+bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why, bool proba = false);
 cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, const float* x, int64_t n_rows,
-                           int32_t* labels, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream);
+                           int32_t* labels, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream,
+                           float* proba = nullptr);
 cudaError_t launch_mlp_rescore_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows,
                                    const MlpTcLaunch& out, const FlagList& flags, bool all_rows, int sm_count,
                                    cudaStream_t stream);
@@ -195,6 +198,12 @@ bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why);
 std::vector<float> mlp_tc_build_w1_tiles(const float* w1, int H, int F, int f_pad);
 cudaError_t launch_mlp_tc(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
                           const FlagList& flags, int sm_count, cudaStream_t stream, bool* rescore_kernel_needed);
+// class probabilities softmax(logits) of every row into l.proba: tensor-core kernel (rows that are tf32 values), and
+// the fp64 scorer with a float64 softmax for shapes no tile kernel takes
+cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, int sm_count,
+                                cudaStream_t stream);
+cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, float* proba,
+                                 int sm_count, cudaStream_t stream);
 // int32 labels (device) -> every target vector of a fused exchange (int32 or uint8 wire), for kernels without peer stores
 cudaError_t launch_labels_scatter(const int32_t* labels, int64_t n, void* const* peers, int n_peers, int wire_u8,
                                   int64_t row_offset, int sm_count, cudaStream_t stream);

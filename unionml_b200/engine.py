@@ -276,6 +276,25 @@ class Engine:
             self._check(st)  # under the lock: uml_last_error is per engine, another thread's call may overwrite it
         return out, stats.as_dict() if stats else None
 
+    def predict_mlp_proba(self, model: MlpModel, batch: Batch, out_device_ptr: Optional[int] = None,
+                          want_stats: bool = False) -> Tuple[Optional[np.ndarray], Optional[dict]]:
+        """``softmax(W2 relu(W1 x + b1) + b2)`` per row (fp32), ``(n_rows, n_classes)``: what the torch quickstart's
+        ``PytorchModel.forward`` returns.  With ``out_device_ptr`` the rows are written there and ``None`` is returned."""
+        stats = N.Stats() if want_stats else None
+        with self._lock:
+            if out_device_ptr is not None:
+                st = N.lib().uml_mlp_predict_proba(
+                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, C.byref(stats) if stats else None
+                )
+                self._check(st)
+                return None, stats.as_dict() if stats else None
+            out = np.empty((batch.n_rows, model.n_classes), dtype=np.float32)
+            st = N.lib().uml_mlp_predict_proba(
+                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, C.byref(stats) if stats else None
+            )
+            self._check(st)
+        return out, stats.as_dict() if stats else None
+
     def predict_mlp_peers(self, model: MlpModel, batch: Batch, peer_ptrs, row_offset: int, exact: bool = True,
                           want_stats: bool = False, label_bytes: int = 4) -> Optional[dict]:
         """Fused compute + all-gather for the MLP predictor (same contract as :meth:`predict_peers`)."""

@@ -327,3 +327,20 @@ def mlp_argmax(module: Any, features: Any) -> List[float]:
     out, stats = engine.predict_host_list(dm, arr, dm.class_table, exact=_exact_default())
     _note_ambiguous(stats)
     return out
+
+
+def mlp_predict_proba(module: Any, features: Any) -> np.ndarray:
+    """``module(process_features(features))`` of the torch quickstart on the GPU: class probabilities, an
+    ``(n_rows, n_out)`` float32 ndarray.  The result is ``softmax`` of the module's ``Linear -> ReLU -> Linear`` stack,
+    whatever its ``forward`` does.  Features are cast to float32 as ``process_features`` does; NaN/Inf or a wrong
+    feature count raise ``ValueError``.  The frame is staged on the device in one piece (no chunk pipeline)."""
+    engine = get_engine()
+    dm = device_mlp(module, engine)
+    arr = features.to_numpy() if hasattr(features, "to_numpy") else np.asarray(features)
+    _check_min_samples(arr)
+    batch = engine.stage(arr, keep_f64=False)
+    try:
+        out, _ = engine.predict_mlp_proba(dm, batch)
+        return out
+    finally:
+        batch.free()
