@@ -397,11 +397,10 @@ def mlp_report():
     return fails
 
 
-@pytest.mark.parametrize("mode", ["queue", "kernel"])
-def test_mlp_routes(mode):
-    """mlp_rescore_f64_kernel behind the CUDA-core kernel (path 3), the tensor-core kernel's re-score (path 5) as the
-    queue and as a second kernel, and the generic shapes (path 2) at ragged row counts."""
-    run_report("mlp_report", {"UML_B200_MLP_RESCORE_MODE": mode})
+def test_mlp_routes():
+    """mlp_rescore_f64_kernel behind the CUDA-core kernel (path 3) and behind the tensor-core kernel (path 5), and the
+    generic shapes (path 2) at ragged row counts."""
+    run_report("mlp_report", {})
 
 
 # ---------------------------------------------------------------------------------------------------------------

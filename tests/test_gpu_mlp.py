@@ -138,36 +138,20 @@ def test_tensor_core_kernel_is_safe_on_rows_that_are_not_tf32(engine, mlp_golden
     np.testing.assert_array_equal(got, omlp.predict_indices_f64(Xf, *w).astype(np.int32))
 
 
-def test_tensor_core_queue_and_kernel_rescore_agree(mlp_golden):
-    """UML_B200_MLP_RESCORE_MODE=queue (four fp64 warps inside the scoring launch; loses to the separate kernel and is off by
-    default) vs =kernel (flag list + mlp_rescore_f64_kernel): same labels and counters, also when every row is flagged
-    and the queue backs up."""
-    import os
-    import subprocess
-    import sys
-    from pathlib import Path
-
-    root = Path(__file__).resolve().parent.parent
-    code = (
-        "import sys, numpy as np; sys.path.insert(0, %r)\n"
-        "from unionml_b200.engine import Engine\n"
-        "g = np.load(%r); e = Engine(0); m = e.load_mlp(g['w1'], g['b1'], g['w2'], g['b2'])\n"
-        "X = np.random.default_rng(41).integers(0, 17, size=(1_200_000, 64), dtype=np.uint8).astype(np.float32)\n"
-        "idx, st = e.predict_mlp(m, e.stage(X), exact=True)\n"
-        "print(st['path'], st['kernel_launches'], st['n_flagged'], int(idx.astype(np.int64).sum()), int((idx * np.arange(idx.size) %% 1000003).sum()))\n"
-        "Xf = np.random.default_rng(42).standard_normal((150_000, 64)).astype(np.float32)   # forced onto the tensor cores: all rows flagged\n"
-        "idx2, st2 = e.predict_mlp(m, e.stage(Xf), exact=True)\n"
-        "print(st2['path'], st2['n_flagged'], int(idx2.astype(np.int64).sum()), int((idx2 * np.arange(idx2.size) %% 1000003).sum()))\n"
-    ) % (str(root), str(root / "tests" / "golden" / "mlp_64_32_10.npz"))
-    outs = []
-    for mode in ("queue", "kernel"):
-        env = dict(os.environ, UML_B200_MLP_RESCORE_MODE=mode, UML_B200_MLP_TC="1")
-        r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=300)
-        assert r.returncode == 0, r.stderr[-2000:]
-        outs.append([ln.split() for ln in r.stdout.strip().splitlines()])
-    assert outs[0][0][:2] == ["5", "1"] and outs[1][0][:2] == ["5", "2"]
-    assert outs[0][0][2:] == outs[1][0][2:] and int(outs[0][0][2]) > 0
-    assert outs[0][1] == outs[1][1] and outs[0][1][1] == "150000"
+def test_tensor_core_flagged_rows_rescored_in_float64(engine, mlp_golden, monkeypatch):
+    """The flag list + mlp_rescore_f64_kernel behind the tensor-core kernel: a second launch that gives every flagged
+    row the float64 network's label, also when every row of the batch is flagged."""
+    w = _weights(mlp_golden)
+    m = engine.load_mlp(*w)
+    monkeypatch.setenv("UML_B200_MLP_TC", "1")
+    X = np.random.default_rng(41).integers(0, 17, size=(1_200_000, 64), dtype=np.uint8).astype(np.float32)
+    got, st = engine.predict_mlp(m, engine.stage(X), exact=True)
+    assert st["path"] == 5 and st["kernel_launches"] == 2 and st["n_flagged"] > 0
+    np.testing.assert_array_equal(got, omlp.predict_indices_f64(X, *w).astype(np.int32))
+    Xf = np.random.default_rng(42).standard_normal((150_000, 64)).astype(np.float32)  # forced onto the tensor cores
+    got, st = engine.predict_mlp(m, engine.stage(Xf), exact=True)
+    assert st["path"] == 5 and st["n_flagged"] == 150_000
+    np.testing.assert_array_equal(got, omlp.predict_indices_f64(Xf, *w).astype(np.int32))
 
 
 @pytest.mark.parametrize("shape", [(64, 32, 10), (64, 16, 10), (50, 32, 3), (32, 16, 2), (128, 32, 10), (100, 16, 3)])

@@ -55,8 +55,6 @@ for rows in (10_000_000, 1_250_000):
     out[f"linear_{rows}"] = {"default": run("linear", rows, {}), "rescore_kernel": run("linear", rows, {"UML_B200_RESCORE_MODE": "kernel"}),
                              "no_pdl": run("linear", rows, {"UML_B200_NO_PDL": "1"}), "default_again": run("linear", rows, {})}
 out["linear_784_2000000"] = {"default": run("linear", 2_000_000, {}, 784), "rescore_kernel": run("linear", 2_000_000, {"UML_B200_RESCORE_MODE": "kernel"}, 784)}
-out["mlp_10000000"] = {"tc": run("mlp", 10_000_000, {}), "tc_rescore_kernel": run("mlp", 10_000_000, {"UML_B200_MLP_RESCORE_MODE": "kernel"}),
-                       "ffma": run("mlp", 10_000_000, {"UML_B200_MLP_TC": "0"})}
-out["mlp_1250000"] = {"tc": run("mlp", 1_250_000, {}), "tc_rescore_kernel": run("mlp", 1_250_000, {"UML_B200_MLP_RESCORE_MODE": "kernel"}),
-                      "ffma": run("mlp", 1_250_000, {"UML_B200_MLP_TC": "0"})}
+out["mlp_10000000"] = {"tc": run("mlp", 10_000_000, {}), "ffma": run("mlp", 10_000_000, {"UML_B200_MLP_TC": "0"})}
+out["mlp_1250000"] = {"tc": run("mlp", 1_250_000, {}), "ffma": run("mlp", 1_250_000, {"UML_B200_MLP_TC": "0"})}
 print(json.dumps(out, indent=1))

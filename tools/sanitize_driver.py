@@ -21,7 +21,7 @@ eng.predict_host(m, X, exact=True, chunk_rows=4096)
 buf = eng.device_alloc(b.n_rows)
 eng.predict_peers(m, b, [buf.ptr], 0, exact=True, want_stats=True, label_bytes=1)
 eng.take_labels(buf.ptr, b.n_rows, np.arange(10.0), label_bytes=1)
-# round 2: tensor-core MLP kernel (+ peer stores, queue re-score variant), CUDA-core MLP kernel on float rows, re-score from
+# round 2: tensor-core MLP kernel (+ peer stores), CUDA-core MLP kernel on float rows, re-score from
 # the caller's float64 values, online small-batch kernel, predict_proba, MLP host pipeline, asynchronous host call
 import os as _os
 

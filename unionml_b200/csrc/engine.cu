@@ -1577,15 +1577,12 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       uml::MlpTcLaunch out{};
       out.n_rows = rows;
       out.labels = l.labels;
-      out.x = xc;
-      out.ld = ld;
       FlagList fl{e->d_flag_count, e->d_flag_rows, (int)std::min<int64_t>(e->flag_cap, INT32_MAX), e->d_counters};
       if (mlp_tc && has_map) {
-        bool need_rescore = false;
-        HOST_CUDA(uml::launch_mlp_tc(map, mlp->dm, out, exact, fl, e->info.sm_count, cs, &need_rescore));
+        HOST_CUDA(uml::launch_mlp_tc(map, mlp->dm, out, exact, fl, e->info.sm_count, cs));
         launches += 1;
         path = 5;
-        if (need_rescore) {
+        if (exact) {
           HOST_CUDA(uml::launch_mlp_rescore_f64(mlp->dm, xc, ld, rows, out, fl, false, e->info.sm_count, cs));
           launches += 1;
         }
@@ -1946,8 +1943,6 @@ static int mlp_predict_common(uml_engine* e, const uml_mlp* m, const uml_batch* 
   uml::MlpTcLaunch out{};
   out.n_rows = b->n_rows;
   out.row_offset = row_offset;
-  out.x = b->x;
-  out.ld = b->ld;
   const bool wire_u8 = n_peers > 0 && label_bytes == 1;
   out.wire_u8 = wire_u8 ? 1 : 0;
   int32_t* d_labels = labels_out;
@@ -1977,12 +1972,11 @@ static int mlp_predict_common(uml_engine* e, const uml_mlp* m, const uml_batch* 
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
   if (use_tc) {
     NvtxRange r_score("uml:mlp_score_tc");
-    bool need_rescore = false;
-    UML_CUDA(e, uml::launch_mlp_tc(b->map, m->dm, out, exact, fl, e->info.sm_count, e->stream, &need_rescore));
+    UML_CUDA(e, uml::launch_mlp_tc(b->map, m->dm, out, exact, fl, e->info.sm_count, e->stream));
     launches += 1;
     path = 5;
     if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
-    if (need_rescore) {  // UML_B200_MLP_RESCORE_MODE=kernel; in queue mode four warps of the scoring kernel do it
+    if (exact) {
       NvtxRange r_rescore("uml:mlp_rescore_f64");
       UML_CUDA(e, uml::launch_mlp_rescore_f64(m->dm, b->x, b->ld, b->n_rows, out, fl, false, e->info.sm_count, e->stream));
       launches += 1;

@@ -1,5 +1,5 @@
 // float64 re-score of rows of the 2-layer MLP by one warp, with every operand in shared memory.  Shared by the
-// stand-alone re-score kernel (mlp_kernels.cu) and the re-score warps inside the tensor-core kernel (mlp_tc_kernels.cu).
+// re-score kernel and the float64 probability kernel (mlp_kernels.cu).
 //
 // The kernel is bound by shared-memory bandwidth, not by fp64 math: W1 is F x H doubles and a warp that scores ONE row
 // reads all of it (2 wavefronts per feature) for 1 fma per lane and feature.  mlp_rs_rows<R> therefore scores R rows
@@ -34,7 +34,7 @@ __host__ __device__ inline size_t mlp_rs_weight_doubles(int F, int H, int C) {
   return (n + 1) & ~static_cast<size_t>(1);  // even: 16-byte copies, and the strips behind it stay 16-byte aligned
 }
 // a warp's strip: features and hidden activations of the R rows of one pass
-__host__ __device__ inline size_t mlp_rs_strip_doubles(int F, int H, int R = 1) { return (static_cast<size_t>(F) + H) * R; }
+__host__ __device__ inline size_t mlp_rs_strip_doubles(int F, int H, int R) { return (static_cast<size_t>(F) + H) * R; }
 
 // host: the shared-memory image from the caller's (fp32) weights; w1 is [H][F], w2 is [C][H] as torch holds them
 inline std::vector<double> mlp_rs_build_pack(const float* w1, const float* b1, const float* w2, const float* b2, int F,
@@ -123,7 +123,7 @@ struct MlpRowResult {
 template <int R, bool KEEP_Z = false>
 __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* const (&xr)[R], double* xs, double* hv, int lane,
                                             MlpRowResult (&out)[R], double* zs = nullptr) {
-  static_assert(R == 1 || R == 2 || R == 4, "rows per pass");
+  static_assert(R == 2 || R == 4, "rows per pass");
   const double u = 1.1102230246251565e-16;  // 2^-53
   const int F = v.F, H = v.H, C = v.C, HP = v.H + 1;
   bool bad[R];
@@ -166,15 +166,11 @@ __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* con
 #pragma unroll 4
     for (int f = 0; f < F; ++f) {
       const double w = wcol[f * H];
-      if constexpr (R == 1) {
-        s[0] = fma(xs[f], w, s[0]);
-      } else {
 #pragma unroll
-        for (int r = 0; r < R; r += 2) {
-          const double2 x2 = *reinterpret_cast<const double2*>(xs + f * R + r);  // broadcast 16-byte load: two rows
-          s[r] = fma(x2.x, w, s[r]);
-          s[r + 1] = fma(x2.y, w, s[r + 1]);
-        }
+      for (int r = 0; r < R; r += 2) {
+        const double2 x2 = *reinterpret_cast<const double2*>(xs + f * R + r);  // broadcast 16-byte load: two rows
+        s[r] = fma(x2.x, w, s[r]);
+        s[r + 1] = fma(x2.y, w, s[r + 1]);
       }
     }
     const double b = v.b1s[hn], wm = v.w2m[hn];
@@ -201,15 +197,11 @@ __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* con
 #pragma unroll 4
       for (int nn = 0; nn < H; ++nn) {
         const double w = w2c[nn];
-        if constexpr (R == 1) {
-          s[0] = fma(hv[nn], w, s[0]);
-        } else {
 #pragma unroll
-          for (int r = 0; r < R; r += 2) {
-            const double2 h2 = *reinterpret_cast<const double2*>(hv + nn * R + r);
-            s[r] = fma(h2.x, w, s[r]);
-            s[r + 1] = fma(h2.y, w, s[r + 1]);
-          }
+        for (int r = 0; r < R; r += 2) {
+          const double2 h2 = *reinterpret_cast<const double2*>(hv + nn * R + r);
+          s[r] = fma(h2.x, w, s[r]);
+          s[r + 1] = fma(h2.y, w, s[r + 1]);
         }
       }
     }
@@ -243,15 +235,6 @@ __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* con
     const double err = herr[r] * v.w2sum + (static_cast<double>(H) + 16.0) * u * amax[r];
     out[r].ambiguous = !((top[r].best - top[r].second) > 2.0 * err);
   }
-}
-
-// one row (the re-score warps inside the tensor-core kernel take rows one at a time from their queue)
-__device__ __forceinline__ MlpRowResult mlp_rs_row(const MlpRsView& v, const float* __restrict__ xr, double* xs, double* hv,
-                                                  int lane) {
-  const float* const rows[1] = {xr};
-  MlpRowResult out[1];
-  mlp_rs_rows<1>(v, rows, xs, hv, lane, out);
-  return out[0];
 }
 
 }  // namespace uml

@@ -37,27 +37,18 @@
 
 #include "uml_common.cuh"
 #include "wgmma.cuh"
-#include "mlp_rescore.cuh"
 #include "mlp_proba.cuh"
-
-#ifndef UML_MLP_QUEUE_DEFAULT
-// 0: flagged rows go to the separate fp64 re-score kernel.  The queue variant re-scores them inside the scoring launch,
-// where the fp64 work competes for issue slots with the epilogue warps that bound this kernel.
-#define UML_MLP_QUEUE_DEFAULT 0
-#endif
 
 namespace uml {
 
 constexpr int kTcThreads = 416;
 constexpr int kTcProducerWarp = 12;
-// QUEUE kernels: rows flagged by the epilogue warps are re-scored in fp64 by four more warps of the same launch while
-// the tensor-core pipeline keeps streaming (fp64 units and these issue slots are otherwise idle)
-constexpr int kTcRescoreWarps = 4;
-constexpr int kTcFirstRescoreWarp = 13;
-constexpr int kTcThreadsQueue = kTcThreads + 32 * kTcRescoreWarps;
+// __launch_bounds__ thread count: the register budget of 544 threads, not the 416 the kernel launches with.  Every
+// measurement of this kernel was taken with it; with a bound of 416, ptxas (CUDA 12.9) gives H=32 C=10 EXACT 128
+// registers instead of 95 and H=16 C=10 EXACT 92 instead of 80, and changes their code.  Raising the budget is a
+// performance change to be measured on its own.
+constexpr int kTcRegBudgetThreads = 544;
 constexpr int kTcEpilogueWarps = 8;
-constexpr int kTcQueueCap = 1024;       // power of two
-constexpr int kTcQueueHeadroom = 512;   // a warp publishes only while this many slots are free (8 warps x 32 rows at once)
 constexpr int kTcSlots = 24;       // A1 hand-off slots (scan -> epilogue); > the scan warps' maximum lead over the epilogue
 constexpr int kTcMaxFpad = 128;    // features (padded to 32) the resident W1 tile is sized for
 
@@ -83,30 +74,15 @@ struct MlpTcParams {
   int* flag_count;
   int32_t* flag_rows;
   int flag_cap;
-  // QUEUE kernels: what the in-kernel fp64 re-score needs
-  const float* x;
-  long long ld;
-  int n_in;
-  const double* rs_pack;  // shared-memory image of the fp64 operands (mlp_rs_build_pack)
-  unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] re-scored rows
   float* proba;  // PROBA kernels: [n_rows][C] row-major
 };
-
-template <int H, int C>
-__device__ __forceinline__ void tc_store_final_label(const MlpTcParams<H, C>& p, long long row, int idx) {
-  if (p.labels) p.labels[row] = idx;
-  for (int i = 0; i < p.n_peers; ++i) {
-    if (p.wire_u8) static_cast<uint8_t*>(p.peers[i])[p.row_offset + row] = static_cast<uint8_t>(idx);
-    else static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idx;
-  }
-}
 
 // consumer lane l of warp wq (in its warpgroup) ends the epilogue owning one row of the 128-row tile: the quad
 // (l / 4) holds rows 16 wq + l / 4 (+ 8) of both 64-row halves, and lane l % 4 keeps the (half, +8) pair it names
 __device__ __forceinline__ int tc_row_of_lane(int wq, int l) { return 64 * ((l & 3) >> 1) + 16 * wq + (l >> 2) + 8 * (l & 1); }
 
-template <int H, int C, bool EXACT, bool QUEUE, bool PROBA>
-__global__ void __launch_bounds__(kTcThreadsQueue, 1)
+template <int H, int C, bool EXACT, bool PROBA>
+__global__ void __launch_bounds__(kTcRegBudgetThreads, 1)
 mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ MlpTcParams<H, C> p) {
   constexpr int N = 2 * H;     // accumulator columns per row: [main | small]
   constexpr int NACC = N / 2;  // fp32 accumulator registers per thread and 64-row half
@@ -122,11 +98,6 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(a1_s + kTcSlots * kTileRows);
   uint64_t* empty_bar = full_bar + S;
   uint64_t* a1_bar = empty_bar + S;
-  // QUEUE kernels: flagged-row queue (slot = row + 1, 0 = empty; ctl: 0 tail reserved, 1 head claimed, 2 epilogue
-  // warps done, 3 slots consumed), then the fp64 weights and one strip per epilogue / re-score warp
-  int* q_slots = reinterpret_cast<int*>(a1_bar + kTcSlots);
-  int* q_ctl = q_slots + kTcQueueCap;
-  double* rs_area = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(q_ctl + 4) + 15u) & ~static_cast<uintptr_t>(15));  // 16-byte copies
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -138,14 +109,6 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
     const int n4 = KC * N * 32 / 4;
     for (int i = threadIdx.x; i < n4; i += blockDim.x) dst[i] = __ldg(src + i);
   }
-  MlpRsView rs_view{};
-  if constexpr (EXACT && QUEUE) {
-    for (int i = threadIdx.x; i < kTcQueueCap + 4; i += blockDim.x) q_slots[i] = 0;
-    rs_view = mlp_rs_stage(rs_area, p.rs_pack, p.n_in, H, C);
-    __syncthreads();
-    mlp_rs_finish_stage(rs_view);
-  }
-  double* rs_strips = rs_area + mlp_rs_weight_doubles(p.n_in, H, C);
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
@@ -372,101 +335,15 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
         const bool flagged = in_range && !certain;
         const unsigned mask = __ballot_sync(0xffffffffu, flagged);
         if (mask != 0u) {
-          if constexpr (QUEUE) {
-            // hand the flagged rows to the re-score warps of this launch; the labels stored above are provisional
-            __threadfence();
-            const int total = __popc(mask);
-            int base = -1;
-            if (lane == 0) {
-              const int tail = atomicAdd(&q_ctl[0], 0);
-              const int consumed = atomicAdd(&q_ctl[3], 0);
-              if (tail - consumed <= kTcQueueCap - kTcQueueHeadroom) base = atomicAdd(&q_ctl[0], total);
-            }
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (base >= 0) {
-              if (flagged) {
-                const int slot = (base + __popc(mask & ((1u << lane) - 1u))) & (kTcQueueCap - 1);
-                while (atomicAdd(&q_slots[slot], 0) != 0) {  // only if the slot's previous ticket is claimed but not read yet
-                }
-                atomicExch(&q_slots[slot], static_cast<int>(row) + 1);
-              }
-            } else {
-              // queue backed up (most rows near-ties): this warp re-scores its own rows in fp64
-              double* xs = rs_strips + (warp - 4) * mlp_rs_strip_doubles(p.n_in, H);
-              unsigned m2 = mask;
-              while (m2 != 0u) {
-                const int l = __ffs(static_cast<int>(m2)) - 1;
-                m2 &= m2 - 1u;
-                const long long frow = tile * kTileRows + tc_row_of_lane(wq, l);
-                const MlpRowResult r = mlp_rs_row(rs_view, p.x + frow * p.ld, xs, xs + p.n_in, lane);
-                if (lane == 0) {
-                  tc_store_final_label(p, frow, r.idx);
-                  if (r.bad) atomicAdd(&p.counters[1], 1ull);
-                  if (r.ambiguous) atomicAdd(&p.counters[0], 1ull);
-                }
-              }
-              if (lane == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(total));
-            }
-          } else {
-            int base = 0;
-            if (lane == 0) base = atomicAdd(p.flag_count, __popc(mask));
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (flagged) {
-              const int pos = base + __popc(mask & ((1u << lane) - 1u));
-              if (pos < p.flag_cap) p.flag_rows[pos] = static_cast<int32_t>(row);
-            }
+          int base = 0;
+          if (lane == 0) base = atomicAdd(p.flag_count, __popc(mask));
+          base = __shfl_sync(0xffffffffu, base, 0);
+          if (flagged) {
+            const int pos = base + __popc(mask & ((1u << lane) - 1u));
+            if (pos < p.flag_cap) p.flag_rows[pos] = static_cast<int32_t>(row);
           }
         }
       }
-    }
-    if constexpr (EXACT && QUEUE) {
-      __syncwarp();
-      if (lane == 0) {
-        __threadfence_block();
-        atomicAdd(&q_ctl[2], 1);  // this epilogue warp has published everything it will ever publish
-      }
-    }
-  } else {
-    // ===================== re-score warps 13..16 (QUEUE kernels): fp64 rows from the queue =====================
-    if constexpr (EXACT && QUEUE) {
-      double* xs = rs_strips + (kTcEpilogueWarps + (warp - kTcFirstRescoreWarp)) * mlp_rs_strip_doubles(p.n_in, H);
-      int n_done = 0;
-      for (;;) {
-        // claim the next ticket, then wait until its slot is published (lane 0 polls and broadcasts: the lanes of a
-        // warp need not run in lockstep)
-        int t = 0;
-        if (lane == 0) t = atomicAdd(&q_ctl[1], 1);
-        t = __shfl_sync(0xffffffffu, t, 0);
-        int v = 0;
-        for (;;) {
-          int state = 0;  // 1: nothing will ever be published for this ticket
-          if (lane == 0) {
-            v = atomicAdd(&q_slots[t & (kTcQueueCap - 1)], 0);
-            if (v == 0 && atomicAdd(&q_ctl[2], 0) == kTcEpilogueWarps) {
-              __threadfence_block();
-              if (t >= atomicAdd(&q_ctl[0], 0)) state = 1;
-            }
-          }
-          v = __shfl_sync(0xffffffffu, v, 0);
-          state = __shfl_sync(0xffffffffu, state, 0);
-          if (v != 0 || state == 1) break;
-          __nanosleep(200);
-        }
-        if (v == 0) break;
-        if (lane == 0) {
-          atomicExch(&q_slots[t & (kTcQueueCap - 1)], 0);
-          atomicAdd(&q_ctl[3], 1);
-        }
-        const long long frow = static_cast<long long>(v) - 1;
-        const MlpRowResult r = mlp_rs_row(rs_view, p.x + frow * p.ld, xs, xs + p.n_in, lane);
-        if (lane == 0) {
-          tc_store_final_label(p, frow, r.idx);
-          if (r.bad) atomicAdd(&p.counters[1], 1ull);
-          if (r.ambiguous) atomicAdd(&p.counters[0], 1ull);
-        }
-        ++n_done;
-      }
-      if (lane == 0 && n_done > 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n_done));
     }
   }
 }
@@ -505,28 +382,12 @@ std::vector<float> mlp_tc_build_w1_tiles(const float* w1 /*[H][F]*/, int H, int 
   return tiles;
 }
 
-static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool queue, bool proba = false) {
+static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool proba = false) {
   const size_t kc = m.f_pad / kChunkF;
   size_t bytes = 1024 + kc * (2 * m.n_hidden) * 128 + static_cast<size_t>(kTcSlots) * kTileRows * 4 +
                  (2 * 64 + kTcSlots) * 8 + 16;
-  if (queue)  // flagged-row queue + fp64 weights + one strip per epilogue / re-score warp
-    bytes += (kTcQueueCap + 4) * 4 + 16 +
-             (mlp_rs_weight_doubles(m.n_in, m.n_hidden, m.n_classes) +
-              (kTcEpilogueWarps + kTcRescoreWarps) * mlp_rs_strip_doubles(m.n_in, m.n_hidden)) * 8;
   if (proba) bytes += 16 + static_cast<size_t>(kTcEpilogueWarps) * 32 * m.n_classes * 4;  // one staging strip per epilogue warp
   return bytes;
-}
-
-bool mlp_tc_queue_rescore() {
-  // UML_B200_MLP_RESCORE_MODE=queue: rows flagged by the epilogue go through a shared-memory queue to four fp64
-  // re-score warps of the same launch; =kernel: flag list + mlp_rescore_f64_kernel behind the scoring kernel
-  static const int mode = [] {
-    const char* env = getenv("UML_B200_MLP_RESCORE_MODE");
-    if (env && env[0] == 'q') return 1;
-    if (env && env[0] == 'k') return 0;
-    return UML_MLP_QUEUE_DEFAULT;
-  }();
-  return mode == 1;
 }
 
 bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why) {
@@ -539,10 +400,10 @@ bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why) {
     if (why) *why = "more than 128 features: the resident W1 tile is sized for F_pad <= 128";
     return false;
   }
-  return mlp_tc_fixed_smem(m, true) + 6 * static_cast<size_t>(kStageBytes) <= static_cast<size_t>(kMaxSmemBytes);
+  return mlp_tc_fixed_smem(m) + 6 * static_cast<size_t>(kStageBytes) <= static_cast<size_t>(kMaxSmemBytes);
 }
 
-template <int H, int C, bool EXACT, bool QUEUE, bool PROBA = false>
+template <int H, int C, bool EXACT, bool PROBA = false>
 static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l,
                                      const FlagList& flags, int sm_count, cudaStream_t stream) {
   using Params = MlpTcParams<H, C>;
@@ -592,13 +453,8 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   p.n_rows = l.n_rows;
   p.num_tiles = (l.n_rows + kTileRows - 1) / kTileRows;
   p.kc = m.f_pad / kChunkF;
-  p.x = l.x;
-  p.ld = l.ld;
-  p.n_in = m.n_in;
-  p.rs_pack = m.rs_pack;
-  p.counters = flags.counters;
   p.proba = l.proba;
-  const size_t fixed = mlp_tc_fixed_smem(m, QUEUE, PROBA);
+  const size_t fixed = mlp_tc_fixed_smem(m, PROBA);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kStageBytes);
   stages = std::min(stages, 64);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(4, std::min(stages, atoi(env)));
@@ -610,7 +466,7 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
-  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, QUEUE, PROBA>;
+  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, PROBA>;
   static size_t configured = 0;
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -618,21 +474,17 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
     configured = smem;
   }
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, p.num_tiles)));
-  kern<<<grid, QUEUE ? kTcThreadsQueue : kTcThreads, smem, stream>>>(xmap, p);
+  kern<<<grid, kTcThreads, smem, stream>>>(xmap, p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_mlp_tc(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
-                          const FlagList& flags, int sm_count, cudaStream_t stream, bool* rescore_kernel_needed) {
-  const bool queue = exact && mlp_tc_queue_rescore();
-  if (rescore_kernel_needed) *rescore_kernel_needed = exact && !queue;
+                          const FlagList& flags, int sm_count, cudaStream_t stream) {
   if (l.n_rows <= 0) return cudaSuccess;
-#define UML_TC_CASE(HH, CC)                                                                                      \
-  if (m.n_hidden == HH && m.n_classes == CC) {                                                                   \
-    if (!exact) return mlp_tc_launch_one<HH, CC, false, false>(xmap, m, l, flags, sm_count, stream);             \
-    return queue ? mlp_tc_launch_one<HH, CC, true, true>(xmap, m, l, flags, sm_count, stream)                    \
-                 : mlp_tc_launch_one<HH, CC, true, false>(xmap, m, l, flags, sm_count, stream);                  \
-  }
+#define UML_TC_CASE(HH, CC)                                                                                  \
+  if (m.n_hidden == HH && m.n_classes == CC)                                                                 \
+    return exact ? mlp_tc_launch_one<HH, CC, true>(xmap, m, l, flags, sm_count, stream)                      \
+                 : mlp_tc_launch_one<HH, CC, false>(xmap, m, l, flags, sm_count, stream);
   UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
 #undef UML_TC_CASE
   return cudaErrorInvalidValue;
@@ -643,7 +495,7 @@ cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m
   if (l.n_rows <= 0) return cudaSuccess;
   const FlagList none{};
 #define UML_TC_CASE(HH, CC) \
-  if (m.n_hidden == HH && m.n_classes == CC) return mlp_tc_launch_one<HH, CC, false, false, true>(xmap, m, l, none, sm_count, stream);
+  if (m.n_hidden == HH && m.n_classes == CC) return mlp_tc_launch_one<HH, CC, false, true>(xmap, m, l, none, sm_count, stream);
   UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
 #undef UML_TC_CASE
   return cudaErrorInvalidValue;

@@ -182,9 +182,7 @@ struct MlpTcLaunch {
   int wire_u8;
   long long row_offset;
   long long n_rows;
-  const float* x;  // the batch rows (the in-kernel fp64 re-score of the tensor-core kernel reads flagged rows again)
-  long long ld;
-  float* proba;    // launch_mlp_tc_proba: class probabilities [n_rows][n_classes] (device)
+  float* proba;  // launch_mlp_tc_proba: class probabilities [n_rows][n_classes] (device)
 };
 // proba: the tile kernel's probability form (n_rows x n_classes fp32 instead of labels; exact and flags unused)
 bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why, bool proba = false);
@@ -196,8 +194,9 @@ cudaError_t launch_mlp_rescore_f64(const MlpDeviceModel& m, const float* x, int6
                                    cudaStream_t stream);
 bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why);
 std::vector<float> mlp_tc_build_w1_tiles(const float* w1, int H, int F, int f_pad);
+// exact: flagged rows go to the flag list; the caller launches launch_mlp_rescore_f64 behind it
 cudaError_t launch_mlp_tc(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
-                          const FlagList& flags, int sm_count, cudaStream_t stream, bool* rescore_kernel_needed);
+                          const FlagList& flags, int sm_count, cudaStream_t stream);
 // class probabilities softmax(logits) of every row into l.proba: tensor-core kernel (rows that are tf32 values), and
 // the fp64 scorer with a float64 softmax for shapes no tile kernel takes
 cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, int sm_count,
