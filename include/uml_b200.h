@@ -74,8 +74,8 @@ typedef struct uml_stats {
   int64_t d2h_bytes;
   int32_t kernel_launches; /* kernels of this library launched by the call                                            */
   int32_t path;            /* 1 = TMA fp32 tile kernel, 2 = generic fp64 kernel, 3 = MLP CUDA-core kernel, 5 = MLP tensor-core
-                              (wgmma) kernel, 4 = small-batch fp64
-                              kernel of the online path (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph)                 */
+                              (wgmma) kernel, 4 = small-batch fp64 kernel of the online path, linear or MLP
+                              (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph)                 */
 } uml_stats;
 
 typedef struct uml_device_info {
@@ -202,7 +202,12 @@ UML_API int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_bat
 /* the MLP predictor from HOST rows through the same chunk pipeline as uml_linear_predict_host (pinned bounce buffers,
  * GPU transpose / down-cast to fp32 - the reference predictor casts features to float32 -, scoring kernel, fp64
  * re-score): labels_out[i] = the argmax class index of row i, what `module(features).argmax(1)` yields
- * (quickstart.py:68-70).  _begin is the asynchronous form (uml_async_poll / uml_async_finish as for the linear call). */
+ * (quickstart.py:68-70).  Batches of <= 64 rows whose raw block fits 256 KiB take the online route of
+ * uml_linear_predict_host instead (stats path 4, one kernel replayed as a CUDA graph): the fp64 network on the fp32
+ * cast of the request read straight from pinned host memory, so their labels are the exact-mode labels in either mode;
+ * NaN/Inf in the fp32 features (a finite float64 beyond the fp32 range included) is UML_ERR_NONFINITE, as in the exact
+ * pipeline.  A model too large for one SM's shared memory (fp64 weights plus eight 4-row strips) keeps the pipeline.
+ * _begin is the asynchronous form (uml_async_poll / uml_async_finish as for the linear call). */
 UML_API int uml_mlp_predict_host(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows, int n_features,
                          int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out, int mode,
                          int64_t chunk_rows, uml_stats* stats);

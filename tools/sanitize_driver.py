@@ -48,4 +48,8 @@ X784 = (rng.integers(0, 256, size=(6_001, 784)) / 255.0)
 m784 = eng.load_linear(rng.standard_normal((10, 784)) * 0.05, rng.standard_normal(10))
 eng.predict(m784, eng.stage(X784), exact=True)
 eng.predict_host(m784, X784, exact=True, chunk_rows=2048)
+# MLP online route (mlp_small_kernel): a feature-major float64 block (capture, then replay) and a 1-row int64 request
+eng.predict_mlp_host(mlp, np.asfortranarray(Xf[:32]))
+eng.predict_mlp_host(mlp, np.asfortranarray(Xf[:32]))
+eng.predict_mlp_host(mlp, X[:1].astype(np.int64))
 print("sanitizer driver ok")

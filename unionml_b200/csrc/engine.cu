@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -152,7 +153,7 @@ class CopyPool {
   bool stop_ = false;
 };
 
-struct SmallGraph {  // one captured H2D -> linear_small_kernel -> D2H per (model, rows, features, dtype)
+struct SmallGraph {  // one captured small-batch kernel (linear or MLP) per (model, rows, features, dtype)
   uint64_t model_uid = 0;
   int n_rows = 0, n_features = 0, dtype = 0;
   cudaGraphExec_t exec = nullptr;
@@ -238,6 +239,8 @@ struct uml_batch {
 
 struct uml_mlp {
   uml_engine* e = nullptr;
+  uint64_t uid = 0;  // keys the cached small-batch graphs (from the same counter as uml_model::uid)
+  size_t small_smem = 0;  // dynamic shared memory of mlp_small_kernel; 0: too large, batches keep the chunk pipeline
   uml::MlpDeviceModel dm{};
   float* d_w1t = nullptr;
   float* d_b1 = nullptr;
@@ -1215,12 +1218,14 @@ static bool host_sample_is_tf32(const void* host, const SrcLayout& L, int64_t n_
   return true;
 }
 
-// B <= kSmallRows: request block -> pinned (device-mapped) buffer -> linear_small_kernel (replayed as a CUDA graph) ->
-// labels written straight into pinned host memory.  fp64 from the caller's own values, so the result is the
-// exact-mode result for either mode.
-static int predict_host_small(uml_engine* e, const uml_model* m, const void* host_ptr, int n_rows, int F,
-                              const SrcLayout& L, int src_dtype, int32_t* labels_out, double* values_out,
-                              const double* classes, int n_classes, uml_stats* stats) {
+// B <= kSmallRows: request block -> pinned (device-mapped) buffer -> one small-batch kernel (replayed as a CUDA graph)
+// -> labels written straight into pinned host memory.  The kernel scores in fp64 (linear_small_kernel from the
+// caller's own values, mlp_small_kernel from their fp32 cast), so the result is the exact-mode result for either mode.
+// `launch(view, stream)` enqueues that kernel on the request block; model_uid keys its cached graphs.
+using SmallLaunch = std::function<cudaError_t(const uml::SrcView&, cudaStream_t)>;
+static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaunch& launch, const void* host_ptr,
+                              int n_rows, int F, const SrcLayout& L, int src_dtype, int32_t* labels_out,
+                              double* values_out, const double* classes, int n_classes, uml_stats* stats) {
   NvtxRange r_all("uml:predict_host_small");
   const size_t width = (size_t)F * L.elem;
   const size_t bytes = width * (size_t)n_rows;
@@ -1257,13 +1262,13 @@ static int predict_host_small(uml_engine* e, const uml_model* m, const void* hos
     }
   }
   uml::SrcView view{e->d_req, src_dtype, (long long)F, 1};
-  auto enqueue = [&](cudaStream_t s) -> cudaError_t { return uml::launch_linear_small(m->dm, view, n_rows, e->d_small, s); };
+  auto enqueue = [&](cudaStream_t s) -> cudaError_t { return launch(view, s); };
   static const bool no_graph = getenv("UML_B200_NO_GRAPH") != nullptr;
   bool launched = false;
   if (e->small_graph_ok && !no_graph) {
     SmallGraph* hit = nullptr;
     for (auto& g : e->small_graphs)
-      if (g.model_uid == m->uid && g.n_rows == n_rows && g.n_features == F && g.dtype == src_dtype) hit = &g;
+      if (g.model_uid == model_uid && g.n_rows == n_rows && g.n_features == F && g.dtype == src_dtype) hit = &g;
     if (!hit) {
       cudaGraph_t graph = nullptr;
       cudaGraphExec_t exec = nullptr;
@@ -1286,7 +1291,7 @@ static int predict_host_small(uml_engine* e, const uml_model* m, const void* hos
           cudaGraphExecDestroy(e->small_graphs[lru].exec);
           e->small_graphs.erase(e->small_graphs.begin() + (long)lru);
         }
-        e->small_graphs.push_back({m->uid, n_rows, F, src_dtype, exec, 0});
+        e->small_graphs.push_back({model_uid, n_rows, F, src_dtype, exec, 0});
         hit = &e->small_graphs.back();
       }
     }
@@ -1345,8 +1350,15 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   int rc = classify_layout(e, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, &L);
   if (rc != UML_OK) return rc;
   const int F = n_features;
-  if (!mlp && n_rows <= kSmallRows && (int64_t)F * L.elem * n_rows <= kSmallBytes) {
-    rc = predict_host_small(e, m, host_ptr, (int)n_rows, F, L, src_dtype, labels_out, values_out, classes, n_classes, stats);
+  // an MLP whose weights and strips do not fit one SM's shared memory keeps the chunk pipeline
+  if (n_rows <= kSmallRows && (int64_t)F * L.elem * n_rows <= kSmallBytes && (!mlp || mlp->small_smem > 0)) {
+    const int rows = (int)n_rows;
+    const SmallLaunch launch = [&](const uml::SrcView& v, cudaStream_t s) {
+      return mlp ? uml::launch_mlp_small(mlp->dm, v, rows, e->d_small, mlp->small_smem, s)
+                 : uml::launch_linear_small(m->dm, v, rows, e->d_small, s);
+    };
+    rc = predict_host_small(e, mlp ? mlp->uid : m->uid, launch, host_ptr, rows, F, L, src_dtype, labels_out, values_out,
+                            classes, n_classes, stats);
     if (progress && rc == UML_OK) progress->store(n_rows);
     return rc;
   }
@@ -1717,8 +1729,9 @@ int uml_linear_predict_host_begin(uml_engine* e, const uml_model* m, const void*
                      mode, chunk_rows);
 }
 
-// the MLP predictor through the same chunk pipeline: labels_out[i] = argmax class index of row i, i.e. what
-// `module(features).argmax(1)` yields (tests/integration/pytorch_app/quickstart.py:68-70)
+// the MLP predictor through the same chunk pipeline, or for B <= kSmallRows the same online route (mlp_small_kernel):
+// labels_out[i] = argmax class index of row i, i.e. what `module(features).argmax(1)` yields
+// (tests/integration/pytorch_app/quickstart.py:68-70)
 int uml_mlp_predict_host(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows, int n_features,
                          int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out, int mode,
                          int64_t chunk_rows, uml_stats* stats) {
@@ -1874,6 +1887,14 @@ int uml_mlp_load(uml_engine* e, uml_mlp** out, const float* w1, const float* b1,
   m->dm.w2_abs_row_sum_max = row_sum_max;
   m->dm.w1_tiles = m->d_w1_tiles;
   m->dm.host = &m->host;
+  m->uid = g_model_uid.fetch_add(1);
+  // the online kernel's shared-memory limit is set here, not where its launch is captured into a graph
+  m->small_smem = uml::mlp_small_smem_bytes(F, H, C);
+  if (m->small_smem > 0 && (ce = uml::mlp_small_reserve(m->small_smem)) != cudaSuccess) {
+    e->last_error = std::string("uml_mlp_load: ") + cudaGetErrorString(ce);
+    uml_mlp_free(m);
+    return UML_ERR_CUDA;
+  }
   *out = m;
   return UML_OK;
 }

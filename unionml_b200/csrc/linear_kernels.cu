@@ -28,18 +28,6 @@
 
 namespace uml {
 
-// one element of the caller's raw source chunk as float64 (exact for every dtype the ABI takes)
-__device__ __forceinline__ double load_src(const SrcView& v, long long row, int f) {
-  const long long i = row * v.row_stride + static_cast<long long>(f) * v.col_stride;
-  switch (v.dtype) {
-    case UML_F64: return static_cast<const double*>(v.base)[i];
-    case UML_I64: return static_cast<double>(static_cast<const long long*>(v.base)[i]);
-    case UML_I32: return static_cast<double>(static_cast<const int*>(v.base)[i]);
-    case UML_U8: return static_cast<double>(static_cast<const unsigned char*>(v.base)[i]);
-    default: return static_cast<double>(static_cast<const float*>(v.base)[i]);
-  }
-}
-
 struct RowScore {
   int idx;
   bool bad;        // NaN/Inf in the row

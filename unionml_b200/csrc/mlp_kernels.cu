@@ -13,6 +13,7 @@
 //  * mlp_rescore_f64_kernel: warp per row, lane per hidden unit, fp64; flagged rows of EXACT mode, or every row for
 //    shapes the tile kernel is not instantiated for.
 //  * mlp_proba_f64_kernel: class probabilities for those shapes - the same fp64 scorer, then a float64 softmax.
+//  * mlp_small_kernel: the online path (B <= 64 rows): the same fp64 scorer on the request block in pinned host memory.
 //
 // This is CUDA-core fp32 (FFMA): 4 736 flop/row puts the HBM roofline (25 G rows/s) above the FFMA peak, so this kernel
 // is FMA-pipe bound (~0.66 ms per 10M rows at 1.9 GHz).  It serves batches whose features are NOT tf32 values (general
@@ -413,9 +414,99 @@ __global__ void __launch_bounds__(256) mlp_proba_f64_kernel(const MlpProbaF64Par
   }
 }
 
+// small-batch kernel of the online path (fastapi.py /predict, B <= 64 rows): the fp64 scorer above on the request's
+// raw feature block, which the kernel reads straight from pinned host memory - no staging pass, no tile kernel, no
+// guard, exact by construction.  Each warp casts its four rows to fp32 as the staging kernels do (convert_one: the
+// value as double, then to float), so this route scores the same fp32 features as the chunk pipeline and as the
+// reference predictor (`torch.from_numpy(values).float()`), into an fp32 strip in its own shared memory.
+struct MlpSmallParams {
+  SrcView src;
+  int n_rows;
+  const double* pack;
+  int F, H, C;
+  SmallResult* out;
+};
+
+__global__ void __launch_bounds__(256) mlp_small_kernel(const MlpSmallParams p) {
+  extern __shared__ __align__(16) double rs_smem[];
+  constexpr int R = kMlpRsRows;
+  MlpRsView view = mlp_rs_stage(rs_smem, p.pack, p.F, p.H, p.C);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // per warp: the scorer's strip, then the four rows as fp32 (F x R doubles hold 2 F x R floats: room to spare)
+  double* xs = rs_smem + mlp_rs_weight_doubles(p.F, p.H, p.C) + warp * (mlp_rs_strip_doubles(p.F, p.H, R) + 2 * p.F);
+  double* hv = xs + p.F * R;
+  float* x32 = reinterpret_cast<float*>(hv + p.H * R);
+  __syncthreads();
+  mlp_rs_finish_stage(view);
+
+  const int i = (blockIdx.x * (blockDim.x >> 5) + warp) * R;
+  if (i >= p.n_rows) return;
+  // x32[r F + f] = feature f of row r.  Every load is a PCIe round trip to pinned host memory, so a lane issues a
+  // batch of them before it stores any (a store in between would serialise them: the source may alias shared memory)
+  constexpr int kLoads = 8;
+  const int total = R * p.F;
+  for (int k0 = lane; k0 < total; k0 += 32 * kLoads) {
+    double v[kLoads];
+#pragma unroll
+    for (int j = 0; j < kLoads; ++j) {
+      const int k = min(k0 + 32 * j, total - 1);  // (past the end: a valid element, not stored; no branch per load)
+      const int r = k / p.F;
+      const int row = i + r < p.n_rows ? i + r : i;  // unused slots repeat the first row (result ignored)
+      v[j] = load_src(p.src, row, k - r * p.F);
+    }
+#pragma unroll
+    for (int j = 0; j < kLoads; ++j)
+      if (k0 + 32 * j < total) x32[k0 + 32 * j] = static_cast<float>(v[j]);
+  }
+  const float* xr[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) xr[r] = x32 + r * p.F;
+  __syncwarp();
+  MlpRowResult res[R];
+  mlp_rs_rows<R>(view, xr, xs, hv, lane, res);
+  if (lane < R && i + lane < p.n_rows) {
+    MlpRowResult mine = res[0];
+#pragma unroll
+    for (int r = 1; r < R; ++r)
+      if (lane == r) mine = res[r];
+    p.out[i + lane].label = mine.idx;
+    p.out[i + lane].status = (mine.bad ? 1 : 0) | (mine.ambiguous ? 2 : 0);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
+size_t mlp_small_smem_bytes(int n_in, int n_hidden, int n_classes) {
+  const size_t per_warp = mlp_rs_strip_doubles(n_in, n_hidden, kMlpRsRows) + 2 * static_cast<size_t>(n_in);
+  const size_t smem = (mlp_rs_weight_doubles(n_in, n_hidden, n_classes) + 8 * per_warp) * sizeof(double);
+  return smem > static_cast<size_t>(kMaxSmemBytes) ? 0 : smem;
+}
+
+cudaError_t mlp_small_reserve(size_t smem) {
+  static size_t configured = 0;
+  if (smem <= configured) return cudaSuccess;
+  cudaError_t err = cudaFuncSetAttribute(mlp_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (err == cudaSuccess) configured = smem;
+  return err;
+}
+
+cudaError_t launch_mlp_small(const MlpDeviceModel& m, const SrcView& src, int n_rows, SmallResult* out, size_t smem,
+                             cudaStream_t stream) {
+  if (n_rows <= 0) return cudaSuccess;
+  MlpSmallParams p{};
+  p.src = src;
+  p.n_rows = n_rows;
+  p.pack = m.rs_pack;
+  p.F = m.n_in;
+  p.H = m.n_hidden;
+  p.C = m.n_classes;
+  p.out = out;
+  constexpr int rows_per_block = 8 * kMlpRsRows;
+  mlp_small_kernel<<<(n_rows + rows_per_block - 1) / rows_per_block, 256, smem, stream>>>(p);
+  return cudaGetLastError();
+}
+
 static size_t mlp_fixed_smem(const MlpDeviceModel& m, bool proba = false) {
   return 1024 + (static_cast<size_t>(m.f_pad) * (m.n_hidden + 4) + (m.n_hidden + 4) + static_cast<size_t>(m.n_hidden) * m.cp + m.cp) * 4 +
          2 * 64 * 8 + (proba ? static_cast<size_t>(kMlpConsumerWarps) * 32 * m.n_classes * 4 : 0);  // + a staging strip per warp

@@ -102,6 +102,20 @@ struct SrcView {
   long long col_stride;  // in elements
 };
 
+#ifdef __CUDACC__
+// one element of the caller's raw source chunk as float64 (exact for every dtype the ABI takes)
+__device__ __forceinline__ double load_src(const SrcView& v, long long row, int f) {
+  const long long i = row * v.row_stride + static_cast<long long>(f) * v.col_stride;
+  switch (v.dtype) {
+    case UML_F64: return static_cast<const double*>(v.base)[i];
+    case UML_I64: return static_cast<double>(static_cast<const long long*>(v.base)[i]);
+    case UML_I32: return static_cast<double>(static_cast<const int*>(v.base)[i]);
+    case UML_U8: return static_cast<double>(static_cast<const unsigned char*>(v.base)[i]);
+    default: return static_cast<double>(static_cast<const float*>(v.base)[i]);
+  }
+}
+#endif
+
 struct LinearLaunch {
   const float* x;       // device fp32 row-major
   const double* x64;    // optional fp64 copy of the same rows (lossy staging), else nullptr
@@ -203,6 +217,14 @@ cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m
                                 cudaStream_t stream);
 cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, float* proba,
                                  int sm_count, cudaStream_t stream);
+// small-batch kernel of the online path (B <= 64): four rows per warp through the fp64 scorer, the features read
+// straight from the raw source view and cast to fp32 as the staging kernels cast them.  mlp_small_smem_bytes: its
+// dynamic shared memory for the model's shape, 0 when that exceeds one SM; mlp_small_reserve sets the kernel's
+// shared-memory limit (call it before a launch is captured into a graph)
+size_t mlp_small_smem_bytes(int n_in, int n_hidden, int n_classes);
+cudaError_t mlp_small_reserve(size_t smem);
+cudaError_t launch_mlp_small(const MlpDeviceModel& m, const SrcView& src, int n_rows, SmallResult* out, size_t smem,
+                             cudaStream_t stream);
 // int32 labels (device) -> every target vector of a fused exchange (int32 or uint8 wire), for kernels without peer stores
 cudaError_t launch_labels_scatter(const int32_t* labels, int64_t n, void* const* peers, int n_peers, int wire_u8,
                                   int64_t row_offset, int sm_count, cudaStream_t stream);

@@ -473,8 +473,11 @@ class Engine:
 
     def predict_mlp_host(self, model: MlpModel, features: Any, exact: bool = True, chunk_rows: int = 0,
                          out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, dict]:
-        """Host rows -> argmax class index of the 2-layer MLP per row (int32), through the chunk pipeline (pinned bounce
-        buffers, GPU down-cast to fp32 as the reference predictor does, scoring kernel, fp64 re-score)."""
+        """Host rows -> argmax class index of the 2-layer MLP per row (int32).  Features are cast to fp32 as the
+        reference predictor does.  Up to 64 rows (256 KiB of raw features): the online route, one float64 kernel that
+        reads the request from pinned host memory, replayed as a CUDA graph (stats ``path`` 4, exact labels in either
+        mode).  Larger batches, or a model too large for that kernel's shared memory: the chunk pipeline (pinned bounce
+        buffers, GPU down-cast, scoring kernel, fp64 re-score)."""
         arr = as_feature_array(features)
         if out is None:
             out = np.empty(arr.shape[0], dtype=np.int32)

@@ -301,16 +301,23 @@ def _mlp_layers(module):
 
 
 def device_mlp(module, engine: Engine | None = None) -> MlpModel:
+    """The module's two ``nn.Linear`` layers staged on the device, cached per module.
+
+    The cache key is cheap enough for every online request: per parameter its storage pointer, shape, dtype and
+    ``_version`` (torch bumps it on every in-place write: ``optimizer.step()``, ``load_state_dict``, ``add_``), plus the
+    engine.  The cache entry holds the parameter objects themselves and a hit needs the same objects, so a rebound
+    parameter (``layer.weight = nn.Parameter(...)``) is a miss.  The weights are read back to the host only on a miss."""
     engine = engine or get_engine()
     l1, l2 = _mlp_layers(module)
-    w1, b1, w2, b2 = (t.detach().cpu().numpy() for t in (l1.weight, l1.bias, l2.weight, l2.bias))
-    key = (id(engine), w1.shape, w2.shape, hash(w1.tobytes()), hash(b1.tobytes()), hash(w2.tobytes()), hash(b2.tobytes()))
+    params = (l1.weight, l1.bias, l2.weight, l2.bias)
+    key = (id(engine),) + tuple((t.data_ptr(), tuple(t.shape), t.dtype, t._version) for t in params)
     with _cache_lock:
         hit = _model_cache.get(module)
-        if hit is not None and hit[0] == key:
-            return hit[1]
+        if hit is not None and hit[0] == key and all(a is b for a, b in zip(hit[1], params)):
+            return hit[2]
+        w1, b1, w2, b2 = (t.detach().cpu().numpy() for t in params)
         dm = engine.load_mlp(w1, b1, w2, b2)
-        _model_cache[module] = (key, dm)
+        _model_cache[module] = (key, params, dm)
         return dm
 
 
@@ -318,8 +325,10 @@ def mlp_argmax(module: Any, features: Any) -> List[float]:
     """Drop-in body for the torch quickstart predictor
     ``[float(x) for x in module(process_features(features)).argmax(1)]``: features are cast to float32 exactly as
     ``process_features`` does (``torch.from_numpy(features.values).float()``), the forward pass and argmax run on
-    the GPU, labels come back as Python floats.  Host frames go through the chunk pipeline of the linear predictor
-    (pinned bounce buffers, GPU down-cast); from 1M rows on the list is filled while the batch is still in flight."""
+    the GPU, labels come back as Python floats.  Requests of up to 64 rows (the ``/predict`` shape) take the online
+    route: one float64 kernel replayed as a CUDA graph, exact labels.  Larger frames go through the chunk pipeline of
+    the linear predictor (pinned bounce buffers, GPU down-cast); from 1M rows on the list is filled while the batch is
+    still in flight."""
     engine = get_engine()
     dm = device_mlp(module, engine)
     arr = features.to_numpy() if hasattr(features, "to_numpy") else np.asarray(features)
