@@ -160,6 +160,21 @@ struct SmallGraph {  // one captured small-batch kernel (linear or MLP) per (mod
   uint64_t last_use = 0;
 };
 
+// engine scratch that only grows (see grow): N buffers of `cap` elements each, in device memory or, Pinned, in
+// page-locked host memory
+template <class T, int N = 1, bool Pinned = false>
+struct Scratch {
+  T* p[N] = {};
+  int64_t cap = 0;
+  void release() {
+    for (auto& q : p) {
+      if (q) Pinned ? cudaFreeHost(q) : cudaFree(q);
+      q = nullptr;
+    }
+    cap = 0;
+  }
+};
+
 struct uml_engine {
   int device = 0;
   cudaStream_t own_stream = nullptr, stream = nullptr, copy_stream = nullptr;
@@ -172,24 +187,15 @@ struct uml_engine {
   int* d_flag_count = nullptr;
   unsigned long long* d_counters = nullptr;
   StageResult* d_stage = nullptr;
-  int32_t* d_flag_rows = nullptr;
-  int64_t flag_cap = 0;
-  int32_t* d_labels = nullptr;
-  int64_t labels_cap = 0;
-  float* d_proba = nullptr;  // class probabilities bound for host memory (uml_mlp_predict_proba)
-  int64_t proba_cap = 0;     // floats
-  void* d_chunk[3] = {nullptr, nullptr, nullptr};  // raw source chunks (staging / predict_host)
-  int64_t chunk_cap = 0;
-  float* d_xchunk[3] = {nullptr, nullptr, nullptr};  // converted fp32 chunks (predict_host)
-  int64_t xchunk_cap = 0;
-  double* d_vchunk[3] = {nullptr, nullptr, nullptr};  // class values of a chunk (predict_host_values)
-  int64_t vchunk_cap = 0;
-  double* d_classes = nullptr;
-  int classes_cap = 0;
-  void* h_bounce[3] = {nullptr, nullptr, nullptr};  // pinned bounce buffers for pageable sources
-  int64_t bounce_cap = 0;
-  void* h_result[3] = {nullptr, nullptr, nullptr};  // pinned landing slots for labels / values bound for pageable outputs
-  int64_t result_cap = 0;
+  Scratch<int32_t> d_flag_rows;
+  Scratch<int32_t> d_labels;
+  Scratch<float> d_proba;                // class probabilities bound for host memory (uml_mlp_predict_proba)
+  Scratch<char, 3> d_chunk;              // raw source chunks (staging / predict_host)
+  Scratch<float, 3> d_xchunk;            // converted fp32 chunks (predict_host)
+  Scratch<double, 3> d_vchunk;           // class values of a chunk (predict_host_values)
+  Scratch<double> d_classes;
+  Scratch<char, 3, true> h_bounce;       // pinned bounce buffers for pageable sources
+  Scratch<char, 3, true> h_result;       // pinned landing slots for labels / values bound for pageable outputs
   CopyPool* pool = nullptr;
   // online path (B <= kSmallRows): pinned request buffer, its device twin, result slots, cached graphs
   void* h_req = nullptr;
@@ -267,6 +273,62 @@ struct uml_mlp {
                cudaGetErrorString(_err));                                                              \
     }                                                                                                  \
   } while (0)
+
+// UML_CUDA inside a pipeline (uml_stage_rows, predict_host_impl): both streams are drained before the call returns,
+// because their queued copies still reference the caller's host memory
+#define UML_CUDA_DRAIN(E, CALL)                                                                          \
+  do {                                                                                                   \
+    cudaError_t _ce = (CALL);                                                                            \
+    if (_ce != cudaSuccess) {                                                                            \
+      cudaStreamSynchronize((E)->stream);                                                                \
+      cudaStreamSynchronize((E)->copy_stream);                                                           \
+      UML_FAIL(E, _ce == cudaErrorMemoryAllocation ? UML_ERR_NOMEM : UML_ERR_CUDA, "%s failed: %s", #CALL, \
+               cudaGetErrorString(_ce));                                                                 \
+    }                                                                                                    \
+  } while (0)
+
+// make `s` hold at least n elements per buffer; it never shrinks, and reallocates only when n exceeds its capacity
+template <class T, int N, bool Pinned>
+static int grow(uml_engine* e, Scratch<T, N, Pinned>& s, int64_t n) {
+  if (s.cap >= n) return UML_OK;
+  s.release();
+  for (auto& q : s.p) {
+    void** v = (void**)&q;
+    const size_t bytes = (size_t)n * sizeof(T);
+    if (Pinned) UML_CUDA(e, cudaHostAlloc(v, bytes, cudaHostAllocDefault));
+    else UML_CUDA(e, cudaMalloc(v, bytes));
+  }
+  s.cap = n;
+  return UML_OK;
+}
+
+static FlagList flag_list(const uml_engine* e) {
+  return FlagList{e->d_flag_count, e->d_flag_rows.p[0], (int)std::min<int64_t>(e->d_flag_rows.cap, INT32_MAX),
+                  e->d_counters};
+}
+
+// a synchronous call reads its counters back at the end, so it starts them from zero
+static cudaError_t reset_counters(uml_engine* e, cudaStream_t s) {
+  const cudaError_t ce = cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), s);
+  return ce != cudaSuccess ? ce : cudaMemsetAsync(e->d_flag_count, 0, sizeof(int), s);
+}
+
+// which MLP kernel scores the rows (the stats' path): 5 tensor cores, 3 CUDA cores, 2 the generic fp64 scorer.  Tensor
+// cores when every feature is a tf32 value (integer / pixel domains), CUDA cores otherwise; both read the rows through
+// a tensor map.  UML_B200_MLP_TC=0 / 1 forces the choice; 1 does not apply to class probabilities (labels: rows that
+// are not tf32 values are caught in the kernel and re-scored; the probability kernels have no fp64 re-score behind
+// them).  tf32() is asked only when its answer decides: it may cost a pass over the rows.
+template <class Tf32>
+static int mlp_route(const uml::MlpDeviceModel& m, bool has_map, bool proba, Tf32&& tf32) {
+  if (!has_map) return 2;
+  std::string why;
+  if (uml::mlp_tc_supported(m, &why)) {
+    const char* env = getenv("UML_B200_MLP_TC");
+    const bool off = env && env[0] == '0', on = env && env[0] == '1' && !proba;
+    if (!off && (on || tf32())) return 5;
+  }
+  return uml::mlp_tma_supported(m, &why, proba) ? 3 : 2;
+}
 
 static int dtype_size(int dt) {
   switch (dt) {
@@ -359,17 +421,15 @@ void uml_engine_destroy(uml_engine* e) {
   cudaFree(e->d_flag_count);
   cudaFree(e->d_counters);
   cudaFree(e->d_stage);
-  cudaFree(e->d_flag_rows);
-  cudaFree(e->d_labels);
-  cudaFree(e->d_proba);
-  for (auto p : e->d_chunk) cudaFree(p);
-  for (auto p : e->d_xchunk) cudaFree(p);
-  for (auto p : e->d_vchunk) cudaFree(p);
-  cudaFree(e->d_classes);
-  for (auto p : e->h_bounce)
-    if (p) cudaFreeHost(p);
-  for (auto p : e->h_result)
-    if (p) cudaFreeHost(p);
+  e->d_flag_rows.release();
+  e->d_labels.release();
+  e->d_proba.release();
+  e->d_chunk.release();
+  e->d_xchunk.release();
+  e->d_vchunk.release();
+  e->d_classes.release();
+  e->h_bounce.release();
+  e->h_result.release();
   delete e->pool;
   for (auto& g : e->small_graphs)
     if (g.exec) cudaGraphExecDestroy(g.exec);
@@ -633,18 +693,6 @@ int uml_batch_from_device(uml_engine* e, uml_batch** out, const void* dev_ptr, i
   return UML_OK;
 }
 
-static int ensure_chunks(uml_engine* e, int64_t bytes) {
-  if (e->chunk_cap >= bytes) return UML_OK;
-  for (auto& p : e->d_chunk) {
-    cudaFree(p);
-    p = nullptr;
-  }
-  e->chunk_cap = 0;
-  for (auto& p : e->d_chunk) UML_CUDA(e, cudaMalloc(&p, (size_t)bytes));
-  e->chunk_cap = bytes;
-  return UML_OK;
-}
-
 struct SrcLayout {
   bool feature_major;
   int64_t pitch_elems;
@@ -766,16 +814,9 @@ static int usable_cpus(int* logical = nullptr) {
 }
 
 // pinned bounce buffers (3 slots) + the copy pool, created on first use
-static int ensure_bounce(uml_engine* e, int64_t bytes) {
-  if (e->bounce_cap < bytes) {
-    for (auto& p : e->h_bounce) {
-      if (p) cudaFreeHost(p);
-      p = nullptr;
-    }
-    e->bounce_cap = 0;
-    for (auto& p : e->h_bounce) UML_CUDA(e, cudaHostAlloc(&p, (size_t)bytes, cudaHostAllocDefault));
-    e->bounce_cap = bytes;
-  }
+static int grow_bounce(uml_engine* e, int64_t bytes) {
+  const int rc = grow(e, e->h_bounce, bytes);
+  if (rc != UML_OK) return rc;
   if (!e->pool) {
     int n = 0;
     if (const char* env = getenv("UML_B200_COPY_THREADS")) n = atoi(env);
@@ -818,101 +859,86 @@ int uml_stage_rows(uml_engine* e, uml_batch** out, const void* host_ptr, int64_t
   // float64 / int64 / int32 values may not survive the fp32 down-cast (|int32| > 2^24 does not)
   const bool want64 = (flags & UML_STAGE_KEEP_F64) && (src_dtype == UML_F64 || src_dtype == UML_I64 || src_dtype == UML_I32);
 
-  uml_batch* b = new uml_batch();
+  // the half-built batch is freed on every early return
+  std::unique_ptr<uml_batch, decltype(&uml_batch_free)> b(new uml_batch(), uml_batch_free);
   b->e = e;
   b->n_rows = n_rows;
   b->n_features = F;
   b->ld = ld;
   b->owns = true;
-  auto bail = [&](int code) {
-    uml_batch_free(b);
-    return code;
-  };
   if (n_rows == 0) {
-    *out = b;
+    *out = b.release();
     return UML_OK;
   }
   cudaError_t ce;
   if ((ce = cudaMalloc((void**)&b->x, (size_t)n_rows * ld * 4)) != cudaSuccess) {
     e->last_error = std::string("cudaMalloc(batch): ") + cudaGetErrorString(ce);
-    return bail(ce == cudaErrorMemoryAllocation ? UML_ERR_NOMEM : UML_ERR_CUDA);
+    return ce == cudaErrorMemoryAllocation ? UML_ERR_NOMEM : UML_ERR_CUDA;
   }
   if (want64) {
     b->ld64 = F;
     if ((ce = cudaMalloc((void**)&b->x64, (size_t)n_rows * F * 8)) != cudaSuccess) {
       e->last_error = std::string("cudaMalloc(batch f64): ") + cudaGetErrorString(ce);
-      return bail(ce == cudaErrorMemoryAllocation ? UML_ERR_NOMEM : UML_ERR_CUDA);
+      return ce == cudaErrorMemoryAllocation ? UML_ERR_NOMEM : UML_ERR_CUDA;
     }
   }
   cudaStream_t cs = e->stream;
-#define STAGE_CUDA(CALL)                                                            \
-  do {                                                                              \
-    cudaError_t _e2 = (CALL);                                                       \
-    if (_e2 != cudaSuccess) {                                                       \
-      e->last_error = std::string(#CALL) + ": " + cudaGetErrorString(_e2);          \
-      cudaStreamSynchronize(cs);                                                    \
-      cudaStreamSynchronize(e->copy_stream);                                        \
-      return bail(UML_ERR_CUDA);                                                    \
-    }                                                                               \
-  } while (0)
-  STAGE_CUDA(cudaMemsetAsync(e->d_stage, 0, sizeof(StageResult), cs));
+  UML_CUDA_DRAIN(e, cudaMemsetAsync(e->d_stage, 0, sizeof(StageResult), cs));
 
   // already the resident layout and page-locked: one straight H2D, then the finiteness scan (a large pageable source
   // goes through the chunked path instead, where host threads feed pinned bounce buffers)
   const bool direct = !L.feature_major && src_dtype == UML_F32 && L.pitch_elems == ld &&
                       !want_bounce(host_ptr, n_rows * (int64_t)F * L.elem);
   if (direct) {
-    STAGE_CUDA(cudaMemcpyAsync(b->x, host_ptr, (size_t)n_rows * ld * 4, cudaMemcpyHostToDevice, cs));
-    if (check) STAGE_CUDA(uml::launch_finite_scan(b->x, ld, n_rows, F, e->d_stage, cs));
+    UML_CUDA_DRAIN(e, cudaMemcpyAsync(b->x, host_ptr, (size_t)n_rows * ld * 4, cudaMemcpyHostToDevice, cs));
+    if (check) UML_CUDA_DRAIN(e, uml::launch_finite_scan(b->x, ld, n_rows, F, e->d_stage, cs));
   } else {
     // chunked: H2D of raw source bytes on the copy stream, transpose/convert kernel on the compute stream
     const int64_t row_bytes = (int64_t)F * L.elem;
     int64_t chunk_rows = std::max<int64_t>(1024, (64ll << 20) / row_bytes);
     chunk_rows = std::min<int64_t>((chunk_rows + 31) / 32 * 32, std::max<int64_t>(n_rows, 1));
-    int rc2 = ensure_chunks(e, chunk_rows * row_bytes);
-    if (rc2 != UML_OK) return bail(rc2);
+    if ((rc = grow(e, e->d_chunk, chunk_rows * row_bytes)) != UML_OK) return rc;
     // pageable frames: a few host threads gather each chunk into a pinned bounce buffer (see CopyPool)
     const bool bounce = want_bounce(host_ptr, n_rows * row_bytes);
-    if (bounce && (rc2 = ensure_bounce(e, chunk_rows * row_bytes)) != UML_OK) return bail(rc2);
+    if (bounce && (rc = grow_bounce(e, chunk_rows * row_bytes)) != UML_OK) return rc;
     std::vector<CopyPool::Task> tasks;
     int slot = 0;
     bool used[3] = {false, false, false};
     for (int64_t r0 = 0; r0 < n_rows; r0 += chunk_rows, slot = (slot + 1) % 3) {
       const int64_t rows = std::min(chunk_rows, n_rows - r0);
-      if (used[slot]) STAGE_CUDA(cudaStreamWaitEvent(e->copy_stream, e->chunk_ev[3 + slot], 0));  // convert done
+      char* raw = e->d_chunk.p[slot];
+      if (used[slot]) UML_CUDA_DRAIN(e, cudaStreamWaitEvent(e->copy_stream, e->chunk_ev[3 + slot], 0));  // convert done
       if (bounce) {
-        if (used[slot]) STAGE_CUDA(cudaEventSynchronize(e->chunk_ev[slot]));  // previous H2D has left the bounce buffer
-        build_gather_tasks(tasks, (char*)e->h_bounce[slot], host_ptr, L, r0, rows, F);
+        // previous H2D has left the bounce buffer
+        if (used[slot]) UML_CUDA_DRAIN(e, cudaEventSynchronize(e->chunk_ev[slot]));
+        build_gather_tasks(tasks, e->h_bounce.p[slot], host_ptr, L, r0, rows, F);
         e->pool->run(tasks);
-        STAGE_CUDA(cudaMemcpyAsync(e->d_chunk[slot], e->h_bounce[slot], (size_t)(rows * row_bytes), cudaMemcpyHostToDevice,
-                                   e->copy_stream));
-      } else
-      STAGE_CUDA(copy_chunk_h2d(e->d_chunk[slot], host_ptr, L, r0, rows, F, e->copy_stream));
-      STAGE_CUDA(cudaEventRecord(e->chunk_ev[slot], e->copy_stream));
-      STAGE_CUDA(cudaStreamWaitEvent(cs, e->chunk_ev[slot], 0));
-      STAGE_CUDA(uml::launch_stage_convert(e->d_chunk[slot], src_dtype, L.feature_major, L.feature_major ? rows : F,
-                                           rows, F, b->x + r0 * ld, ld, b->x64 ? b->x64 + r0 * b->ld64 : nullptr,
-                                           b->ld64, e->d_stage, check, cs));
-      STAGE_CUDA(cudaEventRecord(e->chunk_ev[3 + slot], cs));
+        UML_CUDA_DRAIN(e, cudaMemcpyAsync(raw, e->h_bounce.p[slot], (size_t)(rows * row_bytes), cudaMemcpyHostToDevice,
+                                          e->copy_stream));
+      } else {
+        UML_CUDA_DRAIN(e, copy_chunk_h2d(raw, host_ptr, L, r0, rows, F, e->copy_stream));
+      }
+      UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[slot], e->copy_stream));
+      UML_CUDA_DRAIN(e, cudaStreamWaitEvent(cs, e->chunk_ev[slot], 0));
+      UML_CUDA_DRAIN(e, uml::launch_stage_convert(raw, src_dtype, L.feature_major, L.feature_major ? rows : F, rows, F,
+                                                  b->x + r0 * ld, ld, b->x64 ? b->x64 + r0 * b->ld64 : nullptr, b->ld64,
+                                                  e->d_stage, check, cs));
+      UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[3 + slot], cs));
       used[slot] = true;
     }
   }
-  STAGE_CUDA(cudaMemcpyAsync(&e->h->stage, e->d_stage, sizeof(StageResult), cudaMemcpyDeviceToHost, cs));
-  STAGE_CUDA(cudaStreamSynchronize(cs));
-#undef STAGE_CUDA
-  if (check && e->h->stage.nonfinite) {
-    e->last_error = "Input X contains NaN or infinity.";
-    return bail(UML_ERR_NONFINITE);
-  }
+  UML_CUDA_DRAIN(e, cudaMemcpyAsync(&e->h->stage, e->d_stage, sizeof(StageResult), cudaMemcpyDeviceToHost, cs));
+  UML_CUDA_DRAIN(e, cudaStreamSynchronize(cs));
+  if (check && e->h->stage.nonfinite) UML_FAIL(e, UML_ERR_NONFINITE, "Input X contains NaN or infinity.");
   b->lossless = direct ? true : e->h->stage.lossy == 0;
   if (check || !direct) b->tf32_exact = e->h->stage.not_tf32 == 0 ? 1 : 0;  // the scan / conversion pass saw every value
   if (b->x64 && b->lossless) {
     cudaFree(b->x64);
     b->x64 = nullptr;
   }
-  rc = encode_batch_maps(e, b);
-  if (rc != UML_OK && rc != UML_ERR_UNSUPPORTED) return bail(rc);
-  *out = b;
+  rc = encode_batch_maps(e, b.get());
+  if (rc != UML_OK && rc != UML_ERR_UNSUPPORTED) return rc;
+  *out = b.release();
   return UML_OK;
 }
 
@@ -938,41 +964,11 @@ void uml_batch_free(uml_batch* b) {
 // ---------------------------------------------------------------------------------------------------------------
 // predict
 // ---------------------------------------------------------------------------------------------------------------
-static int ensure_flags(uml_engine* e, int64_t rows) {
-  if (e->flag_cap >= rows) return UML_OK;
-  cudaFree(e->d_flag_rows);
-  e->d_flag_rows = nullptr;
-  e->flag_cap = 0;
-  UML_CUDA(e, cudaMalloc((void**)&e->d_flag_rows, (size_t)rows * 4));
-  e->flag_cap = rows;
-  return UML_OK;
-}
-
-static int ensure_labels(uml_engine* e, int64_t rows) {
-  if (e->labels_cap >= rows) return UML_OK;
-  cudaFree(e->d_labels);
-  e->d_labels = nullptr;
-  e->labels_cap = 0;
-  UML_CUDA(e, cudaMalloc((void**)&e->d_labels, (size_t)rows * 4));
-  e->labels_cap = rows;
-  return UML_OK;
-}
-
-static int ensure_proba(uml_engine* e, int64_t n_floats) {
-  if (e->proba_cap >= n_floats) return UML_OK;
-  cudaFree(e->d_proba);
-  e->d_proba = nullptr;
-  e->proba_cap = 0;
-  UML_CUDA(e, cudaMalloc((void**)&e->d_proba, (size_t)n_floats * 4));
-  e->proba_cap = n_floats;
-  return UML_OK;
-}
-
 // enqueue the scoring of one resident block of rows on e->stream; no host synchronisation.
 // ev_k (optional) brackets the scoring kernel, ev_r the fp64 re-score.
 static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch& l, const CUtensorMap* map, int mode,
                            bool timed, int* launches, int* path) {
-  FlagList fl{e->d_flag_count, e->d_flag_rows, (int)std::min<int64_t>(e->flag_cap, INT32_MAX), e->d_counters};
+  const FlagList fl = flag_list(e);
   const bool exact = mode == UML_PREDICT_EXACT;
   std::string why;
   const bool tma = map != nullptr && uml::linear_tma_supported(m->dm, &why);
@@ -1005,6 +1001,49 @@ static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch
   return UML_OK;
 }
 
+// the MLP counterpart of enqueue_predict: the scoring kernel of `route` (mlp_route), the fp64 re-score of its flagged
+// rows when exact, and for the CUDA-core kernel with peers, the scatter of its labels.  `out` holds the row count and
+// where the labels go.  No host synchronisation; ev[1] / ev[2] bracket the scoring kernel, ev[2] / ev[3] the rest.
+static int enqueue_mlp(uml_engine* e, const uml::MlpDeviceModel& m, const CUtensorMap& map, const float* x, int64_t ld,
+                       const uml::MlpTcLaunch& out, bool exact, int route, bool timed, int* launches, int* path) {
+  const FlagList fl = flag_list(e);
+  const int sm = e->info.sm_count;
+  cudaStream_t s = e->stream;
+  *path = route;
+  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], s));
+  if (route == 2) {
+    NvtxRange r_score("uml:mlp_score_f64_generic");
+    UML_CUDA(e, uml::launch_mlp_rescore_f64(m, x, ld, out.n_rows, out, fl, true, sm, s));
+    *launches += 1;
+    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
+  } else {
+    // the CUDA-core kernel has no peer stores: it writes int32 labels to scratch (the caller grew e->d_labels to
+    // n_rows) and a thin kernel scatters them
+    const bool scatter = route == 3 && out.n_peers > 0;
+    uml::MlpTcLaunch own = out;
+    if (scatter) own.labels = e->d_labels.p[0];
+    {
+      NvtxRange r_score(route == 5 ? "uml:mlp_score_tc" : "uml:mlp_score_ffma");
+      if (route == 5) UML_CUDA(e, uml::launch_mlp_tc(map, m, out, exact, fl, sm, s));
+      else UML_CUDA(e, uml::launch_mlp_tma(map, m, x, out.n_rows, own.labels, exact, fl, sm, s));
+      *launches += 1;
+      if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
+    }
+    if (exact) {
+      NvtxRange r_rescore("uml:mlp_rescore_f64");
+      UML_CUDA(e, uml::launch_mlp_rescore_f64(m, x, ld, out.n_rows, own, fl, false, sm, s));
+      *launches += 1;
+    }
+    if (scatter) {
+      UML_CUDA(e, uml::launch_labels_scatter(own.labels, out.n_rows, out.peers, out.n_peers, out.wire_u8, out.row_offset,
+                                             sm, s));
+      *launches += 1;
+    }
+  }
+  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], s));
+  return UML_OK;
+}
+
 static int finish_stats(uml_engine* e, uml_stats* stats, int64_t n_rows, int launches, int path, bool timed,
                         bool kernel_events = true) {
   // counters -> pinned mirror, then synchronise and report
@@ -1034,86 +1073,90 @@ static int finish_stats(uml_engine* e, uml_stats* stats, int64_t n_rows, int lau
   return UML_OK;
 }
 
-static int predict_common(uml_engine* e, const uml_model* m, const uml_batch* b, int32_t* labels_out,
-                          int labels_on_device, void* const* peers, int n_peers, int64_t row_offset, int label_bytes,
-                          int mode, uml_stats* stats) {
-  if (!e || !m || !b) return UML_ERR_INVALID;
+// One predict call on a resident batch, linear or MLP.  `model` names the model in the feature-count message
+// ("estimator" as scikit-learn words it, "module" as the torch app does).  prepare() makes the model's host-side
+// choices before the first timed stream operation; score(labels, timed, &launches, &path) enqueues its scoring step.
+// labels: host-label scratch or the caller's device vector; nullptr with peers, which each model's step serves.
+extern "C++" {  // a template cannot have the C linkage of the ABI section around it
+template <class Prepare, class Score>
+static int predict_resident(uml_engine* e, const uml_batch* b, int n_classes, int n_features, const char* model,
+                            int32_t* labels_out, int labels_on_device, int n_peers, int label_bytes, int mode,
+                            uml_stats* stats, Prepare&& prepare, Score&& score) {
+  if (!e || !b) return UML_ERR_INVALID;
   if (!labels_out && b->n_rows > 0 && n_peers == 0) return UML_ERR_INVALID;
   if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
   if (n_peers < 0 || n_peers > 8) UML_FAIL(e, UML_ERR_INVALID, "n_peers %d (max 8)", n_peers);
   if (n_peers > 0 && label_bytes != 1 && label_bytes != 4) UML_FAIL(e, UML_ERR_INVALID, "label_bytes %d", label_bytes);
-  if (n_peers > 0 && label_bytes == 1 && m->dm.n_classes > 256)
-    UML_FAIL(e, UML_ERR_UNSUPPORTED, "byte labels need n_classes <= 256 (model has %d)", m->dm.n_classes);
-  if (b->n_features != m->n_features_in)
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the estimator is expecting %d features as input.",
-             b->n_features, m->n_features_in);
+  if (n_peers > 0 && label_bytes == 1 && n_classes > 256)
+    UML_FAIL(e, UML_ERR_UNSUPPORTED, "byte labels need n_classes <= 256 (model has %d)", n_classes);
+  if (b->n_features != n_features)
+    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the %s is expecting %d features as input.", b->n_features, model,
+             n_features);
   UML_CUDA(e, cudaSetDevice(e->device));
   (void)cudaGetLastError();
   if (stats) memset(stats, 0, sizeof(*stats));
   if (b->n_rows == 0) return UML_OK;
-  const bool exact = mode == UML_PREDICT_EXACT;
   const bool timed = stats != nullptr;
+  const bool sync_call = stats || !labels_on_device;
   int rc;
-  if (exact && (rc = ensure_flags(e, b->n_rows)) != UML_OK) return rc;
+  if (mode == UML_PREDICT_EXACT && (rc = grow(e, e->d_flag_rows, b->n_rows)) != UML_OK) return rc;
+  if ((rc = prepare()) != UML_OK) return rc;
   int32_t* d_labels = labels_out;
-  const bool wire_u8 = n_peers > 0 && label_bytes == 1;
-  if (!labels_out && n_peers > 0 && !wire_u8) {
-    // fused exchange: entry 0 is this rank's own full-length vector -> it is the local label target
-    d_labels = static_cast<int32_t*>(peers[0]) + row_offset;
-    peers += 1;
-    n_peers -= 1;
-  } else if (!labels_out && wire_u8) {
-    d_labels = nullptr;  // byte vectors everywhere (own vector included among the peers); no int32 copy kept
-  } else if (!labels_on_device || !labels_out) {
-    if ((rc = ensure_labels(e, b->n_rows)) != UML_OK) return rc;
-    d_labels = e->d_labels;
+  if (!labels_on_device) {
+    if ((rc = grow(e, e->d_labels, b->n_rows)) != UML_OK) return rc;
+    d_labels = e->d_labels.p[0];
   }
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
-  if (stats || !labels_on_device) {
-    // synchronous call: the counters are read back at the end, start them from zero.  The asynchronous step (device
-    // labels, no stats) needs no memset at all: the flag list is handed back empty by the previous re-score kernel.
-    UML_CUDA(e, cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), e->stream));
-    UML_CUDA(e, cudaMemsetAsync(e->d_flag_count, 0, sizeof(int), e->stream));
-  }
-  LinearLaunch l{};
-  l.x = b->x;
-  l.x64 = b->x64;
-  l.ld = b->ld;
-  l.ld64 = b->ld64;
-  l.n_rows = b->n_rows;
-  l.labels = d_labels;
-  l.n_peers = n_peers;
-  l.wire_u8 = wire_u8 ? 1 : 0;
-  for (int i = 0; i < n_peers; ++i) l.peers[i] = peers[i];
-  l.row_offset = row_offset;
+  // The asynchronous step (device labels, no stats) needs no memset at all: the flag list is handed back empty by the
+  // previous re-score kernel.
+  if (sync_call) UML_CUDA(e, reset_counters(e, e->stream));
   int launches = 0, path = 0;
-  rc = enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, mode, timed, &launches, &path);
-  if (rc != UML_OK) return rc;
-  int64_t d2h = 0;
-  if (!labels_on_device && labels_out) {
+  if ((rc = score(d_labels, timed, &launches, &path)) != UML_OK) return rc;
+  if (!sync_call) return UML_OK;
+  if (!labels_on_device)
     UML_CUDA(e, cudaMemcpyAsync(labels_out, d_labels, (size_t)b->n_rows * 4, cudaMemcpyDeviceToHost, e->stream));
-    d2h = b->n_rows * 4;
-  }
-  if (stats || !labels_on_device) {
-    rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
-    if (stats) {
-      stats->d2h_bytes = d2h;
-    }
-    return rc;
-  }
-  return UML_OK;
+  rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
+  if (stats) stats->d2h_bytes = labels_on_device ? 0 : b->n_rows * 4;
+  return rc;
+}
+}  // extern "C++"
+
+static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_batch* b, int32_t* labels_out,
+                                   int labels_on_device, void* const* peers, int n_peers, int64_t row_offset,
+                                   int label_bytes, int mode, uml_stats* stats) {
+  if (!m) return UML_ERR_INVALID;
+  auto score = [&](int32_t* labels, bool timed, int* launches, int* path) {
+    LinearLaunch l{};
+    l.x = b->x;
+    l.x64 = b->x64;
+    l.ld = b->ld;
+    l.ld64 = b->ld64;
+    l.n_rows = b->n_rows;
+    l.labels = labels;
+    l.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
+    l.row_offset = row_offset;
+    // fused int32 exchange: entry 0 is this rank's own full-length vector, the local label target.  Byte vectors are
+    // all peers (own vector included); no int32 copy is kept.
+    const int own = n_peers > 0 && !l.wire_u8 ? 1 : 0;
+    if (own) l.labels = static_cast<int32_t*>(peers[0]) + row_offset;
+    l.n_peers = n_peers - own;
+    for (int i = 0; i < l.n_peers; ++i) l.peers[i] = peers[own + i];
+    return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, mode, timed, launches, path);
+  };
+  return predict_resident(e, b, m->dm.n_classes, m->n_features_in, "estimator", labels_out, labels_on_device, n_peers,
+                          label_bytes, mode, stats, [] { return (int)UML_OK; }, score);
 }
 
 int uml_linear_predict(uml_engine* e, const uml_model* m, const uml_batch* b, int32_t* labels_out,
                        int labels_on_device, int mode, uml_stats* stats) {
-  return predict_common(e, m, b, labels_out, labels_on_device, nullptr, 0, 0, 4, mode, stats);
+  return linear_predict_resident(e, m, b, labels_out, labels_on_device, nullptr, 0, 0, 4, mode, stats);
 }
 
 int uml_linear_predict_peers(uml_engine* e, const uml_model* m, const uml_batch* b, void* const* peer_labels,
                              int n_peers, int64_t row_offset, int label_bytes, int mode, uml_stats* stats) {
   if (!peer_labels || n_peers < 1) return UML_ERR_INVALID;
   // peer_labels[0] must be this rank's own vector (local target); labels land at peer_labels[i] + row_offset for all i
-  return predict_common(e, m, b, nullptr, 1, peer_labels, n_peers, row_offset, label_bytes, mode, stats);
+  return linear_predict_resident(e, m, b, nullptr, 1, peer_labels, n_peers, row_offset, label_bytes, mode, stats);
 }
 
 // labels (device, int32 or uint8 indices) -> classes_[idx] as float64 in HOST memory: the device-side classes_.take of
@@ -1373,54 +1416,22 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   // pageable sources of any size worth the trouble go through pinned bounce buffers filled by the copy pool
   const bool bounce = want_bounce(host_ptr, n_rows * row_bytes);
 
-  if (!direct && (rc = ensure_chunks(e, chunk_rows * row_bytes)) != UML_OK) return rc;
-  if (e->xchunk_cap < chunk_rows * ld) {
-    for (auto& p : e->d_xchunk) {
-      cudaFree(p);
-      p = nullptr;
-    }
-    e->xchunk_cap = 0;
-    for (auto& p : e->d_xchunk) UML_CUDA(e, cudaMalloc((void**)&p, (size_t)chunk_rows * ld * 4));
-    e->xchunk_cap = chunk_rows * ld;
-  }
+  if (!direct && (rc = grow(e, e->d_chunk, chunk_rows * row_bytes)) != UML_OK) return rc;
+  if ((rc = grow(e, e->d_xchunk, chunk_rows * ld)) != UML_OK) return rc;
   // bytes of one row as it travels: `direct` rows keep their padding up to ld
   const int64_t wire_row_bytes = direct ? ld * 4 : row_bytes;
-  if (bounce && (rc = ensure_bounce(e, chunk_rows * wire_row_bytes)) != UML_OK) return rc;
-  if (values_out) {
-    if (e->vchunk_cap < chunk_rows) {
-      for (auto& p : e->d_vchunk) {
-        cudaFree(p);
-        p = nullptr;
-      }
-      e->vchunk_cap = 0;
-      for (auto& p : e->d_vchunk) UML_CUDA(e, cudaMalloc((void**)&p, (size_t)chunk_rows * 8));
-      e->vchunk_cap = chunk_rows;
-    }
-    if (e->classes_cap < n_classes) {
-      cudaFree(e->d_classes);
-      e->d_classes = nullptr;
-      e->classes_cap = 0;
-      UML_CUDA(e, cudaMalloc((void**)&e->d_classes, (size_t)n_classes * 8));
-      e->classes_cap = n_classes;
-    }
-  }
-  if ((rc = ensure_labels(e, 3 * chunk_rows)) != UML_OK) return rc;
-  if (exact && (rc = ensure_flags(e, chunk_rows)) != UML_OK) return rc;
+  if (bounce && (rc = grow_bounce(e, chunk_rows * wire_row_bytes)) != UML_OK) return rc;
+  if (values_out && (rc = grow(e, e->d_vchunk, chunk_rows)) != UML_OK) return rc;
+  if (values_out && (rc = grow(e, e->d_classes, n_classes)) != UML_OK) return rc;
+  if ((rc = grow(e, e->d_labels, 3 * chunk_rows)) != UML_OK) return rc;
+  if (exact && (rc = grow(e, e->d_flag_rows, chunk_rows)) != UML_OK) return rc;
   // A device-to-host copy into PAGEABLE memory blocks the calling thread until the chunk's whole pipeline has drained,
   // which would serialise gather / H2D / scoring.  Pageable outputs therefore land in pinned slots first and are
   // copied out by the host when the slot comes round again (three chunks later) or at the end.
   // (the asynchronous variant always does: the flush is also where a finished prefix is published to the poller)
   const bool result_bounce = progress != nullptr || (labels_out && !host_ptr_is_pinned(labels_out)) ||
                              (values_out && !host_ptr_is_pinned(values_out));
-  if (result_bounce && e->result_cap < chunk_rows * 12) {
-    for (auto& p : e->h_result) {
-      if (p) cudaFreeHost(p);
-      p = nullptr;
-    }
-    e->result_cap = 0;
-    for (auto& p : e->h_result) UML_CUDA(e, cudaHostAlloc(&p, (size_t)(chunk_rows * 12), cudaHostAllocDefault));
-    e->result_cap = chunk_rows * 12;
-  }
+  if (result_bounce && (rc = grow(e, e->h_result, chunk_rows * 12)) != UML_OK) return rc;
   struct Pending {
     int64_t r0 = 0, rows = 0;
     bool live = false;
@@ -1429,7 +1440,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     if (!pending[sl].live) return cudaSuccess;
     cudaError_t fe = cudaEventSynchronize(e->chunk_ev[3 + sl]);  // recorded after the slot's D2H copies
     if (fe != cudaSuccess) return fe;
-    const char* base = (const char*)e->h_result[sl];
+    const char* base = e->h_result.p[sl];
     if (values_out) memcpy(values_out + pending[sl].r0, base, (size_t)pending[sl].rows * 8);
     if (labels_out) memcpy(labels_out + pending[sl].r0, base + (size_t)chunk_rows * 8, (size_t)pending[sl].rows * 4);
     pending[sl].live = false;
@@ -1437,41 +1448,23 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     return cudaSuccess;
   };
 
-  // MLP: tensor cores when the features look like tf32 values (a host-side sample of the first rows decides; rows that
-  // are not are caught in the kernel and re-scored, so a wrong guess costs time, never labels), CUDA cores otherwise
-  bool mlp_tc = false, mlp_ffma = false;
-  if (mlp) {
-    std::string why;
-    mlp_tc = uml::mlp_tc_supported(mlp->dm, &why);
-    if (mlp_tc) {
-      const char* env = getenv("UML_B200_MLP_TC");
-      if (env && env[0] == '0') mlp_tc = false;
-      else if (!(env && env[0] == '1')) mlp_tc = host_sample_is_tf32(host_ptr, L, n_rows, F, src_dtype);
-    }
-    mlp_ffma = !mlp_tc && uml::mlp_tma_supported(mlp->dm, &why);
-  }
+  // MLP: the tensor cores' tf32 question is answered by a host-side sample of the first rows (rows that are not tf32
+  // values are caught in the kernel and re-scored, so a wrong guess costs time, never labels); taken once
+  int sample_tf32 = -1;
+  auto tf32 = [&] {
+    if (sample_tf32 < 0) sample_tf32 = host_sample_is_tf32(host_ptr, L, n_rows, F, src_dtype) ? 1 : 0;
+    return sample_tf32 == 1;
+  };
 
   const bool timed = stats != nullptr;
   cudaStream_t cs = e->stream;
-  // errors inside the pipeline: both streams must be idle before returning - async copies still reference the
-  // caller's host_ptr / labels_out
-#define HOST_CUDA(CALL)                                                          \
-  do {                                                                           \
-    cudaError_t _e3 = (CALL);                                                    \
-    if (_e3 != cudaSuccess) {                                                    \
-      cudaStreamSynchronize(cs);                                                 \
-      cudaStreamSynchronize(e->copy_stream);                                     \
-      UML_FAIL(e, _e3 == cudaErrorMemoryAllocation ? UML_ERR_NOMEM : UML_ERR_CUDA, "%s failed: %s", #CALL, \
-               cudaGetErrorString(_e3));                                         \
-    }                                                                            \
-  } while (0)
-  if (timed) HOST_CUDA(cudaEventRecord(e->ev[0], cs));
-  HOST_CUDA(cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), cs));
-  HOST_CUDA(cudaMemsetAsync(e->d_flag_count, 0, sizeof(int), cs));
-  HOST_CUDA(cudaMemsetAsync(e->d_stage, 0, sizeof(StageResult), cs));
-  if (values_out) HOST_CUDA(cudaMemcpyAsync(e->d_classes, classes, (size_t)n_classes * 8, cudaMemcpyHostToDevice, cs));
-  HOST_CUDA(cudaEventRecord(e->chunk_ev[6], cs));
-  HOST_CUDA(cudaStreamWaitEvent(e->copy_stream, e->chunk_ev[6], 0));
+  if (timed) UML_CUDA_DRAIN(e, cudaEventRecord(e->ev[0], cs));
+  UML_CUDA_DRAIN(e, reset_counters(e, cs));
+  UML_CUDA_DRAIN(e, cudaMemsetAsync(e->d_stage, 0, sizeof(StageResult), cs));
+  if (values_out)
+    UML_CUDA_DRAIN(e, cudaMemcpyAsync(e->d_classes.p[0], classes, (size_t)n_classes * 8, cudaMemcpyHostToDevice, cs));
+  UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[6], cs));
+  UML_CUDA_DRAIN(e, cudaStreamWaitEvent(e->copy_stream, e->chunk_ev[6], 0));
   int launches = 0, path = 0;
   int64_t h2d = 0, d2h = 0;
   bool used[3] = {false, false, false};
@@ -1496,20 +1489,21 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       for (auto& ev : row) cudaEventCreate(&ev);
   for (int64_t r0 = 0; r0 < n_rows; r0 += chunk_rows, slot = (slot + 1) % 3) {
     const int64_t rows = std::min(chunk_rows, n_rows - r0);
-    float* xc = e->d_xchunk[slot];
-    void* raw = direct ? (void*)xc : e->d_chunk[slot];
+    float* xc = e->d_xchunk.p[slot];
+    void* raw = direct ? (void*)xc : e->d_chunk.p[slot];
     const int tli = (prof && tl_n < kTl) ? tl_n++ : -1;
     bool chunk_narrow = false;  // this chunk crossed PCIe as fp32 (lossless float64 source)
     // (1) H2D on the copy stream, once the previous user of this slot has finished scoring (the re-score reads the
     //     raw chunk, so that includes it)
-    if (used[slot]) HOST_CUDA(cudaStreamWaitEvent(e->copy_stream, e->chunk_ev[3 + slot], 0));
-    if (result_bounce) HOST_CUDA(flush_slot(slot));
+    if (used[slot]) UML_CUDA_DRAIN(e, cudaStreamWaitEvent(e->copy_stream, e->chunk_ev[3 + slot], 0));
+    if (result_bounce) UML_CUDA_DRAIN(e, flush_slot(slot));
     if (tli >= 0) cudaEventRecord(tl[tli][0], e->copy_stream);
     {
       NvtxRange r_h2d("uml:h2d");
       if (bounce) {
         auto t0 = now();
-        if (used[slot]) HOST_CUDA(cudaEventSynchronize(e->chunk_ev[slot]));  // the slot's previous H2D has left the bounce buffer
+        // the slot's previous H2D has left the bounce buffer
+        if (used[slot]) UML_CUDA_DRAIN(e, cudaEventSynchronize(e->chunk_ev[slot]));
         auto t1 = now();
         t_wait += secs(t0, t1);
         if (direct) {  // already the resident layout (padding included): one contiguous run
@@ -1517,7 +1511,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
           const char* src0 = (const char*)host_ptr + (size_t)r0 * ld * 4;
           const size_t total = (size_t)rows * ld * 4, piece = 1u << 20;
           for (size_t o = 0; o < total; o += piece)
-            tasks.push_back({(char*)e->h_bounce[slot] + o, src0 + o, std::min(piece, total - o)});
+            tasks.push_back({e->h_bounce.p[slot] + o, src0 + o, std::min(piece, total - o)});
         }
         auto t2 = now();
         if (direct) {
@@ -1529,7 +1523,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
           chunk_narrow = wire_f32;
           if (chunk_narrow) {
             std::atomic<int> lossy{0};
-            build_gather_tasks(tasks, (char*)e->h_bounce[slot], host_ptr, L, r0, rows, F, &lossy);
+            build_gather_tasks(tasks, e->h_bounce.p[slot], host_ptr, L, r0, rows, F, &lossy);
             e->pool->run(tasks);
             if (lossy.load()) {
               wire_f32 = false;
@@ -1537,35 +1531,37 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
             }
           }
           if (!chunk_narrow) {
-            build_gather_tasks(tasks, (char*)e->h_bounce[slot], host_ptr, L, r0, rows, F);
+            build_gather_tasks(tasks, e->h_bounce.p[slot], host_ptr, L, r0, rows, F);
             e->pool->run(tasks);
           }
         }
         auto t3 = now();
         t_gather += secs(t2, t3);
-        HOST_CUDA(cudaMemcpyAsync(raw, e->h_bounce[slot], (size_t)(rows * (chunk_narrow ? wire_row_bytes / 2 : wire_row_bytes)),
-                                  cudaMemcpyHostToDevice, e->copy_stream));
+        UML_CUDA_DRAIN(e, cudaMemcpyAsync(raw, e->h_bounce.p[slot],
+                                          (size_t)(rows * (chunk_narrow ? wire_row_bytes / 2 : wire_row_bytes)),
+                                          cudaMemcpyHostToDevice, e->copy_stream));
         t_enqueue += secs(t3, now());
       } else if (direct) {
-        HOST_CUDA(cudaMemcpyAsync(xc, (const char*)host_ptr + (size_t)r0 * ld * 4, (size_t)rows * ld * 4,
-                                  cudaMemcpyHostToDevice, e->copy_stream));
+        UML_CUDA_DRAIN(e, cudaMemcpyAsync(xc, (const char*)host_ptr + (size_t)r0 * ld * 4, (size_t)rows * ld * 4,
+                                          cudaMemcpyHostToDevice, e->copy_stream));
       } else {
-        HOST_CUDA(copy_chunk_h2d(raw, host_ptr, L, r0, rows, F, e->copy_stream));
+        UML_CUDA_DRAIN(e, copy_chunk_h2d(raw, host_ptr, L, r0, rows, F, e->copy_stream));
       }
     }
     h2d += rows * (chunk_narrow ? wire_row_bytes / 2 : wire_row_bytes);
     if (tli >= 0) cudaEventRecord(tl[tli][1], e->copy_stream);
-    HOST_CUDA(cudaEventRecord(e->chunk_ev[slot], e->copy_stream));
-    HOST_CUDA(cudaStreamWaitEvent(cs, e->chunk_ev[slot], 0));
+    UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[slot], e->copy_stream));
+    UML_CUDA_DRAIN(e, cudaStreamWaitEvent(cs, e->chunk_ev[slot], 0));
     if (tli >= 0) cudaEventRecord(tl[tli][2], cs);
     // (2) transpose / down-cast (+ finiteness) on the compute stream
     if (!direct) {
       NvtxRange r_stage("uml:stage_convert");
-      HOST_CUDA(uml::launch_stage_convert(raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major,
-                                          L.feature_major ? rows : F, rows, F, xc, ld, nullptr, 0, e->d_stage, true, cs));
+      UML_CUDA_DRAIN(e, uml::launch_stage_convert(raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major,
+                                                  L.feature_major ? rows : F, rows, F, xc, ld, nullptr, 0, e->d_stage,
+                                                  true, cs));
       launches += 1;
     } else if (!exact) {
-      HOST_CUDA(uml::launch_finite_scan(xc, ld, rows, F, e->d_stage, cs));
+      UML_CUDA_DRAIN(e, uml::launch_finite_scan(xc, ld, rows, F, e->d_stage, cs));
       launches += 1;
     }
     // (3) score
@@ -1575,7 +1571,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     l.x = xc;
     l.ld = ld;
     l.n_rows = rows;
-    l.labels = e->d_labels + (int64_t)slot * chunk_rows;
+    l.labels = e->d_labels.p[0] + (int64_t)slot * chunk_rows;
     if (!mlp && exact && !direct && !chunk_narrow && lossy_capable(src_dtype)) {  // (the reference MLP predictor casts to
       // float32; a chunk that travelled as fp32 was checked lossless on the host: its fp32 rows ARE the caller's values)
       // flagged rows are re-scored from the caller's own values (the raw chunk is still resident): float64 / int
@@ -1589,29 +1585,8 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       uml::MlpTcLaunch out{};
       out.n_rows = rows;
       out.labels = l.labels;
-      FlagList fl{e->d_flag_count, e->d_flag_rows, (int)std::min<int64_t>(e->flag_cap, INT32_MAX), e->d_counters};
-      if (mlp_tc && has_map) {
-        HOST_CUDA(uml::launch_mlp_tc(map, mlp->dm, out, exact, fl, e->info.sm_count, cs));
-        launches += 1;
-        path = 5;
-        if (exact) {
-          HOST_CUDA(uml::launch_mlp_rescore_f64(mlp->dm, xc, ld, rows, out, fl, false, e->info.sm_count, cs));
-          launches += 1;
-        }
-      } else if (mlp_ffma && has_map) {
-        HOST_CUDA(uml::launch_mlp_tma(map, mlp->dm, xc, rows, out.labels, exact, fl, e->info.sm_count, cs));
-        launches += 1;
-        path = 3;
-        if (exact) {
-          HOST_CUDA(uml::launch_mlp_rescore_f64(mlp->dm, xc, ld, rows, out, fl, false, e->info.sm_count, cs));
-          launches += 1;
-        }
-      } else {
-        HOST_CUDA(uml::launch_mlp_rescore_f64(mlp->dm, xc, ld, rows, out, fl, true, e->info.sm_count, cs));
-        launches += 1;
-        path = 2;
-      }
-      rc = UML_OK;
+      rc = enqueue_mlp(e, mlp->dm, map, xc, ld, out, exact, mlp_route(mlp->dm, has_map, false, tf32), false, &launches,
+                       &path);
     } else {
       rc = enqueue_predict(e, m, l, has_map ? &map : nullptr, mode, false, &launches, &path);
     }
@@ -1621,17 +1596,18 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       return rc;
     }
     // (4) labels (or class values) back
-    char* land = result_bounce ? (char*)e->h_result[slot] : nullptr;
+    char* land = result_bounce ? e->h_result.p[slot] : nullptr;
     if (values_out) {
-      HOST_CUDA(uml::launch_labels_take(l.labels, 4, rows, e->d_classes, n_classes, e->d_vchunk[slot], cs));
+      UML_CUDA_DRAIN(e, uml::launch_labels_take(l.labels, 4, rows, e->d_classes.p[0], n_classes, e->d_vchunk.p[slot],
+                                                cs));
       launches += 1;
-      HOST_CUDA(cudaMemcpyAsync(land ? (void*)land : (void*)(values_out + r0), e->d_vchunk[slot], (size_t)rows * 8,
-                                cudaMemcpyDeviceToHost, cs));
+      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)land : (void*)(values_out + r0), e->d_vchunk.p[slot],
+                                        (size_t)rows * 8, cudaMemcpyDeviceToHost, cs));
       d2h += rows * 8;
     }
     if (labels_out) {
-      HOST_CUDA(cudaMemcpyAsync(land ? (void*)(land + (size_t)chunk_rows * 8) : (void*)(labels_out + r0), l.labels,
-                                (size_t)rows * 4, cudaMemcpyDeviceToHost, cs));
+      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)(land + (size_t)chunk_rows * 8) : (void*)(labels_out + r0), l.labels,
+                                        (size_t)rows * 4, cudaMemcpyDeviceToHost, cs));
       d2h += rows * 4;
     }
     if (result_bounce) {
@@ -1640,11 +1616,10 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       pending[slot].live = true;
     }
     if (tli >= 0) cudaEventRecord(tl[tli][3], cs);
-    HOST_CUDA(cudaEventRecord(e->chunk_ev[3 + slot], cs));
+    UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[3 + slot], cs));
     used[slot] = true;
   }
-  HOST_CUDA(cudaMemcpyAsync(&e->h->stage, e->d_stage, sizeof(StageResult), cudaMemcpyDeviceToHost, cs));
-#undef HOST_CUDA
+  UML_CUDA_DRAIN(e, cudaMemcpyAsync(&e->h->stage, e->d_stage, sizeof(StageResult), cudaMemcpyDeviceToHost, cs));
   if (prof && tl_n > 0) {
     cudaStreamSynchronize(cs);
     cudaStreamSynchronize(e->copy_stream);
@@ -1927,126 +1902,39 @@ static int batch_tf32_exact(uml_engine* e, const uml_batch* b) {
   return b->tf32_exact;
 }
 
-static int mlp_predict_common(uml_engine* e, const uml_mlp* m, const uml_batch* b, int32_t* labels_out,
-                              int labels_on_device, void* const* peers, int n_peers, int64_t row_offset,
-                              int label_bytes, int mode, uml_stats* stats) {
-  if (!e || !m || !b) return UML_ERR_INVALID;
-  if (!labels_out && b->n_rows > 0 && n_peers == 0) return UML_ERR_INVALID;
-  if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
-  if (n_peers < 0 || n_peers > 8) UML_FAIL(e, UML_ERR_INVALID, "n_peers %d (max 8)", n_peers);
-  if (n_peers > 0 && label_bytes != 1 && label_bytes != 4) UML_FAIL(e, UML_ERR_INVALID, "label_bytes %d", label_bytes);
-  if (n_peers > 0 && label_bytes == 1 && m->dm.n_classes > 256)
-    UML_FAIL(e, UML_ERR_UNSUPPORTED, "byte labels need n_classes <= 256 (model has %d)", m->dm.n_classes);
-  if (b->n_features != m->dm.n_in)
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the module is expecting %d features as input.", b->n_features,
-             m->dm.n_in);
-  UML_CUDA(e, cudaSetDevice(e->device));
-  (void)cudaGetLastError();
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (b->n_rows == 0) return UML_OK;
-  const bool exact = mode == UML_PREDICT_EXACT;
-  const bool timed = stats != nullptr;
-  const bool sync_call = stats || (!labels_on_device && labels_out);
-  int rc;
-  if (exact && (rc = ensure_flags(e, b->n_rows)) != UML_OK) return rc;
-
-  // kernel choice: tensor cores when every feature is a tf32 value (integer / pixel domains), CUDA cores otherwise.
-  // UML_B200_MLP_TC=0 / 1 forces the choice (1: rows that are not tf32-exact are caught in the kernel and re-scored)
-  std::string why;
-  bool use_tc = b->has_map && uml::mlp_tc_supported(m->dm, &why);
-  if (use_tc) {
-    const char* env = getenv("UML_B200_MLP_TC");
-    if (env && env[0] == '0') use_tc = false;
-    else if (!(env && env[0] == '1')) use_tc = batch_tf32_exact(e, b) == 1;
-  }
-  const bool use_ffma = !use_tc && b->has_map && uml::mlp_tma_supported(m->dm, &why);
-
-  uml::MlpTcLaunch out{};
-  out.n_rows = b->n_rows;
-  out.row_offset = row_offset;
-  const bool wire_u8 = n_peers > 0 && label_bytes == 1;
-  out.wire_u8 = wire_u8 ? 1 : 0;
-  int32_t* d_labels = labels_out;
-  if (n_peers > 0) {
-    out.n_peers = n_peers;
+static int mlp_predict_resident(uml_engine* e, const uml_mlp* m, const uml_batch* b, int32_t* labels_out,
+                                int labels_on_device, void* const* peers, int n_peers, int64_t row_offset,
+                                int label_bytes, int mode, uml_stats* stats) {
+  if (!m) return UML_ERR_INVALID;
+  int route = 2;
+  auto prepare = [&] {
+    route = mlp_route(m->dm, b->has_map, false, [&] { return batch_tf32_exact(e, b) == 1; });
+    // scratch for the CUDA-core kernel's labels on their way to the peers (enqueue_mlp)
+    return route == 3 && n_peers > 0 ? grow(e, e->d_labels, b->n_rows) : (int)UML_OK;
+  };
+  auto score = [&](int32_t* labels, bool timed, int* launches, int* path) {
+    uml::MlpTcLaunch out{};
+    out.labels = labels;
+    out.n_rows = b->n_rows;
+    out.row_offset = row_offset;
+    out.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
+    out.n_peers = n_peers;  // every peer vector, this rank's own included
     for (int i = 0; i < n_peers; ++i) out.peers[i] = peers[i];
-    d_labels = nullptr;
-  } else if (!labels_on_device) {
-    if ((rc = ensure_labels(e, b->n_rows)) != UML_OK) return rc;
-    d_labels = e->d_labels;
-  }
-  out.labels = d_labels;
-  // the CUDA-core kernel has no peer stores: it writes int32 labels to scratch and a thin kernel scatters them
-  uml::MlpTcLaunch ffma_out = out;
-  if (use_ffma && n_peers > 0) {
-    if ((rc = ensure_labels(e, b->n_rows)) != UML_OK) return rc;
-    ffma_out.labels = e->d_labels;
-  }
-
-  FlagList fl{e->d_flag_count, e->d_flag_rows, (int)std::min<int64_t>(e->flag_cap, INT32_MAX), e->d_counters};
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
-  if (sync_call) {
-    UML_CUDA(e, cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), e->stream));
-    UML_CUDA(e, cudaMemsetAsync(e->d_flag_count, 0, sizeof(int), e->stream));
-  }
-  int launches = 0, path = 3;
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
-  if (use_tc) {
-    NvtxRange r_score("uml:mlp_score_tc");
-    UML_CUDA(e, uml::launch_mlp_tc(b->map, m->dm, out, exact, fl, e->info.sm_count, e->stream));
-    launches += 1;
-    path = 5;
-    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
-    if (exact) {
-      NvtxRange r_rescore("uml:mlp_rescore_f64");
-      UML_CUDA(e, uml::launch_mlp_rescore_f64(m->dm, b->x, b->ld, b->n_rows, out, fl, false, e->info.sm_count, e->stream));
-      launches += 1;
-    }
-  } else if (use_ffma) {
-    NvtxRange r_score("uml:mlp_score_ffma");
-    UML_CUDA(e, uml::launch_mlp_tma(b->map, m->dm, b->x, b->n_rows, ffma_out.labels, exact, fl, e->info.sm_count, e->stream));
-    launches += 1;
-    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
-    if (exact) {
-      UML_CUDA(e, uml::launch_mlp_rescore_f64(m->dm, b->x, b->ld, b->n_rows, ffma_out, fl, false, e->info.sm_count, e->stream));
-      launches += 1;
-    }
-    if (n_peers > 0) {
-      UML_CUDA(e, uml::launch_labels_scatter(e->d_labels, b->n_rows, out.peers, n_peers, out.wire_u8, row_offset,
-                                             e->info.sm_count, e->stream));
-      launches += 1;
-    }
-  } else {
-    NvtxRange r_score("uml:mlp_score_f64_generic");
-    UML_CUDA(e, uml::launch_mlp_rescore_f64(m->dm, b->x, b->ld, b->n_rows, out, fl, true, e->info.sm_count, e->stream));
-    launches += 1;
-    path = 2;
-    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
-  }
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
-  int64_t d2h = 0;
-  if (!labels_on_device && labels_out) {
-    UML_CUDA(e, cudaMemcpyAsync(labels_out, d_labels, (size_t)b->n_rows * 4, cudaMemcpyDeviceToHost, e->stream));
-    d2h = b->n_rows * 4;
-  }
-  if (sync_call) {
-    rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
-    if (stats) stats->d2h_bytes = d2h;
-    return rc;
-  }
-  return UML_OK;
+    return enqueue_mlp(e, m->dm, b->map, b->x, b->ld, out, mode == UML_PREDICT_EXACT, route, timed, launches, path);
+  };
+  return predict_resident(e, b, m->dm.n_classes, m->dm.n_in, "module", labels_out, labels_on_device, n_peers,
+                          label_bytes, mode, stats, prepare, score);
 }
 
 int uml_mlp_predict(uml_engine* e, const uml_mlp* m, const uml_batch* b, int32_t* labels_out, int labels_on_device,
                     int mode, uml_stats* stats) {
-  if (b && !labels_out && b->n_rows > 0) return UML_ERR_INVALID;
-  return mlp_predict_common(e, m, b, labels_out, labels_on_device, nullptr, 0, 0, 4, mode, stats);
+  return mlp_predict_resident(e, m, b, labels_out, labels_on_device, nullptr, 0, 0, 4, mode, stats);
 }
 
 int uml_mlp_predict_peers(uml_engine* e, const uml_mlp* m, const uml_batch* b, void* const* peer_labels, int n_peers,
                           int64_t row_offset, int label_bytes, int mode, uml_stats* stats) {
   if (!peer_labels || n_peers < 1) return UML_ERR_INVALID;
-  return mlp_predict_common(e, m, b, nullptr, 1, peer_labels, n_peers, row_offset, label_bytes, mode, stats);
+  return mlp_predict_resident(e, m, b, nullptr, 1, peer_labels, n_peers, row_offset, label_bytes, mode, stats);
 }
 
 int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, float* proba_out, int proba_on_device,
@@ -2060,21 +1948,13 @@ int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, f
   if (stats) memset(stats, 0, sizeof(*stats));
   if (b->n_rows == 0) return UML_OK;
   NvtxRange r_all("uml:mlp_proba");
-  // the labels' kernel choice, except that UML_B200_MLP_TC=1 does not send rows that are not tf32 values to the
-  // tensor cores: the probability kernels have no fp64 re-score behind them
-  std::string why;
-  bool use_tc = b->has_map && uml::mlp_tc_supported(m->dm, &why);
-  if (use_tc) {
-    const char* env = getenv("UML_B200_MLP_TC");
-    use_tc = !(env && env[0] == '0') && batch_tf32_exact(e, b) == 1;
-  }
-  const bool use_ffma = !use_tc && b->has_map && uml::mlp_tma_supported(m->dm, &why, true);
+  const int path = mlp_route(m->dm, b->has_map, true, [&] { return batch_tf32_exact(e, b) == 1; });
   const int64_t n_floats = b->n_rows * m->dm.n_classes;
   float* d_out = proba_out;
   int rc;
   if (!proba_on_device) {
-    if ((rc = ensure_proba(e, n_floats)) != UML_OK) return rc;
-    d_out = e->d_proba;
+    if ((rc = grow(e, e->d_proba, n_floats)) != UML_OK) return rc;
+    d_out = e->d_proba.p[0];
   }
   const bool timed = stats != nullptr;
   if (timed) {
@@ -2082,20 +1962,16 @@ int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, f
     UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
     UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
   }
-  int path;
-  if (use_tc) {
+  if (path == 5) {
     uml::MlpTcLaunch out{};
     out.n_rows = b->n_rows;
     out.proba = d_out;
     UML_CUDA(e, uml::launch_mlp_tc_proba(b->map, m->dm, out, e->info.sm_count, e->stream));
-    path = 5;
-  } else if (use_ffma) {
-    UML_CUDA(e, uml::launch_mlp_tma(b->map, m->dm, b->x, b->n_rows, nullptr, false, FlagList{}, e->info.sm_count, e->stream,
+  } else if (path == 3) {  // (no labels, so no flag list)
+    UML_CUDA(e, uml::launch_mlp_tma(b->map, m->dm, b->x, b->n_rows, nullptr, false, {}, e->info.sm_count, e->stream,
                                     d_out));
-    path = 3;
   } else {
     UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, b->x, b->ld, b->n_rows, d_out, e->info.sm_count, e->stream));
-    path = 2;
   }
   if (timed) {
     UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
