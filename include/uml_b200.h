@@ -75,7 +75,8 @@ typedef struct uml_stats {
   int32_t kernel_launches; /* kernels of this library launched by the call                                            */
   int32_t path;            /* 1 = TMA fp32 tile kernel, 2 = generic fp64 kernel, 3 = MLP CUDA-core kernel, 5 = MLP tensor-core
                               (wgmma) kernel, 4 = small-batch fp64 kernel of the online path, linear or MLP
-                              (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph)                 */
+                              (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph), 6 = float64
+                              decision_function scores kernel                                                             */
 } uml_stats;
 
 typedef struct uml_device_info {
@@ -184,6 +185,21 @@ UML_API int uml_async_finish(uml_engine* e, uml_stats* stats);
  * proba_out: n_rows x n_classes row-major fp32 (n_classes = 2 for a binary model), host or device memory. */
 UML_API int uml_linear_predict_proba(uml_engine* e, const uml_model* m, const uml_batch* b, float* proba_out,
                              int proba_on_device);
+/* scores of a resident batch: LinearClassifierMixin.decision_function (sklearn/linear_model/_base.py:366-396),
+ * X @ coef_.T + intercept_ in float64 from the caller's own values - the batch's float64 copy when it has one
+ * (UML_STAGE_KEEP_F64), else its fp32 rows, which must then be the caller's values (a lossy batch without the copy is
+ * UML_ERR_UNSUPPORTED).  scores_out: n_rows x n_classes row-major float64, or n_rows doubles (the score s) for a binary
+ * model, host or device memory (8-byte aligned).  Every score is within ((F + 3) 2^-53 + fold) a_c + (F + 3) 2^-1074 of
+ * the exact score (DESIGN.md 3.7); finite features whose scores overflow give inf / NaN as numpy does, NaN / Inf
+ * features give UML_ERR_NONFINITE.  Synchronous; stats (optional): path 6, kernel_ms, d2h_bytes. */
+UML_API int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_batch* b, double* scores_out,
+                                         int scores_on_device, uml_stats* stats);
+/* the same scores from HOST rows of any layout and dtype uml_linear_predict_host takes, through its chunk pipeline
+ * (pinned bounce buffers, lossless float64 -> fp32 narrowing on the gather threads, the raw chunk scored on the device,
+ * pageable scores_out through pinned result slots); batches of <= 64 rows take the pipeline too. */
+UML_API int uml_linear_decision_function_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows,
+                                              int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes,
+                                              int src_dtype, double* scores_out, int64_t chunk_rows, uml_stats* stats);
 
 /* ---- 2-layer MLP predictor (tests/integration/pytorch_app/quickstart.py:14-24,68-70) -------------------------- */
 /* w1: hidden x in, b1: hidden, w2: out x hidden, b2: out (torch nn.Linear layout, fp32).  Labels = argmax of

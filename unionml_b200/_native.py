@@ -96,6 +96,11 @@ SIGNATURES = {
     "uml_async_poll": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
     "uml_async_finish": (C.c_int, [_P, C.POINTER(Stats)]),
     "uml_linear_predict_proba": (C.c_int, [_P, _P, _P, _P, C.c_int]),
+    "uml_linear_decision_function": (C.c_int, [_P, _P, _P, _P, C.c_int, C.POINTER(Stats)]),
+    "uml_linear_decision_function_host": (
+        C.c_int,
+        [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, _P, C.c_int64, C.POINTER(Stats)],
+    ),
     "uml_mlp_load": (C.c_int, [_P, _PP, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int]),
     "uml_mlp_free": (None, [_P]),
     "uml_mlp_predict": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.POINTER(Stats)]),

@@ -170,6 +170,12 @@ cudaError_t launch_linear_small(const LinearDeviceModel& m, const SrcView& src, 
 // (sigmoid for the binary layout), fp32 scores and exp; proba[n_rows][n_classes] row-major fp32
 cudaError_t launch_linear_proba(const LinearDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, float* proba,
                                 int sm_count, cudaStream_t stream);
+// float64 decision_function scores (LinearClassifierMixin.decision_function, sklearn/linear_model/_base.py:366-396) of
+// every row of `src` (linear_scores.cu): out[n_rows][linear_scores_width(m)] row-major, one sequential fp64 FMA chain
+// per class plus the bias (DESIGN.md 3.7); rows with NaN / Inf features are counted into *nonfinite
+inline int linear_scores_width(const LinearDeviceModel& m) { return m.binary ? 1 : m.n_classes; }
+cudaError_t launch_linear_scores_f64(const LinearDeviceModel& m, const SrcView& src, int64_t n_rows, double* out,
+                                     unsigned long long* nonfinite, int sm_count, cudaStream_t stream);
 
 // 2-layer MLP (mlp_kernels.cu, mlp_tc_kernels.cu)
 struct MlpHostModel {  // the caller's fp32 weights, torch nn.Linear layout

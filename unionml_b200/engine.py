@@ -80,12 +80,15 @@ def as_feature_array(features: Any) -> np.ndarray:
 class LinearModel:
     """``coef_``/``intercept_`` of a linear classifier resident on the device (fp32 tile operands + fp64 copy)."""
 
-    def __init__(self, engine: "Engine", handle: int, n_features: int, n_classes: int, classes: Optional[np.ndarray]):
+    def __init__(self, engine: "Engine", handle: int, n_features: int, n_classes: int, classes: Optional[np.ndarray],
+                 binary: bool = False):
         self.engine = engine
         self._h = handle
         self.n_features = n_features
         self.n_classes = n_classes
         self.classes = classes
+        #: one coef_ row (sklearn's binary layout): decision_function returns one score per row
+        self.binary = binary
         # numeric class labels as float64, ready for the device-side classes_.take (None for string labels)
         self.classes_f64 = None
         if classes is not None and np.asarray(classes).dtype.kind in "iufb":
@@ -240,7 +243,8 @@ class Engine:
                 N.UML_F32 if dt == np.float32 else N.UML_F64,
             )
             self._check(st)
-        return LinearModel(self, h.value, n_features, max(n_classes, 2), None if classes is None else np.asarray(classes))
+        return LinearModel(self, h.value, n_features, max(n_classes, 2), None if classes is None else np.asarray(classes),
+                           binary=n_classes == 1)
 
     def load_mlp(self, w1, b1, w2, b2) -> MlpModel:
         """``torch.nn.Linear`` layout: ``w1`` (hidden, in), ``b1`` (hidden), ``w2`` (out, hidden), ``b2`` (out); fp32."""
@@ -570,6 +574,59 @@ class Engine:
             out = np.empty((batch.n_rows, model.n_classes), dtype=np.float32)
             self._check(N.lib().uml_linear_predict_proba(self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0))
         return out
+
+    @staticmethod
+    def _scores_shape(model: LinearModel, n_rows: int) -> tuple:
+        return (n_rows,) if model.binary else (n_rows, model.n_classes)
+
+    def decision_function(self, model: LinearModel, batch: Batch, out_device_ptr: Optional[int] = None,
+                          want_stats: bool = False) -> Tuple[Optional[np.ndarray], Optional[dict]]:
+        """``X @ coef_.T + intercept_`` per row in float64 (``LinearClassifierMixin.decision_function``): ``(n_rows,)``
+        for a binary model, else ``(n_rows, n_classes)``.  Scored from the batch's float64 copy when it has one
+        (``stage(keep_f64=True)``), else from its fp32 rows, which must then be the caller's values.  With
+        ``out_device_ptr`` (8-byte aligned) the scores are written there and ``None`` is returned."""
+        stats = N.Stats() if want_stats else None
+        with self._lock:
+            if out_device_ptr is not None:
+                st = N.lib().uml_linear_decision_function(
+                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, C.byref(stats) if stats else None
+                )
+                self._check(st)
+                return None, stats.as_dict() if stats else None
+            out = np.empty(self._scores_shape(model, batch.n_rows), dtype=np.float64)
+            st = N.lib().uml_linear_decision_function(
+                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, C.byref(stats) if stats else None
+            )
+            self._check(st)
+        return out, stats.as_dict() if stats else None
+
+    def decision_function_host(self, model: LinearModel, features: Any, chunk_rows: int = 0,
+                               out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, dict]:
+        """Host rows (any order, f32/f64/int) -> float64 scores through the chunk pipeline of :meth:`predict_host`,
+        from the caller's own values; shapes as :meth:`decision_function`."""
+        arr = as_feature_array(features)
+        shape = self._scores_shape(model, arr.shape[0])
+        if out is None:
+            out = np.empty(shape, dtype=np.float64)
+        elif out.dtype != np.float64 or out.shape != shape or not out.flags.c_contiguous:
+            raise ValueError(f"out must be a C-contiguous float64 array of shape {shape}")
+        stats = N.Stats()
+        with self._lock:
+            st = N.lib().uml_linear_decision_function_host(
+                self._h,
+                model._h,
+                C.c_void_p(arr.ctypes.data),
+                arr.shape[0],
+                arr.shape[1],
+                arr.strides[0],
+                arr.strides[1],
+                _DTYPES[arr.dtype],
+                out.ctypes.data_as(C.c_void_p),
+                chunk_rows,
+                C.byref(stats),
+            )
+            self._check(st)
+        return out, stats.as_dict()
 
 
 _default_engine: Optional[Engine] = None

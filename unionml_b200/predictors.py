@@ -284,6 +284,23 @@ def linear_predict_proba(estimator: Any, features: Any) -> np.ndarray:
         batch.free()
 
 
+def linear_decision_function(estimator: Any, features: Any) -> np.ndarray:
+    """``estimator.decision_function(features)`` on the GPU (``sklearn/linear_model/_base.py:366-396``,
+    ``X @ coef_.T + intercept_``): float64, shape ``(n,)`` for a binary model and ``(n, n_classes)`` otherwise.  The
+    confidence of classifiers without ``predict_proba`` (``LinearSVC``, ``RidgeClassifier``, ``Perceptron``,
+    ``SGDClassifier(loss="hinge")``).  Computed in float64 from the caller's own values through the chunk pipeline;
+    every score is within ``((F + 3)·2⁻⁵³ + fold)·a_c + (F + 3)·2⁻¹⁰⁷⁴`` of the exact score of those values
+    (``a_c = Σ_f |x_f w_cf| + |b_c|``, DESIGN.md §3.7), not bit-equal to a BLAS.  The guards of :func:`linear_argmax`
+    apply (fitted, classifier with dense ``coef_``, feature names, non-empty batch, NaN / Inf -> ``ValueError``)."""
+    engine = get_engine()
+    dm = device_model(estimator, engine)
+    _check_feature_names(estimator, features)
+    _check_min_samples(features)
+    scores, stats = engine.decision_function_host(dm, features)
+    _note_ambiguous(stats)
+    return scores
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # PyTorch 2-layer MLP predictor (reference: tests/integration/pytorch_app/quickstart.py:14-24, 31-32, 68-70)
 # ---------------------------------------------------------------------------------------------------------------
