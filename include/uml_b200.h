@@ -214,6 +214,21 @@ UML_API int uml_mlp_predict(uml_engine* e, const uml_mlp* m, const uml_batch* b,
  * stats (optional): path 5 / 3 / 2 as for uml_mlp_predict, kernel_ms, kernel_launches. */
 UML_API int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, float* proba_out,
                                   int proba_on_device, uml_stats* stats);
+/* the k most probable classes of every row and their probabilities: `values, indices = torch.topk(softmax(module(x)),
+ * k)` of the quickdraw template's predictor (unionml/templates/quickdraw/.../app.py:62-71).  idx_out: n_rows x k int32
+ * class indices in descending order of the logits, ties to the lower index (column 0 is uml_mlp_predict's label in the
+ * same mode); proba_out (may be NULL): n_rows x k fp32, bit-equal to uml_mlp_predict_proba's value at that index on
+ * the same route, except for rows re-scored in float64 (float64 softmax, rounded once).  Both host or both device
+ * memory (out_on_device).  UML_PREDICT_EXACT: the indices are those of the float64 network - rows whose top k + 1
+ * logits are not separated by the fp32 error bound are re-scored in float64 (stats n_flagged, DESIGN.md 3.8).  Routed
+ * as uml_mlp_predict; k > 5 takes the float64 kernel (path 2) for every row.  1 <= k <= n_out, else UML_ERR_INVALID. */
+UML_API int uml_mlp_predict_topk(uml_engine* e, const uml_mlp* m, const uml_batch* b, int k, int32_t* idx_out,
+                                 float* proba_out, int out_on_device, int mode, uml_stats* stats);
+/* top-k hit counts of the quickdraw template's accuracy(output, target, topk) (quickdraw/model.py:20-27) from n x k
+ * class indices in device memory (uml_mlp_predict_topk): hits_out[j] = rows whose target_host[i] equals
+ * classes_host[idx[i][j']] for some j' <= j, for every j < k - top-1 and top-5 accuracy from one call. */
+UML_API int uml_topk_count_hits(uml_engine* e, const int32_t* idx_dev, int k, int64_t n, const double* classes_host,
+                                int n_classes, const double* targets_host, int64_t* hits_out);
 
 /* the MLP predictor from HOST rows through the same chunk pipeline as uml_linear_predict_host (pinned bounce buffers,
  * GPU transpose / down-cast to fp32 - the reference predictor casts features to float32 -, scoring kernel, fp64

@@ -52,4 +52,15 @@ eng.predict_host(m784, X784, exact=True, chunk_rows=2048)
 eng.predict_mlp_host(mlp, np.asfortranarray(Xf[:32]))
 eng.predict_mlp_host(mlp, np.asfortranarray(Xf[:32]))
 eng.predict_mlp_host(mlp, X[:1].astype(np.int64))
+# MLP top-k: tensor-core and CUDA-core top-k forms with their fp64 re-score, the fp64 kernel for k > 5, device outputs
+# 4 bytes off 16-byte alignment, indices only, and the hit count
+for batch in (b, bf):
+    for k in (1, 3, 5, 10):
+        eng.predict_mlp_topk(mlp, batch, k, exact=True)
+        eng.predict_mlp_topk(mlp, batch, k, exact=False, want_proba=False)
+kb = eng.device_alloc(4 * (3 * b.n_rows + 1))
+pb = eng.device_alloc(4 * (3 * b.n_rows + 1))
+eng.predict_mlp_topk(mlp, b, 3, idx_device_ptr=kb.ptr + 4, proba_device_ptr=pb.ptr + 4)
+eng.predict_mlp_topk(mlp, b, 3, want_proba=False, idx_device_ptr=kb.ptr)
+eng.count_topk_hits(kb.ptr, 3, b.n_rows, np.arange(10.0), np.zeros(b.n_rows))
 print("sanitizer driver ok")

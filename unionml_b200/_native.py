@@ -105,6 +105,8 @@ SIGNATURES = {
     "uml_mlp_free": (None, [_P]),
     "uml_mlp_predict": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.POINTER(Stats)]),
     "uml_mlp_predict_proba": (C.c_int, [_P, _P, _P, _P, C.c_int, C.POINTER(Stats)]),
+    "uml_mlp_predict_topk": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_int, C.c_int, C.POINTER(Stats)]),
+    "uml_topk_count_hits": (C.c_int, [_P, _P, C.c_int, C.c_int64, _P, C.c_int, _P, _P]),
     "uml_mlp_predict_host": (
         C.c_int,
         [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, _P, C.c_int, C.c_int64, C.POINTER(Stats)],

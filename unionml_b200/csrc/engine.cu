@@ -19,6 +19,7 @@
 
 #include "uml_common.cuh"
 #include "mlp_rescore.cuh"
+#include "mlp_topk.cuh"
 
 // NVTX ranges around the phases of a call (stage / score / re-score / exchange); free when no tool is attached
 struct NvtxRange {
@@ -195,6 +196,8 @@ struct uml_engine {
   Scratch<float, 3> d_xchunk;            // converted fp32 chunks (predict_host)
   Scratch<double, 3> d_vchunk;           // class values (predict_host_values) or scores (decision_function_host) of a chunk
   Scratch<double> d_classes;
+  Scratch<double> d_targets;             // uml_topk_count_hits: targets and first-hit counters
+  Scratch<unsigned long long> d_hits;
   Scratch<char, 3, true> h_bounce;       // pinned bounce buffers for pageable sources
   Scratch<char, 3, true> h_result;       // pinned landing slots for labels / values bound for pageable outputs
   CopyPool* pool = nullptr;
@@ -319,16 +322,17 @@ static cudaError_t reset_counters(uml_engine* e, cudaStream_t s) {
 // a tensor map.  UML_B200_MLP_TC=0 / 1 forces the choice; 1 does not apply to class probabilities (labels: rows that
 // are not tf32 values are caught in the kernel and re-scored; the probability kernels have no fp64 re-score behind
 // them).  tf32() is asked only when its answer decides: it may cost a pass over the rows.
+// topk: the tile kernels' top-k form, routed as the labels are (it has the same fp64 re-score behind it)
 template <class Tf32>
-static int mlp_route(const uml::MlpDeviceModel& m, bool has_map, bool proba, Tf32&& tf32) {
+static int mlp_route(const uml::MlpDeviceModel& m, bool has_map, bool proba, Tf32&& tf32, bool topk = false) {
   if (!has_map) return 2;
   std::string why;
-  if (uml::mlp_tc_supported(m, &why)) {
+  if (uml::mlp_tc_supported(m, &why, topk)) {
     const char* env = getenv("UML_B200_MLP_TC");
     const bool off = env && env[0] == '0', on = env && env[0] == '1' && !proba;
     if (!off && (on || tf32())) return 5;
   }
-  return uml::mlp_tma_supported(m, &why, proba) ? 3 : 2;
+  return uml::mlp_tma_supported(m, &why, proba, topk) ? 3 : 2;
 }
 
 static int dtype_size(int dt) {
@@ -430,6 +434,8 @@ void uml_engine_destroy(uml_engine* e) {
   e->d_xchunk.release();
   e->d_vchunk.release();
   e->d_classes.release();
+  e->d_targets.release();
+  e->d_hits.release();
   e->h_bounce.release();
   e->h_result.release();
   delete e->pool;
@@ -1228,6 +1234,33 @@ int uml_labels_count_equal(uml_engine* e, const void* labels_dev, int label_byte
   }
   *count_out = (int64_t)e->h->counters[0];
   return done(UML_OK);
+}
+
+// top-k hit counts of the quickdraw template's accuracy(output, target, topk) (quickdraw/model.py:20-27):
+// hits_out[j] = rows whose target is among their first j + 1 classes, for every j < k, in one pass
+int uml_topk_count_hits(uml_engine* e, const int32_t* idx_dev, int k, int64_t n, const double* classes_host,
+                        int n_classes, const double* targets_host, int64_t* hits_out) {
+  if (!e || (!idx_dev && n > 0) || k < 1 || n < 0 || !classes_host || n_classes < 1 || (!targets_host && n > 0) || !hits_out)
+    return UML_ERR_INVALID;
+  UML_CUDA(e, cudaSetDevice(e->device));
+  for (int j = 0; j < k; ++j) hits_out[j] = 0;
+  if (n == 0) return UML_OK;
+  int rc;
+  if ((rc = grow(e, e->d_classes, n_classes)) != UML_OK || (rc = grow(e, e->d_targets, n)) != UML_OK ||
+      (rc = grow(e, e->d_hits, k)) != UML_OK)
+    return rc;
+  std::vector<unsigned long long> first(k);
+  cudaStream_t s = e->stream;
+  UML_CUDA(e, cudaMemcpyAsync(e->d_classes.p[0], classes_host, (size_t)n_classes * 8, cudaMemcpyHostToDevice, s));
+  UML_CUDA(e, cudaMemcpyAsync(e->d_targets.p[0], targets_host, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+  UML_CUDA(e, cudaMemsetAsync(e->d_hits.p[0], 0, (size_t)k * 8, s));
+  UML_CUDA(e, uml::launch_topk_first_hits(idx_dev, k, n, e->d_classes.p[0], n_classes, e->d_targets.p[0],
+                                          e->d_hits.p[0], s));
+  UML_CUDA(e, cudaMemcpyAsync(first.data(), e->d_hits.p[0], (size_t)k * 8, cudaMemcpyDeviceToHost, s));
+  UML_CUDA(e, cudaStreamSynchronize(s));
+  int64_t run = 0;
+  for (int j = 0; j < k; ++j) hits_out[j] = run += (int64_t)first[j];
+  return UML_OK;
 }
 
 int uml_labels_push(uml_engine* e, const void* src, void* const* dst, int n_dst, int64_t bytes) {
@@ -2069,6 +2102,78 @@ int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, f
   }
   if (!proba_on_device) UML_CUDA(e, cudaStreamSynchronize(e->stream));
   return UML_OK;
+}
+
+int uml_mlp_predict_topk(uml_engine* e, const uml_mlp* m, const uml_batch* b, int k, int32_t* idx_out, float* proba_out,
+                         int out_on_device, int mode, uml_stats* stats) {
+  if (!e || !m || !b || (!idx_out && b->n_rows > 0)) return UML_ERR_INVALID;
+  const int C = m->dm.n_classes;
+  if (k < 1 || k > C) UML_FAIL(e, UML_ERR_INVALID, "k = %d: the module has %d classes (need 1 <= k <= %d)", k, C, C);
+  if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
+  if (b->n_features != m->dm.n_in)
+    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the module is expecting %d features as input.", b->n_features,
+             m->dm.n_in);
+  UML_CUDA(e, cudaSetDevice(e->device));
+  (void)cudaGetLastError();
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (b->n_rows == 0) return UML_OK;
+  NvtxRange r_all("uml:mlp_topk");
+  const bool exact = mode == UML_PREDICT_EXACT;
+  // k beyond what the tile kernels select in registers: the float64 kernel serves every row
+  const int path = k > uml::kMlpTopkMax ? 2 : mlp_route(m->dm, b->has_map, false, [&] { return batch_tf32_exact(e, b) == 1; }, true);
+  const int64_t n_out = b->n_rows * k;
+  int32_t* d_idx = idx_out;
+  float* d_proba = proba_out;
+  int rc;
+  if (exact && path != 2 && (rc = grow(e, e->d_flag_rows, b->n_rows)) != UML_OK) return rc;
+  if (!out_on_device) {
+    if ((rc = grow(e, e->d_labels, n_out)) != UML_OK) return rc;
+    d_idx = e->d_labels.p[0];
+    if (proba_out) {
+      if ((rc = grow(e, e->d_proba, n_out)) != UML_OK) return rc;
+      d_proba = e->d_proba.p[0];
+    }
+  }
+  const FlagList fl = flag_list(e);
+  const int sm = e->info.sm_count;
+  cudaStream_t s = e->stream;
+  const bool timed = stats != nullptr;
+  const bool sync_call = timed || !out_on_device;
+  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[0], s));
+  // as for the labels: an asynchronous call finds the flag list handed back empty by the previous re-score
+  if (sync_call) UML_CUDA(e, reset_counters(e, s));
+  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], s));
+  int launches = 1;
+  if (path == 2) {
+    UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, b->x, b->ld, b->n_rows, k, d_idx, d_proba, fl, true, sm, s));
+    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
+  } else {
+    if (path == 5) {
+      uml::MlpTcLaunch out{};
+      out.n_rows = b->n_rows;
+      out.topk_idx = d_idx;
+      out.topk_proba = d_proba;
+      out.topk_k = k;
+      UML_CUDA(e, uml::launch_mlp_tc_topk(b->map, m->dm, out, exact, fl, sm, s));
+    } else {
+      UML_CUDA(e, uml::launch_mlp_tma_topk(b->map, m->dm, b->n_rows, k, d_idx, d_proba, exact, fl, sm, s));
+    }
+    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
+    if (exact) {
+      NvtxRange r_rescore("uml:mlp_topk_f64");
+      UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, b->x, b->ld, b->n_rows, k, d_idx, d_proba, fl, false, sm, s));
+      ++launches;
+    }
+  }
+  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], s));
+  if (!sync_call) return UML_OK;
+  if (!out_on_device) {
+    UML_CUDA(e, cudaMemcpyAsync(idx_out, d_idx, (size_t)n_out * 4, cudaMemcpyDeviceToHost, s));
+    if (proba_out) UML_CUDA(e, cudaMemcpyAsync(proba_out, d_proba, (size_t)n_out * 4, cudaMemcpyDeviceToHost, s));
+  }
+  rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
+  if (stats) stats->d2h_bytes = out_on_device ? 0 : n_out * 4 * (proba_out ? 2 : 1);
+  return rc;
 }
 
 }  // extern "C"

@@ -10,6 +10,9 @@
 //    rows whose logit margin is inside the propagated fp32 error bound in fp64.
 //    PROBA instantiations store softmax(logits) instead of the label: each warp's 32 consecutive rows per j leave as one
 //    coalesced run through shared memory (mlp_proba.cuh).
+//    TOPK instantiations store the k largest logits' class indices (and probabilities) the same way; EXACT ones flag
+//    rows whose top k + 1 logits are not separated by the bound (mlp_topk.cuh, DESIGN.md 3.8).
+//  * mlp_topk_f64_kernel: the fp64 top-k of those flagged rows, or of every row for shapes / k no tile kernel takes.
 //  * mlp_rescore_f64_kernel: warp per row, lane per hidden unit, fp64; flagged rows of EXACT mode, or every row for
 //    shapes the tile kernel is not instantiated for.
 //  * mlp_proba_f64_kernel: class probabilities for those shapes - the same fp64 scorer, then a float64 softmax.
@@ -25,6 +28,7 @@
 #include "tma_ring.cuh"
 #include "mlp_rescore.cuh"
 #include "mlp_proba.cuh"
+#include "mlp_topk.cuh"
 
 #ifndef UML_MLP_UNROLL_Q
 #define UML_MLP_UNROLL_Q 8  // feature-quad unroll of the layer-1 loop
@@ -63,9 +67,17 @@ struct MlpKernelParams {
   float* proba;  // PROBA kernels: [n_rows][C] row-major
 };
 
-template <int H, int C, bool EXACT, bool PROBA>
+// TOPK kernels take the parameters in this longer form (a longer MlpKernelParams changes the code ptxas makes for
+// every other instantiation)
+struct MlpTopkKernelParams : MlpKernelParams {
+  int32_t* topk_idx;  // [n_rows][topk_k] class indices
+  float* topk_proba;  // [n_rows][topk_k] their probabilities, or nullptr: not written
+  int topk_k;
+};
+
+template <int H, int C, bool EXACT, bool PROBA, bool TOPK = false, class Params = MlpKernelParams>
 __global__ void __launch_bounds__(kMlpThreads, 1)
-mlp_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const MlpKernelParams p) {
+mlp_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) {
   constexpr int HP = H + 4;
   constexpr int CP = (C + 1 + 3) / 4 * 4;
   constexpr int NC2 = C + (EXACT ? 1 : 0);
@@ -242,6 +254,41 @@ mlp_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const MlpKernelP
             __syncwarp();  // the strip is rewritten for the next run
             continue;
           }
+          if constexpr (TOPK) {
+            // lane l's k indices at l k of the warp's strip, its k probabilities at l k of the strip's second half
+            constexpr int M = C < kMlpTopkMax + 1 ? C : kMlpTopkMax + 1;
+            const int k = p.topk_k;
+            const bool want_p = p.topk_proba != nullptr;
+            float pr[C];
+            if (want_p) {
+              mlp_softmax_f32<C>(z[j], pr);
+            } else {
+#pragma unroll
+              for (int c = 0; c < C; ++c) pr[c] = 0.f;
+            }
+            float v[M], pv[M];
+            int id[M];
+            mlp_topk_select<C, M>(z[j], pr, v, id, pv);
+            int32_t* si = reinterpret_cast<int32_t*>(empty_bar + S) + warp * kMlpTopkStripWords;
+            float* sp = reinterpret_cast<float*>(si + 32 * kMlpTopkMax);
+#pragma unroll
+            for (int r = 0; r < M; ++r) {
+              if (r < k) {
+                si[lane * k + r] = id[r];
+                sp[lane * k + r] = pv[r];
+              }
+            }
+            __syncwarp();
+            mlp_topk_store_run<32>(si, p.topk_idx, row - lane, p.n_rows, k, lane);
+            if (want_p) mlp_topk_store_run<32>(sp, p.topk_proba, row - lane, p.n_rows, k, lane);
+            __syncwarp();  // the strip is rewritten for the next run
+            if (EXACT) {
+              const float err = p.e1_scale * a1[j] + p.e2_scale * z[j][C];
+              const bool certain = mlp_topk_certain<M>(v, min(k, C - 1), 2.0f * err);
+              mlp_topk_flag(row < p.n_rows && !certain, row, p.flag_count, p.flag_rows, p.flag_cap, lane);
+            }
+            continue;
+          }
           float best = z[j][0];
           float second = -INFINITY;
           int idx = 0;
@@ -414,6 +461,106 @@ __global__ void __launch_bounds__(256) mlp_proba_f64_kernel(const MlpProbaF64Par
   }
 }
 
+// top-k of the float64 network: the flagged rows of a TOPK tile kernel in EXACT mode, or every row for a shape or k no
+// tile kernel takes.  The fp64 scorer above (logits kept), then per row and lane per class: the class's rank in the
+// stable descending order (the logits above it, and equal logits of lower index) - no sort, any k <= C.  A class of
+// rank r < k writes slot r of its row's indices and, when requested, the float64 softmax of mlp_proba_f64_kernel
+// rounded once to fp32.  A row where a consecutive gap among ranks 0 .. min(k, C - 1) is within twice the fp64 logit
+// bound counts as ambiguous, as the labels' top-2 margin does.
+struct MlpTopkF64Params {
+  const float* x;
+  long long ld;
+  long long n_rows;
+  const double* pack;
+  int F, H, C;
+  int k;
+  int32_t* idx;   // [n_rows][k]
+  float* proba;   // [n_rows][k] or nullptr
+  const int* flag_count;
+  const int32_t* flag_rows;
+  int flag_cap;
+  int all_rows;
+  unsigned long long* counters;
+};
+
+__global__ void __launch_bounds__(256) mlp_topk_f64_kernel(const MlpTopkF64Params p) {
+  extern __shared__ __align__(16) double rs_smem[];
+  constexpr int R = kMlpRsRows;
+  MlpRsView view = mlp_rs_stage(rs_smem, p.pack, p.F, p.H, p.C);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double* xs = rs_smem + mlp_rs_weight_doubles(p.F, p.H, p.C) + warp * (mlp_rs_strip_doubles(p.F, p.H, R) + p.C * R);
+  double* hv = xs + p.F * R;
+  double* zs = hv + p.H * R;  // the pass's logits, [c][R]
+  __syncthreads();
+  mlp_rs_finish_stage(view);
+
+  pdl_wait_for_predecessor();  // flagged mode: the flag list and outputs of the tile kernel this launch depends on
+  const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const long long warps_total = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  const long long n = p.all_rows ? p.n_rows : static_cast<long long>(min(*p.flag_count, p.flag_cap));
+  if (!p.all_rows && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n));
+  const int C = p.C, k = p.k, kk = min(p.k, p.C - 1);
+  for (long long i = warp_global * R; i < n; i += warps_total * R) {
+    long long row[R];
+    const float* xr[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const long long j = i + r < n ? i + r : i;  // unused slots repeat the first row (result ignored)
+      row[r] = p.all_rows ? j : static_cast<long long>(p.flag_rows[j]);
+      xr[r] = p.x + row[r] * p.ld;
+    }
+    MlpRowResult res[R];
+    double err[R];
+    mlp_rs_rows<R, true, true>(view, xr, xs, hv, lane, res, zs, err);
+    for (int r = 0; r < R && i + r < n; ++r) {
+      const double* zr = zs + r;  // logit c at zr[c R]
+      const long long out_row = p.all_rows ? i + r : static_cast<long long>(p.flag_rows[i + r]);
+      double m = -INFINITY;
+      for (int c = lane; c < C; c += 32) m = fmax(m, zr[c * R]);
+      m = warp_max(m, 1);
+      double s = 0.0;
+      for (int c = lane; c < C; c += 32) s += exp(zr[c * R] - m);
+      s = warp_sum(s);
+      bool ambiguous = false;
+      for (int c = lane; c < C; c += 32) {
+        const double zc = zr[c * R];
+        int rank = 0;
+        double above = INFINITY;  // the smallest logit ranked above c: its neighbour one rank up
+        for (int o = 0; o < C; ++o) {
+          const double zo = zr[o * R];
+          if (zo > zc || (zo == zc && o < c)) {
+            ++rank;
+            above = fmin(above, zo);
+          }
+        }
+        if (rank < k) {
+          const long long at = out_row * k + rank;
+          p.idx[at] = c;
+          if (p.proba) p.proba[at] = static_cast<float>(exp(zc - m) / s);
+        }
+        if (rank >= 1 && rank <= kk && !((above - zc) > 2.0 * err[r])) ambiguous = true;
+      }
+      ambiguous = __any_sync(0xffffffffu, ambiguous);
+      if (lane == 0) {
+        if (res[r].bad) atomicAdd(&p.counters[1], 1ull);
+        if (ambiguous) atomicAdd(&p.counters[0], 1ull);
+      }
+    }
+    __syncwarp();  // the strip is rewritten by the next pass
+  }
+  // hand the flag list back empty (see mlp_rescore_f64_kernel)
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const unsigned long long ticket = atomicAdd(&p.counters[3], 1ull);
+    if (ticket == static_cast<unsigned long long>(gridDim.x) - 1ull) {
+      *const_cast<int*>(p.flag_count) = 0;
+      p.counters[3] = 0ull;
+      __threadfence();
+    }
+  }
+}
+
 // small-batch kernel of the online path (fastapi.py /predict, B <= 64 rows): the fp64 scorer above on the request's
 // raw feature block, which the kernel reads straight from pinned host memory - no staging pass, no tile kernel, no
 // guard, exact by construction.  Each warp casts its four rows to fp32 as the staging kernels do (convert_one: the
@@ -507,28 +654,28 @@ cudaError_t launch_mlp_small(const MlpDeviceModel& m, const SrcView& src, int n_
   return cudaGetLastError();
 }
 
-static size_t mlp_fixed_smem(const MlpDeviceModel& m, bool proba = false) {
+static size_t mlp_fixed_smem(const MlpDeviceModel& m, bool proba = false, bool topk = false) {
   return 1024 + (static_cast<size_t>(m.f_pad) * (m.n_hidden + 4) + (m.n_hidden + 4) + static_cast<size_t>(m.n_hidden) * m.cp + m.cp) * 4 +
-         2 * 64 * 8 + (proba ? static_cast<size_t>(kMlpConsumerWarps) * 32 * m.n_classes * 4 : 0);  // + a staging strip per warp
+         2 * 64 * 8 + (proba ? static_cast<size_t>(kMlpConsumerWarps) * 32 * m.n_classes * 4 : 0) +  // + a staging strip per warp
+         (topk ? static_cast<size_t>(kMlpConsumerWarps) * kMlpTopkStripWords * 4 : 0);
 }
 
-bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why, bool proba) {
+bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why, bool proba, bool topk) {
   const bool shape_ok = (m.n_hidden == 32 || m.n_hidden == 16) && (m.n_classes == 10 || m.n_classes == 2 || m.n_classes == 3);
   if (!shape_ok) {
     if (why) *why = "tile kernel instantiated for hidden in {16, 32} and classes in {2, 3, 10}";
     return false;
   }
-  if (mlp_fixed_smem(m, proba) + kMlpPairs * static_cast<size_t>(kMlpStageBytes) > static_cast<size_t>(kMaxSmemBytes)) {
+  if (mlp_fixed_smem(m, proba, topk) + kMlpPairs * static_cast<size_t>(kMlpStageBytes) > static_cast<size_t>(kMaxSmemBytes)) {
     if (why) *why = "W1^T does not fit in shared memory next to a 4-stage ring";
     return false;
   }
   return true;
 }
 
-template <int H, int C, bool EXACT, bool PROBA = false>
-static cudaError_t mlp_launch_one(const CUtensorMap& xmap, const MlpKernelParams& p, int grid, size_t smem,
-                                  cudaStream_t stream) {
-  auto kern = mlp_argmax_tma_kernel<H, C, EXACT, PROBA>;
+template <int H, int C, bool EXACT, bool PROBA = false, bool TOPK = false, class Params = MlpKernelParams>
+static cudaError_t mlp_launch_one(const CUtensorMap& xmap, const Params& p, int grid, size_t smem, cudaStream_t stream) {
+  auto kern = mlp_argmax_tma_kernel<H, C, EXACT, PROBA, TOPK, Params>;
   static size_t configured = 0;
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -539,22 +686,19 @@ static cudaError_t mlp_launch_one(const CUtensorMap& xmap, const MlpKernelParams
   return cudaGetLastError();
 }
 
-template <bool EXACT, bool PROBA = false>
-static cudaError_t mlp_dispatch(int H, int C, const CUtensorMap& xmap, const MlpKernelParams& p, int grid, size_t smem,
+template <bool EXACT, bool PROBA = false, bool TOPK = false, class Params = MlpKernelParams>
+static cudaError_t mlp_dispatch(int H, int C, const CUtensorMap& xmap, const Params& p, int grid, size_t smem,
                                 cudaStream_t stream) {
 #define UML_MLP_CASE(HH, CC) \
-  if (H == HH && C == CC) return mlp_launch_one<HH, CC, EXACT, PROBA>(xmap, p, grid, smem, stream);
+  if (H == HH && C == CC) return mlp_launch_one<HH, CC, EXACT, PROBA, TOPK, Params>(xmap, p, grid, smem, stream);
   UML_MLP_CASE(32, 10) UML_MLP_CASE(32, 2) UML_MLP_CASE(32, 3) UML_MLP_CASE(16, 10) UML_MLP_CASE(16, 2) UML_MLP_CASE(16, 3)
 #undef UML_MLP_CASE
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, const float* x, int64_t n_rows,
-                           int32_t* labels, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream,
-                           float* proba) {
-  (void)x;
-  if (n_rows <= 0) return cudaSuccess;
-  const bool want_proba = proba != nullptr;
+// the parameters, grid and shared memory of one tile-kernel launch; `fixed` = mlp_fixed_smem of the kernel's form
+static MlpKernelParams mlp_tma_params(const MlpDeviceModel& m, int64_t n_rows, int32_t* labels, const FlagList& flags,
+                                      float* proba, size_t fixed, int sm_count, int* grid, size_t* smem) {
   MlpKernelParams p{};
   p.w1t = m.w1t;
   p.b1 = m.b1;
@@ -565,7 +709,6 @@ cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, con
   p.num_tiles = (n_rows + kMlpTileRows - 1) / kMlpTileRows;
   p.f_pad = m.f_pad;
   p.kc = m.f_pad / kChunkF;
-  const size_t fixed = mlp_fixed_smem(m, want_proba);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kMlpStageBytes);
   stages = std::min(stages, 64);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(kMlpPairs, std::min(stages, atoi(env)));
@@ -578,12 +721,40 @@ cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, con
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
   p.proba = proba;
-  const size_t smem = fixed + static_cast<size_t>(stages) * kMlpStageBytes;
+  *smem = fixed + static_cast<size_t>(stages) * kMlpStageBytes;
   const long long slots = (p.num_tiles + kMlpPairs - 1) / kMlpPairs;
-  const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
+  *grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
+  return p;
+}
+
+cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, const float* x, int64_t n_rows,
+                           int32_t* labels, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream,
+                           float* proba) {
+  (void)x;
+  if (n_rows <= 0) return cudaSuccess;
+  const bool want_proba = proba != nullptr;
+  int grid = 0;
+  size_t smem = 0;
+  const MlpKernelParams p = mlp_tma_params(m, n_rows, labels, flags, proba, mlp_fixed_smem(m, want_proba), sm_count, &grid, &smem);
   if (want_proba) return mlp_dispatch<false, true>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream);
   return exact ? mlp_dispatch<true>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream)
                : mlp_dispatch<false>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream);
+}
+
+cudaError_t launch_mlp_tma_topk(const CUtensorMap& xmap, const MlpDeviceModel& m, int64_t n_rows, int k, int32_t* idx,
+                                float* proba, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream) {
+  if (n_rows <= 0) return cudaSuccess;
+  if (k < 1 || k > std::min(m.n_classes, kMlpTopkMax)) return cudaErrorInvalidValue;
+  int grid = 0;
+  size_t smem = 0;
+  MlpTopkKernelParams p{};
+  static_cast<MlpKernelParams&>(p) =
+      mlp_tma_params(m, n_rows, nullptr, flags, nullptr, mlp_fixed_smem(m, false, true), sm_count, &grid, &smem);
+  p.topk_idx = idx;
+  p.topk_proba = proba;
+  p.topk_k = k;
+  return exact ? mlp_dispatch<true, false, true>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream)
+               : mlp_dispatch<false, false, true>(m.n_hidden, m.n_classes, xmap, p, grid, smem, stream);
 }
 
 cudaError_t launch_mlp_rescore_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows,
@@ -652,6 +823,44 @@ cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mlp_proba_f64_kernel, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
   const long long blocks = std::min<long long>(static_cast<long long>(sm_count) * per_sm, (n_rows + 8 * kMlpRsRows - 1) / (8 * kMlpRsRows));
   mlp_proba_f64_kernel<<<static_cast<int>(std::max<long long>(1, blocks)), 256, smem, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_mlp_topk_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, int k, int32_t* idx,
+                                float* proba, const FlagList& flags, bool all_rows, int sm_count, cudaStream_t stream) {
+  if (n_rows <= 0) return cudaSuccess;
+  MlpTopkF64Params p{};
+  p.x = x;
+  p.ld = ld;
+  p.n_rows = n_rows;
+  p.pack = m.rs_pack;
+  p.F = m.n_in;
+  p.H = m.n_hidden;
+  p.C = m.n_classes;
+  p.k = k;
+  p.idx = idx;
+  p.proba = proba;
+  p.flag_count = flags.count;
+  p.flag_rows = flags.rows;
+  p.flag_cap = flags.capacity;
+  p.all_rows = all_rows ? 1 : 0;
+  p.counters = flags.counters;
+  // the shared memory of mlp_proba_f64_kernel
+  const size_t strip = mlp_rs_strip_doubles(m.n_in, m.n_hidden, kMlpRsRows) + static_cast<size_t>(m.n_classes) * kMlpRsRows;
+  const size_t smem = (mlp_rs_weight_doubles(m.n_in, m.n_hidden, m.n_classes) + 8 * strip) * sizeof(double);
+  if (smem > static_cast<size_t>(kMaxSmemBytes)) return cudaErrorInvalidValue;
+  static size_t configured = 0;
+  if (smem > configured) {
+    cudaError_t err = cudaFuncSetAttribute(mlp_topk_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (err != cudaSuccess) return err;
+    configured = smem;
+  }
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mlp_topk_f64_kernel, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  long long blocks = static_cast<long long>(sm_count) * per_sm;  // persistent: every resident warp loops over rows
+  if (all_rows) blocks = std::min<long long>(blocks, (n_rows + 8 * kMlpRsRows - 1) / (8 * kMlpRsRows));
+  cudaError_t lerr = launch_dependent(mlp_topk_f64_kernel, static_cast<int>(std::max<long long>(1, blocks)), 256, smem, stream, p);
+  if (lerr != cudaSuccess) return lerr;
   return cudaGetLastError();
 }
 

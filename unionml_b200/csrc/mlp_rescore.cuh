@@ -119,10 +119,11 @@ struct MlpRowResult {
 
 // One warp, R rows per pass.  xr[r] = row r's fp32 features in global memory (callers pass a valid row for unused
 // slots and ignore that result); xs / hv = the warp's strip, F x R and H x R doubles, 16-byte aligned.  KEEP_Z: the
-// logits are also left in zs[c R + r] (C x R doubles, visible to the whole warp on return).
-template <int R, bool KEEP_Z = false>
+// logits are also left in zs[c R + r] (C x R doubles, visible to the whole warp on return).  KEEP_ERR: errs[r] = the
+// bound on row r's fp64 logit errors that decides `ambiguous` (the same value in every lane).
+template <int R, bool KEEP_Z = false, bool KEEP_ERR = false>
 __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* const (&xr)[R], double* xs, double* hv, int lane,
-                                            MlpRowResult (&out)[R], double* zs = nullptr) {
+                                            MlpRowResult (&out)[R], double* zs = nullptr, double* errs = nullptr) {
   static_assert(R == 2 || R == 4, "rows per pass");
   const double u = 1.1102230246251565e-16;  // 2^-53
   const int F = v.F, H = v.H, C = v.C, HP = v.H + 1;
@@ -234,6 +235,7 @@ __device__ __forceinline__ void mlp_rs_rows(const MlpRsView& v, const float* con
     // fp64 error of a logit: the hidden units' own errors carried through W2, plus the output layer's chain
     const double err = herr[r] * v.w2sum + (static_cast<double>(H) + 16.0) * u * amax[r];
     out[r].ambiguous = !((top[r].best - top[r].second) > 2.0 * err);
+    if constexpr (KEEP_ERR) errs[r] = err;
   }
 }
 

@@ -29,7 +29,8 @@
 //             the resident W1 tile as B), then from the accumulator registers: + b1, ReLU, layer 2 over the lane's
 //             hidden units, a quad reduce-scatter that leaves each lane one row's logits, argmax (first maximum
 //             wins), margin guard, label store (+ peer stores); PROBA kernels instead take the softmax of the logits
-//             and store each warp's two 16-row runs of probabilities through shared memory (mlp_proba.cuh)
+//             and store each warp's two 16-row runs of probabilities through shared memory (mlp_proba.cuh); TOPK
+//             kernels select the k largest logits and store indices / probabilities the same way (mlp_topk.cuh)
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -38,6 +39,7 @@
 #include "uml_common.cuh"
 #include "wgmma.cuh"
 #include "mlp_proba.cuh"
+#include "mlp_topk.cuh"
 
 namespace uml {
 
@@ -75,13 +77,17 @@ struct MlpTcParams {
   int32_t* flag_rows;
   int flag_cap;
   float* proba;  // PROBA kernels: [n_rows][C] row-major
+  // TOPK kernels: [n_rows][topk_k] class indices and (optional, nullptr: not written) their probabilities
+  int32_t* topk_idx;
+  float* topk_proba;
+  int topk_k;
 };
 
 // consumer lane l of warp wq (in its warpgroup) ends the epilogue owning one row of the 128-row tile: the quad
 // (l / 4) holds rows 16 wq + l / 4 (+ 8) of both 64-row halves, and lane l % 4 keeps the (half, +8) pair it names
 __device__ __forceinline__ int tc_row_of_lane(int wq, int l) { return 64 * ((l & 3) >> 1) + 16 * wq + (l >> 2) + 8 * (l & 1); }
 
-template <int H, int C, bool EXACT, bool PROBA>
+template <int H, int C, bool EXACT, bool PROBA, bool TOPK = false>
 __global__ void __launch_bounds__(kTcRegBudgetThreads, 1)
 mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ MlpTcParams<H, C> p) {
   constexpr int N = 2 * H;     // accumulator columns per row: [main | small]
@@ -283,6 +289,48 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
         __syncwarp();  // the strip is rewritten by this warp's next tile
         continue;
       }
+      if constexpr (TOPK) {
+        // this warp's staging strip, laid out as the PROBA strip with k words per row: indices, then probabilities
+        constexpr int M = C < kMlpTopkMax + 1 ? C : kMlpTopkMax + 1;
+        const int k = p.topk_k;
+        const bool want_p = p.topk_proba != nullptr;
+        float pr[C];
+        if (want_p) {
+          mlp_softmax_f32<C>(z, pr);
+        } else {
+#pragma unroll
+          for (int c = 0; c < C; ++c) pr[c] = 0.f;
+        }
+        float v[M], pv[M];
+        int id[M];
+        mlp_topk_select<C, M>(z, pr, v, id, pv);
+        int32_t* si = reinterpret_cast<int32_t*>((reinterpret_cast<uintptr_t>(a1_bar + kTcSlots) + 15u) & ~static_cast<uintptr_t>(15)) +
+                      (warp - 4) * kMlpTopkStripWords;
+        float* sp = reinterpret_cast<float*>(si + 32 * kMlpTopkMax);
+        const int mine = (16 * ((lane & 3) >> 1) + (lane >> 2) + 8 * (lane & 1)) * k;
+#pragma unroll
+        for (int r = 0; r < M; ++r) {
+          if (r < k) {
+            si[mine + r] = id[r];
+            sp[mine + r] = pv[r];
+          }
+        }
+        __syncwarp();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const long long row0 = tile * kTileRows + 64 * h + 16 * wq;
+          mlp_topk_store_run<16>(si + 16 * h * k, p.topk_idx, row0, p.n_rows, k, lane);
+          if (want_p) mlp_topk_store_run<16>(sp + 16 * h * k, p.topk_proba, row0, p.n_rows, k, lane);
+        }
+        __syncwarp();  // the strip is rewritten by this warp's next tile
+        if (EXACT) {
+          const long long row = tile * kTileRows + row_in_tile;
+          const float err = p.e1_scale * a1 + p.e2_scale * z[C];
+          const bool certain = mlp_topk_certain<M>(v, min(k, C - 1), 2.0f * err);
+          mlp_topk_flag(row < p.n_rows && !certain, row, p.flag_count, p.flag_rows, p.flag_cap, lane);
+        }
+        continue;
+      }
       const long long row = tile * kTileRows + row_in_tile;
       float best = z[0];
       float second = -INFINITY;
@@ -382,15 +430,16 @@ std::vector<float> mlp_tc_build_w1_tiles(const float* w1 /*[H][F]*/, int H, int 
   return tiles;
 }
 
-static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool proba = false) {
+static size_t mlp_tc_fixed_smem(const MlpDeviceModel& m, bool proba = false, bool topk = false) {
   const size_t kc = m.f_pad / kChunkF;
   size_t bytes = 1024 + kc * (2 * m.n_hidden) * 128 + static_cast<size_t>(kTcSlots) * kTileRows * 4 +
                  (2 * 64 + kTcSlots) * 8 + 16;
   if (proba) bytes += 16 + static_cast<size_t>(kTcEpilogueWarps) * 32 * m.n_classes * 4;  // one staging strip per epilogue warp
+  if (topk) bytes += 16 + static_cast<size_t>(kTcEpilogueWarps) * kMlpTopkStripWords * 4;
   return bytes;
 }
 
-bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why) {
+bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why, bool topk) {
   const bool shape_ok = (m.n_hidden == 32 || m.n_hidden == 16) && (m.n_classes == 10 || m.n_classes == 2 || m.n_classes == 3);
   if (!shape_ok) {
     if (why) *why = "tensor-core kernel instantiated for hidden in {16, 32} and classes in {2, 3, 10}";
@@ -400,10 +449,10 @@ bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why) {
     if (why) *why = "more than 128 features: the resident W1 tile is sized for F_pad <= 128";
     return false;
   }
-  return mlp_tc_fixed_smem(m) + 6 * static_cast<size_t>(kStageBytes) <= static_cast<size_t>(kMaxSmemBytes);
+  return mlp_tc_fixed_smem(m, false, topk) + 6 * static_cast<size_t>(kStageBytes) <= static_cast<size_t>(kMaxSmemBytes);
 }
 
-template <int H, int C, bool EXACT, bool PROBA = false>
+template <int H, int C, bool EXACT, bool PROBA = false, bool TOPK = false>
 static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l,
                                      const FlagList& flags, int sm_count, cudaStream_t stream) {
   using Params = MlpTcParams<H, C>;
@@ -454,7 +503,10 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   p.num_tiles = (l.n_rows + kTileRows - 1) / kTileRows;
   p.kc = m.f_pad / kChunkF;
   p.proba = l.proba;
-  const size_t fixed = mlp_tc_fixed_smem(m, PROBA);
+  p.topk_idx = l.topk_idx;
+  p.topk_proba = l.topk_proba;
+  p.topk_k = l.topk_k;
+  const size_t fixed = mlp_tc_fixed_smem(m, PROBA, TOPK);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kStageBytes);
   stages = std::min(stages, 64);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(4, std::min(stages, atoi(env)));
@@ -466,7 +518,7 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
-  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, PROBA>;
+  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, PROBA, TOPK>;
   static size_t configured = 0;
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -496,6 +548,19 @@ cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m
   const FlagList none{};
 #define UML_TC_CASE(HH, CC) \
   if (m.n_hidden == HH && m.n_classes == CC) return mlp_tc_launch_one<HH, CC, false, true>(xmap, m, l, none, sm_count, stream);
+  UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
+#undef UML_TC_CASE
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_mlp_tc_topk(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
+                               const FlagList& flags, int sm_count, cudaStream_t stream) {
+  if (l.n_rows <= 0) return cudaSuccess;
+  if (l.topk_k < 1 || l.topk_k > std::min(m.n_classes, kMlpTopkMax)) return cudaErrorInvalidValue;
+#define UML_TC_CASE(HH, CC)                                                                                  \
+  if (m.n_hidden == HH && m.n_classes == CC)                                                                 \
+    return exact ? mlp_tc_launch_one<HH, CC, true, false, true>(xmap, m, l, flags, sm_count, stream)         \
+                 : mlp_tc_launch_one<HH, CC, false, false, true>(xmap, m, l, flags, sm_count, stream);
   UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
 #undef UML_TC_CASE
   return cudaErrorInvalidValue;

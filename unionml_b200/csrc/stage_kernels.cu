@@ -326,6 +326,45 @@ __global__ void __launch_bounds__(256) labels_count_equal_kernel(const void* __r
   if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
 }
 
+// top-k hits (the quickdraw template's accuracy(output, target, topk)): per row the first rank j whose class value is
+// the target, counted per j in shared memory; the host's running sum gives the hits within the first k' classes
+constexpr int kTopkHitsShared = 1024;  // ranks counted in shared memory; a later first hit (k > 1024) goes to global
+
+__global__ void __launch_bounds__(256) topk_first_hits_kernel(const int32_t* __restrict__ idx, int k, long long n,
+                                                              const double* __restrict__ classes, int n_classes,
+                                                              const double* __restrict__ targets,
+                                                              unsigned long long* first_hits) {
+  __shared__ unsigned long long hist[kTopkHitsShared];
+  const int ks = min(k, kTopkHitsShared);
+  for (int j = threadIdx.x; j < ks; j += blockDim.x) hist[j] = 0ull;
+  __syncthreads();
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const double t = targets[i];
+    const int32_t* row = idx + i * k;
+    for (int j = 0; j < k; ++j) {
+      const int c = row[j];
+      if (c >= 0 && c < n_classes && __ldg(classes + c) == t) {
+        if (j < ks) atomicAdd(&hist[j], 1ull);
+        else atomicAdd(&first_hits[j], 1ull);
+        break;
+      }
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < ks; j += blockDim.x)
+    if (hist[j]) atomicAdd(&first_hits[j], hist[j]);
+}
+
+cudaError_t launch_topk_first_hits(const int32_t* idx, int k, int64_t n, const double* classes, int n_classes,
+                                   const double* targets, unsigned long long* first_hits, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  const long long want = (n + 255) / 256;
+  const int grid = static_cast<int>(want < 132 * 4 ? want : 132 * 4);
+  topk_first_hits_kernel<<<grid, 256, 0, stream>>>(idx, k, n, classes, n_classes, targets, first_hits);
+  return cudaGetLastError();
+}
+
 // int32 labels -> every target vector of a fused exchange
 struct ScatterParams {
   const int32_t* labels;

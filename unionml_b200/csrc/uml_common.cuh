@@ -203,16 +203,21 @@ struct MlpTcLaunch {
   long long row_offset;
   long long n_rows;
   float* proba;  // launch_mlp_tc_proba: class probabilities [n_rows][n_classes] (device)
+  // launch_mlp_tc_topk: [n_rows][topk_k] class indices and probabilities (device; topk_proba may be nullptr)
+  int32_t* topk_idx;
+  float* topk_proba;
+  int topk_k;
 };
-// proba: the tile kernel's probability form (n_rows x n_classes fp32 instead of labels; exact and flags unused)
-bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why, bool proba = false);
+// proba: the tile kernel's probability form (n_rows x n_classes fp32 instead of labels; exact and flags unused);
+// topk: its top-k form (mlp_topk.cuh)
+bool mlp_tma_supported(const MlpDeviceModel& m, std::string* why, bool proba = false, bool topk = false);
 cudaError_t launch_mlp_tma(const CUtensorMap& xmap, const MlpDeviceModel& m, const float* x, int64_t n_rows,
                            int32_t* labels, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream,
                            float* proba = nullptr);
 cudaError_t launch_mlp_rescore_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows,
                                    const MlpTcLaunch& out, const FlagList& flags, bool all_rows, int sm_count,
                                    cudaStream_t stream);
-bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why);
+bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why, bool topk = false);
 std::vector<float> mlp_tc_build_w1_tiles(const float* w1, int H, int F, int f_pad);
 // exact: flagged rows go to the flag list; the caller launches launch_mlp_rescore_f64 behind it
 cudaError_t launch_mlp_tc(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
@@ -223,6 +228,19 @@ cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m
                                 cudaStream_t stream);
 cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, float* proba,
                                  int sm_count, cudaStream_t stream);
+// top-k class indices [n_rows][k] (and probabilities, proba != nullptr) of every row, 1 <= k <= min(C, kMlpTopkMax):
+// the tile kernels' top-k forms.  exact: rows the rank guard cannot certify go to the flag list; the caller launches
+// launch_mlp_topk_f64 (all_rows = false) behind them.  launch_mlp_topk_f64 with all_rows: any shape and any k <= C.
+cudaError_t launch_mlp_tc_topk(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
+                               const FlagList& flags, int sm_count, cudaStream_t stream);
+cudaError_t launch_mlp_tma_topk(const CUtensorMap& xmap, const MlpDeviceModel& m, int64_t n_rows, int k, int32_t* idx,
+                                float* proba, bool exact, const FlagList& flags, int sm_count, cudaStream_t stream);
+cudaError_t launch_mlp_topk_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, int k, int32_t* idx,
+                                float* proba, const FlagList& flags, bool all_rows, int sm_count, cudaStream_t stream);
+// top-k hits (stage_kernels.cu): first_hits[j] += rows whose target is classes[idx[row][j]] and no earlier rank's
+// class; the running sum over j is the number of rows with the target among their first j + 1 classes
+cudaError_t launch_topk_first_hits(const int32_t* idx, int k, int64_t n, const double* classes, int n_classes,
+                                   const double* targets, unsigned long long* first_hits, cudaStream_t stream);
 // small-batch kernel of the online path (B <= 64): four rows per warp through the fp64 scorer, the features read
 // straight from the raw source view and cast to fp32 as the staging kernels cast them.  mlp_small_smem_bytes: its
 // dynamic shared memory for the model's shape, 0 when that exceeds one SM; mlp_small_reserve sets the kernel's

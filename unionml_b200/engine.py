@@ -299,6 +299,50 @@ class Engine:
             self._check(st)
         return out, stats.as_dict() if stats else None
 
+    def predict_mlp_topk(self, model: MlpModel, batch: Batch, k: int, exact: bool = True, want_proba: bool = True,
+                         idx_device_ptr: Optional[int] = None, proba_device_ptr: Optional[int] = None,
+                         want_stats: bool = True) -> Tuple[Optional[np.ndarray], Optional[np.ndarray], Optional[dict]]:
+        """The ``k`` most probable classes per row, ``(indices int32 (n, k), probabilities float32 (n, k) | None,
+        stats)``: descending logits, ties to the lower class index; column 0 is :meth:`predict_mlp`'s label in the same
+        mode.  ``exact``: the indices of the float64 network (rows the fp32 rank guard cannot certify are re-scored in
+        float64).  With ``idx_device_ptr`` (and ``proba_device_ptr`` when ``want_proba``) the results are written to
+        device memory and ``None`` is returned in their place."""
+        mode = N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
+        stats = N.Stats() if want_stats else None
+        on_device = idx_device_ptr is not None
+        if on_device and want_proba and proba_device_ptr is None:
+            raise ValueError("want_proba with device outputs needs proba_device_ptr")
+        with self._lock:
+            if on_device:
+                idx_p, proba_p = C.c_void_p(idx_device_ptr), C.c_void_p(proba_device_ptr) if want_proba else None
+                idx = proba = None
+            else:
+                idx = np.empty((batch.n_rows, max(int(k), 0)), dtype=np.int32)
+                proba = np.empty((batch.n_rows, max(int(k), 0)), dtype=np.float32) if want_proba else None
+                idx_p = idx.ctypes.data_as(C.c_void_p)
+                proba_p = None if proba is None else proba.ctypes.data_as(C.c_void_p)
+            st = N.lib().uml_mlp_predict_topk(
+                self._h, model._h, batch._h, int(k), idx_p, proba_p, 1 if on_device else 0, mode,
+                C.byref(stats) if stats else None
+            )
+            self._check(st)
+        return idx, proba, stats.as_dict() if stats else None
+
+    def count_topk_hits(self, idx_ptr: int, k: int, n: int, classes, targets) -> np.ndarray:
+        """``hits[j]`` = rows whose target is ``classes[idx[row, j']]`` for some ``j' <= j`` (int64, length ``k``), from
+        ``n x k`` int32 class indices in device memory (:meth:`predict_mlp_topk`), reduced on the device."""
+        classes = np.ascontiguousarray(classes, dtype=np.float64)
+        targets = np.ascontiguousarray(targets, dtype=np.float64)
+        if targets.shape != (n,):
+            raise ValueError("targets must be a vector of length n")
+        hits = np.zeros(max(int(k), 1), dtype=np.int64)
+        with self._lock:
+            st = N.lib().uml_topk_count_hits(self._h, C.c_void_p(idx_ptr), int(k), n, classes.ctypes.data_as(C.c_void_p),
+                                             len(classes), targets.ctypes.data_as(C.c_void_p),
+                                             hits.ctypes.data_as(C.c_void_p))
+            self._check(st)
+        return hits[:k]
+
     def predict_mlp_peers(self, model: MlpModel, batch: Batch, peer_ptrs, row_offset: int, exact: bool = True,
                           want_stats: bool = False, label_bytes: int = 4) -> Optional[dict]:
         """Fused compute + all-gather for the MLP predictor (same contract as :meth:`predict_peers`)."""

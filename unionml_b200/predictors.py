@@ -370,3 +370,79 @@ def mlp_predict_proba(module: Any, features: Any) -> np.ndarray:
         return out
     finally:
         batch.free()
+
+
+def _check_topk(k, n_classes: int) -> int:
+    if isinstance(k, bool) or int(k) != k or not 1 <= int(k) <= n_classes:
+        raise ValueError(f"k = {k}: selected index k out of range (the module has {n_classes} classes)")
+    return int(k)
+
+
+def mlp_predict_topk(module: Any, features: Any, k: int = 3) -> tuple:
+    """``torch.topk(module(process_features(features)), k)`` of the quickdraw template's predictor on the GPU:
+    ``(values, indices)``, the ``k`` largest class probabilities per row as a float32 ``(n, k)`` ndarray and their
+    class indices as int64 ``(n, k)``, in descending order.  Probabilities are those of :func:`mlp_predict_proba`;
+    the indices are the float64 network's ranks (``UNIONML_B200_MODE=fast``: the fp32 kernel's), ties to the lower
+    class index.  The guards of :func:`mlp_predict_proba` apply; ``k`` outside ``1 .. n_out`` raises ``ValueError``."""
+    engine = get_engine()
+    dm = device_mlp(module, engine)
+    k = _check_topk(k, dm.n_classes)
+    arr = features.to_numpy() if hasattr(features, "to_numpy") else np.asarray(features)
+    _check_min_samples(arr)
+    batch = engine.stage(arr, keep_f64=False)
+    try:
+        idx, proba, stats = engine.predict_mlp_topk(dm, batch, k, exact=_exact_default())
+    finally:
+        batch.free()
+    _note_ambiguous(stats)
+    return proba, idx.astype(np.int64)
+
+
+def _mlp_staged_targets(engine, features, target):
+    arr = features.to_numpy() if hasattr(features, "to_numpy") else np.asarray(features)
+    _check_min_samples(arr)
+    batch = engine.stage(arr, keep_f64=False)
+    y = np.asarray(target.to_numpy() if hasattr(target, "to_numpy") else target, dtype=np.float64).reshape(-1)
+    if y.shape[0] != batch.n_rows:
+        batch.free()
+        raise ValueError(f"Found input variables with inconsistent numbers of samples: [{y.shape[0]}, {batch.n_rows}]")
+    return batch, y
+
+
+def mlp_accuracy(module: Any, features: Any, target: Any) -> float:
+    """The torch quickstart's evaluator ``accuracy_score(target, predictor(module, features))`` with the predictor
+    :func:`mlp_argmax` (``float(class index)`` per row) on the device: the labels and the match count never leave
+    the GPU.  Labels are exact by default (``UNIONML_B200_MODE``)."""
+    engine = get_engine()
+    dm = device_mlp(module, engine)
+    batch, y = _mlp_staged_targets(engine, features, target)
+    try:
+        labels = engine.device_alloc(4 * batch.n_rows)
+        _, stats = engine.predict_mlp(dm, batch, exact=_exact_default(), out_device_ptr=labels.ptr, want_stats=True)
+        _note_ambiguous(stats)
+        hits = engine.count_equal(labels.ptr, batch.n_rows, np.arange(dm.n_classes, dtype=np.float64), y)
+        return hits / batch.n_rows
+    finally:
+        batch.free()
+
+
+def mlp_topk_accuracy(module: Any, features: Any, target: Any, topk=(1, 5)) -> list:
+    """The quickdraw template's ``accuracy(module(x), target, topk)`` (``quickdraw/model.py:20-27``) on the device, as
+    fractions: one entry per ``k`` in ``topk``, the share of rows whose target class index is among their first
+    ``min(k, n_out)`` classes.  One top-k call and one hit count serve every entry."""
+    engine = get_engine()
+    dm = device_mlp(module, engine)
+    ks = [int(k) for k in topk]
+    if not ks or min(ks) < 1:
+        raise ValueError(f"topk = {tuple(topk)}: every k must be >= 1")
+    kmax = min(max(ks), dm.n_classes)
+    batch, y = _mlp_staged_targets(engine, features, target)
+    try:
+        idx = engine.device_alloc(4 * batch.n_rows * kmax)
+        _, _, stats = engine.predict_mlp_topk(dm, batch, kmax, exact=_exact_default(), want_proba=False,
+                                              idx_device_ptr=idx.ptr, want_stats=True)
+        _note_ambiguous(stats)
+        hits = engine.count_topk_hits(idx.ptr, kmax, batch.n_rows, np.arange(dm.n_classes, dtype=np.float64), y)
+        return [float(hits[min(k, kmax) - 1]) / batch.n_rows for k in ks]
+    finally:
+        batch.free()
