@@ -77,6 +77,8 @@ typedef struct uml_stats {
                               (wgmma) kernel, 4 = small-batch fp64 kernel of the online path, linear or MLP
                               (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph), 6 = float64
                               decision_function scores kernel                                                             */
+  int32_t x_elem_bytes;    /* predict calls on a resident batch: bytes per feature of the rows the scoring kernel read -
+                              2 = the batch's compact fp16 copy (linear tile kernel), 4 = its fp32 rows; 0 otherwise    */
 } uml_stats;
 
 typedef struct uml_device_info {
@@ -117,7 +119,10 @@ UML_API int uml_linear_set_affine(uml_engine* e, uml_model* m, const double* shi
 /* ---- batch: Dataset.get_features output (dataset.py:350-359) staged once into HBM ---------------------------- */
 /* host rows -> device fp32 row-major (transpose / down-cast on the GPU).  Strides are in bytes; a pandas block is
  * feature-major (col_stride < row_stride is NOT required: either order is taken).  Checks finiteness like
- * check_array (validation.py:107) unless UML_STAGE_SKIP_FINITE_CHECK. */
+ * check_array (validation.py:107) unless UML_STAGE_SKIP_FINITE_CHECK.  When F <= 64 and the staging pass saw every value
+ * to be an fp16 value (integer features up to 2048, pixels 0..255, ...), the batch also keeps a compact fp16 copy (2 F
+ * bytes per row on top of the 4 F of the fp32 rows) that the linear predictor reads instead: same labels, half the
+ * bytes. */
 UML_API int uml_stage_rows(uml_engine* e, uml_batch** out, const void* host_ptr, int64_t n_rows, int n_features,
                    int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, uint32_t flags);
 /* wrap rows that already live in HBM (fp32, row-major, leading dimension ld floats, ld % 4 == 0, 16-byte aligned) */

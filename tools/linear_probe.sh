@@ -1,5 +1,7 @@
 #!/bin/bash
-# Read ceiling + feed-only + wait-clock + timeline breakdown of the linear tile kernel (tools/linear_probe.cu), on GPU 0.
+# Read ceiling + feed-only + wait-clock + timeline breakdown of the linear tile kernel (tools/linear_probe.cu), on GPU 0,
+# for each schedule: chunked and whole fp32 rows, and the compact fp16 rows (whose feed-only and wait-clock lines say
+# whether that schedule is bound by its feed or by its scoring warps).
 # Writes MEASURED_PEAKS.json (the read ceiling bench.py's roofline divides by) and the probe's JSON lines to
 # ${1:-build/probe}/linear_probe.jsonl.  Binaries go to build/probe/.
 set -euo pipefail
@@ -24,7 +26,7 @@ nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noh
 python3 - "$out/linear_probe.jsonl" <<'PY'
 import json, sys
 rows = [json.loads(l) for l in open(sys.argv[1]) if l.startswith("{")]
-ceiling = [r for r in rows if r["probe"] == "read_ceiling"][-1]
+ceiling = [r for r in rows if r["probe"] == "read_ceiling"][-1]  # the 2.56 GB one (fp32 rows of the cfg2 shape)
 json.dump({"hbm_gbs": ceiling["hbm_gbs"], "device": ceiling["device"],
            "method": "tools/linear_probe.cu read_kernel, 2.56 GB, 16-byte ld.global.nc.L1::no_allocate, >= 0.5 s"},
           open("MEASURED_PEAKS.json", "w"))

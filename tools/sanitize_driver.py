@@ -63,4 +63,20 @@ pb = eng.device_alloc(4 * (3 * b.n_rows + 1))
 eng.predict_mlp_topk(mlp, b, 3, idx_device_ptr=kb.ptr + 4, proba_device_ptr=pb.ptr + 4)
 eng.predict_mlp_topk(mlp, b, 3, want_proba=False, idx_device_ptr=kb.ptr)
 eng.count_topk_hits(kb.ptr, 3, b.n_rows, np.arange(10.0), np.zeros(b.n_rows))
+# compact fp16 rows: `b` holds integers, so staging packed its fp16 copy and the linear predicts above ran the tile
+# kernel's fp16 schedule; here also pinned float32 rows (finite-scan staging), F = 7 (the box's first 32 features
+# only) with peer stores at an odd offset, and the same batch on the fp32 route through the test hook
+bp = eng.pinned_empty(X.shape, np.float32)
+bp[:] = X
+b16 = eng.stage(bp)
+for exact in (True, False):
+    assert eng.predict(m, b16, exact=exact)[1]["x_elem_bytes"] == 2
+m7 = eng.load_linear(rng.standard_normal((10, 7)), rng.standard_normal(10))
+b7 = eng.stage(X[:, :7])
+eng.predict(m7, b7, exact=True)
+buf7 = eng.device_alloc(b7.n_rows + 3)
+eng.predict_peers(m7, b7, [buf7.ptr], 3, exact=True, want_stats=True, label_bytes=1)
+_os.environ["UML_B200_COMPACT_ROWS"] = "0"
+assert eng.predict(m, b16, exact=True)[1]["x_elem_bytes"] == 4
+del _os.environ["UML_B200_COMPACT_ROWS"]
 print("sanitizer driver ok")

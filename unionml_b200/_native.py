@@ -31,6 +31,7 @@ class Stats(C.Structure):
         ("d2h_bytes", C.c_int64),
         ("kernel_launches", C.c_int32),
         ("path", C.c_int32),
+        ("x_elem_bytes", C.c_int32),
     ]
 
     def as_dict(self) -> dict:

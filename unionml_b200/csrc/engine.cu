@@ -245,6 +245,12 @@ struct uml_batch {
   bool has_map = false;
   CUtensorMap map{};      // boxes of 128 rows x 32 features (MLP kernels)
   CUtensorMap lin_map{};  // boxes of uml::linear_box_rows(f_pad) rows x 32 features (linear tile kernel)
+  // compact fp16 copy of the rows (staged batches with F <= 64 whose every value is an fp16 value): what the linear
+  // tile kernel reads instead of x, through half_map's {64 features, 128 rows} boxes.  ldh = uml::linear_half_ld(F).
+  void* xh = nullptr;
+  int64_t ldh = 0;
+  bool has_half = false;
+  CUtensorMap half_map{};
 };
 
 struct uml_mlp {
@@ -678,6 +684,40 @@ static int encode_batch_maps(uml_engine* e, uml_batch* b) {
   return rc;
 }
 
+// the compact fp16 copy of a staged batch whose staging pass found every value to be an fp16 value (stage.not_f16 == 0):
+// one pack kernel from the fp32 rows and its tensor map.  The copy is an optimisation: when there is no room for it the
+// batch keeps the fp32 route, and the call still succeeds.
+static int build_half_copy(uml_engine* e, uml_batch* b) {
+  const int F = b->n_features;
+  const int64_t ldh = uml::linear_half_ld(F);
+  if (cudaMalloc(&b->xh, (size_t)b->n_rows * ldh * 2) != cudaSuccess) {
+    (void)cudaGetLastError();
+    b->xh = nullptr;
+    return UML_OK;
+  }
+  b->ldh = ldh;
+  UML_CUDA(e, uml::launch_pack_half(b->x, b->ld, b->n_rows, F, b->xh, ldh, e->stream));
+  cuuint64_t gdim[2] = {(cuuint64_t)F, (cuuint64_t)b->n_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)ldh * 2};
+  cuuint32_t box[2] = {(cuuint32_t)uml::kHalfBoxF, (cuuint32_t)uml::kTileRows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = e->encode(&b->half_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, b->xh, gdim, gstride, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) UML_FAIL(e, UML_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for the fp16 copy, %lld x %d", (int)r,
+                                  (long long)b->n_rows, F);
+  UML_CUDA(e, cudaStreamSynchronize(e->stream));  // later calls may run on another stream (uml_engine_set_stream)
+  b->has_half = true;
+  return UML_OK;
+}
+
+// UML_B200_COMPACT_ROWS=0 makes the linear tile kernel read the fp32 rows of a batch that has an fp16 copy (test and A/B
+// hook, read per call)
+static bool compact_rows_enabled() {
+  const char* env = getenv("UML_B200_COMPACT_ROWS");
+  return !(env && env[0] == '0');
+}
+
 int uml_batch_from_device(uml_engine* e, uml_batch** out, const void* dev_ptr, int64_t n_rows, int n_features,
                           int64_t ld) {
   if (!e || !out || (!dev_ptr && n_rows > 0) || n_rows < 0 || n_features < 1 || ld < n_features) return UML_ERR_INVALID;
@@ -946,6 +986,9 @@ int uml_stage_rows(uml_engine* e, uml_batch** out, const void* host_ptr, int64_t
   }
   rc = encode_batch_maps(e, b.get());
   if (rc != UML_OK && rc != UML_ERR_UNSUPPORTED) return rc;
+  if (rc == UML_OK && (check || !direct) && e->h->stage.not_f16 == 0 && F <= uml::kHalfBoxF &&
+      (rc = build_half_copy(e, b.get())) != UML_OK)
+    return rc;
   *out = b.release();
   return UML_OK;
 }
@@ -966,6 +1009,7 @@ void uml_batch_free(uml_batch* b) {
   if (b->e) cudaSetDevice(b->e->device);
   if (b->owns) cudaFree(b->x);
   cudaFree(b->x64);
+  cudaFree(b->xh);
   delete b;
 }
 
@@ -973,9 +1017,11 @@ void uml_batch_free(uml_batch* b) {
 // predict
 // ---------------------------------------------------------------------------------------------------------------
 // enqueue the scoring of one resident block of rows on e->stream; no host synchronisation.
-// ev_k (optional) brackets the scoring kernel, ev_r the fp64 re-score.
-static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch& l, const CUtensorMap* map, int mode,
-                           bool timed, int* launches, int* path) {
+// ev_k (optional) brackets the scoring kernel, ev_r the fp64 re-score.  half_map (optional): the rows' compact fp16
+// copy, which the tile kernel then reads; *x_elem_bytes (optional) gets the bytes per feature it read (2 or 4).
+static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch& l, const CUtensorMap* map,
+                           const CUtensorMap* half_map, int mode, bool timed, int* launches, int* path,
+                           int* x_elem_bytes = nullptr) {
   const FlagList fl = flag_list(e);
   const bool exact = mode == UML_PREDICT_EXACT;
   std::string why;
@@ -985,10 +1031,13 @@ static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch
     NvtxRange r_score("uml:score");
     std::string err;
     bool need_rescore = false;
-    cudaError_t ce = uml::launch_linear_tma(*map, m->dm, l, exact, fl, e->info.sm_count, e->stream, &err, &need_rescore);
+    if (half_map && !uml::linear_half_rows_ok(m->dm.f_pad)) half_map = nullptr;
+    cudaError_t ce = uml::launch_linear_tma(*map, half_map, m->dm, l, exact, fl, e->info.sm_count, e->stream, &err,
+                                            &need_rescore);
     if (ce != cudaSuccess) UML_FAIL(e, UML_ERR_CUDA, "linear_argmax_tma launch: %s %s", cudaGetErrorString(ce), err.c_str());
     *launches += 1;
     *path = 1;
+    if (x_elem_bytes) *x_elem_bytes = half_map ? 2 : 4;
     if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
     if (need_rescore) {  // UML_B200_RESCORE_MODE=kernel; in queue mode flagged rows are re-scored by a warp of the tile kernel
       NvtxRange r_rescore("uml:rescore_f64");
@@ -1083,8 +1132,9 @@ static int finish_stats(uml_engine* e, uml_stats* stats, int64_t n_rows, int lau
 
 // One predict call on a resident batch, linear or MLP.  `model` names the model in the feature-count message
 // ("estimator" as scikit-learn words it, "module" as the torch app does).  prepare() makes the model's host-side
-// choices before the first timed stream operation; score(labels, timed, &launches, &path) enqueues its scoring step.
-// labels: host-label scratch or the caller's device vector; nullptr with peers, which each model's step serves.
+// choices before the first timed stream operation; score(labels, timed, &launches, &path, &x_elem_bytes) enqueues its
+// scoring step (x_elem_bytes: bytes per feature its kernel read, preset to 4).  labels: host-label scratch or the
+// caller's device vector; nullptr with peers, which each model's step serves.
 extern "C++" {  // a template cannot have the C linkage of the ABI section around it
 template <class Prepare, class Score>
 static int predict_resident(uml_engine* e, const uml_batch* b, int n_classes, int n_features, const char* model,
@@ -1118,13 +1168,16 @@ static int predict_resident(uml_engine* e, const uml_batch* b, int n_classes, in
   // The asynchronous step (device labels, no stats) needs no memset at all: the flag list is handed back empty by the
   // previous re-score kernel.
   if (sync_call) UML_CUDA(e, reset_counters(e, e->stream));
-  int launches = 0, path = 0;
-  if ((rc = score(d_labels, timed, &launches, &path)) != UML_OK) return rc;
+  int launches = 0, path = 0, elem_bytes = 4;
+  if ((rc = score(d_labels, timed, &launches, &path, &elem_bytes)) != UML_OK) return rc;
   if (!sync_call) return UML_OK;
   if (!labels_on_device)
     UML_CUDA(e, cudaMemcpyAsync(labels_out, d_labels, (size_t)b->n_rows * 4, cudaMemcpyDeviceToHost, e->stream));
   rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
-  if (stats) stats->d2h_bytes = labels_on_device ? 0 : b->n_rows * 4;
+  if (stats) {
+    stats->d2h_bytes = labels_on_device ? 0 : b->n_rows * 4;
+    stats->x_elem_bytes = elem_bytes;
+  }
   return rc;
 }
 }  // extern "C++"
@@ -1133,7 +1186,7 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
                                    int labels_on_device, void* const* peers, int n_peers, int64_t row_offset,
                                    int label_bytes, int mode, uml_stats* stats) {
   if (!m) return UML_ERR_INVALID;
-  auto score = [&](int32_t* labels, bool timed, int* launches, int* path) {
+  auto score = [&](int32_t* labels, bool timed, int* launches, int* path, int* elem_bytes) {
     LinearLaunch l{};
     l.x = b->x;
     l.x64 = b->x64;
@@ -1149,7 +1202,8 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
     if (own) l.labels = static_cast<int32_t*>(peers[0]) + row_offset;
     l.n_peers = n_peers - own;
     for (int i = 0; i < l.n_peers; ++i) l.peers[i] = peers[own + i];
-    return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, mode, timed, launches, path);
+    const CUtensorMap* half = b->has_half && compact_rows_enabled() ? &b->half_map : nullptr;
+    return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, half, mode, timed, launches, path, elem_bytes);
   };
   return predict_resident(e, b, m->dm.n_classes, m->n_features_in, "estimator", labels_out, labels_on_device, n_peers,
                           label_bytes, mode, stats, [] { return (int)UML_OK; }, score);
@@ -1646,7 +1700,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
         rc = enqueue_mlp(e, mlp->dm, map, xc, ld, out, exact, mlp_route(mlp->dm, has_map, false, tf32), false, &launches,
                          &path);
       } else {
-        rc = enqueue_predict(e, m, l, has_map ? &map : nullptr, mode, false, &launches, &path);
+        rc = enqueue_predict(e, m, l, has_map ? &map : nullptr, nullptr, mode, false, &launches, &path);
       }
     }
     if (rc != UML_OK) {
@@ -2028,7 +2082,7 @@ static int mlp_predict_resident(uml_engine* e, const uml_mlp* m, const uml_batch
     // scratch for the CUDA-core kernel's labels on their way to the peers (enqueue_mlp)
     return route == 3 && n_peers > 0 ? grow(e, e->d_labels, b->n_rows) : (int)UML_OK;
   };
-  auto score = [&](int32_t* labels, bool timed, int* launches, int* path) {
+  auto score = [&](int32_t* labels, bool timed, int* launches, int* path, int*) {  // the MLP kernels read fp32 rows
     uml::MlpTcLaunch out{};
     out.labels = labels;
     out.n_rows = b->n_rows;

@@ -3,9 +3,10 @@
 // Replaces the numeric body of sklearn's LinearClassifierMixin.predict (sklearn/linear_model/_base.py:366-427), which
 // is what the reference's canonical predictor runs (unionml:README.md:87-92).
 //
-//  * linear_argmax_tma_kernel<C, EXACT, QUEUE, WHOLE>: persistent, warp-specialised.  One producer warp streams X
+//  * linear_argmax_tma_kernel<C, EXACT, QUEUE, SCHED>: persistent, warp-specialised.  One producer warp streams X
 //    through a 16 KiB-per-stage shared-memory ring with TMA + mbarriers: 128-row x 32-feature boxes (128B-swizzled), or
-//    at 33 <= F <= 64 (WHOLE) stages of 64 complete rows; eight consumer warps each own one tile at a time (4 or 2
+//    at 33 <= F <= 64 (kWhole) stages of 64 complete rows, or (kHalf) stages of 128 complete rows from the batch's
+//    compact fp16 copy; eight consumer warps each own one tile at a time (4 or 2
 //    rows per lane), read X with conflict-free LDS.128, W as warp-uniform broadcast
 //    LDS.128 from a transposed copy in shared memory, keep C (+1) fp32 accumulators per row in registers, and fuse
 //    bias, argmax (first maximum wins, like np.argmax) and the label store.  In EXACT mode one extra accumulator
@@ -13,6 +14,8 @@
 //    rounding error (2 (F+4) 2^-24 A) are appended to a list and re-scored in fp64 by rescore_f64_kernel.
 //  * rescore_f64_kernel: warp per row, lanes over features, fp64 FMA + shuffle reduction; serves the flagged rows of
 //    EXACT mode and is the generic (any F, any C) path when the tile kernel's shape limits do not hold.
+#include <cuda_fp16.h>
+
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -179,7 +182,7 @@ __device__ __noinline__ int rescore_row_inline(const TmaKernelParams& p, long lo
   return r.idx;
 }
 
-constexpr int kTileSentinel = -1;        // WHOLE: ring item that ends a scoring warp's loop
+constexpr int kTileSentinel = -1;        // claimed schedules: ring item that ends a scoring warp's loop
 constexpr int kQueueCap = 2048;           // flagged-row queue of the QUEUE kernels (power of two)
 constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this many slots are free (8 warps x 128 rows)
 constexpr int kThreadsQueue = kThreads + 32;  // + 1 fp64 re-score warp
@@ -236,19 +239,29 @@ __device__ __forceinline__ unsigned long long probe_globaltimer() {
 #define UML_PROBE_RELEASED()
 #endif
 
-// WHOLE (f_pad == 64, linear_whole_rows): one ring stage is one 64-row tile with all its features, loaded as two
-// {32 features, 64 rows} boxes onto one barrier; the producer claims the tiles in groups of 8 from a global counter
-// and ring item n goes to warp n % 8 (2 rows per lane).  Otherwise one stage is a 128-row x 32-feature box, a tile
-// takes f_pad / 32 stages (4 rows per lane) and the CTA scores tiles blockIdx.x, blockIdx.x + gridDim.x, ...
-template <int C, bool EXACT, bool QUEUE, bool WHOLE>
+// How the ring is fed (the schedule):
+//  kChunked  one stage is a 128-row x 32-feature fp32 box, a tile takes f_pad / 32 stages (4 rows per lane) and the
+//            CTA scores tiles blockIdx.x, blockIdx.x + gridDim.x, ...
+//  kWhole    (f_pad == 64, linear_whole_rows) one stage is one 64-row tile with all its features, loaded as two
+//            {32 features, 64 rows} fp32 boxes onto one barrier (2 rows per lane)
+//  kHalf     (f_pad <= 64, the batch has a compact fp16 copy) one stage is one 128-row tile with all its features, one
+//            {64 features, 128 rows} fp16 box (4 rows per lane)
+// kWhole and kHalf claim their tiles in groups of 8 from a global counter; ring item n goes to warp n % 8.
+enum class LinearSched { kChunked, kWhole, kHalf };
+
+template <int C, bool EXACT, bool QUEUE, LinearSched SCHED>
 __global__ void __launch_bounds__(kThreadsQueue, 1)
 linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ TmaKernelParams p) {
   constexpr int NCOL = C + (EXACT ? 1 : 0);  // accumulators per row (classes + error-bound column)
   constexpr int CP = (C + 1 + 3) / 4 * 4;    // padded columns of wt in shared memory (layout shared by both modes)
   constexpr int NW4 = (NCOL + 3) / 4;        // float4 loads of W per feature
+  constexpr bool WHOLE = SCHED == LinearSched::kWhole;
+  constexpr bool HALF = SCHED == LinearSched::kHalf;
+  constexpr bool CLAIMED = WHOLE || HALF;                    // tiles claimed from p.counters[4], one tile per stage
   constexpr int TILE = WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = rows per TMA box
   constexpr int R = TILE / 32;                               // rows per lane
-  constexpr int BOX_BYTES = TILE * kChunkF * 4;              // one {32, TILE} box: 8 KiB (two per stage) or 16 KiB
+  constexpr int BOX_BYTES = TILE * kChunkF * 4;              // one box: 8 KiB (two per kWhole stage) or 16 KiB
+  static_assert(!HALF || BOX_BYTES == kTileRows * kHalfBoxF * 2, "an fp16 box is one stage");
   constexpr bool USE_F2 = EXACT;  // fp32x2 accumulator pairs (see the accumulator comment below)
 
   extern __shared__ uint8_t smem_raw[];
@@ -264,7 +277,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   // warps done, ctl[3] = slots consumed
   int* q_slots = reinterpret_cast<int*>(empty_bar + S);
   int* q_ctl = q_slots + kQueueCap;
-  // WHOLE: the tile each stage holds, written by the producer before the stage's `full` arrive (whose release makes it
+  // CLAIMED: the tile each stage holds, written by the producer before the stage's `full` arrive (whose release makes it
   // visible to the waiters); kTileSentinel ends a scoring warp's loop
   int* tile_slot = q_ctl + 4;
 
@@ -317,7 +330,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           phase ^= 1u;
         }
       };
-      if constexpr (WHOLE) {
+      if constexpr (CLAIMED) {
         // Tiles are claimed, kConsumerWarps at a time, from a counter shared by the grid: with a static split, CTAs
         // with equal tile counts finished up to ~0.24 ms apart (SMs draw unequal shares of HBM bandwidth), and the
         // launch lasted as long as the slowest one.  Ring item n is one tile with both halves of its rows and goes to
@@ -338,7 +351,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
               uint8_t* dst = smem + static_cast<size_t>(stage) * kStageBytes;
               const int row = static_cast<int>(tile * TILE);
               tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
-              tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], kChunkF, row, policy);
+              if constexpr (WHOLE) tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], kChunkF, row, policy);
 #ifdef UML_PROBE_TIMELINE
               if (probe_first_issue) UML_PROBE_STAMP(1);
               probe_first_issue = false;
@@ -389,7 +402,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     // lane l owns rows l, l+32, ... of the tile.  In every box row r sits at byte r*128 with its 16-byte chunks
     // XOR-swizzled by (r & 7); r & 7 == l & 7 for all of a lane's rows, so one swizzle term serves them all and the
     // eight lanes of every LDS.128 phase (lanes 8i..8i+7: l & 7 = 0..7) hit eight distinct bank groups.  The whole-row
-    // stage is two such boxes (features 0-31, then 32-63 at +8 KiB), so the same holds in both halves.
+    // stage is two such boxes (features 0-31, then 32-63 at +8 KiB), so the same holds in both halves; an fp16 row is
+    // 64 halves in the same 128 bytes, so the same addresses serve it.
     const uint32_t lanebase = static_cast<uint32_t>(lane) * 128u + static_cast<uint32_t>(lane & 7) * 16u;
 #ifdef UML_PROBE_WAIT_CLOCKS
     long long probe_hold = 0;
@@ -419,6 +433,20 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         }
       }
     };
+    // one feature x of row j with wv = its W^T row: every class accumulator and the bound column
+    auto fma_feature = [&](int j, float x, const float* wv) {
+      if constexpr (USE_F2) {
+        const uint64_t xx = pack2(x, x);
+#pragma unroll
+        for (int i = 0; i < NPAIR; ++i) acc2[j][i] = fma2(xx, pack2(wv[2 * i], wv[2 * i + 1]), acc2[j][i]);
+        if (ODD) acc_last[j] = fmaf(x, wv[C - 1], acc_last[j]);
+        if (EXACT) acc_bound[j] = fmaf(fabsf(x), wv[C], acc_bound[j]);
+      } else {
+#pragma unroll
+        for (int c = 0; c < C; ++c) acc[j][c] = fmaf(x, wv[c], acc[j][c]);
+        if (EXACT) acc[j][C] = fmaf(fabsf(x), wv[C], acc[j][C]);
+      }
+    };
     // features kChunkF*k .. +31 of the lane's rows from box xs, with wk = the W^T rows of those features; every row's
     // FMAs run in feature order, so scores do not depend on the schedule
     auto fma_box = [&](const uint8_t* xs, const float* wk) {
@@ -441,19 +469,38 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             wv[m * 4 + 3] = t.w;
           }
 #pragma unroll
+          for (int j = 0; j < R; ++j) fma_feature(j, e == 0 ? xv[j].x : e == 1 ? xv[j].y : e == 2 ? xv[j].z : xv[j].w, wv);
+        }
+      }
+    };
+
+    // kHalf: features 32*h .. 32*h + 31 of the lane's rows from the fp16 box (16-byte chunks 4h .. 4h + 3, eight
+    // features each).  cvt.f32.f16 is exact, so every FMA gets the operands the fp32 route gives it, in the same order
+    // and the same fma2 pairing: scores, flags and labels are those of the fp32 rows bit for bit.
+    auto fma_half = [&](const uint8_t* xs, int h) {
+      if constexpr (kFeedOnly) return;
+      const float* wk = wt_s + h * kChunkF * CP;
+#pragma unroll
+      for (int q = 0; q < kChunkF / 8; ++q) {
+        uint4 hv[R];
+        const uint32_t off = lanebase ^ static_cast<uint32_t>((4 * h + q) * 16);
+#pragma unroll
+        for (int j = 0; j < R; ++j) hv[j] = *reinterpret_cast<const uint4*>(xs + off + j * 32 * 128);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          float wv[NW4 * 4];
+#pragma unroll
+          for (int m = 0; m < NW4; ++m) {
+            const float4 t = *reinterpret_cast<const float4*>(wk + (q * 8 + e) * CP + m * 4);
+            wv[m * 4 + 0] = t.x;
+            wv[m * 4 + 1] = t.y;
+            wv[m * 4 + 2] = t.z;
+            wv[m * 4 + 3] = t.w;
+          }
+#pragma unroll
           for (int j = 0; j < R; ++j) {
-            const float x = e == 0 ? xv[j].x : e == 1 ? xv[j].y : e == 2 ? xv[j].z : xv[j].w;
-            if constexpr (USE_F2) {
-              const uint64_t xx = pack2(x, x);
-#pragma unroll
-              for (int i = 0; i < NPAIR; ++i) acc2[j][i] = fma2(xx, pack2(wv[2 * i], wv[2 * i + 1]), acc2[j][i]);
-              if (ODD) acc_last[j] = fmaf(x, wv[C - 1], acc_last[j]);
-              if (EXACT) acc_bound[j] = fmaf(fabsf(x), wv[C], acc_bound[j]);
-            } else {
-#pragma unroll
-              for (int c = 0; c < C; ++c) acc[j][c] = fmaf(x, wv[c], acc[j][c]);
-              if (EXACT) acc[j][C] = fmaf(fabsf(x), wv[C], acc[j][C]);
-            }
+            const uint32_t word = e < 2 ? hv[j].x : e < 4 ? hv[j].y : e < 6 ? hv[j].z : hv[j].w;
+            fma_feature(j, __half2float(__ushort_as_half(static_cast<unsigned short>((e & 1) ? word >> 16 : word & 0xffffu))), wv);
           }
         }
       }
@@ -593,7 +640,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       }
     };
 
-    if constexpr (WHOLE) {
+    if constexpr (CLAIMED) {
       // this warp's ring items are n = warp, warp + 8, ... (stage n % S, phase (n / S) & 1); S >= 8 lets stage and
       // phase advance without a division.  Both waits keep the invariant argued below: the next item is n + 8 <= n + S.
       uint32_t stage = static_cast<uint32_t>(warp), phase = 0;
@@ -606,8 +653,13 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         const bool scored = tile >= 0 && tile < num_tiles;
         if (scored) {
           const uint8_t* xs = smem + static_cast<size_t>(stage) * kStageBytes;
-          fma_box(xs, wt_s);
-          fma_box(xs + BOX_BYTES, wt_s + kChunkF * CP);
+          if constexpr (HALF) {
+            fma_half(xs, 0);
+            if (p.f_pad > kChunkF) fma_half(xs, 1);  // f_pad 32: the box's zero columns 32-63 are not scored
+          } else {
+            fma_box(xs, wt_s);
+            fma_box(xs + BOX_BYTES, wt_s + kChunkF * CP);
+          }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[stage]);  // hand the stage back to the producer
@@ -967,11 +1019,11 @@ cudaError_t launch_linear_proba(const LinearDeviceModel& m, const float* x, int6
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-static size_t tma_fixed_smem(const LinearDeviceModel& m) {
+static size_t tma_fixed_smem(const LinearDeviceModel& m, bool claimed = false) {
   // alignment slack + W^T + bias + barriers (64 stages max) + the flagged-row queue of the QUEUE kernels (+ the tile
-  // index of each stage, whole-row schedule)
+  // index of each stage, claimed schedules)
   return 1024 + static_cast<size_t>(m.f_pad) * m.cp * 4 + static_cast<size_t>(m.cp) * 4 + 2 * 64 * 8 + (kQueueCap + 4) * 4 +
-         (linear_whole_rows(m.f_pad) ? 64 * 4 : 0);
+         (claimed || linear_whole_rows(m.f_pad) ? 64 * 4 : 0);
 }
 
 bool linear_tma_supported(const LinearDeviceModel& m, std::string* why) {
@@ -987,10 +1039,10 @@ bool linear_tma_supported(const LinearDeviceModel& m, std::string* why) {
   return true;
 }
 
-template <int C, bool EXACT, bool QUEUE, bool WHOLE>
+template <int C, bool EXACT, bool QUEUE, LinearSched SCHED>
 static cudaError_t launch_one(const CUtensorMap& xmap, const TmaKernelParams& p, int grid, size_t smem,
                               cudaStream_t stream) {
-  auto kern = linear_argmax_tma_kernel<C, EXACT, QUEUE, WHOLE>;
+  auto kern = linear_argmax_tma_kernel<C, EXACT, QUEUE, SCHED>;
   static size_t configured = 0;  // per instantiation (one device per process): set the attribute once, not per launch
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -1001,13 +1053,13 @@ static cudaError_t launch_one(const CUtensorMap& xmap, const TmaKernelParams& p,
   return cudaGetLastError();
 }
 
-template <bool EXACT, bool QUEUE, bool WHOLE>
+template <bool EXACT, bool QUEUE, LinearSched SCHED>
 static cudaError_t dispatch_classes(int C, const CUtensorMap& xmap, const TmaKernelParams& p, int grid, size_t smem,
                                     cudaStream_t stream) {
   switch (C) {
 #define UML_CASE(N) \
   case N:           \
-    return launch_one<N, EXACT, QUEUE, WHOLE>(xmap, p, grid, smem, stream);
+    return launch_one<N, EXACT, QUEUE, SCHED>(xmap, p, grid, smem, stream);
     UML_CASE(2) UML_CASE(3) UML_CASE(4) UML_CASE(5) UML_CASE(6) UML_CASE(7) UML_CASE(8) UML_CASE(9) UML_CASE(10)
     UML_CASE(11) UML_CASE(12) UML_CASE(13) UML_CASE(14) UML_CASE(15) UML_CASE(16)
 #undef UML_CASE
@@ -1029,9 +1081,9 @@ bool linear_queue_rescore() {
   return mode == 1;
 }
 
-cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& m, const LinearLaunch& l, bool exact,
-                              const FlagList& flags, int sm_count, cudaStream_t stream, std::string* err,
-                              bool* rescore_kernel_needed) {
+cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const LinearDeviceModel& m,
+                              const LinearLaunch& l, bool exact, const FlagList& flags, int sm_count,
+                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed) {
   // the in-kernel queue re-scores rows with W in global memory / L2: fine for a 5 KB model, not for 62 KB of fp64
   // weights per row (cfg 3) - wide models take the re-score kernel, which stages W in shared memory
   const bool small_model = static_cast<size_t>(m.w64_stride) * m.n_features * sizeof(double) <= 16 * 1024;
@@ -1048,12 +1100,13 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& 
   for (int i = 0; i < 8; ++i) p.peers[i] = i < l.n_peers ? l.peers[i] : nullptr;
   p.row_offset = l.row_offset;
   p.n_rows = l.n_rows;
-  const bool whole = linear_whole_rows(m.f_pad);
-  const int tile_rows = linear_box_rows(m.f_pad);
+  const bool half = half_map != nullptr && linear_half_rows_ok(m.f_pad);
+  const LinearSched sched = half ? LinearSched::kHalf : linear_whole_rows(m.f_pad) ? LinearSched::kWhole : LinearSched::kChunked;
+  const int tile_rows = half ? kTileRows : linear_box_rows(m.f_pad);
   p.num_tiles = (l.n_rows + tile_rows - 1) / tile_rows;
   p.f_pad = m.f_pad;
   p.kc = m.f_pad / kChunkF;
-  const size_t fixed = tma_fixed_smem(m);
+  const size_t fixed = tma_fixed_smem(m, half);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kStageBytes);
   stages = std::min(stages, 64);
   // test hook: the shallowest legal ring (stages == consumer warps) stresses the barrier protocol
@@ -1080,14 +1133,21 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& 
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
   const long long slots = (p.num_tiles + kConsumerWarps - 1) / kConsumerWarps;
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
-  if (whole) {
-    if (!exact) return dispatch_classes<false, false, true>(m.n_classes, xmap, p, grid, smem, stream);
-    return inline_rescore ? dispatch_classes<true, true, true>(m.n_classes, xmap, p, grid, smem, stream)
-                          : dispatch_classes<true, false, true>(m.n_classes, xmap, p, grid, smem, stream);
+  using S = LinearSched;
+  if (sched == S::kHalf) {
+    const CUtensorMap& hmap = *half_map;
+    if (!exact) return dispatch_classes<false, false, S::kHalf>(m.n_classes, hmap, p, grid, smem, stream);
+    return inline_rescore ? dispatch_classes<true, true, S::kHalf>(m.n_classes, hmap, p, grid, smem, stream)
+                          : dispatch_classes<true, false, S::kHalf>(m.n_classes, hmap, p, grid, smem, stream);
   }
-  if (!exact) return dispatch_classes<false, false, false>(m.n_classes, xmap, p, grid, smem, stream);
-  return inline_rescore ? dispatch_classes<true, true, false>(m.n_classes, xmap, p, grid, smem, stream)
-                        : dispatch_classes<true, false, false>(m.n_classes, xmap, p, grid, smem, stream);
+  if (sched == S::kWhole) {
+    if (!exact) return dispatch_classes<false, false, S::kWhole>(m.n_classes, xmap, p, grid, smem, stream);
+    return inline_rescore ? dispatch_classes<true, true, S::kWhole>(m.n_classes, xmap, p, grid, smem, stream)
+                          : dispatch_classes<true, false, S::kWhole>(m.n_classes, xmap, p, grid, smem, stream);
+  }
+  if (!exact) return dispatch_classes<false, false, S::kChunked>(m.n_classes, xmap, p, grid, smem, stream);
+  return inline_rescore ? dispatch_classes<true, true, S::kChunked>(m.n_classes, xmap, p, grid, smem, stream)
+                        : dispatch_classes<true, false, S::kChunked>(m.n_classes, xmap, p, grid, smem, stream);
 }
 
 cudaError_t launch_rescore_f64(const LinearDeviceModel& m, const LinearLaunch& l, const FlagList& flags, bool all_rows,

@@ -5,6 +5,8 @@
 // 506-520: pd.DataFrame(features)[cols]) and sklearn's check_array finiteness scan
 // (sklearn/utils/validation.py:107): the scan for NaN/Inf and the "is the fp32 copy lossless" test are fused into
 // the conversion pass, so each element is touched once.
+#include <cuda_fp16.h>
+
 #include <cstring>
 #include <type_traits>
 
@@ -17,8 +19,14 @@ __device__ __forceinline__ double load_as_double(const T* p) {
   return static_cast<double>(*p);
 }
 
-// flag bits accumulated per thread: 1 = NaN/Inf, 2 = fp32 copy differs from the source value, 4 = fp32 value is not
-// a tf32 value (low 13 mantissa bits set)
+// the fp32 value is a finite fp16 value: the round trip through fp16 gives it back bit for bit (|v| <= 65504, no
+// bits below the fp16 spacing, fp16 subnormals and -0.0 included)
+__device__ __forceinline__ bool f16_exact(float f) {
+  return isfinite(f) && __float_as_uint(__half2float(__float2half_rn(f))) == __float_as_uint(f);
+}
+
+// flag bits accumulated per thread: 1 = NaN/Inf; in `lossy`: 1 = fp32 copy differs from the source value, 2 = fp32
+// value is not a tf32 value (low 13 mantissa bits set), 4 = fp32 value is not a finite fp16 value
 template <typename T>
 __device__ __forceinline__ void convert_one(T v, float* out32, double* out64, unsigned& nonfinite, unsigned& lossy) {
   const double d = static_cast<double>(v);
@@ -31,12 +39,14 @@ __device__ __forceinline__ void convert_one(T v, float* out32, double* out64, un
     lossy |= 1u;
   }
   if (__float_as_uint(f) & 0x1fffu) lossy |= 2u;  // second bit of `lossy`: not a tf32 value
+  if (!f16_exact(f)) lossy |= 4u;
 }
 
 __device__ __forceinline__ void publish_flags(unsigned nonfinite, unsigned lossy, StageResult* result) {
   if (__any_sync(0xffffffffu, nonfinite) && (threadIdx.x & 31) == 0) atomicAdd(&result->nonfinite, 1ull);
   if (__any_sync(0xffffffffu, lossy & 1u) && (threadIdx.x & 31) == 0) atomicAdd(&result->lossy, 1ull);
   if (__any_sync(0xffffffffu, lossy & 2u) && (threadIdx.x & 31) == 0) atomicAdd(&result->not_tf32, 1ull);
+  if (__any_sync(0xffffffffu, lossy & 4u) && (threadIdx.x & 31) == 0) atomicAdd(&result->not_f16, 1ull);
 }
 
 // source is row-major: element (r, f) at src[r * pitch + f]
@@ -125,7 +135,7 @@ __global__ void __launch_bounds__(256) stage_featmajor_kernel(const T* __restric
 // finiteness scan of rows that are already fp32 row-major on the device (no conversion needed)
 __global__ void __launch_bounds__(256) finite_scan_kernel(const float* __restrict__ x, long long ld, long long rows,
                                                           int F, StageResult* result) {
-  unsigned nonfinite = 0, low = 0;
+  unsigned nonfinite = 0, low = 0, not_f16 = 0;
   const long long total = rows * static_cast<long long>(ld);
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -134,15 +144,16 @@ __global__ void __launch_bounds__(256) finite_scan_kernel(const float* __restric
       const float v = x[i];
       if (!isfinite(v)) nonfinite = 1u;
       low |= __float_as_uint(v);
+      if (!f16_exact(v)) not_f16 = 4u;
     }
   }
-  publish_flags(nonfinite, (low & 0x1fffu) ? 2u : 0u, result);
+  publish_flags(nonfinite, ((low & 0x1fffu) ? 2u : 0u) | not_f16, result);
 }
 
 // dense variants (ld == F, source pitch == F): no per-element index arithmetic, 16-byte accesses
 __global__ void __launch_bounds__(256) finite_scan_dense_kernel(const float4* __restrict__ x, long long n4,
                                                                 StageResult* result) {
-  unsigned nonfinite = 0, low = 0;
+  unsigned nonfinite = 0, low = 0, not_f16 = 0;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float4 v = __ldg(x + i);
@@ -150,8 +161,9 @@ __global__ void __launch_bounds__(256) finite_scan_dense_kernel(const float4* __
     const float t = (v.x - v.x) + (v.y - v.y) + (v.z - v.z) + (v.w - v.w);
     if (!(t == 0.f)) nonfinite = 1u;
     low |= __float_as_uint(v.x) | __float_as_uint(v.y) | __float_as_uint(v.z) | __float_as_uint(v.w);
+    if (!(f16_exact(v.x) && f16_exact(v.y) && f16_exact(v.z) && f16_exact(v.w))) not_f16 = 4u;
   }
-  publish_flags(nonfinite, (low & 0x1fffu) ? 2u : 0u, result);
+  publish_flags(nonfinite, ((low & 0x1fffu) ? 2u : 0u) | not_f16, result);
 }
 
 // four consecutive source elements with 16-byte loads where the type allows it
@@ -254,6 +266,43 @@ cudaError_t launch_stage_convert(const void* src, int src_dtype, bool feature_ma
     default:
       return cudaErrorInvalidValue;
   }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// compact fp16 copy of resident rows (read by the linear tile kernel's fp16 schedule): one thread per 8 features of a
+// row, two 16-byte loads, one 16-byte store.  fp32 -> fp16 is exact for the values the staging pass let through
+// (not_f16 == 0); columns F..ldh-1 are written as zero, whatever the fp32 rows hold there.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) pack_half_kernel(const float* __restrict__ x, long long ld, long long rows, int F,
+                                                        uint4* __restrict__ xh, long long ldh) {
+  const long long groups = ldh / 8;
+  const long long total = rows * groups;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long r = i / groups;
+    const int f0 = static_cast<int>(i - r * groups) * 8;
+    const float* xr = x + r * ld + f0;
+    float v[8];
+    const float4 a = f0 < ld ? __ldg(reinterpret_cast<const float4*>(xr)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 b = f0 + 4 < ld ? __ldg(reinterpret_cast<const float4*>(xr + 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    v[0] = a.x, v[1] = a.y, v[2] = a.z, v[3] = a.w, v[4] = b.x, v[5] = b.y, v[6] = b.z, v[7] = b.w;
+    uint32_t w[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const __half2 h = __floats2half2_rn(f0 + 2 * k < F ? v[2 * k] : 0.f, f0 + 2 * k + 1 < F ? v[2 * k + 1] : 0.f);
+      w[k] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    xh[i] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+cudaError_t launch_pack_half(const float* x, int64_t ld, int64_t rows, int n_features, void* xh, int64_t ldh,
+                             cudaStream_t stream) {
+  if (rows <= 0) return cudaSuccess;
+  const long long want = (rows * (ldh / 8) + 255) / 256;
+  const int grid = static_cast<int>(want < 132 * 16 ? want : 132 * 16);
+  pack_half_kernel<<<grid, 256, 0, stream>>>(x, ld, rows, n_features, static_cast<uint4*>(xh), ldh);
+  return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------------------------

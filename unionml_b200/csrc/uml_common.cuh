@@ -31,6 +31,11 @@ constexpr int kWholeTileRows = kStageBytes / (2 * kChunkF * 4);  // 64
 __host__ __device__ inline bool linear_whole_rows(int f_pad) { return f_pad == 2 * kChunkF; }
 // rows per box of the tensor map the linear tile kernel reads (its feature width is always kChunkF)
 __host__ __device__ inline int linear_box_rows(int f_pad) { return linear_whole_rows(f_pad) ? kWholeTileRows : kTileRows; }
+// Compact fp16 rows (F <= 64, every value an fp16 value): one stage is one {64 features, 128 rows} fp16 box = 128
+// whole rows in kStageBytes, read through the batch's half_map
+constexpr int kHalfBoxF = 2 * kChunkF;  // 64 halves = 128 bytes per row, the SWIZZLE_128B span
+__host__ __device__ inline bool linear_half_rows_ok(int f_pad) { return f_pad <= kHalfBoxF; }
+__host__ __device__ inline int linear_half_ld(int F) { return (F + 7) / 8 * 8; }  // halves per row: 16-byte row pitch
 
 struct LinearDeviceModel {
   // fp32 operands of the tile kernel: wt[f][cp] (feature-major, classes padded to cp = 4*ceil((C+1)/4), column C holds
@@ -152,10 +157,12 @@ inline cudaError_t launch_dependent(void (*kern)(Params), int grid, int block, s
 
 // scoring kernels (linear_kernels.cu)
 // *rescore_kernel_needed: exact mode with the inline re-score switched off -> the caller launches launch_rescore_f64
-// xmap: the rows as a 2-D map {F, n_rows} with {kChunkF, linear_box_rows(m.f_pad)} boxes, SWIZZLE_128B
-cudaError_t launch_linear_tma(const CUtensorMap& xmap, const LinearDeviceModel& m, const LinearLaunch& l, bool exact,
-                              const FlagList& flags, int sm_count, cudaStream_t stream, std::string* err,
-                              bool* rescore_kernel_needed);
+// xmap: the rows as a 2-D map {F, n_rows} with {kChunkF, linear_box_rows(m.f_pad)} boxes, SWIZZLE_128B.
+// half_map (optional): the batch's compact fp16 copy of the same rows, {kHalfBoxF, kTileRows} boxes, SWIZZLE_128B;
+// when given and linear_half_rows_ok(m.f_pad), the kernel reads it instead of xmap (same labels, half the bytes)
+cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const LinearDeviceModel& m,
+                              const LinearLaunch& l, bool exact, const FlagList& flags, int sm_count,
+                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed);
 bool linear_tma_supported(const LinearDeviceModel& m, std::string* why);
 cudaError_t launch_rescore_f64(const LinearDeviceModel& m, const LinearLaunch& l, const FlagList& flags, bool all_rows,
                                int sm_count, cudaStream_t stream);
@@ -258,9 +265,14 @@ struct StageResult {  // device-side counters
   unsigned long long nonfinite;
   unsigned long long lossy;
   unsigned long long not_tf32;  // fp32 values with any of the low 13 mantissa bits set (tensor-core path needs none)
+  unsigned long long not_f16;   // fp32 values that are not finite fp16 values (the compact fp16 copy needs none)
 };
 cudaError_t launch_stage_convert(const void* src, int src_dtype, bool feature_major, int64_t src_pitch_elems,
                                  int64_t rows, int n_features, float* dst, int64_t ld, double* dst64, int64_t ld64,
                                  StageResult* result, bool check_finite, cudaStream_t stream);
+// fp32 rows [rows][ld] -> fp16 rows [rows][ldh] (ldh = linear_half_ld(F), columns >= F zero); exact when the staging
+// pass found not_f16 == 0
+cudaError_t launch_pack_half(const float* x, int64_t ld, int64_t rows, int n_features, void* xh, int64_t ldh,
+                             cudaStream_t stream);
 
 }  // namespace uml
