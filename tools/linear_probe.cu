@@ -1,5 +1,5 @@
 // Where the time of the linear tile kernel goes, on 10M x 64 fp32 rows (2.56 GB, the cfg2 shape) and on their compact
-// fp16 copy (1.28 GB), against the card's own read ceiling.  Built four times by tools/linear_probe.sh from
+// fp16 copy (1.28 GB), against the card's own read ceiling.  Built nine times by tools/linear_probe.sh from
 // linear_kernels.cu itself:
 //   plain                   read ceiling (streaming 16-byte non-allocating loads) over 2.56 GB and over 1.28 GB + the
 //                           tile kernel, all three schedules
@@ -9,6 +9,11 @@
 //                           warps' `full` waits, and over the time the scoring warps hold a landed stage
 //   -DUML_PROBE_TIMELINE    the tile kernel with %globaltimer stamps per CTA (entry, first issue, first landing, last
 //                           release, exit) over two back-to-back launches: ramp, exit spread, launch gap
+//   -DUML_PROBE_NO_W, -DUML_PROBE_NO_X, both   the fp16 schedule without its W loads, without its x loads and
+//                           conversions, and with neither (the FMAs and the epilogue alone): which of the scoring
+//                           warps' operands the time above the feed pays for.  Wrong scores by design.
+//   -DUML_PROBE_HALF_ONLY   the fp16 schedule alone, and once more with -DUML_HALF_CONSUMER_WARPS=8: the script runs the
+//                           two alternately, eight scoring warps against the library's twelve
 // Every figure is CUDA-event time over >= 0.5 s of back-to-back launches.  Prints one JSON object per line.
 #include "../unionml_b200/csrc/linear_kernels.cu"
 
@@ -125,12 +130,23 @@ int main() {
   fill_kernel<<<prop.multiProcessorCount * 8, 512>>>(x, xh, kRows * kF);
   CK(cudaDeviceSynchronize());
 
-#if defined(UML_PROBE_FEED_ONLY)
+#if defined(UML_PROBE_NO_W) || defined(UML_PROBE_NO_X)
+#define UML_PROBE_HALF_ONLY
+#endif
+#if defined(UML_PROBE_NO_W) && defined(UML_PROBE_NO_X)
+  const char* build = "math_only";
+#elif defined(UML_PROBE_NO_W)
+  const char* build = "no_w_loads";
+#elif defined(UML_PROBE_NO_X)
+  const char* build = "no_x_loads";
+#elif defined(UML_PROBE_FEED_ONLY)
   const char* build = "feed_only";
 #elif defined(UML_PROBE_WAIT_CLOCKS)
   const char* build = "wait_clocks";
 #elif defined(UML_PROBE_TIMELINE)
   const char* build = "timeline";
+#elif defined(UML_PROBE_HALF_ONLY)
+  const char* build = "half_only";
 #else
   const char* build = "plain";
   {
@@ -260,9 +276,9 @@ int main() {
     };
     const double ms = time_ms(launch);
     printf("{\"probe\": \"tile_kernel\", \"build\": \"%s\", \"schedule\": \"%s\", \"l2_promotion\": \"%s\", \"stages\": %d, "
-           "\"ms\": %.4f, \"bytes_read\": %.0f, \"gbs\": %.1f",
-           build, half ? "half_rows_128x64" : whole ? "whole_rows_64" : "chunked_128x32", promo_name, p.num_stages, ms,
-           read_bytes, read_bytes / ms * 1e-6);
+           "\"scoring_warps\": %d, \"ms\": %.4f, \"bytes_read\": %.0f, \"gbs\": %.1f",
+           build, half ? "half_rows_128x64" : whole ? "whole_rows_64" : "chunked_128x32", promo_name, p.num_stages,
+           linear_consumer_warps(sched), ms, read_bytes, read_bytes / ms * 1e-6);
 #ifdef UML_PROBE_WAIT_CLOCKS
     // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time
     CK(cudaMemset(counters + 8, 0, 5 * sizeof(unsigned long long)));
@@ -279,7 +295,7 @@ int main() {
     CK(cudaMemcpy(c, counters + 8, sizeof(c), cudaMemcpyDeviceToHost));
     // mean stages per CTA landed and not yet released (one scoring warp per stage): the scoring warps' summed hold time
     // over one warp's loop time, per CTA
-    const int scoring_warps = grid * kConsumerWarps;
+    const int scoring_warps = grid * linear_consumer_warps(sched);
     const double held_stages = static_cast<double>(c[4]) / (static_cast<double>(c[3]) / scoring_warps) / grid;
     printf(", \"producer_empty_wait_frac\": %.4f, \"consumer_full_wait_frac\": %.4f, \"held_stages\": %.3f, "
            "\"ring_stages\": %d, \"sm_clock_mhz_under_load\": %.0f",
@@ -341,6 +357,10 @@ int main() {
     printf("}\n");
     fflush(stdout);
   };
+#ifdef UML_PROBE_HALF_ONLY
+  run(LinearSched::kHalf, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
+  return 0;
+#endif
   run(LinearSched::kChunked, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
   run(LinearSched::kWhole, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
   run(LinearSched::kHalf, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");

@@ -1,7 +1,9 @@
 #!/bin/bash
 # Read ceiling + feed-only + wait-clock + timeline breakdown of the linear tile kernel (tools/linear_probe.cu), on GPU 0,
 # for each schedule: chunked and whole fp32 rows, and the compact fp16 rows (whose feed-only and wait-clock lines say
-# whether that schedule is bound by its feed or by its scoring warps).
+# whether that schedule is bound by its feed or by its scoring warps); then the fp16 schedule without its W loads,
+# without its x loads, and with neither; then the fp16 schedule with eight scoring warps and with the library's twelve,
+# alternating.
 # Writes MEASURED_PEAKS.json (the read ceiling bench.py's roofline divides by) and the probe's JSON lines to
 # ${1:-build/probe}/linear_probe.jsonl.  Binaries go to build/probe/.
 set -euo pipefail
@@ -9,9 +11,12 @@ cd "$(dirname "$0")/.."
 out=${1:-build/probe}
 mkdir -p build/probe "$out"
 nvcc=${NVCC:-$(command -v nvcc || echo /usr/local/cuda/bin/nvcc)}
-flags=(-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo)
-declare -A defs=([plain]="" [feed_only]="-DUML_PROBE_FEED_ONLY" [wait_clocks]="-DUML_PROBE_WAIT_CLOCKS" [timeline]="-DUML_PROBE_TIMELINE")
-for v in plain feed_only wait_clocks timeline; do
+flags=(-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -DUML_PROBE_CLASSES=10)
+declare -A defs=([plain]="" [feed_only]="-DUML_PROBE_FEED_ONLY" [wait_clocks]="-DUML_PROBE_WAIT_CLOCKS" [timeline]="-DUML_PROBE_TIMELINE"
+                 [no_w_loads]="-DUML_PROBE_NO_W" [no_x_loads]="-DUML_PROBE_NO_X" [math_only]="-DUML_PROBE_NO_W -DUML_PROBE_NO_X"
+                 [half_only]="-DUML_PROBE_HALF_ONLY" [half_only_warps8]="-DUML_PROBE_HALF_ONLY -DUML_HALF_CONSUMER_WARPS=8")
+variants=(plain feed_only wait_clocks timeline no_w_loads no_x_loads math_only half_only_warps8 half_only)
+for v in "${variants[@]}"; do
   bin=build/probe/linear_probe_$v
   if [ ! -x "$bin" ] || [ tools/linear_probe.cu -nt "$bin" ] || [ unionml_b200/csrc/linear_kernels.cu -nt "$bin" ]; then
     "$nvcc" "${flags[@]}" ${defs[$v]} tools/linear_probe.cu -o "$bin" &
@@ -19,7 +24,7 @@ for v in plain feed_only wait_clocks timeline; do
 done
 wait
 nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noheader | sed 's/^/# before: /' | tee -a "$out/linear_probe.jsonl"
-for v in plain feed_only wait_clocks timeline; do
+for v in "${variants[@]}" half_only_warps8 half_only; do
   build/probe/linear_probe_$v | tee -a "$out/linear_probe.jsonl"
 done
 nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noheader | sed 's/^/# after: /' | tee -a "$out/linear_probe.jsonl"

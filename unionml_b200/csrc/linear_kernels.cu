@@ -6,7 +6,7 @@
 //  * linear_argmax_tma_kernel<C, EXACT, QUEUE, SCHED>: persistent, warp-specialised.  One producer warp streams X
 //    through a 16 KiB-per-stage shared-memory ring with TMA + mbarriers: 128-row x 32-feature boxes (128B-swizzled), or
 //    at 33 <= F <= 64 (kWhole) stages of 64 complete rows, or (kHalf) stages of 128 complete rows from the batch's
-//    compact fp16 copy; eight consumer warps each own one tile at a time (4 or 2
+//    compact fp16 copy; eight consumer warps (twelve in kHalf) each own one tile at a time (4 or 2
 //    rows per lane), read X with conflict-free LDS.128, W as warp-uniform broadcast
 //    LDS.128 from a transposed copy in shared memory, keep C (+1) fp32 accumulators per row in registers, and fuse
 //    bias, argmax (first maximum wins, like np.argmax) and the label store.  In EXACT mode one extra accumulator
@@ -185,7 +185,6 @@ __device__ __noinline__ int rescore_row_inline(const TmaKernelParams& p, long lo
 constexpr int kTileSentinel = -1;        // claimed schedules: ring item that ends a scoring warp's loop
 constexpr int kQueueCap = 2048;           // flagged-row queue of the QUEUE kernels (power of two)
 constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this many slots are free (8 warps x 128 rows)
-constexpr int kThreadsQueue = kThreads + 32;  // + 1 fp64 re-score warp
 
 // the final label of a re-scored row into every target the launch writes (one lane)
 __device__ __forceinline__ void store_final_label(const TmaKernelParams& p, long long row, int idx) {
@@ -204,6 +203,20 @@ __device__ __forceinline__ void store_final_label(const TmaKernelParams& p, long
 //                         hold a landed stage (from the return of the `full` wait to the `empty` arrive)
 //  UML_PROBE_TIMELINE     %globaltimer per CTA into p.probe_timeline[blockIdx.x][5]: [0] entry, [1] the producer's first
 //                         issue, [2] the first stage landed (warp 0), [3] the last `empty` arrive, [4] exit
+//  UML_PROBE_NO_W         kHalf only, wrong scores: every feature's W^T row is one set of registers loaded once per warp,
+//                         so the scoring loop issues no W loads
+//  UML_PROBE_NO_X         kHalf only, wrong scores: every feature of a row is one register set once per warp, so the
+//                         scoring loop issues no x loads and no fp16 conversions (both defines: the FMAs alone)
+#ifdef UML_PROBE_NO_W
+constexpr bool kProbeNoW = true;
+#else
+constexpr bool kProbeNoW = false;
+#endif
+#ifdef UML_PROBE_NO_X
+constexpr bool kProbeNoX = true;
+#else
+constexpr bool kProbeNoX = false;
+#endif
 #ifdef UML_PROBE_FEED_ONLY
 constexpr bool kFeedOnly = true;
 #else
@@ -246,11 +259,16 @@ __device__ __forceinline__ unsigned long long probe_globaltimer() {
 //            {32 features, 64 rows} fp32 boxes onto one barrier (2 rows per lane)
 //  kHalf     (f_pad <= 64, the batch has a compact fp16 copy) one stage is one 128-row tile with all its features, one
 //            {64 features, 128 rows} fp16 box (4 rows per lane)
-// kWhole and kHalf claim their tiles in groups of 8 from a global counter; ring item n goes to warp n % 8.
+// kWhole and kHalf claim their tiles in groups of NCW (their scoring warps: 8, and kHalfConsumerWarps) from a global
+// counter; ring item n goes to warp n % NCW.
 enum class LinearSched { kChunked, kWhole, kHalf };
 
+// scoring warps of a schedule; the producer is warp NCW and the QUEUE kernels' re-score warp NCW + 1
+__host__ __device__ constexpr int linear_consumer_warps(LinearSched s) { return s == LinearSched::kHalf ? kHalfConsumerWarps : kConsumerWarps; }
+__host__ __device__ constexpr int linear_threads(LinearSched s, bool queue) { return (linear_consumer_warps(s) + (queue ? 2 : 1)) * 32; }
+
 template <int C, bool EXACT, bool QUEUE, LinearSched SCHED>
-__global__ void __launch_bounds__(kThreadsQueue, 1)
+__global__ void __launch_bounds__(linear_threads(SCHED, true), 1)
 linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ TmaKernelParams p) {
   constexpr int NCOL = C + (EXACT ? 1 : 0);  // accumulators per row (classes + error-bound column)
   constexpr int CP = (C + 1 + 3) / 4 * 4;    // padded columns of wt in shared memory (layout shared by both modes)
@@ -258,11 +276,18 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr bool WHOLE = SCHED == LinearSched::kWhole;
   constexpr bool HALF = SCHED == LinearSched::kHalf;
   constexpr bool CLAIMED = WHOLE || HALF;                    // tiles claimed from p.counters[4], one tile per stage
+  constexpr int NCW = linear_consumer_warps(SCHED);
+  // free queue slots a scoring warp wants before it publishes: every scoring warp may publish a whole tile at once
+  constexpr int HEADROOM = HALF ? NCW * kTileRows : kQueueHeadroom;
+  static_assert(HEADROOM <= kQueueCap, "the queue holds one tile of every scoring warp");
   constexpr int TILE = WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = rows per TMA box
   constexpr int R = TILE / 32;                               // rows per lane
   constexpr int BOX_BYTES = TILE * kChunkF * 4;              // one box: 8 KiB (two per kWhole stage) or 16 KiB
   static_assert(!HALF || BOX_BYTES == kTileRows * kHalfBoxF * 2, "an fp16 box is one stage");
-  constexpr bool USE_F2 = EXACT;  // fp32x2 accumulator pairs (see the accumulator comment below)
+  // fp32x2 accumulator pairs (see the accumulator comment below).  Not in the fp16 schedule: fma2 is two fmaf, so the
+  // scores are the same bits, and without the 64-bit register pairs ptxas schedules its 128 registers better
+  // (0.534 -> 0.523 ms at cfg 2, DESIGN.md 5.1)
+  constexpr bool USE_F2 = EXACT && !HALF;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // SWIZZLE_128B wants 1 KiB alignment
@@ -314,7 +339,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   const long long probe_start = clock64();
 #endif
 
-  if (warp == kConsumerWarps) {
+  if (warp == NCW) {
     // ===================== TMA producer (one elected lane) =====================
     if (elect_one_sync()) {
       tma_prefetch_desc(&xmap);
@@ -331,18 +356,17 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         }
       };
       if constexpr (CLAIMED) {
-        // Tiles are claimed, kConsumerWarps at a time, from a counter shared by the grid: with a static split, CTAs
+        // Tiles are claimed, NCW at a time, from a counter shared by the grid: with a static split, CTAs
         // with equal tile counts finished up to ~0.24 ms apart (SMs draw unequal shares of HBM bandwidth), and the
         // launch lasted as long as the slowest one.  Ring item n is one tile with both halves of its rows and goes to
-        // warp n % kConsumerWarps; a group claimed past the end hands every warp kTileSentinel.  The next group is
+        // warp n % NCW; a group claimed past the end hands every warp kTileSentinel.  The next group is
         // claimed while this one is issued, so the atomic's round trip stays off the ring.
         unsigned long long* claim = p.counters + 4;  // [0] next unclaimed tile, [1] CTAs done claiming
-        long long base = static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(kConsumerWarps)));
+        long long base = static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(NCW)));
         for (;;) {
           const long long next =
-              base < num_tiles ? static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(kConsumerWarps)))
-                               : base;
-          for (int w = 0; w < kConsumerWarps; ++w) {
+              base < num_tiles ? static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(NCW))) : base;
+          for (int w = 0; w < NCW; ++w) {
             const long long tile = base + w;
             UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u));
             tile_slot[stage] = base < num_tiles ? static_cast<int>(tile) : kTileSentinel;
@@ -398,7 +422,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     }
   } else {
     // ===================== consumers: one tile per warp at a time (warp 9 of the QUEUE kernels: re-score) ==========
-    const bool scoring_warp = warp < kConsumerWarps;
+    const bool scoring_warp = warp < NCW;
     // lane l owns rows l, l+32, ... of the tile.  In every box row r sits at byte r*128 with its 16-byte chunks
     // XOR-swizzled by (r & 7); r & 7 == l & 7 for all of a lane's rows, so one swizzle term serves them all and the
     // eight lanes of every LDS.128 phase (lanes 8i..8i+7: l & 7 = 0..7) hit eight distinct bank groups.  The whole-row
@@ -476,31 +500,52 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
 
     // kHalf: features 32*h .. 32*h + 31 of the lane's rows from the fp16 box (16-byte chunks 4h .. 4h + 3, eight
     // features each).  cvt.f32.f16 is exact, so every FMA gets the operands the fp32 route gives it, in the same order
-    // and the same fma2 pairing: scores, flags and labels are those of the fp32 rows bit for bit.
+    // (fma2 pairs there, plain fmaf here: the same IEEE operations): scores, flags and labels are those of the fp32
+    // rows bit for bit.
+    [[maybe_unused]] float probe_w[NW4 * 4], probe_x[R];  // UML_PROBE_NO_W / UML_PROBE_NO_X
+    if constexpr (kProbeNoW) {
+#pragma unroll
+      for (int c = 0; c < NW4 * 4; ++c) probe_w[c] = wt_s[c];
+    }
+    if constexpr (kProbeNoX) {
+#pragma unroll
+      for (int j = 0; j < R; ++j) probe_x[j] = p.thr * static_cast<float>(lane + 32 * j + 1);
+    }
     auto fma_half = [&](const uint8_t* xs, int h) {
       if constexpr (kFeedOnly) return;
       const float* wk = wt_s + h * kChunkF * CP;
 #pragma unroll
       for (int q = 0; q < kChunkF / 8; ++q) {
-        uint4 hv[R];
+        [[maybe_unused]] uint4 hv[R];
         const uint32_t off = lanebase ^ static_cast<uint32_t>((4 * h + q) * 16);
+        if constexpr (!kProbeNoX) {
 #pragma unroll
-        for (int j = 0; j < R; ++j) hv[j] = *reinterpret_cast<const uint4*>(xs + off + j * 32 * 128);
+          for (int j = 0; j < R; ++j) hv[j] = *reinterpret_cast<const uint4*>(xs + off + j * 32 * 128);
+        }
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           float wv[NW4 * 4];
 #pragma unroll
           for (int m = 0; m < NW4; ++m) {
-            const float4 t = *reinterpret_cast<const float4*>(wk + (q * 8 + e) * CP + m * 4);
-            wv[m * 4 + 0] = t.x;
-            wv[m * 4 + 1] = t.y;
-            wv[m * 4 + 2] = t.z;
-            wv[m * 4 + 3] = t.w;
+            if constexpr (kProbeNoW) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) wv[m * 4 + i] = probe_w[m * 4 + i];
+            } else {
+              const float4 t = *reinterpret_cast<const float4*>(wk + (q * 8 + e) * CP + m * 4);
+              wv[m * 4 + 0] = t.x;
+              wv[m * 4 + 1] = t.y;
+              wv[m * 4 + 2] = t.z;
+              wv[m * 4 + 3] = t.w;
+            }
           }
 #pragma unroll
           for (int j = 0; j < R; ++j) {
-            const uint32_t word = e < 2 ? hv[j].x : e < 4 ? hv[j].y : e < 6 ? hv[j].z : hv[j].w;
-            fma_feature(j, __half2float(__ushort_as_half(static_cast<unsigned short>((e & 1) ? word >> 16 : word & 0xffffu))), wv);
+            if constexpr (kProbeNoX) {
+              fma_feature(j, probe_x[j], wv);
+            } else {
+              const uint32_t word = e < 2 ? hv[j].x : e < 4 ? hv[j].y : e < 6 ? hv[j].z : hv[j].w;
+              fma_feature(j, __half2float(__ushort_as_half(static_cast<unsigned short>((e & 1) ? word >> 16 : word & 0xffffu))), wv);
+            }
           }
         }
       }
@@ -603,7 +648,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           if (lane == 0) {
             const int tail = atomicAdd(&q_ctl[0], 0);
             const int consumed = atomicAdd(&q_ctl[3], 0);
-            if (tail - consumed <= kQueueCap - kQueueHeadroom) base = atomicAdd(&q_ctl[0], total);
+            if (tail - consumed <= kQueueCap - HEADROOM) base = atomicAdd(&q_ctl[0], total);
           }
           base = __shfl_sync(0xffffffffu, base, 0);
           if (base >= 0) {
@@ -641,8 +686,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     };
 
     if constexpr (CLAIMED) {
-      // this warp's ring items are n = warp, warp + 8, ... (stage n % S, phase (n / S) & 1); S >= 8 lets stage and
-      // phase advance without a division.  Both waits keep the invariant argued below: the next item is n + 8 <= n + S.
+      // this warp's ring items are n = warp, warp + NCW, ... (stage n % S, phase (n / S) & 1); S >= NCW lets stage and
+      // phase advance without a division.  Both waits keep the invariant argued below: the next item is n + NCW <= n + S.
       uint32_t stage = static_cast<uint32_t>(warp), phase = 0;
       for (bool first = true; scoring_warp; first = false) {
         init_acc();
@@ -666,7 +711,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         UML_PROBE_SINCE(probe_hold, probe_landed);
         UML_PROBE_RELEASED();
         if (tile == kTileSentinel) break;
-        stage += kConsumerWarps;
+        stage += NCW;
         if (stage >= static_cast<uint32_t>(S)) {
           stage -= S;
           phase ^= 1u;
@@ -717,7 +762,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     }
 #endif
     if constexpr (EXACT && QUEUE) {
-      if (warp < kConsumerWarps) {
+      if (warp < NCW) {
         __syncwarp();
         if (lane == 0) {
           __threadfence_block();
@@ -739,7 +784,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           int state = 0;  // 1: nothing will ever be published for this ticket
           if (lane == 0) {
             v = atomicAdd(&q_slots[t & (kQueueCap - 1)], 0);
-            if (v == 0 && atomicAdd(&q_ctl[2], 0) == kConsumerWarps) {
+            if (v == 0 && atomicAdd(&q_ctl[2], 0) == NCW) {
               __threadfence_block();
               if (t >= atomicAdd(&q_ctl[0], 0)) state = 1;
             }
@@ -1049,7 +1094,7 @@ static cudaError_t launch_one(const CUtensorMap& xmap, const TmaKernelParams& p,
     if (err != cudaSuccess) return err;
     configured = smem;
   }
-  kern<<<grid, QUEUE ? kThreadsQueue : kThreads, smem, stream>>>(xmap, p);
+  kern<<<grid, linear_threads(SCHED, QUEUE), smem, stream>>>(xmap, p);
   return cudaGetLastError();
 }
 
@@ -1060,8 +1105,12 @@ static cudaError_t dispatch_classes(int C, const CUtensorMap& xmap, const TmaKer
 #define UML_CASE(N) \
   case N:           \
     return launch_one<N, EXACT, QUEUE, SCHED>(xmap, p, grid, smem, stream);
+#ifdef UML_PROBE_CLASSES  // diagnostic builds compile only the class count they launch
+    UML_CASE(UML_PROBE_CLASSES)
+#else
     UML_CASE(2) UML_CASE(3) UML_CASE(4) UML_CASE(5) UML_CASE(6) UML_CASE(7) UML_CASE(8) UML_CASE(9) UML_CASE(10)
     UML_CASE(11) UML_CASE(12) UML_CASE(13) UML_CASE(14) UML_CASE(15) UML_CASE(16)
+#endif
 #undef UML_CASE
     default:
       return cudaErrorInvalidValue;
@@ -1100,6 +1149,9 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   for (int i = 0; i < 8; ++i) p.peers[i] = i < l.n_peers ? l.peers[i] : nullptr;
   p.row_offset = l.row_offset;
   p.n_rows = l.n_rows;
+  // (at f_pad <= 64 the fp16 schedule's shortest ring always fits beside the largest W^T, 16 classes)
+  static_assert(1024 + (kHalfBoxF + 1) * 20 * 4 + 2 * 64 * 8 + (kQueueCap + 4) * 4 + 64 * 4 +
+                        kHalfConsumerWarps * kStageBytes <= kMaxSmemBytes, "kHalfConsumerWarps stages do not fit");
   const bool half = half_map != nullptr && linear_half_rows_ok(m.f_pad);
   const LinearSched sched = half ? LinearSched::kHalf : linear_whole_rows(m.f_pad) ? LinearSched::kWhole : LinearSched::kChunked;
   const int tile_rows = half ? kTileRows : linear_box_rows(m.f_pad);
@@ -1109,8 +1161,9 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   const size_t fixed = tma_fixed_smem(m, half);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kStageBytes);
   stages = std::min(stages, 64);
-  // test hook: the shallowest legal ring (stages == consumer warps) stresses the barrier protocol
-  if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(kConsumerWarps, std::min(stages, atoi(env)));
+  // test hook: the shallowest legal ring (stages == scoring warps) stresses the barrier protocol
+  const int warps = linear_consumer_warps(sched);
+  if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(warps, std::min(stages, atoi(env)));
   p.num_stages = stages;
   // margin > 2 err guarantees the fp32 argmax is the exact argmax; err <= (F+4) 2^-24 A (1 + F 2^-21), see DESIGN.md
   p.thr = linear_margin_thr(m.n_features);
@@ -1131,7 +1184,7 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   p.binary = m.binary;
   p.counters = flags.counters;
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
-  const long long slots = (p.num_tiles + kConsumerWarps - 1) / kConsumerWarps;
+  const long long slots = (p.num_tiles + warps - 1) / warps;
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
   using S = LinearSched;
   if (sched == S::kHalf) {

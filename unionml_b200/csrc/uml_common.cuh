@@ -36,6 +36,13 @@ __host__ __device__ inline int linear_box_rows(int f_pad) { return linear_whole_
 constexpr int kHalfBoxF = 2 * kChunkF;  // 64 halves = 128 bytes per row, the SWIZZLE_128B span
 __host__ __device__ inline bool linear_half_rows_ok(int f_pad) { return f_pad <= kHalfBoxF; }
 __host__ __device__ inline int linear_half_ld(int F) { return (F + 7) / 8 * 8; }  // halves per row: 16-byte row pitch
+// Scoring warps of the fp16 schedule: 3 per SM sub-partition.  Its feed outruns eight warps (their cost per row is the
+// limit, DESIGN.md 5.1), and a third warp per scheduler fills issue slots the other two leave while they wait for
+// their shared-memory operands.  The ring must hold at least this many stages.
+#ifndef UML_HALF_CONSUMER_WARPS
+#define UML_HALF_CONSUMER_WARPS 12
+#endif
+constexpr int kHalfConsumerWarps = UML_HALF_CONSUMER_WARPS;
 
 struct LinearDeviceModel {
   // fp32 operands of the tile kernel: wt[f][cp] (feature-major, classes padded to cp = 4*ceil((C+1)/4), column C holds
