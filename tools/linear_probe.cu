@@ -12,8 +12,9 @@
 //   -DUML_PROBE_NO_W, -DUML_PROBE_NO_X, both   the fp16 schedule without its W loads, without its x loads and
 //                           conversions, and with neither (the FMAs and the epilogue alone): which of the scoring
 //                           warps' operands the time above the feed pays for.  Wrong scores by design.
-//   -DUML_PROBE_HALF_ONLY   the fp16 schedule alone, and once more with -DUML_HALF_CONSUMER_WARPS=8: the script runs the
-//                           two alternately, eight scoring warps against the library's twelve
+//   -DUML_PROBE_HALF_ONLY   the fp16 schedule alone, and once more with -DUML_PROBE_HALF_PASS_ROWS=4 (256-row stages
+//                           scored in two passes of 4 rows per lane by the same four warps): the script runs the two
+//                           alternately, which separates the W reuse of 8 rows per lane from the warp count
 // Every figure is CUDA-event time over >= 0.5 s of back-to-back launches.  Prints one JSON object per line.
 #include "../unionml_b200/csrc/linear_kernels.cu"
 
@@ -145,6 +146,8 @@ int main() {
   const char* build = "wait_clocks";
 #elif defined(UML_PROBE_TIMELINE)
   const char* build = "timeline";
+#elif defined(UML_PROBE_HALF_ONLY) && defined(UML_PROBE_HALF_PASS_ROWS)
+  const char* build = "half_only_rows4";
 #elif defined(UML_PROBE_HALF_ONLY)
   const char* build = "half_only";
 #else
@@ -234,8 +237,8 @@ int main() {
   // the EXACT + QUEUE kernel bench.py runs (uint8 labels to one target), in each schedule
   auto run = [&](LinearSched sched, CUtensorMapL2promotion promo, const char* promo_name) {
     const bool whole = sched == LinearSched::kWhole, half = sched == LinearSched::kHalf;
-    const int tile = whole ? kWholeTileRows : kTileRows;
-    const CUtensorMap map = half ? make_map(xh, tile, promo, true) : make_map(x, tile, promo);
+    const int tile = whole ? kWholeTileRows : half ? kHalfTileRows : kTileRows;
+    const CUtensorMap map = half ? make_map(xh, kTileRows, promo, true) : make_map(x, tile, promo);
     const double read_bytes = half ? bytes / 2 : bytes;
     TmaKernelParams p{};
     p.wt = m.wt;
@@ -248,7 +251,8 @@ int main() {
     p.f_pad = kF;
     p.kc = kF / kChunkF;
     const size_t fixed = tma_fixed_smem(m, half);
-    p.num_stages = std::min(64, static_cast<int>((kMaxSmemBytes - fixed) / kStageBytes));
+    const int stage_bytes = linear_stage_bytes(sched);
+    p.num_stages = std::min(64, static_cast<int>((kMaxSmemBytes - fixed) / stage_bytes));
     p.thr = static_cast<float>(2.0 * (kF + 4.0) * 5.9604644775390625e-08 * (1.0 + kF * 4.76837158203125e-07) * 1.0001);
     p.x = x;
     p.ld = kF;
@@ -266,7 +270,7 @@ int main() {
 #ifdef UML_PROBE_TIMELINE
     p.probe_timeline = timeline;
 #endif
-    const size_t smem = fixed + static_cast<size_t>(p.num_stages) * kStageBytes;
+    const size_t smem = fixed + static_cast<size_t>(p.num_stages) * stage_bytes;
     const int grid = prop.multiProcessorCount;
     auto launch = [&] {
       const cudaError_t err = half    ? launch_one<kC, true, true, LinearSched::kHalf>(map, p, grid, smem, 0)
@@ -276,9 +280,10 @@ int main() {
     };
     const double ms = time_ms(launch);
     printf("{\"probe\": \"tile_kernel\", \"build\": \"%s\", \"schedule\": \"%s\", \"l2_promotion\": \"%s\", \"stages\": %d, "
-           "\"scoring_warps\": %d, \"ms\": %.4f, \"bytes_read\": %.0f, \"gbs\": %.1f",
-           build, half ? "half_rows_128x64" : whole ? "whole_rows_64" : "chunked_128x32", promo_name, p.num_stages,
-           linear_consumer_warps(sched), ms, read_bytes, read_bytes / ms * 1e-6);
+           "\"scoring_warps\": %d, \"rows_per_lane_per_pass\": %d, \"ms\": %.4f, \"bytes_read\": %.0f, \"gbs\": %.1f",
+           build, half ? "half_rows_256x64" : whole ? "whole_rows_64" : "chunked_128x32", promo_name, p.num_stages,
+           linear_consumer_warps(sched), half ? kHalfPassRows : tile / 32, ms, read_bytes,
+           read_bytes / ms * 1e-6);
 #ifdef UML_PROBE_WAIT_CLOCKS
     // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time
     CK(cudaMemset(counters + 8, 0, 5 * sizeof(unsigned long long)));

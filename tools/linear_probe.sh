@@ -2,8 +2,8 @@
 # Read ceiling + feed-only + wait-clock + timeline breakdown of the linear tile kernel (tools/linear_probe.cu), on GPU 0,
 # for each schedule: chunked and whole fp32 rows, and the compact fp16 rows (whose feed-only and wait-clock lines say
 # whether that schedule is bound by its feed or by its scoring warps); then the fp16 schedule without its W loads,
-# without its x loads, and with neither; then the fp16 schedule with eight scoring warps and with the library's twelve,
-# alternating.
+# without its x loads, and with neither; then the fp16 schedule with 4 rows per lane per pass and with the library's 8,
+# alternating (both with four scoring warps and 256-row stages).
 # Writes MEASURED_PEAKS.json (the read ceiling bench.py's roofline divides by) and the probe's JSON lines to
 # ${1:-build/probe}/linear_probe.jsonl.  Binaries go to build/probe/.
 set -euo pipefail
@@ -14,17 +14,18 @@ nvcc=${NVCC:-$(command -v nvcc || echo /usr/local/cuda/bin/nvcc)}
 flags=(-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -DUML_PROBE_CLASSES=10)
 declare -A defs=([plain]="" [feed_only]="-DUML_PROBE_FEED_ONLY" [wait_clocks]="-DUML_PROBE_WAIT_CLOCKS" [timeline]="-DUML_PROBE_TIMELINE"
                  [no_w_loads]="-DUML_PROBE_NO_W" [no_x_loads]="-DUML_PROBE_NO_X" [math_only]="-DUML_PROBE_NO_W -DUML_PROBE_NO_X"
-                 [half_only]="-DUML_PROBE_HALF_ONLY" [half_only_warps8]="-DUML_PROBE_HALF_ONLY -DUML_HALF_CONSUMER_WARPS=8")
-variants=(plain feed_only wait_clocks timeline no_w_loads no_x_loads math_only half_only_warps8 half_only)
+                 [half_only]="-DUML_PROBE_HALF_ONLY" [half_only_rows4]="-DUML_PROBE_HALF_ONLY -DUML_PROBE_HALF_PASS_ROWS=4")
+variants=(plain feed_only wait_clocks timeline no_w_loads no_x_loads math_only half_only_rows4 half_only)
 for v in "${variants[@]}"; do
   bin=build/probe/linear_probe_$v
-  if [ ! -x "$bin" ] || [ tools/linear_probe.cu -nt "$bin" ] || [ unionml_b200/csrc/linear_kernels.cu -nt "$bin" ]; then
+  if [ ! -x "$bin" ] || [ tools/linear_probe.cu -nt "$bin" ] || [ unionml_b200/csrc/linear_kernels.cu -nt "$bin" ] ||
+     [ unionml_b200/csrc/uml_common.cuh -nt "$bin" ]; then
     "$nvcc" "${flags[@]}" ${defs[$v]} tools/linear_probe.cu -o "$bin" &
   fi
 done
 wait
 nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noheader | sed 's/^/# before: /' | tee -a "$out/linear_probe.jsonl"
-for v in "${variants[@]}" half_only_warps8 half_only; do
+for v in "${variants[@]}" half_only_rows4 half_only; do
   build/probe/linear_probe_$v | tee -a "$out/linear_probe.jsonl"
 done
 nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noheader | sed 's/^/# after: /' | tee -a "$out/linear_probe.jsonl"

@@ -79,4 +79,17 @@ eng.predict_peers(m7, b7, [buf7.ptr], 3, exact=True, want_stats=True, label_byte
 _os.environ["UML_B200_COMPACT_ROWS"] = "0"
 assert eng.predict(m, b16, exact=True)[1]["x_elem_bytes"] == 4
 del _os.environ["UML_B200_COMPACT_ROWS"]
+# 256-row items of the fp16 schedule with the ring at its 4-item floor: ragged last items (40_001 = 156 x 256 + 65 rows
+# ends inside the item's first box, 155 x 256 + 200 inside its second), uint8 peer stores at an odd offset, and a
+# 16-class model (8 rows of 17 accumulators per lane, 255 registers)
+_os.environ["UML_B200_STAGES"] = "4"
+m16 = eng.load_linear(rng.standard_normal((16, 64)), rng.standard_normal(16))
+b200 = eng.stage(X[: 155 * 256 + 200])
+buf16 = eng.device_alloc(b16.n_rows + 1)
+for mm in (m, m16):
+    for bb in (b16, b200):
+        for exact in (True, False):
+            assert eng.predict(mm, bb, exact=exact)[1]["x_elem_bytes"] == 2
+        eng.predict_peers(mm, bb, [buf16.ptr], 1, exact=True, want_stats=True, label_bytes=1)
+del _os.environ["UML_B200_STAGES"]
 print("sanitizer driver ok")

@@ -5,8 +5,8 @@
 //
 //  * linear_argmax_tma_kernel<C, EXACT, QUEUE, SCHED>: persistent, warp-specialised.  One producer warp streams X
 //    through a 16 KiB-per-stage shared-memory ring with TMA + mbarriers: 128-row x 32-feature boxes (128B-swizzled), or
-//    at 33 <= F <= 64 (kWhole) stages of 64 complete rows, or (kHalf) stages of 128 complete rows from the batch's
-//    compact fp16 copy; eight consumer warps (twelve in kHalf) each own one tile at a time (4 or 2
+//    at 33 <= F <= 64 (kWhole) stages of 64 complete rows, or (kHalf) 32 KiB stages of 256 complete rows from the
+//    batch's compact fp16 copy; eight consumer warps (four in kHalf) each own one tile at a time (4, 2 or 8
 //    rows per lane), read X with conflict-free LDS.128, W as warp-uniform broadcast
 //    LDS.128 from a transposed copy in shared memory, keep C (+1) fp32 accumulators per row in registers, and fuse
 //    bias, argmax (first maximum wins, like np.argmax) and the label store.  In EXACT mode one extra accumulator
@@ -257,8 +257,8 @@ __device__ __forceinline__ unsigned long long probe_globaltimer() {
 //            CTA scores tiles blockIdx.x, blockIdx.x + gridDim.x, ...
 //  kWhole    (f_pad == 64, linear_whole_rows) one stage is one 64-row tile with all its features, loaded as two
 //            {32 features, 64 rows} fp32 boxes onto one barrier (2 rows per lane)
-//  kHalf     (f_pad <= 64, the batch has a compact fp16 copy) one stage is one 128-row tile with all its features, one
-//            {64 features, 128 rows} fp16 box (4 rows per lane)
+//  kHalf     (f_pad <= 64, the batch has a compact fp16 copy) one stage is one 256-row tile with all its features, two
+//            {64 features, 128 rows} fp16 boxes onto one barrier (8 rows per lane)
 // kWhole and kHalf claim their tiles in groups of NCW (their scoring warps: 8, and kHalfConsumerWarps) from a global
 // counter; ring item n goes to warp n % NCW.
 enum class LinearSched { kChunked, kWhole, kHalf };
@@ -266,6 +266,18 @@ enum class LinearSched { kChunked, kWhole, kHalf };
 // scoring warps of a schedule; the producer is warp NCW and the QUEUE kernels' re-score warp NCW + 1
 __host__ __device__ constexpr int linear_consumer_warps(LinearSched s) { return s == LinearSched::kHalf ? kHalfConsumerWarps : kConsumerWarps; }
 __host__ __device__ constexpr int linear_threads(LinearSched s, bool queue) { return (linear_consumer_warps(s) + (queue ? 2 : 1)) * 32; }
+// bytes of one ring stage: in kHalf two 16 KiB fp16 boxes
+__host__ __device__ constexpr int linear_stage_bytes(LinearSched s) { return s == LinearSched::kHalf ? 2 * kStageBytes : kStageBytes; }
+
+// kHalf: rows per lane scored in one pass over a 256-row stage (NPASS = 8 / this passes).  All 8 rows of a lane at
+// once for every class count: their 8 NCOL accumulators and the operands in flight fit in 255 registers without a
+// spill up to C = 16 in FAST, EXACT and EXACT + QUEUE (ptxas -v, DESIGN.md 5.1).  The diagnostic builds' two passes
+// of 4 rows separate the W reuse of 8 rows from the warp count.
+#ifdef UML_PROBE_HALF_PASS_ROWS
+constexpr int kHalfPassRows = UML_PROBE_HALF_PASS_ROWS;
+#else
+constexpr int kHalfPassRows = 8;
+#endif
 
 template <int C, bool EXACT, bool QUEUE, LinearSched SCHED>
 __global__ void __launch_bounds__(linear_threads(SCHED, true), 1)
@@ -277,13 +289,19 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr bool HALF = SCHED == LinearSched::kHalf;
   constexpr bool CLAIMED = WHOLE || HALF;                    // tiles claimed from p.counters[4], one tile per stage
   constexpr int NCW = linear_consumer_warps(SCHED);
+  constexpr int TILE = HALF ? kHalfTileRows : WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = per ring stage
   // free queue slots a scoring warp wants before it publishes: every scoring warp may publish a whole tile at once
-  constexpr int HEADROOM = HALF ? NCW * kTileRows : kQueueHeadroom;
+  constexpr int HEADROOM = HALF ? NCW * TILE : kQueueHeadroom;
   static_assert(HEADROOM <= kQueueCap, "the queue holds one tile of every scoring warp");
-  constexpr int TILE = WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = rows per TMA box
-  constexpr int R = TILE / 32;                               // rows per lane
-  constexpr int BOX_BYTES = TILE * kChunkF * 4;              // one box: 8 KiB (two per kWhole stage) or 16 KiB
-  static_assert(!HALF || BOX_BYTES == kTileRows * kHalfBoxF * 2, "an fp16 box is one stage");
+  // rows per lane held in registers at once (kHalf: one pass, NPASS passes per tile)
+  constexpr int R = HALF ? kHalfPassRows : TILE / 32;
+  constexpr int NPASS = TILE / 32 / R;
+  static_assert(NPASS * R * 32 == TILE && (!HALF || R % 4 == 0), "a pass is whole 128-row boxes");
+  // one box: 8 KiB (two per kWhole stage) or 16 KiB (two per kHalf stage)
+  constexpr int BOX_BYTES = (HALF ? kTileRows : TILE) * kChunkF * 4;
+  constexpr int STAGE_BYTES = linear_stage_bytes(SCHED);
+  static_assert(!HALF || (BOX_BYTES == kTileRows * kHalfBoxF * 2 && STAGE_BYTES == 2 * BOX_BYTES),
+                "an fp16 stage is two boxes");
   // fp32x2 accumulator pairs (see the accumulator comment below).  Not in the fp16 schedule: fma2 is two fmaf, so the
   // scores are the same bits, and without the 64-bit register pairs ptxas schedules its 128 registers better
   // (0.534 -> 0.523 ms at cfg 2, DESIGN.md 5.1)
@@ -293,7 +311,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // SWIZZLE_128B wants 1 KiB alignment
 
   const int S = p.num_stages;
-  float* wt_s = reinterpret_cast<float*>(smem + static_cast<size_t>(S) * kStageBytes);
+  float* wt_s = reinterpret_cast<float*>(smem + static_cast<size_t>(S) * STAGE_BYTES);
   float* bias_s = wt_s + p.f_pad * CP;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + CP);
   uint64_t* empty_bar = full_bar + S;
@@ -371,11 +389,22 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u));
             tile_slot[stage] = base < num_tiles ? static_cast<int>(tile) : kTileSentinel;
             if (tile < num_tiles) {
-              mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-              uint8_t* dst = smem + static_cast<size_t>(stage) * kStageBytes;
-              const int row = static_cast<int>(tile * TILE);
-              tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
-              if constexpr (WHOLE) tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], kChunkF, row, policy);
+              if constexpr (HALF) {
+                // rows 128-255 of the last tile may all lie past the batch: that box is not loaded (its rows are
+                // scored from stale shared memory and never stored)
+                uint8_t* dst = smem + static_cast<size_t>(stage) * STAGE_BYTES;
+                const int row = static_cast<int>(tile * TILE);
+                const bool second = row + kTileRows < p.n_rows;
+                mbar_arrive_expect_tx(&full_bar[stage], second ? STAGE_BYTES : BOX_BYTES);
+                tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
+                if (second) tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], 0, row + kTileRows, policy);
+              } else {
+                mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+                uint8_t* dst = smem + static_cast<size_t>(stage) * kStageBytes;
+                const int row = static_cast<int>(tile * TILE);
+                tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
+                if constexpr (WHOLE) tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], kChunkF, row, policy);
+              }
 #ifdef UML_PROBE_TIMELINE
               if (probe_first_issue) UML_PROBE_STAMP(1);
               probe_first_issue = false;
@@ -427,7 +456,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     // XOR-swizzled by (r & 7); r & 7 == l & 7 for all of a lane's rows, so one swizzle term serves them all and the
     // eight lanes of every LDS.128 phase (lanes 8i..8i+7: l & 7 = 0..7) hit eight distinct bank groups.  The whole-row
     // stage is two such boxes (features 0-31, then 32-63 at +8 KiB), so the same holds in both halves; an fp16 row is
-    // 64 halves in the same 128 bytes, so the same addresses serve it.
+    // 64 halves in the same 128 bytes, so the same addresses serve it, and the fp16 stage's second box (rows 128-255
+    // at +16 KiB) puts every one of its 256 rows at r*128.
     const uint32_t lanebase = static_cast<uint32_t>(lane) * 128u + static_cast<uint32_t>(lane & 7) * 16u;
 #ifdef UML_PROBE_WAIT_CLOCKS
     long long probe_hold = 0;
@@ -498,10 +528,13 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       }
     };
 
-    // kHalf: features 32*h .. 32*h + 31 of the lane's rows from the fp16 box (16-byte chunks 4h .. 4h + 3, eight
-    // features each).  cvt.f32.f16 is exact, so every FMA gets the operands the fp32 route gives it, in the same order
-    // (fma2 pairs there, plain fmaf here: the same IEEE operations): scores, flags and labels are those of the fp32
-    // rows bit for bit.
+    // kHalf: features 0 .. f_pad - 1 of the lane's rows from an fp16 stage, eight features (one 16-byte chunk of each
+    // row) per iteration.  cvt.f32.f16 is exact, so every FMA gets the operands the fp32 route gives it, in the same
+    // order (fma2 pairs there, plain fmaf here: the same IEEE operations): scores, flags and labels are those of the
+    // fp32 rows bit for bit.  The loop over the chunks stays rolled: unrolled over 64 features, 8 rows of 11 columns
+    // are ~7 000 instructions (112 KB of SASS), no other warp on the scheduler covers their instruction fetches, and
+    // the kernel ran 3.7x slower (2x unrolled by 2, DESIGN.md 5.1).  The next chunk's x is loaded while this one is
+    // scored.
     [[maybe_unused]] float probe_w[NW4 * 4], probe_x[R];  // UML_PROBE_NO_W / UML_PROBE_NO_X
     if constexpr (kProbeNoW) {
 #pragma unroll
@@ -511,17 +544,22 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
 #pragma unroll
       for (int j = 0; j < R; ++j) probe_x[j] = p.thr * static_cast<float>(lane + 32 * j + 1);
     }
-    auto fma_half = [&](const uint8_t* xs, int h) {
+    auto load_chunk = [&](uint4* hv, const uint8_t* xs, int k) {
+      if constexpr (!kProbeNoX) {
+        const uint32_t off = lanebase ^ static_cast<uint32_t>(k * 16);
+#pragma unroll
+        for (int j = 0; j < R; ++j) hv[j] = *reinterpret_cast<const uint4*>(xs + off + j * 32 * 128);
+      }
+    };
+    auto fma_half = [&](const uint8_t* xs) {
       if constexpr (kFeedOnly) return;
-      const float* wk = wt_s + h * kChunkF * CP;
-#pragma unroll
-      for (int q = 0; q < kChunkF / 8; ++q) {
-        [[maybe_unused]] uint4 hv[R];
-        const uint32_t off = lanebase ^ static_cast<uint32_t>((4 * h + q) * 16);
-        if constexpr (!kProbeNoX) {
-#pragma unroll
-          for (int j = 0; j < R; ++j) hv[j] = *reinterpret_cast<const uint4*>(xs + off + j * 32 * 128);
-        }
+      const int nk = p.f_pad / 8;  // f_pad 32: the box's zero columns 32-63 are not scored
+      [[maybe_unused]] uint4 hv[R], hn[R];
+      load_chunk(hv, xs, 0);
+#pragma unroll 1
+      for (int k = 0; k < nk; ++k) {
+        load_chunk(hn, xs, k + 1 < nk ? k + 1 : k);
+        const float* wk = wt_s + k * 8 * CP;
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           float wv[NW4 * 4];
@@ -531,7 +569,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
 #pragma unroll
               for (int i = 0; i < 4; ++i) wv[m * 4 + i] = probe_w[m * 4 + i];
             } else {
-              const float4 t = *reinterpret_cast<const float4*>(wk + (q * 8 + e) * CP + m * 4);
+              const float4 t = *reinterpret_cast<const float4*>(wk + e * CP + m * 4);
               wv[m * 4 + 0] = t.x;
               wv[m * 4 + 1] = t.y;
               wv[m * 4 + 2] = t.z;
@@ -548,11 +586,14 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             }
           }
         }
+#pragma unroll
+        for (int j = 0; j < R; ++j) hv[j] = hn[j];
       }
     };
 
-    // ---- fused epilogue: argmax (first maximum wins), margin guard, label store (+ peer stores) ----
-    auto finish_tile = [&](long long tile) {
+    // ---- fused epilogue of the rows row0 + lane + 32 j, j < R: argmax (first maximum wins), margin guard, label store
+    // (+ peer stores) ----
+    auto finish_rows = [&](long long row0) {
       if constexpr (USE_F2) {
 #pragma unroll
         for (int j = 0; j < R; ++j) {
@@ -562,7 +603,6 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           acc[j][C] = acc_bound[j];
         }
       }
-      const long long row0 = tile * TILE;
       int idxs[R];
       bool flag[R];
 #pragma unroll
@@ -608,28 +648,34 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         }
       }
       if (p.wire_u8 && p.n_peers > 0) {
-        // byte labels: transpose through shuffles so lane l < TILE/4 holds rows 4l..4l+3 of the tile and the whole
-        // tile leaves as ONE coalesced TILE-byte store per target (instead of R int32 stores).  Row 4l+t sits in byte
-        // (4l+t)/32 = l/8 of lane (4l+t) % 32's packed word.
-        uint32_t packed = 0, word = 0;
+        // byte labels: transpose through shuffles so lane l < GR/4 holds rows 4l..4l+3 of a group of GR = 32 RG rows
+        // and the group leaves as ONE coalesced GR-byte store per target (instead of RG int32 stores).  Row 4l+t sits
+        // in byte (4l+t)/32 = l/8 of lane (4l+t) % 32's packed word.  One group per pass, except kHalf's 8 rows per
+        // lane: two 128-row groups.
+        constexpr int NG = HALF ? R / 4 : 1;
+        constexpr int RG = R / NG;
 #pragma unroll
-        for (int j = 0; j < R; ++j) packed |= static_cast<uint32_t>(idxs[j]) << (8 * j);
+        for (int g = 0; g < NG; ++g) {
+          uint32_t packed = 0, word = 0;
 #pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
-          word |= ((w >> (8 * (lane >> 3))) & 0xffu) << (8 * t);
-        }
-        const long long row4 = row0 + 4 * lane;
-        const long long at = p.row_offset + row4;
-        if (4 * lane < TILE) {
-          if (row4 + 3 < p.n_rows && (at & 3) == 0) {
-            for (int i = 0; i < p.n_peers; ++i)
-              *reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(p.peers[i]) + at) = word;
-          } else {
-            for (int t = 0; t < 4; ++t)
-              if (row4 + t < p.n_rows)
-                for (int i = 0; i < p.n_peers; ++i)
-                  static_cast<uint8_t*>(p.peers[i])[at + t] = static_cast<uint8_t>((word >> (8 * t)) & 0xffu);
+          for (int j = 0; j < RG; ++j) packed |= static_cast<uint32_t>(idxs[g * RG + j]) << (8 * j);
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {
+            const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
+            word |= ((w >> (8 * (lane >> 3))) & 0xffu) << (8 * t);
+          }
+          const long long row4 = row0 + g * 32 * RG + 4 * lane;
+          const long long at = p.row_offset + row4;
+          if (4 * lane < 32 * RG) {
+            if (row4 + 3 < p.n_rows && (at & 3) == 0) {
+              for (int i = 0; i < p.n_peers; ++i)
+                *reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(p.peers[i]) + at) = word;
+            } else {
+              for (int t = 0; t < 4; ++t)
+                if (row4 + t < p.n_rows)
+                  for (int i = 0; i < p.n_peers; ++i)
+                    static_cast<uint8_t*>(p.peers[i])[at + t] = static_cast<uint8_t>((word >> (8 * t)) & 0xffu);
+            }
           }
         }
       }
@@ -697,10 +743,17 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         const int tile = tile_slot[stage];
         const bool scored = tile >= 0 && tile < num_tiles;
         if (scored) {
-          const uint8_t* xs = smem + static_cast<size_t>(stage) * kStageBytes;
+          const uint8_t* xs = smem + static_cast<size_t>(stage) * STAGE_BYTES;
           if constexpr (HALF) {
-            fma_half(xs, 0);
-            if (p.f_pad > kChunkF) fma_half(xs, 1);  // f_pad 32: the box's zero columns 32-63 are not scored
+            // NPASS > 1: every pass but the last is finished while the stage is held, the last one after its release
+#pragma unroll
+            for (int pass = 0; pass < NPASS; ++pass) {
+              if (pass > 0) {
+                finish_rows(static_cast<long long>(tile) * TILE + (pass - 1) * 32 * R);
+                init_acc();
+              }
+              fma_half(xs + pass * 32 * R * 128);
+            }
           } else {
             fma_box(xs, wt_s);
             fma_box(xs + BOX_BYTES, wt_s + kChunkF * CP);
@@ -716,7 +769,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           stage -= S;
           phase ^= 1u;
         }
-        if (scored) finish_tile(tile);
+        if (scored) finish_rows(static_cast<long long>(tile) * TILE + (NPASS - 1) * 32 * R);
       }
     } else {
       uint32_t seq_base = 0;
@@ -746,7 +799,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             UML_PROBE_SINCE(probe_hold, probe_landed);
             UML_PROBE_RELEASED();
           }
-          finish_tile(tile);
+          finish_rows(tile * TILE);
         }
         seq_base += static_cast<uint32_t>(KC * nv);
       }
@@ -1151,15 +1204,17 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   p.n_rows = l.n_rows;
   // (at f_pad <= 64 the fp16 schedule's shortest ring always fits beside the largest W^T, 16 classes)
   static_assert(1024 + (kHalfBoxF + 1) * 20 * 4 + 2 * 64 * 8 + (kQueueCap + 4) * 4 + 64 * 4 +
-                        kHalfConsumerWarps * kStageBytes <= kMaxSmemBytes, "kHalfConsumerWarps stages do not fit");
+                        kHalfConsumerWarps * linear_stage_bytes(LinearSched::kHalf) <= kMaxSmemBytes,
+                "kHalfConsumerWarps stages do not fit");
   const bool half = half_map != nullptr && linear_half_rows_ok(m.f_pad);
   const LinearSched sched = half ? LinearSched::kHalf : linear_whole_rows(m.f_pad) ? LinearSched::kWhole : LinearSched::kChunked;
-  const int tile_rows = half ? kTileRows : linear_box_rows(m.f_pad);
+  const int tile_rows = half ? kHalfTileRows : linear_box_rows(m.f_pad);
   p.num_tiles = (l.n_rows + tile_rows - 1) / tile_rows;
   p.f_pad = m.f_pad;
   p.kc = m.f_pad / kChunkF;
   const size_t fixed = tma_fixed_smem(m, half);
-  int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / kStageBytes);
+  const int stage_bytes = linear_stage_bytes(sched);
+  int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / stage_bytes);
   stages = std::min(stages, 64);
   // test hook: the shallowest legal ring (stages == scoring warps) stresses the barrier protocol
   const int warps = linear_consumer_warps(sched);
@@ -1183,7 +1238,7 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   p.fold_rel = m.fold_rel;
   p.binary = m.binary;
   p.counters = flags.counters;
-  const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
+  const size_t smem = fixed + static_cast<size_t>(stages) * stage_bytes;
   const long long slots = (p.num_tiles + warps - 1) / warps;
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
   using S = LinearSched;

@@ -31,18 +31,18 @@ constexpr int kWholeTileRows = kStageBytes / (2 * kChunkF * 4);  // 64
 __host__ __device__ inline bool linear_whole_rows(int f_pad) { return f_pad == 2 * kChunkF; }
 // rows per box of the tensor map the linear tile kernel reads (its feature width is always kChunkF)
 __host__ __device__ inline int linear_box_rows(int f_pad) { return linear_whole_rows(f_pad) ? kWholeTileRows : kTileRows; }
-// Compact fp16 rows (F <= 64, every value an fp16 value): one stage is one {64 features, 128 rows} fp16 box = 128
-// whole rows in kStageBytes, read through the batch's half_map
+// Compact fp16 rows (F <= 64, every value an fp16 value): one {64 features, 128 rows} fp16 box = 128 whole rows in
+// kStageBytes, read through the batch's half_map
 constexpr int kHalfBoxF = 2 * kChunkF;  // 64 halves = 128 bytes per row, the SWIZZLE_128B span
 __host__ __device__ inline bool linear_half_rows_ok(int f_pad) { return f_pad <= kHalfBoxF; }
 __host__ __device__ inline int linear_half_ld(int F) { return (F + 7) / 8 * 8; }  // halves per row: 16-byte row pitch
-// Scoring warps of the fp16 schedule: 3 per SM sub-partition.  Its feed outruns eight warps (their cost per row is the
-// limit, DESIGN.md 5.1), and a third warp per scheduler fills issue slots the other two leave while they wait for
-// their shared-memory operands.  The ring must hold at least this many stages.
-#ifndef UML_HALF_CONSUMER_WARPS
-#define UML_HALF_CONSUMER_WARPS 12
-#endif
-constexpr int kHalfConsumerWarps = UML_HALF_CONSUMER_WARPS;
+// Ring items of the fp16 schedule: 256 whole rows, two {64, 128} fp16 boxes on one barrier (32 KiB), so a lane scores
+// 8 rows and every broadcast W load feeds 8 FMA chains per class instead of 4.  Its feed outruns the scoring warps
+// (their cost per row is the limit, DESIGN.md 5.1).
+constexpr int kHalfTileRows = 2 * kTileRows;
+// Scoring warps of the fp16 schedule: one per SM sub-partition, with up to 255 registers for its 8 rows of
+// accumulators and the operands of the next feature.  The ring must hold at least this many items.
+constexpr int kHalfConsumerWarps = 4;
 
 struct LinearDeviceModel {
   // fp32 operands of the tile kernel: wt[f][cp] (feature-major, classes padded to cp = 4*ceil((C+1)/4), column C holds
