@@ -101,17 +101,20 @@ def build_pylist(force: bool = False) -> Path:
 
 PROBE_SRC = PKG.parent / "tests" / "cuda" / "wgmma_accum_probe.cu"
 PROBE_LIB = PKG.parent / "build" / "tests" / "libwgmma_accum_probe.so"
+F16_PROBE_SRC = PKG.parent / "tests" / "cuda" / "wgmma_f16_accum_probe.cu"
+F16_PROBE_LIB = PKG.parent / "build" / "tests" / "libwgmma_f16_accum_probe.so"
 
 
 def build_test_probes(force: bool = False) -> Path:
-    """Test-only library of tests/test_gpu_wgmma_accum.py (the product never loads it): the wgmma accumulation probe,
-    compiled against the product's own wgmma.cuh."""
+    """Test-only libraries of tests/test_gpu_wgmma_accum.py and tests/test_gpu_wgmma_f16_accum.py (the product never
+    loads them): the tf32 and f16 wgmma accumulation probes, compiled against the product's own wgmma.cuh."""
     PROBE_LIB.parent.mkdir(parents=True, exist_ok=True)
-    if force or _stale(PROBE_LIB, [PROBE_SRC, *CSRC.glob("*.cuh")]):
-        cmd = [nvcc(), *NVCC_FLAGS, "-shared", str(PROBE_SRC), "-o", str(PROBE_LIB)]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f"nvcc failed for {PROBE_SRC.name}:\n{r.stdout}\n{r.stderr}")
+    for src, lib in ((PROBE_SRC, PROBE_LIB), (F16_PROBE_SRC, F16_PROBE_LIB)):
+        if force or _stale(lib, [src, *CSRC.glob("*.cuh")]):
+            cmd = [nvcc(), *NVCC_FLAGS, "-shared", str(src), "-o", str(lib)]
+            r = subprocess.run(cmd, capture_output=True, text=True)
+            if r.returncode != 0:
+                raise RuntimeError(f"nvcc failed for {src.name}:\n{r.stdout}\n{r.stderr}")
     return PROBE_LIB
 
 

@@ -231,6 +231,7 @@ struct uml_model {
   float* d_bias = nullptr;
   double* d_w64 = nullptr;
   double* d_b64 = nullptr;
+  void* d_tc = nullptr;  // dm.tc_ops
 };
 
 struct uml_batch {
@@ -250,6 +251,7 @@ struct uml_batch {
   void* xh = nullptr;
   int64_t ldh = 0;
   bool has_half = false;
+  bool half_nonneg = false;  // the fp16 copy holds no value < 0 (the linear tile kernel's tensor-core schedule needs that)
   CUtensorMap half_map{};
 };
 
@@ -508,6 +510,85 @@ int uml_host_free(uml_engine* e, void* p) {
 // ---------------------------------------------------------------------------------------------------------------
 // model
 // ---------------------------------------------------------------------------------------------------------------
+// ---- tensor-core operands of the linear tile kernel (DESIGN.md 3.1, 3.2) ----
+// the fp16 value nearest to v (ties to even; up: the smallest fp16 value >= v), for |v| below 2^16
+static double f16_round(double v, bool up = false) {
+  if (v == 0.0) return v;
+  int e = 0;
+  std::frexp(std::fabs(v), &e);  // |v| in [2^(e-1), 2^e): 11 significant bits, or the subnormal spacing 2^-24
+  const int q = std::max(e - 11, -24);
+  const double m = std::ldexp(v, -q);
+  return std::ldexp(up ? std::ceil(m) : std::nearbyint(m), q);
+}
+// bit pattern of an fp16 value held exactly in v
+static uint16_t f16_bits(double v) {
+  const uint16_t sign = std::signbit(v) ? 0x8000u : 0u;
+  const double a = std::fabs(v);
+  if (a < 0x1p-14) return sign | (uint16_t)std::ldexp(a, 24);
+  int e = 0;
+  const double m = std::frexp(a, &e);  // a = m 2^e, m in [0.5, 1)
+  return sign | (uint16_t)((e + 14) << 10) | (uint16_t)std::ldexp(m * 2.0 - 1.0, 10);
+}
+// per-k16-step budget of the f16 wgmma accumulation, in u = 2^-24 of the running |.| sum (DESIGN.md 3.2): above the
+// 36u of a truncating aligner without guard bits over 16 products and the accumulator ((2 x 17 + 2) u, the model of
+// 3.3), and at least 4x the worst that tests/test_gpu_wgmma_f16_accum.py measures on the hardware
+constexpr double kTcStepBudget = 64.0;
+// The B operand image of LinearDeviceModel::tc_ops and the certification factor, or false when the model does not take
+// the tensor-core schedule: a folded affine map (its score error is bounded in the fp64 terms only), non-finite weights,
+// or magnitudes at which the scaled A of DESIGN.md 3.2 could leave the normal fp32 range.  wt / bias are the fp32
+// route's operands (its bound column and bias bound are what tier 1 must dominate).
+static bool build_tc_operands(const std::vector<double>& w, const std::vector<double>& b, const std::vector<float>& wt,
+                              const std::vector<float>& bias, int C, int F, int f_pad, int cp, double fold_rel,
+                              std::vector<uint8_t>* image, float* kappa) {
+  if (f_pad > uml::kHalfBoxF || fold_rel != 0.0) return false;
+  double wabs = 0.0;
+  for (double v : w) {
+    if (!std::isfinite(v)) return false;
+    wabs = std::max(wabs, std::fabs(v));
+  }
+  for (int c = 0; c < C; ++c)
+    if (!std::isfinite(b[c])) return false;
+  int ex = 0;
+  if (wabs > 0.0) std::frexp(wabs, &ex);  // wabs < 2^ex
+  const int sigma = 15 - ex;               // max |w| 2^sigma in [2^14, 2^15): every hi piece is a normal fp16 value
+  double wsum = 0.0;
+  for (int f = 0; f < F; ++f) wsum += wt[(size_t)f * cp + C];
+  const double a32 = (double)bias[C] + 65504.0 * wsum;  // the fp32 route's A of the largest fp16 row
+  if (!(std::ldexp(a32, std::max(sigma, 0)) < 0x1p100) || !(std::ldexp((double)bias[C], sigma) > 0x1p-100)) return false;
+  const int NH = uml::linear_tc_hi_cols(C), N = uml::linear_tc_cols(C);
+  std::vector<uint16_t> bt((size_t)N * uml::kHalfBoxF, 0);
+  // column n's 128-byte row, its 16-byte chunks XOR-swizzled by (n & 7): the SWIZZLE_128B K-major layout
+  auto put = [&](int n, int f, double v) { bt[(size_t)n * 64 + (((f / 8) ^ (n & 7)) * 8) + f % 8] = f16_bits(v); };
+  for (int f = 0; f < F; ++f) {
+    double wmax = std::ldexp((double)wt[(size_t)f * cp + C], sigma);
+    for (int c = 0; c < C; ++c) {
+      const double v = std::ldexp(w[(size_t)c * F + f], sigma);
+      const double hi = f16_round(v);
+      put(c, f, hi);
+      put(NH + c, f, f16_round(v - hi));
+      wmax = std::max(wmax, std::fabs(v));
+    }
+    // floored at 2^-3 so that 2^-22 of it covers the 2^-25 a subnormal piece errs by (hi + lo errs by <= 2^-21 of it).
+    // The fp32 route's FLT_MIN floor can scale past fp16 when every weight is below 2^-127: no route then.
+    const double wb = f16_round(std::max(wmax, 0.125), true);
+    if (!(wb <= 65504.0)) return false;
+    put(C, f, wb);
+  }
+  std::vector<float> tb(NH, 0.f);
+  for (int c = 0; c < C; ++c) tb[c] = (float)std::ldexp(b[c], sigma);
+  tb[C] = (float)std::ldexp((double)bias[C], sigma);  // exact: a power-of-two multiple of an fp32 value in range
+  image->assign((size_t)N * 128 + tb.size() * 4, 0);
+  std::memcpy(image->data(), bt.data(), (size_t)N * 128);
+  std::memcpy(image->data() + (size_t)N * 128, tb.data(), tb.size() * 4);
+  // tier 1 certifies iff margin > 2 Etc + 2.5 thr A32+ (DESIGN.md 3.2): Etc <= e_rel A, A <= Ahat / (1 - step)
+  const double u = uml::kU;
+  const double step = kTcStepBudget * u * (f_pad / 16);
+  const double e_rel = (0x1p-21 + step * (1.0 + 0x1p-10) + 4.0 * u) * (1.0 + 0x1p-10);
+  const double thr = uml::linear_margin_thr(F);
+  *kappa = (float)((2.0 * e_rel + 2.5 * thr * (1.0 + (F + 2.0) * u)) / (1.0 - step) * (1.0 + 0x1p-10));
+  return true;
+}
+
 // bmag[c] >= |b_c| is the bias magnitude both bounds use (|b_c| + sum_f |shift_f w'_cf| for a folded affine map) and
 // fold_rel the fp64 bound's extra relative term of such a map (DESIGN.md 3.2)
 static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& w, const std::vector<double>& b,
@@ -560,6 +641,16 @@ static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& 
   UML_CUDA(e, cudaMemcpy(m->d_bias, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice));
   UML_CUDA(e, cudaMemcpy(m->d_w64, w64t.data(), w64t.size() * 8, cudaMemcpyHostToDevice));
   UML_CUDA(e, cudaMemcpy(m->d_b64, b64.data(), b64.size() * 8, cudaMemcpyHostToDevice));
+  std::vector<uint8_t> tc;
+  float kappa = 0.f;
+  if (m->d_tc) cudaFree(m->d_tc);
+  m->d_tc = nullptr;
+  if (build_tc_operands(w, b, wt, bias, C, F, f_pad, cp, fold_rel, &tc, &kappa)) {
+    UML_CUDA(e, cudaMalloc(&m->d_tc, tc.size()));
+    UML_CUDA(e, cudaMemcpy(m->d_tc, tc.data(), tc.size(), cudaMemcpyHostToDevice));
+  }
+  m->dm.tc_ops = m->d_tc;
+  m->dm.tc_kappa = kappa;
   m->dm.wt = m->d_wt;
   m->dm.bias = m->d_bias;
   m->dm.w64 = m->d_w64;
@@ -650,6 +741,7 @@ void uml_model_free(uml_model* m) {
   if (m->e) cudaSetDevice(m->e->device);
   cudaFree(m->d_wt);
   cudaFree(m->d_bias);
+  cudaFree(m->d_tc);
   cudaFree(m->d_w64);
   cudaFree(m->d_b64);
   delete m;
@@ -696,7 +788,10 @@ static int build_half_copy(uml_engine* e, uml_batch* b) {
     return UML_OK;
   }
   b->ldh = ldh;
-  UML_CUDA(e, uml::launch_pack_half(b->x, b->ld, b->n_rows, F, b->xh, ldh, e->stream));
+  UML_CUDA(e, cudaMemsetAsync(&e->d_stage->negative, 0, sizeof(unsigned long long), e->stream));
+  UML_CUDA(e, uml::launch_pack_half(b->x, b->ld, b->n_rows, F, b->xh, ldh, &e->d_stage->negative, e->stream));
+  UML_CUDA(e, cudaMemcpyAsync(&e->h->stage.negative, &e->d_stage->negative, sizeof(unsigned long long),
+                              cudaMemcpyDeviceToHost, e->stream));
   cuuint64_t gdim[2] = {(cuuint64_t)F, (cuuint64_t)b->n_rows};
   cuuint64_t gstride[1] = {(cuuint64_t)ldh * 2};
   cuuint32_t box[2] = {(cuuint32_t)uml::kHalfBoxF, (cuuint32_t)uml::kTileRows};
@@ -708,6 +803,7 @@ static int build_half_copy(uml_engine* e, uml_batch* b) {
                                   (long long)b->n_rows, F);
   UML_CUDA(e, cudaStreamSynchronize(e->stream));  // later calls may run on another stream (uml_engine_set_stream)
   b->has_half = true;
+  b->half_nonneg = e->h->stage.negative == 0;
   return UML_OK;
 }
 
@@ -1021,7 +1117,7 @@ void uml_batch_free(uml_batch* b) {
 // copy, which the tile kernel then reads; *x_elem_bytes (optional) gets the bytes per feature it read (2 or 4).
 static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch& l, const CUtensorMap* map,
                            const CUtensorMap* half_map, int mode, bool timed, int* launches, int* path,
-                           int* x_elem_bytes = nullptr) {
+                           int* x_elem_bytes = nullptr, bool half_nonneg = false) {
   const FlagList fl = flag_list(e);
   const bool exact = mode == UML_PREDICT_EXACT;
   std::string why;
@@ -1033,7 +1129,7 @@ static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch
     bool need_rescore = false;
     if (half_map && !uml::linear_half_rows_ok(m->dm.f_pad)) half_map = nullptr;
     cudaError_t ce = uml::launch_linear_tma(*map, half_map, m->dm, l, exact, fl, e->info.sm_count, e->stream, &err,
-                                            &need_rescore);
+                                            &need_rescore, half_nonneg);
     if (ce != cudaSuccess) UML_FAIL(e, UML_ERR_CUDA, "linear_argmax_tma launch: %s %s", cudaGetErrorString(ce), err.c_str());
     *launches += 1;
     *path = 1;
@@ -1203,7 +1299,8 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
     l.n_peers = n_peers - own;
     for (int i = 0; i < l.n_peers; ++i) l.peers[i] = peers[own + i];
     const CUtensorMap* half = b->has_half && compact_rows_enabled() ? &b->half_map : nullptr;
-    return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, half, mode, timed, launches, path, elem_bytes);
+    return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, half, mode, timed, launches, path, elem_bytes,
+                           b->half_nonneg);
   };
   return predict_resident(e, b, m->dm.n_classes, m->n_features_in, "estimator", labels_out, labels_on_device, n_peers,
                           label_bytes, mode, stats, [] { return (int)UML_OK; }, score);

@@ -23,6 +23,7 @@
 #include "uml_common.cuh"
 #include "tma_ring.cuh"
 #include "rescore_util.cuh"
+#include "wgmma.cuh"
 
 #ifndef UML_RESCORE_QUEUE_DEFAULT
 #define UML_RESCORE_QUEUE_DEFAULT 1  // one launch per step; the few flagged rows (0.02 % on digits) cost the queue little
@@ -160,6 +161,8 @@ struct TmaKernelParams {
 #ifdef UML_PROBE_TIMELINE
   unsigned long long* probe_timeline;  // [gridDim.x][5], see the diagnostic builds below
 #endif
+  const void* tc_ops;  // kHalfMma: LinearDeviceModel::tc_ops
+  float tc_kappa;
 };
 
 // fp64 scores of one row by the whole warp (kept out of line so the hot loop's register allocation is untouched)
@@ -259,15 +262,76 @@ __device__ __forceinline__ unsigned long long probe_globaltimer() {
 //            {32 features, 64 rows} fp32 boxes onto one barrier (2 rows per lane)
 //  kHalf     (f_pad <= 64, the batch has a compact fp16 copy) one stage is one 256-row tile with all its features, two
 //            {64 features, 128 rows} fp16 boxes onto one barrier (8 rows per lane)
-// kWhole and kHalf claim their tiles in groups of NCW (their scoring warps: 8, and kHalfConsumerWarps) from a global
-// counter; ring item n goes to warp n % NCW.
-enum class LinearSched { kChunked, kWhole, kHalf };
+//  kHalfMma  (EXACT + QUEUE, the same stages, every fp16 value >= 0, the model has tc_ops) two warpgroups score the
+//            stages on the tensor cores (wgmma, f16 x f16 -> fp32, W^T as scaled hi | lo pieces); ring item n goes to
+//            warpgroup n % 2.  Rows the tensor-core guard does not certify go through the queue, where the re-score warp
+//            first replays the fp32 route on them (DESIGN.md 3.1, 3.2)
+// kWhole, kHalf and kHalfMma claim their tiles in groups of NCU (the units that take ring items: the scoring warps, or
+// kHalfMma's two warpgroups) from a global counter; ring item n goes to unit n % NCU.
+enum class LinearSched { kChunked, kWhole, kHalf, kHalfMma };
 
 // scoring warps of a schedule; the producer is warp NCW and the QUEUE kernels' re-score warp NCW + 1
 __host__ __device__ constexpr int linear_consumer_warps(LinearSched s) { return s == LinearSched::kHalf ? kHalfConsumerWarps : kConsumerWarps; }
+// units that take ring items (and the ring's floor): warps, or kHalfMma's warpgroups
+__host__ __device__ constexpr int linear_ring_units(LinearSched s) { return s == LinearSched::kHalfMma ? kConsumerWarps / 4 : linear_consumer_warps(s); }
 __host__ __device__ constexpr int linear_threads(LinearSched s, bool queue) { return (linear_consumer_warps(s) + (queue ? 2 : 1)) * 32; }
-// bytes of one ring stage: in kHalf two 16 KiB fp16 boxes
-__host__ __device__ constexpr int linear_stage_bytes(LinearSched s) { return s == LinearSched::kHalf ? 2 * kStageBytes : kStageBytes; }
+// bytes of one ring stage: in kHalf and kHalfMma two 16 KiB fp16 boxes
+__host__ __device__ constexpr int linear_stage_bytes(LinearSched s) {
+  return s == LinearSched::kHalf || s == LinearSched::kHalfMma ? 2 * kStageBytes : kStageBytes;
+}
+// kHalfMma: bytes of the B operand in shared memory (rounded up to the 1 KiB that keeps what follows aligned)
+__host__ __device__ constexpr int linear_tc_b_bytes(int C) { return (linear_tc_cols(C) * 128 + 1023) / 1024 * 1024; }
+
+// kHalfMma's tier 2 (DESIGN.md 3.2): the fp32 route's scores of one row, replayed bit for bit by one warp: lane c <= C
+// runs column c's FMA chain in feature order from bias_s[c] over the caller's fp32 row (zeros past F, as the fp32 route's
+// boxes hold), the bound column on |x|; lane 0's sequential best / second loop of finish_rows on the gathered C + 1
+// values and the same p.thr comparison.  True: that route certifies the row, *idx is its label.
+__device__ __noinline__ bool replay_fp32_row(const TmaKernelParams& p, const float* wt_s, const float* bias_s, int cp,
+                                             long long row, int lane, int* idx) {
+  const int C = p.n_classes, F = p.n_features;
+  const float* xr = p.x + row * p.ld;
+  const float x0 = lane < F ? xr[lane] : 0.f, x1 = lane + 32 < F ? xr[lane + 32] : 0.f;
+  const int col = lane <= C ? lane : C;
+  float acc = bias_s[col];
+  // unrolled so that the W loads and shuffles of later features issue ahead of the FMA chain, which alone is serial
+#pragma unroll 16
+  for (int f = 0; f < p.f_pad; ++f) {
+    const float xf = __shfl_sync(0xffffffffu, f < 32 ? x0 : x1, f & 31);
+    const float wv = wt_s[f * cp + col];
+    acc = lane < C ? fmaf(xf, wv, acc) : fmaf(fabsf(xf), wv, acc);
+  }
+  float best = __shfl_sync(0xffffffffu, acc, 0);
+  float second = -INFINITY;
+  int bi = 0;
+  for (int c = 1; c < C; ++c) {
+    const float v = __shfl_sync(0xffffffffu, acc, c);
+    if (v > best) {
+      second = best;
+      best = v;
+      bi = c;
+    } else {
+      second = fmaxf(second, v);
+    }
+  }
+  const float bound = __shfl_sync(0xffffffffu, acc, C);
+  *idx = bi;
+  return (best - second) > p.thr * bound;
+}
+
+// tier 2 of one row the tensor-core guard left, by the whole warp: the fp32 route's decision first, fp64 only where that
+// route would flag the row; stores the final label.  Returns 1 when the row went to fp64 (it counts in n_flagged).
+// The scoring warps' only call site in the tensor-core schedule, so their registers are not saved around two calls.
+__device__ __noinline__ int settle_row_tc(const TmaKernelParams& p, const float* wt_s, const float* bias_s, int cp,
+                                          long long row, int lane) {
+  int idx = 0;
+  int f64 = 0;
+  if (!replay_fp32_row(p, wt_s, bias_s, cp, row, lane, &idx)) {
+    idx = rescore_row_inline(p, row, lane);
+    f64 = 1;
+  }
+  if (lane == 0) store_final_label(p, row, idx);
+  return f64;
+}
 
 // kHalf: rows per lane scored in one pass over a 256-row stage (NPASS = 8 / this passes).  All 8 rows of a lane at
 // once for every class count: their 8 NCOL accumulators and the operands in flight fit in 255 registers without a
@@ -287,20 +351,25 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr int NW4 = (NCOL + 3) / 4;        // float4 loads of W per feature
   constexpr bool WHOLE = SCHED == LinearSched::kWhole;
   constexpr bool HALF = SCHED == LinearSched::kHalf;
-  constexpr bool CLAIMED = WHOLE || HALF;                    // tiles claimed from p.counters[4], one tile per stage
+  constexpr bool MMA = SCHED == LinearSched::kHalfMma;
+  constexpr bool F16 = HALF || MMA;                          // 256-row stages of the compact fp16 rows
+  constexpr bool CLAIMED = WHOLE || F16;                     // tiles claimed from p.counters[4], one tile per stage
   constexpr int NCW = linear_consumer_warps(SCHED);
-  constexpr int TILE = HALF ? kHalfTileRows : WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = per ring stage
+  constexpr int NCU = linear_ring_units(SCHED);
+  static_assert(!MMA || (EXACT && QUEUE), "the tensor-core schedule certifies rows through the queue's replay");
+  constexpr int TILE = F16 ? kHalfTileRows : WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = per ring stage
   // free queue slots a scoring warp wants before it publishes: every scoring warp may publish a whole tile at once
-  constexpr int HEADROOM = HALF ? NCW * TILE : kQueueHeadroom;
+  // (kHalfMma: the 64 rows of the tile a warp stores)
+  constexpr int HEADROOM = HALF ? NCW * TILE : MMA ? NCW * 64 : kQueueHeadroom;
   static_assert(HEADROOM <= kQueueCap, "the queue holds one tile of every scoring warp");
   // rows per lane held in registers at once (kHalf: one pass, NPASS passes per tile)
   constexpr int R = HALF ? kHalfPassRows : TILE / 32;
   constexpr int NPASS = TILE / 32 / R;
   static_assert(NPASS * R * 32 == TILE && (!HALF || R % 4 == 0), "a pass is whole 128-row boxes");
   // one box: 8 KiB (two per kWhole stage) or 16 KiB (two per kHalf stage)
-  constexpr int BOX_BYTES = (HALF ? kTileRows : TILE) * kChunkF * 4;
+  constexpr int BOX_BYTES = (F16 ? kTileRows : TILE) * kChunkF * 4;
   constexpr int STAGE_BYTES = linear_stage_bytes(SCHED);
-  static_assert(!HALF || (BOX_BYTES == kTileRows * kHalfBoxF * 2 && STAGE_BYTES == 2 * BOX_BYTES),
+  static_assert(!F16 || (BOX_BYTES == kTileRows * kHalfBoxF * 2 && STAGE_BYTES == 2 * BOX_BYTES),
                 "an fp16 stage is two boxes");
   // fp32x2 accumulator pairs (see the accumulator comment below).  Not in the fp16 schedule: fma2 is two fmaf, so the
   // scores are the same bits, and without the 64-bit register pairs ptxas schedules its 128 registers better
@@ -311,7 +380,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // SWIZZLE_128B wants 1 KiB alignment
 
   const int S = p.num_stages;
-  float* wt_s = reinterpret_cast<float*>(smem + static_cast<size_t>(S) * STAGE_BYTES);
+  // kHalfMma: the B operand (1 KiB aligned, as SWIZZLE_128B wants) between the ring and W^T
+  float* wt_s = reinterpret_cast<float*>(smem + static_cast<size_t>(S) * STAGE_BYTES + (MMA ? linear_tc_b_bytes(C) : 0));
   float* bias_s = wt_s + p.f_pad * CP;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + CP);
   uint64_t* empty_bar = full_bar + S;
@@ -335,6 +405,12 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     const int n4 = p.f_pad * CP / 4;
     for (int i = threadIdx.x; i < n4; i += blockDim.x) dst[i] = __ldg(src + i);
     if (threadIdx.x < CP) bias_s[threadIdx.x] = __ldg(p.bias + threadIdx.x);
+    if constexpr (MMA) {
+      const uint4* bsrc = static_cast<const uint4*>(p.tc_ops);
+      uint4* bdst = reinterpret_cast<uint4*>(smem + static_cast<size_t>(S) * STAGE_BYTES);
+      for (int i = threadIdx.x; i < linear_tc_cols(C) * 8; i += blockDim.x) bdst[i] = __ldg(bsrc + i);
+      fence_proxy_async_smem();  // st.shared -> visible to the wgmma reads
+    }
     if constexpr (QUEUE) {
       for (int i = threadIdx.x; i < kQueueCap + 4; i += blockDim.x) q_slots[i] = 0;
     }
@@ -342,7 +418,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], MMA ? 4 : 1);  // kHalfMma: every warp of the warpgroup hands the stage back
     }
     fence_barrier_init();
   }
@@ -380,16 +456,16 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         // warp n % NCW; a group claimed past the end hands every warp kTileSentinel.  The next group is
         // claimed while this one is issued, so the atomic's round trip stays off the ring.
         unsigned long long* claim = p.counters + 4;  // [0] next unclaimed tile, [1] CTAs done claiming
-        long long base = static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(NCW)));
+        long long base = static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(NCU)));
         for (;;) {
           const long long next =
-              base < num_tiles ? static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(NCW))) : base;
-          for (int w = 0; w < NCW; ++w) {
+              base < num_tiles ? static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(NCU))) : base;
+          for (int w = 0; w < NCU; ++w) {
             const long long tile = base + w;
             UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u));
             tile_slot[stage] = base < num_tiles ? static_cast<int>(tile) : kTileSentinel;
             if (tile < num_tiles) {
-              if constexpr (HALF) {
+              if constexpr (F16) {
                 // rows 128-255 of the last tile may all lie past the batch: that box is not loaded (its rows are
                 // scored from stale shared memory and never stored)
                 uint8_t* dst = smem + static_cast<size_t>(stage) * STAGE_BYTES;
@@ -731,7 +807,171 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       }
     };
 
-    if constexpr (CLAIMED) {
+    if constexpr (MMA) {
+      // ===== kHalfMma: warpgroup wg = warp / 4 takes ring items wg, wg + 2, ...; per item four m64 blocks of 64 rows x
+      // NT columns, f_pad / 16 k16 steps each, one commit group; the stage goes back after the wait, the epilogue runs
+      // from registers.  Fragment (WgmmaTf32's layout): thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 and the
+      // row 8 below of each block, columns 8 i + 2 (l % 4) + {0, 1}: class c's hi piece at c, its lo piece at NH + c,
+      // the bound column at C - all of a row in one quad ----
+      constexpr int NH = linear_tc_hi_cols(C), NT = linear_tc_cols(C), NL = NT - NH;
+      const int q = lane & 3;
+      const long long row_in = 16 * (warp & 3) + (lane >> 2);  // row of fragment row-half 0 in block 0
+      const float* tcb = reinterpret_cast<const float*>(static_cast<const uint8_t*>(p.tc_ops) + NT * 128);
+      float bz[NH / 8][2];
+#pragma unroll
+      for (int i = 0; i < NH / 8; ++i) {
+        bz[i][0] = __ldg(tcb + 8 * i + 2 * q);
+        bz[i][1] = __ldg(tcb + 8 * i + 2 * q + 1);
+      }
+      const uint32_t b_base = smem_u32(smem + static_cast<size_t>(S) * STAGE_BYTES);
+      const int nk = p.f_pad / 16;
+      const float kappa = p.tc_kappa;
+      // scores, top-2 and the tier-1 guard of the 8 rows whose columns this thread's quad holds; quad lane q then stores
+      // and (if not certified) publishes the two rows of block q, so every row leaves once
+      auto finish_mma = [&](float (&d)[4][NT / 2], long long row0) {
+        int lab[4][2];
+        bool flg[4][2];
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float best = -INFINITY, second = -INFINITY, bound = 0.f;
+            int bi = C;  // a thread without classes loses every tie
+#pragma unroll
+            for (int i = 0; i < NH / 8; ++i) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int c = 8 * i + 2 * q + e;
+                const float lo = i < NL / 8 ? d[b][4 * (NH / 8 + i) + 2 * h + e] : 0.f;
+                const float v = (d[b][4 * i + 2 * h + e] + lo) + bz[i][e];
+                if (c < C) {
+                  if (v > best) {
+                    second = best;
+                    best = v;
+                    bi = c;
+                  } else {
+                    second = fmaxf(second, v);
+                  }
+                } else if (c == C) {
+                  bound = v;
+                }
+              }
+            }
+            // merge over the quad: the larger score wins, the lower class on a tie (first maximum, like np.argmax)
+#pragma unroll
+            for (int off = 1; off <= 2; off <<= 1) {
+              const float ob = __shfl_xor_sync(0xffffffffu, best, off);
+              const float os = __shfl_xor_sync(0xffffffffu, second, off);
+              const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+              if (ob > best || (ob == best && oi < bi)) {
+                second = fmaxf(best, os);
+                best = ob;
+                bi = oi;
+              } else {
+                second = fmaxf(second, ob);
+              }
+            }
+            const float a = __shfl_sync(0xffffffffu, bound, (lane & ~3) | ((C % 8) / 2));
+            const long long row = row0 + b * 64 + row_in + 8 * h;
+            lab[b][h] = bi;
+            // tier 1: certain iff margin > kappa A; NaN / Inf anywhere makes the comparison false
+            flg[b][h] = row < p.n_rows && !((best - second) > kappa * a);
+          }
+        }
+        unsigned masks[2];
+        int total = 0;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int idx = q == 0 ? lab[0][h] : q == 1 ? lab[1][h] : q == 2 ? lab[2][h] : lab[3][h];
+          const bool flag = q == 0 ? flg[0][h] : q == 1 ? flg[1][h] : q == 2 ? flg[2][h] : flg[3][h];
+          const long long row = row0 + q * 64 + row_in + 8 * h;
+          if (row < p.n_rows) {
+            if (p.labels) p.labels[row] = idx;
+            for (int i = 0; i < p.n_peers; ++i) {
+              if (p.wire_u8) static_cast<uint8_t*>(p.peers[i])[p.row_offset + row] = static_cast<uint8_t>(idx);
+              else static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idx;
+            }
+          }
+          masks[h] = __ballot_sync(0xffffffffu, flag);
+          total += __popc(masks[h]);
+        }
+        if (total == 0) return;
+        // the (few) uncertified rows go to the re-score warp, as in finish_rows: the labels above are provisional.  When
+        // the queue is backed up (most rows near-ties) the warp waits for room instead of settling its rows itself: a
+        // call from this loop made ptxas save the loop's live registers around it, spill stores and loads in the hot
+        // path at every class count (-Xptxas -v).  The drain never waits for a scoring warp, so the wait ends.
+        auto row_of = [&](int l, int h) { return row0 + (l & 3) * 64 + 16 * (warp & 3) + (l >> 2) + 8 * h; };
+        __threadfence();
+        int base = -1;
+        if (lane == 0) {
+          for (;;) {
+            const int tail = atomicAdd(&q_ctl[0], 0);
+            const int consumed = atomicAdd(&q_ctl[3], 0);
+            if (tail - consumed <= kQueueCap - HEADROOM) break;
+            __nanosleep(500);
+          }
+          base = atomicAdd(&q_ctl[0], total);
+        }
+        base = __shfl_sync(0xffffffffu, base, 0);
+        int off = base;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if ((masks[h] >> lane) & 1u) {
+            const int slot = (off + __popc(masks[h] & ((1u << lane) - 1u))) & (kQueueCap - 1);
+            while (atomicAdd(&q_slots[slot], 0) != 0) {
+            }
+            atomicExch(&q_slots[slot], static_cast<int>(row_of(lane, h)) + 1);
+          }
+          off += __popc(masks[h]);
+        }
+      };
+      uint32_t stage = static_cast<uint32_t>(warp >> 2), phase = 0;
+      for (bool first = true; scoring_warp; first = false) {
+        UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
+        UML_PROBE_CLOCK(probe_landed);
+        UML_PROBE_LANDED(first);
+        const int tile = tile_slot[stage];
+        const bool scored = !kFeedOnly && tile >= 0 && tile < num_tiles;
+        float d[4][NT / 2];
+        if (scored) {
+          const uint32_t a_base = smem_u32(smem + static_cast<size_t>(stage) * STAGE_BYTES);
+#pragma unroll
+          for (int b = 0; b < 4; ++b)
+#pragma unroll
+            for (int r = 0; r < NT / 2; ++r) {
+              d[b][r] = 0.f;
+              wgmma_fence_operand(d[b][r]);
+            }
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kHalfBoxF / 16; ++k) {
+            if (k < nk) {  // f_pad 32: the box's zero columns 32-63 are not multiplied
+              const uint64_t bd = wgmma_desc_k_sw128(b_base + 32 * k);
+#pragma unroll
+              for (int b = 0; b < 4; ++b)
+                WgmmaF16<NT>::mma(d[b], wgmma_desc_k_sw128(a_base + b * 64 * 128 + 32 * k), bd, k != 0 ? 1u : 0u);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+#pragma unroll
+          for (int b = 0; b < 4; ++b)
+#pragma unroll
+            for (int r = 0; r < NT / 2; ++r) wgmma_fence_operand(d[b][r]);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);  // the fourth warp's arrive hands the stage back
+        UML_PROBE_SINCE(probe_hold, probe_landed);
+        UML_PROBE_RELEASED();
+        if (tile == kTileSentinel) break;
+        stage += NCU;
+        if (stage >= static_cast<uint32_t>(S)) {
+          stage -= S;
+          phase ^= 1u;
+        }
+        if (scored) finish_mma(d, static_cast<long long>(tile) * TILE);
+      }
+    } else if constexpr (CLAIMED) {
       // this warp's ring items are n = warp, warp + NCW, ... (stage n % S, phase (n / S) & 1); S >= NCW lets stage and
       // phase advance without a division.  Both waits keep the invariant argued below: the next item is n + NCW <= n + S.
       uint32_t stage = static_cast<uint32_t>(warp), phase = 0;
@@ -853,9 +1093,14 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           atomicAdd(&q_ctl[3], 1);
         }
         const long long row = static_cast<long long>(v) - 1;
-        const int idx64 = rescore_row_inline(p, row, lane);
-        if (lane == 0) store_final_label(p, row, idx64);
-        ++n_done;
+        if constexpr (MMA) {
+          // tier 2: the fp32 route's own decision first; only the rows it would flag go to fp64 (and are counted)
+          n_done += settle_row_tc(p, wt_s, bias_s, CP, row, lane);
+        } else {
+          const int idx64 = rescore_row_inline(p, row, lane);
+          if (lane == 0) store_final_label(p, row, idx64);
+          ++n_done;
+        }
       }
       if (lane == 0 && n_done > 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n_done));
     }
@@ -1185,7 +1430,7 @@ bool linear_queue_rescore() {
 
 cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const LinearDeviceModel& m,
                               const LinearLaunch& l, bool exact, const FlagList& flags, int sm_count,
-                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed) {
+                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed, bool half_nonneg) {
   // the in-kernel queue re-scores rows with W in global memory / L2: fine for a 5 KB model, not for 62 KB of fp64
   // weights per row (cfg 3) - wide models take the re-score kernel, which stages W in shared memory
   const bool small_model = static_cast<size_t>(m.w64_stride) * m.n_features * sizeof(double) <= 16 * 1024;
@@ -1207,17 +1452,32 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
                         kHalfConsumerWarps * linear_stage_bytes(LinearSched::kHalf) <= kMaxSmemBytes,
                 "kHalfConsumerWarps stages do not fit");
   const bool half = half_map != nullptr && linear_half_rows_ok(m.f_pad);
-  const LinearSched sched = half ? LinearSched::kHalf : linear_whole_rows(m.f_pad) ? LinearSched::kWhole : LinearSched::kChunked;
+  // the tensor-core schedule: EXACT with the queue (its uncertified rows are replayed there), a model with tc_ops, an
+  // fp16 copy without negative values (its bound column is a product with x, not |x|).  UML_B200_LINEAR_TC=0 (read per
+  // call) keeps such a batch on kHalf: a test and A/B hook.
+  const char* tc_env = getenv("UML_B200_LINEAR_TC");
+  const bool tc = half && half_nonneg && inline_rescore && m.tc_ops != nullptr && l.x != nullptr && !(tc_env && tc_env[0] == '0');
+  // UML_B200_LINEAR_TC=1: the call fails unless it takes the tensor-core schedule (tests assert the dispatch with it)
+  if (tc_env && tc_env[0] == '1' && !tc) {
+    if (err) *err = "UML_B200_LINEAR_TC=1, but the batch or the model does not take the tensor-core schedule";
+    return cudaErrorInvalidValue;
+  }
+  const LinearSched sched = tc     ? LinearSched::kHalfMma
+                            : half ? LinearSched::kHalf
+                            : linear_whole_rows(m.f_pad) ? LinearSched::kWhole
+                                                         : LinearSched::kChunked;
   const int tile_rows = half ? kHalfTileRows : linear_box_rows(m.f_pad);
   p.num_tiles = (l.n_rows + tile_rows - 1) / tile_rows;
   p.f_pad = m.f_pad;
   p.kc = m.f_pad / kChunkF;
-  const size_t fixed = tma_fixed_smem(m, half);
+  p.tc_ops = m.tc_ops;
+  p.tc_kappa = m.tc_kappa;
+  const size_t fixed = tma_fixed_smem(m, half) + (tc ? linear_tc_b_bytes(m.n_classes) : 0);
   const int stage_bytes = linear_stage_bytes(sched);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / stage_bytes);
   stages = std::min(stages, 64);
   // test hook: the shallowest legal ring (stages == scoring warps) stresses the barrier protocol
-  const int warps = linear_consumer_warps(sched);
+  const int warps = linear_ring_units(sched);
   if (const char* env = getenv("UML_B200_STAGES")) stages = std::max(warps, std::min(stages, atoi(env)));
   p.num_stages = stages;
   // margin > 2 err guarantees the fp32 argmax is the exact argmax; err <= (F+4) 2^-24 A (1 + F 2^-21), see DESIGN.md
@@ -1242,6 +1502,7 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   const long long slots = (p.num_tiles + warps - 1) / warps;
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
   using S = LinearSched;
+  if (sched == S::kHalfMma) return dispatch_classes<true, true, S::kHalfMma>(m.n_classes, *half_map, p, grid, smem, stream);
   if (sched == S::kHalf) {
     const CUtensorMap& hmap = *half_map;
     if (!exact) return dispatch_classes<false, false, S::kHalf>(m.n_classes, hmap, p, grid, smem, stream);

@@ -271,10 +271,13 @@ cudaError_t launch_stage_convert(const void* src, int src_dtype, bool feature_ma
 // ---------------------------------------------------------------------------------------------------------------
 // compact fp16 copy of resident rows (read by the linear tile kernel's fp16 schedule): one thread per 8 features of a
 // row, two 16-byte loads, one 16-byte store.  fp32 -> fp16 is exact for the values the staging pass let through
-// (not_f16 == 0); columns F..ldh-1 are written as zero, whatever the fp32 rows hold there.
+// (not_f16 == 0); columns F..ldh-1 are written as zero, whatever the fp32 rows hold there.  A warp that saw a value < 0
+// raises *negative (the tensor-core schedule takes only batches without one).
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) pack_half_kernel(const float* __restrict__ x, long long ld, long long rows, int F,
-                                                        uint4* __restrict__ xh, long long ldh) {
+                                                        uint4* __restrict__ xh, long long ldh,
+                                                        unsigned long long* __restrict__ negative) {
+  bool neg = false;
   const long long groups = ldh / 8;
   const long long total = rows * groups;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
@@ -289,19 +292,22 @@ __global__ void __launch_bounds__(256) pack_half_kernel(const float* __restrict_
     uint32_t w[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const __half2 h = __floats2half2_rn(f0 + 2 * k < F ? v[2 * k] : 0.f, f0 + 2 * k + 1 < F ? v[2 * k + 1] : 0.f);
+      const float lo = f0 + 2 * k < F ? v[2 * k] : 0.f, hi = f0 + 2 * k + 1 < F ? v[2 * k + 1] : 0.f;
+      neg |= lo < 0.f || hi < 0.f;
+      const __half2 h = __floats2half2_rn(lo, hi);
       w[k] = *reinterpret_cast<const uint32_t*>(&h);
     }
     xh[i] = make_uint4(w[0], w[1], w[2], w[3]);
   }
+  if (__any_sync(0xffffffffu, neg) && (threadIdx.x & 31) == 0) atomicAdd(negative, 1ull);
 }
 
 cudaError_t launch_pack_half(const float* x, int64_t ld, int64_t rows, int n_features, void* xh, int64_t ldh,
-                             cudaStream_t stream) {
+                             unsigned long long* negative, cudaStream_t stream) {
   if (rows <= 0) return cudaSuccess;
   const long long want = (rows * (ldh / 8) + 255) / 256;
   const int grid = static_cast<int>(want < 132 * 16 ? want : 132 * 16);
-  pack_half_kernel<<<grid, 256, 0, stream>>>(x, ld, rows, n_features, static_cast<uint4*>(xh), ldh);
+  pack_half_kernel<<<grid, 256, 0, stream>>>(x, ld, rows, n_features, static_cast<uint4*>(xh), ldh, negative);
   return cudaGetLastError();
 }
 

@@ -60,7 +60,17 @@ struct LinearDeviceModel {
   int n_features;  // F
   int cp;          // padded class columns in wt
   int f_pad;       // rows of wt = 32 * ceil(F / 32), zero padded
+  // tensor-core schedule of the fp16 rows (DESIGN.md 3.1, 3.2), nullptr when the model does not qualify: the B operand
+  // [n][64] fp16, n = linear_tc_cols(C), W^T scaled by 2^sigma as hi | lo pieces with the bound column at hi column C,
+  // pre-swizzled (SWIZZLE_128B, one 128-byte row per column) so one linear copy fills shared memory; then the scaled
+  // biases as fp32 at byte n * 128 (hi columns: b_c for c < C, the bound column's bias at C, 0 past it)
+  const void* tc_ops;
+  float tc_kappa;  // a row is certain iff margin > tc_kappa * A (scaled scores, DESIGN.md 3.2)
 };
+// hi and lo column blocks of the tensor-core B operand: the C classes and the bound column, then the C lo pieces, each
+// padded to a multiple of 8 so that a class's hi and lo accumulators sit in the same thread of the wgmma fragment
+__host__ __device__ constexpr int linear_tc_hi_cols(int C) { return (C + 1 + 7) / 8 * 8; }
+__host__ __device__ constexpr int linear_tc_cols(int C) { return linear_tc_hi_cols(C) + (C + 7) / 8 * 8; }
 
 // doubles per feature of the fp64 weight table: a lane reads the classes of ITS feature as 16-byte pairs, so the row
 // length in 16-byte units must be odd for the eight lanes of a quarter-warp to land in eight different bank groups of
@@ -169,7 +179,8 @@ inline cudaError_t launch_dependent(void (*kern)(Params), int grid, int block, s
 // when given and linear_half_rows_ok(m.f_pad), the kernel reads it instead of xmap (same labels, half the bytes)
 cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const LinearDeviceModel& m,
                               const LinearLaunch& l, bool exact, const FlagList& flags, int sm_count,
-                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed);
+                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed,
+                              bool half_nonneg = false);
 bool linear_tma_supported(const LinearDeviceModel& m, std::string* why);
 cudaError_t launch_rescore_f64(const LinearDeviceModel& m, const LinearLaunch& l, const FlagList& flags, bool all_rows,
                                int sm_count, cudaStream_t stream);
@@ -273,13 +284,15 @@ struct StageResult {  // device-side counters
   unsigned long long lossy;
   unsigned long long not_tf32;  // fp32 values with any of the low 13 mantissa bits set (tensor-core path needs none)
   unsigned long long not_f16;   // fp32 values that are not finite fp16 values (the compact fp16 copy needs none)
+  unsigned long long negative;  // values < 0 in the compact fp16 copy (written by launch_pack_half; -0 is not one)
 };
 cudaError_t launch_stage_convert(const void* src, int src_dtype, bool feature_major, int64_t src_pitch_elems,
                                  int64_t rows, int n_features, float* dst, int64_t ld, double* dst64, int64_t ld64,
                                  StageResult* result, bool check_finite, cudaStream_t stream);
 // fp32 rows [rows][ld] -> fp16 rows [rows][ldh] (ldh = linear_half_ld(F), columns >= F zero); exact when the staging
 // pass found not_f16 == 0
+// (*negative is raised when any value is < 0: the tensor-core schedule needs none)
 cudaError_t launch_pack_half(const float* x, int64_t ld, int64_t rows, int n_features, void* xh, int64_t ldh,
-                             cudaStream_t stream);
+                             unsigned long long* negative, cudaStream_t stream);
 
 }  // namespace uml

@@ -73,6 +73,35 @@ struct WgmmaTf32<32> {
   }
 };
 
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, f16 x f16 -> fp32, one K = 16 step (32 bytes of f16 per row), both operands
+// K-major (transpose immediates 0, 0); scale_d = 0 overwrites D.  Same fragment layout as WgmmaTf32.  N: the widths the
+// linear tile kernel's tensor-core schedule uses (linear_tc_cols).
+template <int N>
+struct WgmmaF16;
+
+#define UML_WGMMA_F16(N, REGS, NA, NB, NS, ...)                                                               \
+  template <>                                                                                                 \
+  struct WgmmaF16<N> {                                                                                        \
+    static __device__ __forceinline__ void mma(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc,           \
+                                               uint32_t scale_d) {                                            \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" NS ", 0;\n\t"                                     \
+                   "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 {" REGS "}, %" NA ", %" NB         \
+                   ", p, 1, 1, 0, 0;\n\t}"                                                                    \
+                   : __VA_ARGS__                                                                              \
+                   : "l"(a_desc), "l"(b_desc), "r"(scale_d)                                                   \
+                   : "memory");                                                                               \
+    }                                                                                                         \
+  };
+#define UML_R4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+UML_WGMMA_F16(16, "%0, %1, %2, %3, %4, %5, %6, %7", "8", "9", "10", UML_R4(0), UML_R4(4))
+UML_WGMMA_F16(24, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11", "12", "13", "14", UML_R4(0), UML_R4(4), UML_R4(8))
+UML_WGMMA_F16(32, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15", "16", "17", "18", UML_R4(0),
+              UML_R4(4), UML_R4(8), UML_R4(12))
+UML_WGMMA_F16(40, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19", "20",
+              "21", "22", UML_R4(0), UML_R4(4), UML_R4(8), UML_R4(12), UML_R4(16))
+#undef UML_R4
+#undef UML_WGMMA_F16
+
 // generic-proxy writes to shared memory (st.shared) -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
