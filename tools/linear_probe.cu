@@ -243,9 +243,9 @@ int main() {
     TmaKernelParams p{};
     p.wt = m.wt;
     p.bias = m.bias;
-    p.peers[0] = labels;
-    p.n_peers = 1;
-    p.wire_u8 = 1;
+    p.targets.peers[0] = labels;
+    p.targets.n_peers = 1;
+    p.targets.wire_u8 = 1;
     p.n_rows = kRows;
     p.num_tiles = (kRows + tile - 1) / tile;
     p.f_pad = kF;

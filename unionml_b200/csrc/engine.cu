@@ -56,7 +56,7 @@ constexpr int64_t kSmallBytes = 256 << 10;   // ... when their raw feature block
 struct HostMirror {  // pinned; device counters are copied here
   int flag_count;
   int pad;
-  unsigned long long counters[4];
+  unsigned long long counters[uml::kCounterTileClaim];  // the slots a synchronous call zeroes and reads back
   StageResult stage;
   uml::SmallResult small[kSmallRows];
 };
@@ -321,7 +321,7 @@ static FlagList flag_list(const uml_engine* e) {
 
 // a synchronous call reads its counters back at the end, so it starts them from zero
 static cudaError_t reset_counters(uml_engine* e, cudaStream_t s) {
-  const cudaError_t ce = cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), s);
+  const cudaError_t ce = cudaMemsetAsync(e->d_counters, 0, sizeof(e->h->counters), s);
   return ce != cudaSuccess ? ce : cudaMemsetAsync(e->d_flag_count, 0, sizeof(int), s);
 }
 
@@ -409,14 +409,16 @@ int uml_engine_create(uml_engine** out, int device_id) {
   for (auto& ev : e->chunk_ev)
     if ((err = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", err);
   if ((err = cudaMalloc(&e->d_flag_count, sizeof(int))) != cudaSuccess) return fail("cudaMalloc", err);
-  if ((err = cudaMalloc(&e->d_counters, 6 * sizeof(unsigned long long))) != cudaSuccess) return fail("cudaMalloc", err);
+  if ((err = cudaMalloc(&e->d_counters, uml::kCounterSlots * sizeof(unsigned long long))) != cudaSuccess)
+    return fail("cudaMalloc", err);
   if ((err = cudaMalloc(&e->d_stage, sizeof(StageResult))) != cudaSuccess) return fail("cudaMalloc", err);
   if ((err = cudaHostAlloc((void**)&e->h, sizeof(HostMirror), cudaHostAllocMapped)) != cudaSuccess)
     return fail("cudaHostAlloc", err);
   memset(e->h, 0, sizeof(HostMirror));
-  // the scoring steps do not memset these: the re-score kernel hands the flag list back empty (linear_kernels.cu)
+  // the scoring steps do not memset these: the re-score kernel hands the flag list back empty (label_store.cuh)
   if ((err = cudaMemset(e->d_flag_count, 0, sizeof(int))) != cudaSuccess) return fail("cudaMemset", err);
-  if ((err = cudaMemset(e->d_counters, 0, 6 * sizeof(unsigned long long))) != cudaSuccess) return fail("cudaMemset", err);
+  if ((err = cudaMemset(e->d_counters, 0, uml::kCounterSlots * sizeof(unsigned long long))) != cudaSuccess)
+    return fail("cudaMemset", err);
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   err = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
@@ -1172,13 +1174,13 @@ static int enqueue_mlp(uml_engine* e, const uml::MlpDeviceModel& m, const CUtens
   } else {
     // the CUDA-core kernel has no peer stores: it writes int32 labels to scratch (the caller grew e->d_labels to
     // n_rows) and a thin kernel scatters them
-    const bool scatter = route == 3 && out.n_peers > 0;
+    const bool scatter = route == 3 && out.targets.n_peers > 0;
     uml::MlpTcLaunch own = out;
-    if (scatter) own.labels = e->d_labels.p[0];
+    if (scatter) own.targets.labels = e->d_labels.p[0];
     {
       NvtxRange r_score(route == 5 ? "uml:mlp_score_tc" : "uml:mlp_score_ffma");
       if (route == 5) UML_CUDA(e, uml::launch_mlp_tc(map, m, out, exact, fl, sm, s));
-      else UML_CUDA(e, uml::launch_mlp_tma(map, m, x, out.n_rows, own.labels, exact, fl, sm, s));
+      else UML_CUDA(e, uml::launch_mlp_tma(map, m, x, out.n_rows, own.targets.labels, exact, fl, sm, s));
       *launches += 1;
       if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
     }
@@ -1188,8 +1190,7 @@ static int enqueue_mlp(uml_engine* e, const uml::MlpDeviceModel& m, const CUtens
       *launches += 1;
     }
     if (scatter) {
-      UML_CUDA(e, uml::launch_labels_scatter(own.labels, out.n_rows, out.peers, out.n_peers, out.wire_u8, out.row_offset,
-                                             sm, s));
+      UML_CUDA(e, uml::launch_labels_scatter(own.targets.labels, out.n_rows, out.targets, sm, s));
       *launches += 1;
     }
   }
@@ -1201,15 +1202,14 @@ static int finish_stats(uml_engine* e, uml_stats* stats, int64_t n_rows, int lau
                         bool kernel_events = true) {
   // counters -> pinned mirror, then synchronise and report
   UML_CUDA(e, cudaMemcpyAsync(&e->h->flag_count, e->d_flag_count, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  UML_CUDA(e, cudaMemcpyAsync(e->h->counters, e->d_counters, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
-                              e->stream));
+  UML_CUDA(e, cudaMemcpyAsync(e->h->counters, e->d_counters, sizeof(e->h->counters), cudaMemcpyDeviceToHost, e->stream));
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[4], e->stream));
   UML_CUDA(e, cudaStreamSynchronize(e->stream));
   if (stats) {
     stats->n_rows = n_rows;
-    stats->n_ambiguous = (int64_t)e->h->counters[0];
-    stats->n_nonfinite = (int64_t)e->h->counters[1];
-    stats->n_flagged = (int64_t)e->h->counters[2];
+    stats->n_ambiguous = (int64_t)e->h->counters[uml::kCounterAmbiguous];
+    stats->n_nonfinite = (int64_t)e->h->counters[uml::kCounterNonfinite];
+    stats->n_flagged = (int64_t)e->h->counters[uml::kCounterFlagged];
     stats->kernel_launches = launches;
     stats->path = path;
     if (timed) {
@@ -1222,7 +1222,7 @@ static int finish_stats(uml_engine* e, uml_stats* stats, int64_t n_rows, int lau
       (void)cudaGetLastError();  // never leave a stale error behind for the next launch check
     }
   }
-  if (e->h->counters[1] > 0) UML_FAIL(e, UML_ERR_NONFINITE, "Input X contains NaN or infinity.");
+  if (e->h->counters[uml::kCounterNonfinite] > 0) UML_FAIL(e, UML_ERR_NONFINITE, "Input X contains NaN or infinity.");
   return UML_OK;
 }
 
@@ -1289,15 +1289,16 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
     l.ld = b->ld;
     l.ld64 = b->ld64;
     l.n_rows = b->n_rows;
-    l.labels = labels;
-    l.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
-    l.row_offset = row_offset;
+    uml::LabelTargets& t = l.targets;
+    t.labels = labels;
+    t.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
+    t.row_offset = row_offset;
     // fused int32 exchange: entry 0 is this rank's own full-length vector, the local label target.  Byte vectors are
     // all peers (own vector included); no int32 copy is kept.
-    const int own = n_peers > 0 && !l.wire_u8 ? 1 : 0;
-    if (own) l.labels = static_cast<int32_t*>(peers[0]) + row_offset;
-    l.n_peers = n_peers - own;
-    for (int i = 0; i < l.n_peers; ++i) l.peers[i] = peers[own + i];
+    const int own = n_peers > 0 && !t.wire_u8 ? 1 : 0;
+    if (own) t.labels = static_cast<int32_t*>(peers[0]) + row_offset;
+    t.n_peers = n_peers - own;
+    for (int i = 0; i < t.n_peers; ++i) t.peers[i] = peers[own + i];
     const CUtensorMap* half = b->has_half && compact_rows_enabled() ? &b->half_map : nullptr;
     return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, half, mode, timed, launches, path, elem_bytes,
                            b->half_nonneg);
@@ -1376,7 +1377,7 @@ int uml_labels_count_equal(uml_engine* e, const void* labels_dev, int label_byte
   };
   if ((ce = cudaMemcpyAsync(d_classes, classes_host, (size_t)n_classes * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
       (ce = cudaMemcpyAsync(d_targets, targets_host, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
-      (ce = cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), e->stream)) != cudaSuccess ||
+      (ce = cudaMemsetAsync(e->d_counters, 0, sizeof(e->h->counters), e->stream)) != cudaSuccess ||
       (ce = uml::launch_labels_count_equal(labels_dev, label_bytes, n, d_classes, n_classes, d_targets, e->d_counters, e->stream)) != cudaSuccess ||
       (ce = cudaMemcpyAsync(e->h->counters, e->d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream)) != cudaSuccess ||
       (ce = cudaStreamSynchronize(e->stream)) != cudaSuccess) {
@@ -1763,14 +1764,14 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     l.x = xc;
     l.ld = ld;
     l.n_rows = rows;
-    l.labels = e->d_labels.p[0] + (int64_t)slot * chunk_rows;
+    l.targets.labels = e->d_labels.p[0] + (int64_t)slot * chunk_rows;
     if (scores_out) {
       // float64 scores from the chunk as it crossed PCIe: the caller's own values (a float64 chunk that travelled as
       // fp32 was checked lossless by the gather threads)
       NvtxRange r_score("uml:scores_f64");
       uml::SrcView v{raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major ? 1 : F, L.feature_major ? rows : 1};
       if (direct) v = uml::SrcView{xc, UML_F32, ld, 1};
-      const cudaError_t ce = uml::launch_linear_scores_f64(m->dm, v, rows, e->d_vchunk.p[slot], e->d_counters + 1,
+      const cudaError_t ce = uml::launch_linear_scores_f64(m->dm, v, rows, e->d_vchunk.p[slot], e->d_counters + uml::kCounterNonfinite,
                                                            e->info.sm_count, cs);
       if (ce != cudaSuccess) {
         e->last_error = std::string("linear_scores_f64 launch: ") + cudaGetErrorString(ce);
@@ -1793,7 +1794,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       if (mlp) {
         uml::MlpTcLaunch out{};
         out.n_rows = rows;
-        out.labels = l.labels;
+        out.targets.labels = l.targets.labels;
         rc = enqueue_mlp(e, mlp->dm, map, xc, ld, out, exact, mlp_route(mlp->dm, has_map, false, tf32), false, &launches,
                          &path);
       } else {
@@ -1814,7 +1815,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       d2h += (int64_t)bytes;
     }
     if (values_out) {
-      UML_CUDA_DRAIN(e, uml::launch_labels_take(l.labels, 4, rows, e->d_classes.p[0], n_classes, e->d_vchunk.p[slot],
+      UML_CUDA_DRAIN(e, uml::launch_labels_take(l.targets.labels, 4, rows, e->d_classes.p[0], n_classes, e->d_vchunk.p[slot],
                                                 cs));
       launches += 1;
       UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)land : (void*)(values_out + r0), e->d_vchunk.p[slot],
@@ -1822,7 +1823,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       d2h += rows * 8;
     }
     if (labels_out) {
-      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)(land + (size_t)chunk_rows * 8) : (void*)(labels_out + r0), l.labels,
+      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)(land + (size_t)chunk_rows * 8) : (void*)(labels_out + r0), l.targets.labels,
                                         (size_t)rows * 4, cudaMemcpyDeviceToHost, cs));
       d2h += rows * 4;
     }
@@ -2008,7 +2009,7 @@ int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_ba
   UML_CUDA(e, reset_counters(e, e->stream));
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
   const uml::SrcView src = b->x64 ? uml::SrcView{b->x64, UML_F64, b->ld64, 1} : uml::SrcView{b->x, UML_F32, b->ld, 1};
-  UML_CUDA(e, uml::launch_linear_scores_f64(m->dm, src, b->n_rows, d_out, e->d_counters + 1, e->info.sm_count, e->stream));
+  UML_CUDA(e, uml::launch_linear_scores_f64(m->dm, src, b->n_rows, d_out, e->d_counters + uml::kCounterNonfinite, e->info.sm_count, e->stream));
   if (timed) {
     UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
     UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
@@ -2181,12 +2182,13 @@ static int mlp_predict_resident(uml_engine* e, const uml_mlp* m, const uml_batch
   };
   auto score = [&](int32_t* labels, bool timed, int* launches, int* path, int*) {  // the MLP kernels read fp32 rows
     uml::MlpTcLaunch out{};
-    out.labels = labels;
     out.n_rows = b->n_rows;
-    out.row_offset = row_offset;
-    out.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
-    out.n_peers = n_peers;  // every peer vector, this rank's own included
-    for (int i = 0; i < n_peers; ++i) out.peers[i] = peers[i];
+    uml::LabelTargets& t = out.targets;
+    t.labels = labels;
+    t.row_offset = row_offset;
+    t.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
+    t.n_peers = n_peers;  // every peer vector, this rank's own included
+    for (int i = 0; i < n_peers; ++i) t.peers[i] = peers[i];
     return enqueue_mlp(e, m->dm, b->map, b->x, b->ld, out, mode == UML_PREDICT_EXACT, route, timed, launches, path);
   };
   return predict_resident(e, b, m->dm.n_classes, m->dm.n_in, "module", labels_out, labels_on_device, n_peers,
@@ -2225,7 +2227,7 @@ int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, f
   }
   const bool timed = stats != nullptr;
   if (timed) {
-    UML_CUDA(e, cudaMemsetAsync(e->d_counters, 0, 4 * sizeof(unsigned long long), e->stream));
+    UML_CUDA(e, cudaMemsetAsync(e->d_counters, 0, sizeof(e->h->counters), e->stream));
     UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
     UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
   }

@@ -21,6 +21,7 @@
 #include <cstdlib>
 
 #include "uml_common.cuh"
+#include "label_store.cuh"
 #include "tma_ring.cuh"
 #include "rescore_util.cuh"
 #include "wgmma.cuh"
@@ -128,11 +129,7 @@ __device__ __forceinline__ RowScore score_row_f64(LOAD load, const double* __res
 struct TmaKernelParams {
   const float* wt;    // [f_pad][CP]
   const float* bias;  // [CP]
-  int32_t* labels;
-  void* peers[8];
-  int n_peers;
-  int wire_u8;  // peer vectors hold one byte per label (classes <= 256) instead of int32
-  long long row_offset;
+  LabelTargets targets;
   long long n_rows;
   long long num_tiles;
   int f_pad;
@@ -154,7 +151,7 @@ struct TmaKernelParams {
   int n_classes, n_features;
   double fold_rel;  // score_row_f64's extra relative bound term (LinearDeviceModel)
   int binary;
-  unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] re-scored rows
+  unsigned long long* counters;
 #ifdef UML_PROBE_WAIT_CLOCKS
   unsigned long long* probe_clocks;  // [5], see the diagnostic builds below
 #endif
@@ -178,25 +175,13 @@ __device__ __noinline__ int rescore_row_inline(const TmaKernelParams& p, long lo
     const float* xr = p.x + row * p.ld;
     r = score_row_f64([&](int f) { return static_cast<double>(xr[f]); }, p.w64, p.w64_stride, p.b64, p.n_features, p.n_classes, p.fold_rel, p.binary != 0, lane);
   }
-  if (lane == 0) {
-    if (r.bad) atomicAdd(&p.counters[1], 1ull);
-    if (r.ambiguous) atomicAdd(&p.counters[0], 1ull);
-  }
+  if (lane == 0) count_rescored_row(p, r.bad, r.ambiguous);
   return r.idx;
 }
 
 constexpr int kTileSentinel = -1;        // claimed schedules: ring item that ends a scoring warp's loop
 constexpr int kQueueCap = 2048;           // flagged-row queue of the QUEUE kernels (power of two)
 constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this many slots are free (8 warps x 128 rows)
-
-// the final label of a re-scored row into every target the launch writes (one lane)
-__device__ __forceinline__ void store_final_label(const TmaKernelParams& p, long long row, int idx) {
-  if (p.labels) p.labels[row] = idx;
-  for (int i = 0; i < p.n_peers; ++i) {
-    if (p.wire_u8) static_cast<uint8_t*>(p.peers[i])[p.row_offset + row] = static_cast<uint8_t>(idx);
-    else static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idx;
-  }
-}
 
 // Diagnostic builds of this file (tools/linear_probe.cu defines these; the library defines neither):
 //  UML_PROBE_FEED_ONLY    the scoring warps hand each stage back as soon as it has landed, without the math: what the
@@ -329,7 +314,7 @@ __device__ __noinline__ int settle_row_tc(const TmaKernelParams& p, const float*
     idx = rescore_row_inline(p, row, lane);
     f64 = 1;
   }
-  if (lane == 0) store_final_label(p, row, idx);
+  if (lane == 0) store_label(p.targets, row, idx);
   return f64;
 }
 
@@ -353,7 +338,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr bool HALF = SCHED == LinearSched::kHalf;
   constexpr bool MMA = SCHED == LinearSched::kHalfMma;
   constexpr bool F16 = HALF || MMA;                          // 256-row stages of the compact fp16 rows
-  constexpr bool CLAIMED = WHOLE || F16;                     // tiles claimed from p.counters[4], one tile per stage
+  constexpr bool CLAIMED = WHOLE || F16;                     // tiles claimed from kCounterTileClaim, one tile per stage
   constexpr int NCW = linear_consumer_warps(SCHED);
   constexpr int NCU = linear_ring_units(SCHED);
   static_assert(!MMA || (EXACT && QUEUE), "the tensor-core schedule certifies rows through the queue's replay");
@@ -455,7 +440,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         // launch lasted as long as the slowest one.  Ring item n is one tile with both halves of its rows and goes to
         // warp n % NCW; a group claimed past the end hands every warp kTileSentinel.  The next group is
         // claimed while this one is issued, so the atomic's round trip stays off the ring.
-        unsigned long long* claim = p.counters + 4;  // [0] next unclaimed tile, [1] CTAs done claiming
+        unsigned long long* claim = &p.counters[kCounterTileClaim];
+        unsigned long long* claim_done = &p.counters[kCounterTileClaimDone];
         long long base = static_cast<long long>(atomicAdd(claim, static_cast<unsigned long long>(NCU)));
         for (;;) {
           const long long next =
@@ -496,9 +482,9 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         // this CTA claims no more; the last CTA to get here hands the counter back at 0 for the next launch on the
         // stream (no memset between steps, and correct under CUDA-graph replay)
         __threadfence();
-        if (atomicAdd(claim + 1, 1ull) == static_cast<unsigned long long>(gridDim.x) - 1ull) {
-          claim[0] = 0ull;
-          claim[1] = 0ull;
+        if (atomicAdd(claim_done, 1ull) == static_cast<unsigned long long>(gridDim.x) - 1ull) {
+          *claim = 0ull;
+          *claim_done = 0ull;
           __threadfence();
         }
       } else {
@@ -705,25 +691,10 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
 #pragma unroll
       for (int j = 0; j < R; ++j) {
         const long long row = row0 + lane + 32 * j;
-        if (row < p.n_rows) {
-          if (p.labels) p.labels[row] = idxs[j];
-          if (!p.wire_u8)
-            for (int i = 0; i < p.n_peers; ++i) static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idxs[j];
-        }
-        if constexpr (EXACT && !QUEUE) {
-          const unsigned mask = __ballot_sync(0xffffffffu, flag[j]);
-          if (mask != 0u) {
-            int base = 0;
-            if (lane == 0) base = atomicAdd(p.flag_count, __popc(mask));
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (flag[j]) {
-              const int pos = base + __popc(mask & ((1u << lane) - 1u));
-              if (pos < p.flag_cap) p.flag_rows[pos] = static_cast<int32_t>(row);
-            }
-          }
-        }
+        if (row < p.n_rows) store_label_i32(p.targets, row, idxs[j]);
+        if constexpr (EXACT && !QUEUE) flag_rows_warp(flag[j], row, p, lane);
       }
-      if (p.wire_u8 && p.n_peers > 0) {
+      if (p.targets.wire_u8 && p.targets.n_peers > 0) {
         // byte labels: transpose through shuffles so lane l < GR/4 holds rows 4l..4l+3 of a group of GR = 32 RG rows
         // and the group leaves as ONE coalesced GR-byte store per target (instead of RG int32 stores).  Row 4l+t sits
         // in byte (4l+t)/32 = l/8 of lane (4l+t) % 32's packed word.  One group per pass, except kHalf's 8 rows per
@@ -740,19 +711,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
             word |= ((w >> (8 * (lane >> 3))) & 0xffu) << (8 * t);
           }
-          const long long row4 = row0 + g * 32 * RG + 4 * lane;
-          const long long at = p.row_offset + row4;
-          if (4 * lane < 32 * RG) {
-            if (row4 + 3 < p.n_rows && (at & 3) == 0) {
-              for (int i = 0; i < p.n_peers; ++i)
-                *reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(p.peers[i]) + at) = word;
-            } else {
-              for (int t = 0; t < 4; ++t)
-                if (row4 + t < p.n_rows)
-                  for (int i = 0; i < p.n_peers; ++i)
-                    static_cast<uint8_t*>(p.peers[i])[at + t] = static_cast<uint8_t>((word >> (8 * t)) & 0xffu);
-            }
-          }
+          store_label_word_u8(p, row0 + g * 32 * RG + 4 * lane, word, 4 * lane < 32 * RG);
         }
       }
       if constexpr (EXACT && QUEUE) {
@@ -798,10 +757,10 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
                 mask &= mask - 1u;
                 const long long row = row0 + l + 32 * j;
                 const int idx64 = rescore_row_inline(p, row, lane);
-                if (lane == 0) store_final_label(p, row, idx64);
+                if (lane == 0) store_label(p.targets, row, idx64);
               }
             }
-            if (lane == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(total));
+            if (lane == 0) atomicAdd(&p.counters[kCounterFlagged], static_cast<unsigned long long>(total));
           }
         }
       }
@@ -885,13 +844,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           const int idx = q == 0 ? lab[0][h] : q == 1 ? lab[1][h] : q == 2 ? lab[2][h] : lab[3][h];
           const bool flag = q == 0 ? flg[0][h] : q == 1 ? flg[1][h] : q == 2 ? flg[2][h] : flg[3][h];
           const long long row = row0 + q * 64 + row_in + 8 * h;
-          if (row < p.n_rows) {
-            if (p.labels) p.labels[row] = idx;
-            for (int i = 0; i < p.n_peers; ++i) {
-              if (p.wire_u8) static_cast<uint8_t*>(p.peers[i])[p.row_offset + row] = static_cast<uint8_t>(idx);
-              else static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idx;
-            }
-          }
+          if (row < p.n_rows) store_label(p.targets, row, idx);
           masks[h] = __ballot_sync(0xffffffffu, flag);
           total += __popc(masks[h]);
         }
@@ -1098,11 +1051,11 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           n_done += settle_row_tc(p, wt_s, bias_s, CP, row, lane);
         } else {
           const int idx64 = rescore_row_inline(p, row, lane);
-          if (lane == 0) store_final_label(p, row, idx64);
+          if (lane == 0) store_label(p.targets, row, idx64);
           ++n_done;
         }
       }
-      if (lane == 0 && n_done > 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n_done));
+      if (lane == 0 && n_done > 0) atomicAdd(&p.counters[kCounterFlagged], static_cast<unsigned long long>(n_done));
     }
   }
 #ifdef UML_PROBE_TIMELINE
@@ -1127,12 +1080,8 @@ struct RescoreParams {
   const int32_t* flag_rows;
   int flag_cap;
   int all_rows;
-  int32_t* labels;
-  void* peers[8];
-  int n_peers;
-  int wire_u8;
-  long long row_offset;
-  unsigned long long* counters;  // [0] ambiguous, [1] nonfinite, [2] flagged (re-scored) rows
+  LabelTargets targets;
+  unsigned long long* counters;
   int smem_weights;              // W, b staged in dynamic shared memory ((C F + 2 C) doubles)
   double fold_rel;
   int binary;
@@ -1158,13 +1107,8 @@ __device__ __forceinline__ void rescore_rows(const RescoreParams& p, WPTR w64, W
       r = score_row_f64([&](int f) { return static_cast<double>(xr[f]); }, w64, S, b64, F, C, p.fold_rel, p.binary != 0, lane);
     }
     if (lane == 0) {
-      if (p.labels) p.labels[row] = r.idx;
-      for (int q = 0; q < p.n_peers; ++q) {
-        if (p.wire_u8) static_cast<uint8_t*>(p.peers[q])[p.row_offset + row] = static_cast<uint8_t>(r.idx);
-        else static_cast<int32_t*>(p.peers[q])[p.row_offset + row] = r.idx;
-      }
-      if (r.bad) atomicAdd(&p.counters[1], 1ull);
-      if (r.ambiguous) atomicAdd(&p.counters[0], 1ull);
+      store_label(p.targets, row, r.idx);
+      count_rescored_row(p, r.bad, r.ambiguous);
     }
   }
 }
@@ -1186,26 +1130,14 @@ __global__ void __launch_bounds__(256) rescore_f64_kernel(const RescoreParams p)
   const int lane = threadIdx.x & 31;
   const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps_total = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
-  const long long n = p.all_rows ? p.n_rows : static_cast<long long>(min(*p.flag_count, p.flag_cap));
-  if (!p.all_rows && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n));
+  const long long n = flag_list_rows(p);
   if (p.smem_weights) {
     const double* ws = rs_w;
     rescore_rows(p, ws, ws + nw, n, lane, warp_global, warps_total);
   } else {
     rescore_rows(p, p.w64, p.b64, n, lane, warp_global, warps_total);
   }
-  // hand the flag list back empty: every block has read *flag_count before it gets here, so the last one to finish may
-  // reset it (and the ticket) for the next scoring launch on this stream - no memset between steps
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned long long ticket = atomicAdd(&p.counters[3], 1ull);
-    if (ticket == static_cast<unsigned long long>(gridDim.x) - 1ull) {
-      *const_cast<int*>(p.flag_count) = 0;
-      p.counters[3] = 0ull;
-      __threadfence();
-    }
-  }
+  flag_list_hand_back(p);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1441,11 +1373,7 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   TmaKernelParams p{};
   p.wt = m.wt;
   p.bias = m.bias;
-  p.labels = l.labels;
-  p.n_peers = l.n_peers;
-  p.wire_u8 = l.wire_u8;
-  for (int i = 0; i < 8; ++i) p.peers[i] = i < l.n_peers ? l.peers[i] : nullptr;
-  p.row_offset = l.row_offset;
+  p.targets = l.targets;
   p.n_rows = l.n_rows;
   // (at f_pad <= 64 the fp16 schedule's shortest ring always fits beside the largest W^T, 16 classes)
   static_assert(1024 + (kHalfBoxF + 1) * 20 * 4 + 2 * 64 * 8 + (kQueueCap + 4) * 4 + 64 * 4 +
@@ -1538,11 +1466,7 @@ cudaError_t launch_rescore_f64(const LinearDeviceModel& m, const LinearLaunch& l
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
   p.all_rows = all_rows ? 1 : 0;
-  p.labels = l.labels;
-  p.n_peers = l.n_peers;
-  p.wire_u8 = l.wire_u8;
-  for (int i = 0; i < 8; ++i) p.peers[i] = i < l.n_peers ? l.peers[i] : nullptr;
-  p.row_offset = l.row_offset;
+  p.targets = l.targets;
   p.counters = flags.counters;
   p.fold_rel = m.fold_rel;
   p.binary = m.binary;

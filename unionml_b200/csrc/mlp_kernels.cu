@@ -25,6 +25,7 @@
 #include <cstdlib>
 
 #include "uml_common.cuh"
+#include "label_store.cuh"
 #include "tma_ring.cuh"
 #include "mlp_rescore.cuh"
 #include "mlp_proba.cuh"
@@ -308,17 +309,7 @@ mlp_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const Params p) 
             // |z_c - true| <= E1 * sum_n |w2_cn| + (H+4) u A2, E1 = (F+4) u A1 (ReLU is 1-Lipschitz)
             const float err = p.e1_scale * a1[j] + p.e2_scale * z[j][C];
             const bool certain = (best - second) > 2.0f * err;
-            const bool flagged = in_range && !certain;
-            const unsigned mask = __ballot_sync(0xffffffffu, flagged);
-            if (mask != 0u) {
-              int base = 0;
-              if (lane == 0) base = atomicAdd(p.flag_count, __popc(mask));
-              base = __shfl_sync(0xffffffffu, base, 0);
-              if (flagged) {
-                const int pos = base + __popc(mask & ((1u << lane) - 1u));
-                if (pos < p.flag_cap) p.flag_rows[pos] = static_cast<int32_t>(row);
-              }
-            }
+            flag_rows_warp(in_range && !certain, row, p, lane);
           }
         }
       }
@@ -340,11 +331,7 @@ struct MlpRescoreParams {
   const int32_t* flag_rows;
   int flag_cap;
   int all_rows;
-  int32_t* labels;
-  void* peers[8];
-  int n_peers;
-  int wire_u8;
-  long long row_offset;
+  LabelTargets targets;
   unsigned long long* counters;
 };
 
@@ -369,8 +356,7 @@ __global__ void __launch_bounds__(256) mlp_rescore_f64_kernel(const MlpRescorePa
   pdl_wait_for_predecessor();  // from here on: the flag list and labels of the scoring kernel this launch depends on
   const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps_total = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
-  const long long n = p.all_rows ? p.n_rows : static_cast<long long>(min(*p.flag_count, p.flag_cap));
-  if (!p.all_rows && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n));
+  const long long n = flag_list_rows(p);
   // warp w takes entries [w*R, w*R + R) of the list, then strides by all warps: a short list spreads over many warps
   for (long long i = warp_global * R; i < n; i += warps_total * R) {
     long long row[R];
@@ -394,26 +380,11 @@ __global__ void __launch_bounds__(256) mlp_rescore_f64_kernel(const MlpRescorePa
           mine = res[r];
         }
       }
-      if (p.labels) p.labels[my_row] = mine.idx;
-      for (int q = 0; q < p.n_peers; ++q) {
-        if (p.wire_u8) static_cast<uint8_t*>(p.peers[q])[p.row_offset + my_row] = static_cast<uint8_t>(mine.idx);
-        else static_cast<int32_t*>(p.peers[q])[p.row_offset + my_row] = mine.idx;
-      }
-      if (mine.bad) atomicAdd(&p.counters[1], 1ull);
-      if (mine.ambiguous) atomicAdd(&p.counters[0], 1ull);
+      store_label(p.targets, my_row, mine.idx);
+      count_rescored_row(p, mine.bad, mine.ambiguous);
     }
   }
-  // hand the flag list back empty (see rescore_f64_kernel in linear_kernels.cu)
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned long long ticket = atomicAdd(&p.counters[3], 1ull);
-    if (ticket == static_cast<unsigned long long>(gridDim.x) - 1ull) {
-      *const_cast<int*>(p.flag_count) = 0;
-      p.counters[3] = 0ull;
-      __threadfence();
-    }
-  }
+  flag_list_hand_back(p);
 }
 
 // class probabilities for shapes no tile kernel takes: the logits of the fp64 scorer above (mlp_rs_rows), a float64
@@ -497,8 +468,7 @@ __global__ void __launch_bounds__(256) mlp_topk_f64_kernel(const MlpTopkF64Param
   pdl_wait_for_predecessor();  // flagged mode: the flag list and outputs of the tile kernel this launch depends on
   const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps_total = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
-  const long long n = p.all_rows ? p.n_rows : static_cast<long long>(min(*p.flag_count, p.flag_cap));
-  if (!p.all_rows && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&p.counters[2], static_cast<unsigned long long>(n));
+  const long long n = flag_list_rows(p);
   const int C = p.C, k = p.k, kk = min(p.k, p.C - 1);
   for (long long i = warp_global * R; i < n; i += warps_total * R) {
     long long row[R];
@@ -541,24 +511,11 @@ __global__ void __launch_bounds__(256) mlp_topk_f64_kernel(const MlpTopkF64Param
         if (rank >= 1 && rank <= kk && !((above - zc) > 2.0 * err[r])) ambiguous = true;
       }
       ambiguous = __any_sync(0xffffffffu, ambiguous);
-      if (lane == 0) {
-        if (res[r].bad) atomicAdd(&p.counters[1], 1ull);
-        if (ambiguous) atomicAdd(&p.counters[0], 1ull);
-      }
+      if (lane == 0) count_rescored_row(p, res[r].bad, ambiguous);
     }
     __syncwarp();  // the strip is rewritten by the next pass
   }
-  // hand the flag list back empty (see mlp_rescore_f64_kernel)
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned long long ticket = atomicAdd(&p.counters[3], 1ull);
-    if (ticket == static_cast<unsigned long long>(gridDim.x) - 1ull) {
-      *const_cast<int*>(p.flag_count) = 0;
-      p.counters[3] = 0ull;
-      __threadfence();
-    }
-  }
+  flag_list_hand_back(p);
 }
 
 // small-batch kernel of the online path (fastapi.py /predict, B <= 64 rows): the fp64 scorer above on the request's
@@ -773,11 +730,7 @@ cudaError_t launch_mlp_rescore_f64(const MlpDeviceModel& m, const float* x, int6
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
   p.all_rows = all_rows ? 1 : 0;
-  p.labels = out.labels;
-  p.n_peers = out.n_peers;
-  p.wire_u8 = out.wire_u8;
-  for (int i = 0; i < 8; ++i) p.peers[i] = i < out.n_peers ? out.peers[i] : nullptr;
-  p.row_offset = out.row_offset;
+  p.targets = out.targets;
   p.counters = flags.counters;
   // shared memory: W1 + padded W2 + biases + the two bound vectors + one strip (x, hidden values) per warp
   const size_t smem = (mlp_rs_weight_doubles(m.n_in, m.n_hidden, m.n_classes) + 8 * mlp_rs_strip_doubles(m.n_in, m.n_hidden, kMlpRsRows)) * sizeof(double);

@@ -37,6 +37,7 @@
 #include <vector>
 
 #include "uml_common.cuh"
+#include "label_store.cuh"
 #include "wgmma.cuh"
 #include "mlp_proba.cuh"
 #include "mlp_topk.cuh"
@@ -64,11 +65,7 @@ struct MlpTcParams {
   float b1max;
   float e1_scale, e2_scale;
   const float* w1_tiles;    // [KC][2H rows][32 floats], rows 128-byte swizzled exactly as the wgmma descriptor reads them
-  int32_t* labels;
-  void* peers[8];
-  int n_peers;
-  int wire_u8;
-  long long row_offset;
+  LabelTargets targets;
   long long n_rows;
   long long num_tiles;
   int kc;
@@ -327,7 +324,7 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
           const long long row = tile * kTileRows + row_in_tile;
           const float err = p.e1_scale * a1 + p.e2_scale * z[C];
           const bool certain = mlp_topk_certain<M>(v, min(k, C - 1), 2.0f * err);
-          mlp_topk_flag(row < p.n_rows && !certain, row, p.flag_count, p.flag_rows, p.flag_cap, lane);
+          flag_rows_warp(row < p.n_rows && !certain, row, p, lane);
         }
         continue;
       }
@@ -346,12 +343,8 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
         }
       }
       const bool in_range = row < p.n_rows;
-      if (in_range) {
-        if (p.labels) p.labels[row] = idx;
-        if (!p.wire_u8)
-          for (int i = 0; i < p.n_peers; ++i) static_cast<int32_t*>(p.peers[i])[p.row_offset + row] = idx;
-      }
-      if (p.wire_u8 && p.n_peers > 0) {
+      if (in_range) store_label_i32(p.targets, row, idx);
+      if (p.targets.wire_u8 && p.targets.n_peers > 0) {
         // byte labels: the warp's rows are two runs of 16 (rows 16 wq + 0..15 of each half); lanes 0..7 gather 4
         // consecutive rows each -> the warp's 32 labels leave as eight 4-byte words
         const int run = (lane >> 2) & 1;
@@ -363,34 +356,13 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
           const int src = 4 * (r & 7) + 2 * run + (r >> 3);  // the lane that owns row r of the run
           word |= (static_cast<uint32_t>(__shfl_sync(0xffffffffu, idx, src)) & 0xffu) << (8 * t);
         }
-        const long long row4 = tile * kTileRows + 64 * run + 16 * wq + r0;
-        const long long at = p.row_offset + row4;
-        if (lane < 8) {
-          if (row4 + 3 < p.n_rows && (at & 3) == 0) {
-            for (int i = 0; i < p.n_peers; ++i) *reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(p.peers[i]) + at) = word;
-          } else {
-            for (int t = 0; t < 4; ++t)
-              if (row4 + t < p.n_rows)
-                for (int i = 0; i < p.n_peers; ++i)
-                  static_cast<uint8_t*>(p.peers[i])[at + t] = static_cast<uint8_t>((word >> (8 * t)) & 0xffu);
-          }
-        }
+        store_label_word_u8(p, tile * kTileRows + 64 * run + 16 * wq + r0, word, lane < 8);
       }
       if (EXACT) {
         // |z_c - true| <= E1 * max_c sum_n |w2_cn| + (H+4) u A2   (ReLU is 1-Lipschitz); NaN/Inf -> comparison false
         const float err = p.e1_scale * a1 + p.e2_scale * z[C];
         const bool certain = (best - second) > 2.0f * err;
-        const bool flagged = in_range && !certain;
-        const unsigned mask = __ballot_sync(0xffffffffu, flagged);
-        if (mask != 0u) {
-          int base = 0;
-          if (lane == 0) base = atomicAdd(p.flag_count, __popc(mask));
-          base = __shfl_sync(0xffffffffu, base, 0);
-          if (flagged) {
-            const int pos = base + __popc(mask & ((1u << lane) - 1u));
-            if (pos < p.flag_cap) p.flag_rows[pos] = static_cast<int32_t>(row);
-          }
-        }
+        flag_rows_warp(in_range && !certain, row, p, lane);
       }
     }
   }
@@ -494,11 +466,7 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   // (main, small) 8 products and the sum, a subnormal feature |x_f| w1max_f, and 3 for the bias and epilogue adds
   p.b2[C] = mlp_a2_bias_entry(b2max, (18.0 * n_mma + 3.0 + w1max_sum) * kFltMin, m.w2_abs_row_sum_max, H);
   p.w1_tiles = m.w1_tiles;
-  p.labels = l.labels;
-  p.n_peers = l.n_peers;
-  p.wire_u8 = l.wire_u8;
-  for (int i = 0; i < 8; ++i) p.peers[i] = i < l.n_peers ? l.peers[i] : nullptr;
-  p.row_offset = l.row_offset;
+  p.targets = l.targets;
   p.n_rows = l.n_rows;
   p.num_tiles = (l.n_rows + kTileRows - 1) / kTileRows;
   p.kc = m.f_pad / kChunkF;

@@ -78,7 +78,9 @@ __device__ __forceinline__ void mlp_topk_store_run(const T* s, T* out, long long
 // a warp's staging strip: 32 rows x kMlpTopkMax indices, then as many probabilities (4-byte words)
 constexpr int kMlpTopkStripWords = 2 * 32 * kMlpTopkMax;
 
-// flagged rows of a warp onto the flag list (one atomic per warp)
+// flag_rows_warp (label_store.cuh) with the flag list's fields read before the ballot, for the top-k form of
+// mlp_argmax_tma_kernel: read after it, as flag_rows_warp does, ptxas gives that form different code (H = 16, C = 10:
+// 134 registers instead of 128)
 __device__ __forceinline__ void mlp_topk_flag(bool flagged, long long row, int* flag_count, int32_t* flag_rows, int flag_cap,
                                               int lane) {
   const unsigned mask = __ballot_sync(0xffffffffu, flagged);

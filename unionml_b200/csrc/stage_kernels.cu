@@ -11,6 +11,7 @@
 #include <type_traits>
 
 #include "uml_common.cuh"
+#include "label_store.cuh"
 
 namespace uml {
 
@@ -424,33 +425,24 @@ cudaError_t launch_topk_first_hits(const int32_t* idx, int k, int64_t n, const d
 struct ScatterParams {
   const int32_t* labels;
   long long n;
-  void* peers[8];
-  int n_peers;
-  int wire_u8;
-  long long row_offset;
+  LabelTargets targets;  // (targets.labels is nullptr)
 };
 
 __global__ void __launch_bounds__(256) labels_scatter_kernel(const ScatterParams p) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < p.n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int idx = p.labels[i];
-    for (int q = 0; q < p.n_peers; ++q) {
-      if (p.wire_u8) static_cast<unsigned char*>(p.peers[q])[p.row_offset + i] = static_cast<unsigned char>(idx);
-      else static_cast<int32_t*>(p.peers[q])[p.row_offset + i] = idx;
-    }
+    store_label(p.targets, i, p.labels[i]);
   }
 }
 
-cudaError_t launch_labels_scatter(const int32_t* labels, int64_t n, void* const* peers, int n_peers, int wire_u8,
-                                  int64_t row_offset, int sm_count, cudaStream_t stream) {
-  if (n <= 0 || n_peers <= 0) return cudaSuccess;
+cudaError_t launch_labels_scatter(const int32_t* labels, int64_t n, const LabelTargets& out, int sm_count,
+                                  cudaStream_t stream) {
+  if (n <= 0 || out.n_peers <= 0) return cudaSuccess;
   ScatterParams p{};
   p.labels = labels;
   p.n = n;
-  p.n_peers = n_peers;
-  p.wire_u8 = wire_u8;
-  p.row_offset = row_offset;
-  for (int i = 0; i < 8; ++i) p.peers[i] = i < n_peers ? peers[i] : nullptr;
+  p.targets = out;
+  p.targets.labels = nullptr;
   const long long want = (n + 255) / 256;
   const int grid = static_cast<int>(want < static_cast<long long>(sm_count) * 4 ? want : static_cast<long long>(sm_count) * 4);
   labels_scatter_kernel<<<grid, 256, 0, stream>>>(p);

@@ -110,8 +110,18 @@ struct FlagList {
   int* count;        // number of flagged rows appended so far; the re-score kernel's last block resets it to 0
   int32_t* rows;     // flagged row indices
   int capacity;
-  unsigned long long* counters;  // [0] = n_ambiguous, [1] = n_nonfinite, [2] = n_flagged, [3] = re-score blocks done,
-                                 // [4], [5] = the whole-row tile kernel's tile claim (handed back at 0 by every launch)
+  unsigned long long* counters;  // [kCounterSlots]
+};
+// slots of FlagList::counters.  A synchronous call zeroes those before kCounterTileClaim and reads them back; the
+// re-score kernels hand the ticket back at 0, the linear tile kernel both claim slots, so a step needs no memset.
+enum Counter : int {
+  kCounterAmbiguous,      // rows whose float64 margin is inside its rounding bound (uml_stats.n_ambiguous)
+  kCounterNonfinite,      // rows with NaN / Inf (n_nonfinite)
+  kCounterFlagged,        // rows re-scored in float64 (n_flagged)
+  kCounterRescoreTicket,  // re-score blocks done; the last one hands the flag list back empty (label_store.cuh)
+  kCounterTileClaim,      // the linear tile kernel's next unclaimed tile
+  kCounterTileClaimDone,  // its CTAs done claiming; the last one hands both claim slots back at 0
+  kCounterSlots
 };
 
 // The caller's own values for the rows of a launch: the raw source chunk as it was copied to the device (any dtype,
@@ -138,6 +148,16 @@ __device__ __forceinline__ double load_src(const SrcView& v, long long row, int 
 }
 #endif
 
+// Where a launch stores each row's label (device side: label_store.cuh): the local int32 vector (or nullptr), and the
+// fused all-gather epilogue's peer vectors, row r of the launch at peers[i] + row_offset + r for i < n_peers
+struct LabelTargets {
+  int32_t* labels;
+  void* peers[8];
+  int n_peers;
+  int wire_u8;  // 1: peer vectors are uint8 (one byte per label), 0: int32
+  long long row_offset;
+};
+
 struct LinearLaunch {
   const float* x;       // device fp32 row-major
   const double* x64;    // optional fp64 copy of the same rows (lossy staging), else nullptr
@@ -145,12 +165,7 @@ struct LinearLaunch {
   int64_t ld;           // floats per row
   int64_t ld64;
   int64_t n_rows;
-  int32_t* labels;      // local label vector (device)
-  // fused all-gather epilogue: labels are also stored to peers[i] + row_offset for i < n_peers
-  void* peers[8];
-  int n_peers;
-  int wire_u8;  // 1: peer vectors are uint8 (one byte per label), 0: int32
-  int64_t row_offset;
+  LabelTargets targets;
 };
 
 // launch `kern<<<grid, block, smem, stream>>>(p)` as a programmatic dependent of the previous kernel on the stream: its
@@ -219,13 +234,8 @@ struct MlpDeviceModel {
   const float* w1_tiles;
   const MlpHostModel* host;
 };
-// where the labels of an MLP launch go (same contract as LinearLaunch's label fields)
 struct MlpTcLaunch {
-  int32_t* labels;  // local int32 vector or nullptr
-  void* peers[8];
-  int n_peers;
-  int wire_u8;
-  long long row_offset;
+  LabelTargets targets;
   long long n_rows;
   float* proba;  // launch_mlp_tc_proba: class probabilities [n_rows][n_classes] (device)
   // launch_mlp_tc_topk: [n_rows][topk_k] class indices and probabilities (device; topk_proba may be nullptr)
@@ -275,8 +285,8 @@ cudaError_t mlp_small_reserve(size_t smem);
 cudaError_t launch_mlp_small(const MlpDeviceModel& m, const SrcView& src, int n_rows, SmallResult* out, size_t smem,
                              cudaStream_t stream);
 // int32 labels (device) -> every target vector of a fused exchange (int32 or uint8 wire), for kernels without peer stores
-cudaError_t launch_labels_scatter(const int32_t* labels, int64_t n, void* const* peers, int n_peers, int wire_u8,
-                                  int64_t row_offset, int sm_count, cudaStream_t stream);
+cudaError_t launch_labels_scatter(const int32_t* labels, int64_t n, const LabelTargets& out, int sm_count,
+                                  cudaStream_t stream);
 
 // staging kernels (stage_kernels.cu)
 struct StageResult {  // device-side counters
