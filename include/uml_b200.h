@@ -76,7 +76,8 @@ typedef struct uml_stats {
   int32_t path;            /* 1 = TMA fp32 tile kernel, 2 = generic fp64 kernel, 3 = MLP CUDA-core kernel, 5 = MLP tensor-core
                               (wgmma) kernel, 4 = small-batch fp64 kernel of the online path, linear or MLP
                               (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph), 6 = float64
-                              decision_function scores kernel                                                             */
+                              decision_function scores kernel, 7 = float64 probabilities (the same kernel with the
+                              softmax / sigmoid epilogue: predict_proba, predict_log_proba)                               */
   int32_t x_elem_bytes;    /* predict calls on a resident batch: bytes per feature of the rows the scoring kernel read -
                               2 = the batch's compact fp16 copy (linear tile kernel), 4 = its fp32 rows; 0 otherwise    */
 } uml_stats;
@@ -205,6 +206,23 @@ UML_API int uml_linear_decision_function(uml_engine* e, const uml_model* m, cons
 UML_API int uml_linear_decision_function_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows,
                                               int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes,
                                               int src_dtype, double* scores_out, int64_t chunk_rows, uml_stats* stats);
+/* float64 class probabilities of a resident batch: LogisticRegression.predict_proba (sklearn/linear_model/_logistic.py),
+ * or predict_log_proba when log_proba != 0 (np.log of them), from the scores uml_linear_decision_function computes, read
+ * from the same rows (a lossy batch without its float64 copy is UML_ERR_UNSUPPORTED).  Softmax with scikit-learn's formula
+ * and order (extmath.softmax: max, exp(s - max), sum in class order, true division); a binary model gives the columns
+ * [1 - p, p] with p = 1 / (1 + exp(-s)) (scipy's expit).  proba_out: n_rows x n_classes row-major float64 (n_classes = 2
+ * for a binary model), host or device memory (8-byte aligned).  Every element is within the bound of DESIGN.md 3.9 of
+ * the exact value; a probability that rounds to 0 has log -inf, as in scikit-learn; finite features whose scores
+ * overflow give numpy's NaN / 0 / 1 pattern, NaN / Inf features give UML_ERR_NONFINITE.  Synchronous; stats
+ * (optional): path 7, kernel_ms, d2h_bytes. */
+UML_API int uml_linear_predict_proba_f64(uml_engine* e, const uml_model* m, const uml_batch* b, double* proba_out,
+                                         int proba_on_device, int log_proba, uml_stats* stats);
+/* the same from HOST rows of any layout and dtype uml_linear_predict_host takes, through the chunk pipeline of
+ * uml_linear_decision_function_host; batches of <= 64 rows take the pipeline too. */
+UML_API int uml_linear_predict_proba_f64_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows,
+                                              int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes,
+                                              int src_dtype, double* proba_out, int log_proba, int64_t chunk_rows,
+                                              uml_stats* stats);
 
 /* ---- 2-layer MLP predictor (tests/integration/pytorch_app/quickstart.py:14-24,68-70) -------------------------- */
 /* w1: hidden x in, b1: hidden, w2: out x hidden, b2: out (torch nn.Linear layout, fp32).  Labels = argmax of

@@ -92,4 +92,20 @@ for mm in (m, m16):
             assert eng.predict(mm, bb, exact=exact)[1]["x_elem_bytes"] == 2
         eng.predict_peers(mm, bb, [buf16.ptr], 1, exact=True, want_stats=True, label_bytes=1)
 del _os.environ["UML_B200_STAGES"]
+# float64 probabilities (the scores kernel's softmax / sigmoid epilogue): binary, C = 10 (one class group, in the strip),
+# C = 40 (grouped, normalised in global memory), F = 784 (W from global memory), host and resident, a device output
+# 8 bytes off 16-byte alignment
+mb = eng.load_linear(rng.standard_normal((1, 64)), rng.standard_normal(1))
+m40 = eng.load_linear(rng.standard_normal((40, 64)), rng.standard_normal(40))
+b64 = eng.stage(Xf[:3_001], keep_f64=True)
+for mm in (mb, m, m40):
+    for log in (False, True):
+        eng.predict_proba_f64(mm, b64, log=log)
+        eng.predict_proba_f64_host(mm, np.asfortranarray(Xf[:3_001]), log=log, chunk_rows=1024)
+        eng.predict_proba_f64_host(mm, X[:4_001].astype(np.uint8), log=log)
+for log in (False, True):
+    eng.predict_proba_f64(m784, eng.stage(X784, keep_f64=True), log=log)
+    eng.predict_proba_f64_host(m784, X784, log=log, chunk_rows=2048)
+pf = eng.device_alloc(8 * (10 * b64.n_rows + 2))
+eng.predict_proba_f64(m, b64, out_device_ptr=pf.ptr + 8, want_stats=True)
 print("sanitizer driver ok")

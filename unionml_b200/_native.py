@@ -102,6 +102,11 @@ SIGNATURES = {
         C.c_int,
         [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, _P, C.c_int64, C.POINTER(Stats)],
     ),
+    "uml_linear_predict_proba_f64": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.POINTER(Stats)]),
+    "uml_linear_predict_proba_f64_host": (
+        C.c_int,
+        [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, _P, C.c_int, C.c_int64, C.POINTER(Stats)],
+    ),
     "uml_mlp_load": (C.c_int, [_P, _PP, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int]),
     "uml_mlp_free": (None, [_P]),
     "uml_mlp_predict": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.POINTER(Stats)]),

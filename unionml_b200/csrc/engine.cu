@@ -191,10 +191,10 @@ struct uml_engine {
   Scratch<int32_t> d_flag_rows;
   Scratch<int32_t> d_labels;
   Scratch<float> d_proba;                // class probabilities bound for host memory (uml_mlp_predict_proba)
-  Scratch<double> d_scores;              // decision_function scores bound for host memory (uml_linear_decision_function)
+  Scratch<double> d_scores;              // float64 scores / probabilities bound for host memory (linear_f64_resident)
   Scratch<char, 3> d_chunk;              // raw source chunks (staging / predict_host)
   Scratch<float, 3> d_xchunk;            // converted fp32 chunks (predict_host)
-  Scratch<double, 3> d_vchunk;           // class values (predict_host_values) or scores (decision_function_host) of a chunk
+  Scratch<double, 3> d_vchunk;           // class values (predict_host_values) or float64 outputs (f64_out) of a chunk
   Scratch<double> d_classes;
   Scratch<double> d_targets;             // uml_topk_count_hits: targets and first-hit counters
   Scratch<unsigned long long> d_hits;
@@ -1198,6 +1198,9 @@ static int enqueue_mlp(uml_engine* e, const uml::MlpDeviceModel& m, const CUtens
   return UML_OK;
 }
 
+// uml_stats.path of the float64 scores kernel: 6 for decision_function scores, 7 for probabilities or their logs
+static int f64_path(int kind) { return kind == uml::kF64Scores ? 6 : 7; }
+
 static int finish_stats(uml_engine* e, uml_stats* stats, int64_t n_rows, int launches, int path, bool timed,
                         bool kernel_events = true) {
   // counters -> pinned mirror, then synchronise and report
@@ -1558,11 +1561,12 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
                              int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out,
                              double* values_out, const double* classes, int n_classes, int mode, int64_t chunk_rows,
                              uml_stats* stats, std::atomic<int64_t>* progress = nullptr, const uml_mlp* mlp = nullptr,
-                             double* scores_out = nullptr) {
-  // exactly one of m (linear classifier) and mlp (2-layer MLP) scores the chunks.  scores_out (linear only, instead of
-  // labels / values): the float64 decision_function scores, n_rows x linear_scores_width row-major
-  if (!e || (!m && !mlp) || (!host_ptr && n_rows > 0) || (!labels_out && !values_out && !scores_out && n_rows > 0) ||
-      n_rows < 0 || n_features < 1 || (scores_out && !m))
+                             double* f64_out = nullptr, int f64_kind = uml::kF64Scores) {
+  // exactly one of m (linear classifier) and mlp (2-layer MLP) scores the chunks.  f64_out (linear only, instead of
+  // labels / values): the float64 scores, probabilities or log-probabilities (f64_kind), n_rows x linear_f64_width
+  // row-major
+  if (!e || (!m && !mlp) || (!host_ptr && n_rows > 0) || (!labels_out && !values_out && !f64_out && n_rows > 0) ||
+      n_rows < 0 || n_features < 1 || (f64_out && !m))
     return UML_ERR_INVALID;
   if (values_out && (!classes || n_classes < 1)) return UML_ERR_INVALID;
   if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
@@ -1582,8 +1586,9 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   int rc = classify_layout(e, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, &L);
   if (rc != UML_OK) return rc;
   const int F = n_features;
-  // an MLP whose weights and strips do not fit one SM's shared memory keeps the chunk pipeline, and so do scores
-  if (n_rows <= kSmallRows && (int64_t)F * L.elem * n_rows <= kSmallBytes && (!mlp || mlp->small_smem > 0) && !scores_out) {
+  // an MLP whose weights and strips do not fit one SM's shared memory keeps the chunk pipeline, and so do the float64
+  // outputs
+  if (n_rows <= kSmallRows && (int64_t)F * L.elem * n_rows <= kSmallBytes && (!mlp || mlp->small_smem > 0) && !f64_out) {
     const int rows = (int)n_rows;
     const SmallLaunch launch = [&](const uml::SrcView& v, cudaStream_t s) {
       return mlp ? uml::launch_mlp_small(mlp->dm, v, rows, e->d_small, mlp->small_smem, s)
@@ -1599,9 +1604,9 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   const int64_t ld = (F + 3) / 4 * 4;
   const bool exact = mode == UML_PREDICT_EXACT;
   const int64_t row_bytes = (int64_t)F * L.elem;
-  const int n_scores = scores_out ? uml::linear_scores_width(m->dm) : 0;  // doubles per row of scores_out
+  const int n_f64 = f64_out ? uml::linear_f64_width(m->dm, f64_kind) : 0;  // doubles per row of f64_out
   if (chunk_rows <= 0)
-    chunk_rows = std::max<int64_t>(4096, (32ll << 20) / std::max<int64_t>({ld * 4, row_bytes, 8ll * n_scores}));
+    chunk_rows = std::max<int64_t>(4096, (32ll << 20) / std::max<int64_t>({ld * 4, row_bytes, 8ll * n_f64}));
   chunk_rows = std::min<int64_t>((chunk_rows + 127) / 128 * 128, (n_rows + 127) / 128 * 128);
   const bool direct = !L.feature_major && src_dtype == UML_F32 && L.pitch_elems == ld;
   // pageable sources of any size worth the trouble go through pinned bounce buffers filled by the copy pool
@@ -1612,7 +1617,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   // bytes of one row as it travels: `direct` rows keep their padding up to ld
   const int64_t wire_row_bytes = direct ? ld * 4 : row_bytes;
   if (bounce && (rc = grow_bounce(e, chunk_rows * wire_row_bytes)) != UML_OK) return rc;
-  if ((values_out || scores_out) && (rc = grow(e, e->d_vchunk, chunk_rows * std::max(1, n_scores))) != UML_OK) return rc;
+  if ((values_out || f64_out) && (rc = grow(e, e->d_vchunk, chunk_rows * std::max(1, n_f64))) != UML_OK) return rc;
   if (values_out && (rc = grow(e, e->d_classes, n_classes)) != UML_OK) return rc;
   if ((rc = grow(e, e->d_labels, 3 * chunk_rows)) != UML_OK) return rc;
   if (exact && (rc = grow(e, e->d_flag_rows, chunk_rows)) != UML_OK) return rc;
@@ -1622,9 +1627,9 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   // (the asynchronous variant always does: the flush is also where a finished prefix is published to the poller)
   const bool result_bounce = progress != nullptr || (labels_out && !host_ptr_is_pinned(labels_out)) ||
                              (values_out && !host_ptr_is_pinned(values_out)) ||
-                             (scores_out && !host_ptr_is_pinned(scores_out));
-  // a slot holds a chunk's values (8 B per row) and labels (4 B), or its scores (8 B per class)
-  if (result_bounce && (rc = grow(e, e->h_result, chunk_rows * (scores_out ? 8 * n_scores : 12))) != UML_OK) return rc;
+                             (f64_out && !host_ptr_is_pinned(f64_out));
+  // a slot holds a chunk's values (8 B per row) and labels (4 B), or its float64 outputs (8 B per column)
+  if (result_bounce && (rc = grow(e, e->h_result, chunk_rows * (f64_out ? 8 * n_f64 : 12))) != UML_OK) return rc;
   struct Pending {
     int64_t r0 = 0, rows = 0;
     bool live = false;
@@ -1635,7 +1640,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     if (fe != cudaSuccess) return fe;
     const char* base = e->h_result.p[sl];
     if (values_out) memcpy(values_out + pending[sl].r0, base, (size_t)pending[sl].rows * 8);
-    if (scores_out) memcpy(scores_out + pending[sl].r0 * n_scores, base, (size_t)pending[sl].rows * n_scores * 8);
+    if (f64_out) memcpy(f64_out + pending[sl].r0 * n_f64, base, (size_t)pending[sl].rows * n_f64 * 8);
     if (labels_out) memcpy(labels_out + pending[sl].r0, base + (size_t)chunk_rows * 8, (size_t)pending[sl].rows * 4);
     pending[sl].live = false;
     if (progress) progress->store(pending[sl].r0 + pending[sl].rows, std::memory_order_release);  // slots flush in row order
@@ -1747,15 +1752,15 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[slot], e->copy_stream));
     UML_CUDA_DRAIN(e, cudaStreamWaitEvent(cs, e->chunk_ev[slot], 0));
     if (tli >= 0) cudaEventRecord(tl[tli][2], cs);
-    // (2) transpose / down-cast (+ finiteness) on the compute stream; not for scores: their kernel reads the chunk as it
-    // arrived and checks finiteness itself
-    if (!direct && !scores_out) {
+    // (2) transpose / down-cast (+ finiteness) on the compute stream; not for the float64 outputs: their kernel reads the
+    // chunk as it arrived and checks finiteness itself
+    if (!direct && !f64_out) {
       NvtxRange r_stage("uml:stage_convert");
       UML_CUDA_DRAIN(e, uml::launch_stage_convert(raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major,
                                                   L.feature_major ? rows : F, rows, F, xc, ld, nullptr, 0, e->d_stage,
                                                   true, cs));
       launches += 1;
-    } else if (!exact && !scores_out) {
+    } else if (!exact && !f64_out) {
       UML_CUDA_DRAIN(e, uml::launch_finite_scan(xc, ld, rows, F, e->d_stage, cs));
       launches += 1;
     }
@@ -1765,20 +1770,20 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     l.ld = ld;
     l.n_rows = rows;
     l.targets.labels = e->d_labels.p[0] + (int64_t)slot * chunk_rows;
-    if (scores_out) {
-      // float64 scores from the chunk as it crossed PCIe: the caller's own values (a float64 chunk that travelled as
-      // fp32 was checked lossless by the gather threads)
+    if (f64_out) {
+      // float64 scores (or probabilities) from the chunk as it crossed PCIe: the caller's own values (a float64 chunk
+      // that travelled as fp32 was checked lossless by the gather threads)
       NvtxRange r_score("uml:scores_f64");
       uml::SrcView v{raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major ? 1 : F, L.feature_major ? rows : 1};
       if (direct) v = uml::SrcView{xc, UML_F32, ld, 1};
       const cudaError_t ce = uml::launch_linear_scores_f64(m->dm, v, rows, e->d_vchunk.p[slot], e->d_counters + uml::kCounterNonfinite,
-                                                           e->info.sm_count, cs);
+                                                           e->info.sm_count, cs, f64_kind);
       if (ce != cudaSuccess) {
         e->last_error = std::string("linear_scores_f64 launch: ") + cudaGetErrorString(ce);
         rc = UML_ERR_CUDA;
       }
       launches += 1;
-      path = 6;
+      path = f64_path(f64_kind);
     } else {
       CUtensorMap map;  // the MLP kernels' boxes, or the linear tile kernel's
       bool has_map = encode_map(e, &map, xc, rows, F, ld, mlp ? uml::kTileRows : linear_box_rows_for(F)) == UML_OK;
@@ -1806,11 +1811,11 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
       cudaStreamSynchronize(e->copy_stream);
       return rc;
     }
-    // (4) labels (or class values, or scores) back
+    // (4) labels (or class values, or the float64 outputs) back
     char* land = result_bounce ? e->h_result.p[slot] : nullptr;
-    if (scores_out) {
-      const size_t bytes = (size_t)rows * n_scores * 8;
-      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)land : (void*)(scores_out + r0 * n_scores), e->d_vchunk.p[slot],
+    if (f64_out) {
+      const size_t bytes = (size_t)rows * n_f64 * 8;
+      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)land : (void*)(f64_out + r0 * n_f64), e->d_vchunk.p[slot],
                                         bytes, cudaMemcpyDeviceToHost, cs));
       d2h += (int64_t)bytes;
     }
@@ -1980,12 +1985,13 @@ int uml_linear_predict_proba(uml_engine* e, const uml_model* m, const uml_batch*
   return UML_OK;
 }
 
-// float64 decision_function scores of a resident batch (sklearn/linear_model/_base.py:366-396) from the caller's own
-// values: the batch's float64 copy when it has one, else its fp32 rows, which are then the caller's values (lossless
-// staging, or rows wrapped in place).  Synchronous: the scores are written, and NaN / Inf reported, when it returns.
-int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_batch* b, double* scores_out,
-                                 int scores_on_device, uml_stats* stats) {
-  if (!e || !m || !b || (!scores_out && b->n_rows > 0)) return UML_ERR_INVALID;
+// float64 decision_function scores of a resident batch (sklearn/linear_model/_base.py:366-396), or their probabilities /
+// log-probabilities (kind), from the caller's own values: the batch's float64 copy when it has one, else its fp32 rows,
+// which are then the caller's values (lossless staging, or rows wrapped in place).  Synchronous: the output is written,
+// and NaN / Inf reported, when it returns.
+static int linear_f64_resident(uml_engine* e, const uml_model* m, const uml_batch* b, double* out, int on_device,
+                               int kind, uml_stats* stats) {
+  if (!e || !m || !b || (!out && b->n_rows > 0)) return UML_ERR_INVALID;
   if (b->n_features != m->n_features_in)
     UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the estimator is expecting %d features as input.",
              b->n_features, m->n_features_in);
@@ -1995,12 +2001,12 @@ int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_ba
   if (b->n_rows == 0) return UML_OK;
   if (!b->x64 && !b->lossless)
     UML_FAIL(e, UML_ERR_UNSUPPORTED, "the batch's fp32 rows are a lossy cast of the caller's values and it kept no "
-                                     "float64 copy: stage it with UML_STAGE_KEEP_F64 for its float64 scores");
-  NvtxRange r_all("uml:decision_function");
-  const int64_t n_doubles = b->n_rows * uml::linear_scores_width(m->dm);
-  double* d_out = scores_out;
+                                     "float64 copy: stage it with UML_STAGE_KEEP_F64 for its float64 %s",
+             kind == uml::kF64Scores ? "scores" : "probabilities");
+  const int64_t n_doubles = b->n_rows * uml::linear_f64_width(m->dm, kind);
+  double* d_out = out;
   int rc;
-  if (!scores_on_device) {
+  if (!on_device) {
     if ((rc = grow(e, e->d_scores, n_doubles)) != UML_OK) return rc;
     d_out = e->d_scores.p[0];
   }
@@ -2009,16 +2015,21 @@ int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_ba
   UML_CUDA(e, reset_counters(e, e->stream));
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
   const uml::SrcView src = b->x64 ? uml::SrcView{b->x64, UML_F64, b->ld64, 1} : uml::SrcView{b->x, UML_F32, b->ld, 1};
-  UML_CUDA(e, uml::launch_linear_scores_f64(m->dm, src, b->n_rows, d_out, e->d_counters + uml::kCounterNonfinite, e->info.sm_count, e->stream));
+  UML_CUDA(e, uml::launch_linear_scores_f64(m->dm, src, b->n_rows, d_out, e->d_counters + uml::kCounterNonfinite, e->info.sm_count, e->stream, kind));
   if (timed) {
     UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
     UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
   }
-  if (!scores_on_device)
-    UML_CUDA(e, cudaMemcpyAsync(scores_out, d_out, (size_t)n_doubles * 8, cudaMemcpyDeviceToHost, e->stream));
-  rc = finish_stats(e, stats, b->n_rows, 1, 6, timed);
-  if (stats) stats->d2h_bytes = scores_on_device ? 0 : n_doubles * 8;
+  if (!on_device) UML_CUDA(e, cudaMemcpyAsync(out, d_out, (size_t)n_doubles * 8, cudaMemcpyDeviceToHost, e->stream));
+  rc = finish_stats(e, stats, b->n_rows, 1, f64_path(kind), timed);
+  if (stats) stats->d2h_bytes = on_device ? 0 : n_doubles * 8;
   return rc;
+}
+
+int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_batch* b, double* scores_out,
+                                 int scores_on_device, uml_stats* stats) {
+  NvtxRange r_all("uml:decision_function");
+  return linear_f64_resident(e, m, b, scores_out, scores_on_device, uml::kF64Scores, stats);
 }
 
 // the same scores from HOST rows through the chunk pipeline of uml_linear_predict_host (any layout and dtype it takes)
@@ -2029,6 +2040,25 @@ int uml_linear_decision_function_host(uml_engine* e, const uml_model* m, const v
   NvtxRange r_all("uml:decision_function");
   return predict_host_impl(e, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, nullptr,
                            nullptr, nullptr, 0, UML_PREDICT_FAST, chunk_rows, stats, nullptr, nullptr, scores_out);
+}
+
+// float64 probabilities (LogisticRegression.predict_proba) or their logs (predict_log_proba) of a resident batch, from
+// the caller's own values as uml_linear_decision_function reads them
+int uml_linear_predict_proba_f64(uml_engine* e, const uml_model* m, const uml_batch* b, double* proba_out,
+                                 int proba_on_device, int log_proba, uml_stats* stats) {
+  NvtxRange r_all("uml:predict_proba_f64");
+  return linear_f64_resident(e, m, b, proba_out, proba_on_device, log_proba ? uml::kF64LogProba : uml::kF64Proba, stats);
+}
+
+// the same from HOST rows through the chunk pipeline of uml_linear_predict_host (any layout and dtype it takes)
+int uml_linear_predict_proba_f64_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows,
+                                      int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype,
+                                      double* proba_out, int log_proba, int64_t chunk_rows, uml_stats* stats) {
+  if (!e || !m || (!proba_out && n_rows > 0)) return UML_ERR_INVALID;
+  NvtxRange r_all("uml:predict_proba_f64");
+  return predict_host_impl(e, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, nullptr,
+                           nullptr, nullptr, 0, UML_PREDICT_FAST, chunk_rows, stats, nullptr, nullptr, proba_out,
+                           log_proba ? uml::kF64LogProba : uml::kF64Proba);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -15,6 +15,12 @@
 // go in groups of 2 * PAIRS <= 16 (register accumulators); a model with more classes re-reads the tile per group.
 // W sits in shared memory when it fits (WSMEM, zero padded to whole groups), else it is read from global memory.
 // The scores leave through a shared-memory strip in output order, as whole runs of consecutive doubles.
+//
+// KIND selects what leaves: the scores (kF64Scores), or scikit-learn's predict_proba (kF64Proba) or predict_log_proba
+// (kF64LogProba) of them, n_classes doubles per row ([1 - p, p] for a binary model).  proba_row turns a row's scores
+// into them in float64: on the thread's strip row before the store for a model of one class group (C <= 16, binary
+// included), and for a grouped model on the tile's rows in global memory, re-read by the block that wrote them after
+// the tile's last group (DESIGN.md 3.9).
 #include <algorithm>
 
 #include "uml_common.cuh"
@@ -37,8 +43,8 @@ struct ScoresParams {
   const double* w64;  // [F][S], feature-major, zero padded
   const double* b64;  // biases (then the bias magnitudes of the fp64 bound, unused here)
   int S, F, C;
-  int c_first;  // first class written: 1 for the binary layout [0, s], else 0
-  int n_out;    // doubles per output row: C - c_first
+  int c_first;  // 1 for the binary layout [0, s], else 0: the scores output starts at that class, probabilities take both
+  int n_out;    // doubles per output row: C - c_first for the scores, C for the probabilities
   int sp;       // WSMEM: doubles per feature of the shared-memory copy of W (C rounded up to whole groups)
   double* out;
   unsigned long long* nonfinite;  // rows with NaN / Inf features
@@ -78,7 +84,40 @@ __device__ __forceinline__ void load_chunk(const ScoresParams& p, long long row0
   }
 }
 
-template <int PAIRS, bool WSMEM>
+// a row's scores v[0, n) -> their probabilities or log-probabilities, in place, in float64 with scikit-learn's formula
+// and order: softmax of sklearn/utils/extmath.py (m = max, e_c = exp(s_c - m), S = sum of e_c in class order,
+// p_c = e_c / S), or for the binary layout v = [0, s] scipy's expit p = 1 / (1 + exp(-s)) and the columns [1 - p, p]
+// (LinearClassifierMixin._predict_proba_lr); the logs are np.log of those.  NaN propagates through the max as np.max
+// does, so scores that overflowed give numpy's NaN / 0 / 1 pattern.  Not inlined: both epilogues run one body (v is a
+// generic pointer, to shared or global memory), and the kernel around the call keeps the scores form's registers.
+template <int KIND>
+__device__ __noinline__ void proba_row(double* v, int n, bool binary) {
+  constexpr bool kLog = KIND == kF64LogProba;
+  if (binary) {
+    const double p = 1.0 / (1.0 + exp(-v[1]));
+    const double q = 1.0 - p;
+    v[0] = kLog ? log(q) : q;
+    v[1] = kLog ? log(p) : p;
+    return;
+  }
+  double m = v[0];
+  for (int c = 1; c < n; ++c) {
+    const double s = v[c];
+    if (s > m || isnan(s)) m = s;
+  }
+  double sum = 0.0;
+  for (int c = 0; c < n; ++c) {
+    const double e = exp(v[c] - m);
+    v[c] = e;
+    sum += e;
+  }
+  for (int c = 0; c < n; ++c) {
+    const double pc = v[c] / sum;
+    v[c] = kLog ? log(pc) : pc;
+  }
+}
+
+template <int PAIRS, bool WSMEM, int KIND = kF64Scores>
 __global__ void __launch_bounds__(kScoreRows, 3) linear_scores_f64_kernel(const ScoresParams p) {
   extern __shared__ __align__(16) double sc_smem[];
   double* xs = sc_smem;                          // [kScoreRows][kScoreLd]: the staged chunk, then the output strip
@@ -148,15 +187,20 @@ __global__ void __launch_bounds__(kScoreRows, 3) linear_scores_f64_kernel(const 
         const unsigned mask = __ballot_sync(0xffffffffu, bad && t < rows);
         if ((t & 31) == 0 && mask) atomicAdd(p.nonfinite, static_cast<unsigned long long>(__popc(mask)));
       }
-      // this group's output columns [j0, j0 + gc): classes max(c0, c_first) .. min(c0 + G, C) - 1
-      const int cb = max(c0, p.c_first), ce = min(c0 + G, p.C);
-      const int gc = ce - cb, j0 = cb - p.c_first;
+      // this group's output columns [j0, j0 + gc): classes max(c0, c_first) .. min(c0 + G, C) - 1 of the scores, every
+      // class of the probabilities
+      const int c_first = KIND == kF64Scores ? p.c_first : 0;
+      const int cb = max(c0, c_first), ce = min(c0 + G, p.C);
+      const int gc = ce - cb, j0 = cb - c_first;
       __syncthreads();  // xs is free: every thread has read its last chunk
       double* strip = xs;  // [rows][gc] in output order
 #pragma unroll
       for (int q = 0; q < G; ++q) {
         const int c = c0 + q;
         if (c >= cb && c < ce) strip[t * gc + (c - cb)] = acc[q] + p.b64[c];
+      }
+      if constexpr (KIND != kF64Scores) {
+        if (p.C <= G) proba_row<KIND>(strip + t * gc, gc, p.c_first != 0);  // one group: the whole row is in the strip
       }
       __syncthreads();
       // whole runs: one run of rows * n_out doubles when the group covers every output column, else one run of gc
@@ -172,12 +216,18 @@ __global__ void __launch_bounds__(kScoreRows, 3) linear_scores_f64_kernel(const 
         }
       }
     }
+    if constexpr (KIND != kF64Scores) {
+      if (p.C > G) {  // grouped: every group of the tile's rows is written; each thread normalises its own row
+        __syncthreads();  // makes the block's stores of the other threads visible
+        if (t < rows) proba_row<KIND>(p.out + (row0 + t) * p.n_out, p.C, false);
+      }
+    }
   }
 }
 
-template <int PAIRS, bool WSMEM>
+template <int PAIRS, bool WSMEM, int KIND>
 cudaError_t launch_scores(const ScoresParams& p, int sm_count, size_t smem, cudaStream_t stream) {
-  auto kern = linear_scores_f64_kernel<PAIRS, WSMEM>;
+  auto kern = linear_scores_f64_kernel<PAIRS, WSMEM, KIND>;
   static size_t configured = 0;  // per instantiation (one device per process): set the attribute once
   if (smem > configured) {
     const cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -191,24 +241,31 @@ cudaError_t launch_scores(const ScoresParams& p, int sm_count, size_t smem, cuda
   return cudaGetLastError();
 }
 
-template <bool WSMEM>
+template <bool WSMEM, int KIND>
 cudaError_t dispatch_pairs(int pairs, const ScoresParams& p, int sm_count, size_t smem, cudaStream_t stream) {
   switch (pairs) {
-    case 1: return launch_scores<1, WSMEM>(p, sm_count, smem, stream);
-    case 2: return launch_scores<2, WSMEM>(p, sm_count, smem, stream);
-    case 3: return launch_scores<3, WSMEM>(p, sm_count, smem, stream);
-    case 4: return launch_scores<4, WSMEM>(p, sm_count, smem, stream);
-    case 5: return launch_scores<5, WSMEM>(p, sm_count, smem, stream);
-    case 6: return launch_scores<6, WSMEM>(p, sm_count, smem, stream);
-    case 7: return launch_scores<7, WSMEM>(p, sm_count, smem, stream);
-    default: return launch_scores<8, WSMEM>(p, sm_count, smem, stream);
+    case 1: return launch_scores<1, WSMEM, KIND>(p, sm_count, smem, stream);
+    case 2: return launch_scores<2, WSMEM, KIND>(p, sm_count, smem, stream);
+    case 3: return launch_scores<3, WSMEM, KIND>(p, sm_count, smem, stream);
+    case 4: return launch_scores<4, WSMEM, KIND>(p, sm_count, smem, stream);
+    case 5: return launch_scores<5, WSMEM, KIND>(p, sm_count, smem, stream);
+    case 6: return launch_scores<6, WSMEM, KIND>(p, sm_count, smem, stream);
+    case 7: return launch_scores<7, WSMEM, KIND>(p, sm_count, smem, stream);
+    default: return launch_scores<8, WSMEM, KIND>(p, sm_count, smem, stream);
   }
+}
+
+template <int KIND>
+cudaError_t dispatch_smem(int pairs, const ScoresParams& p, int sm_count, size_t w_bytes, cudaStream_t stream) {
+  if (kTileBytes + w_bytes <= static_cast<size_t>(kMaxSmemBytes))
+    return dispatch_pairs<true, KIND>(pairs, p, sm_count, kTileBytes + w_bytes, stream);
+  return dispatch_pairs<false, KIND>(pairs, p, sm_count, kTileBytes, stream);
 }
 
 }  // namespace
 
 cudaError_t launch_linear_scores_f64(const LinearDeviceModel& m, const SrcView& src, int64_t n_rows, double* out,
-                                     unsigned long long* nonfinite, int sm_count, cudaStream_t stream) {
+                                     unsigned long long* nonfinite, int sm_count, cudaStream_t stream, int kind) {
   if (n_rows <= 0) return cudaSuccess;
   ScoresParams p{};
   p.src = src;
@@ -220,15 +277,17 @@ cudaError_t launch_linear_scores_f64(const LinearDeviceModel& m, const SrcView& 
   p.F = m.n_features;
   p.C = m.n_classes;
   p.c_first = m.binary ? 1 : 0;
-  p.n_out = linear_scores_width(m);
+  p.n_out = linear_f64_width(m, kind);
   p.out = out;
   p.nonfinite = nonfinite;
   const int pairs = std::min(kScoreGroup, m.n_classes + (m.n_classes & 1)) / 2;
   p.sp = (m.n_classes + 2 * pairs - 1) / (2 * pairs) * (2 * pairs);
   const size_t w_bytes = static_cast<size_t>(m.n_features) * p.sp * sizeof(double);
-  if (kTileBytes + w_bytes <= static_cast<size_t>(kMaxSmemBytes))
-    return dispatch_pairs<true>(pairs, p, sm_count, kTileBytes + w_bytes, stream);
-  return dispatch_pairs<false>(pairs, p, sm_count, kTileBytes, stream);
+  switch (kind) {
+    case kF64Proba: return dispatch_smem<kF64Proba>(pairs, p, sm_count, w_bytes, stream);
+    case kF64LogProba: return dispatch_smem<kF64LogProba>(pairs, p, sm_count, w_bytes, stream);
+    default: return dispatch_smem<kF64Scores>(pairs, p, sm_count, w_bytes, stream);
+  }
 }
 
 }  // namespace uml

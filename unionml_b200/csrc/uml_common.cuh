@@ -212,10 +212,16 @@ cudaError_t launch_linear_proba(const LinearDeviceModel& m, const float* x, int6
                                 int sm_count, cudaStream_t stream);
 // float64 decision_function scores (LinearClassifierMixin.decision_function, sklearn/linear_model/_base.py:366-396) of
 // every row of `src` (linear_scores.cu): out[n_rows][linear_scores_width(m)] row-major, one sequential fp64 FMA chain
-// per class plus the bias (DESIGN.md 3.7); rows with NaN / Inf features are counted into *nonfinite
+// per class plus the bias (DESIGN.md 3.7); rows with NaN / Inf features are counted into *nonfinite.  kind: the scores,
+// or scikit-learn's float64 predict_proba / predict_log_proba of them (DESIGN.md 3.9), out[n_rows][linear_f64_width]
+enum F64Output { kF64Scores = 0, kF64Proba = 1, kF64LogProba = 2 };
 inline int linear_scores_width(const LinearDeviceModel& m) { return m.binary ? 1 : m.n_classes; }
+inline int linear_f64_width(const LinearDeviceModel& m, int kind) {
+  return kind == kF64Scores ? linear_scores_width(m) : m.n_classes;  // (n_classes is 2 for the binary layout)
+}
 cudaError_t launch_linear_scores_f64(const LinearDeviceModel& m, const SrcView& src, int64_t n_rows, double* out,
-                                     unsigned long long* nonfinite, int sm_count, cudaStream_t stream);
+                                     unsigned long long* nonfinite, int sm_count, cudaStream_t stream,
+                                     int kind = kF64Scores);
 
 // 2-layer MLP (mlp_kernels.cu, mlp_tc_kernels.cu)
 struct MlpHostModel {  // the caller's fp32 weights, torch nn.Linear layout

@@ -672,6 +672,57 @@ class Engine:
             self._check(st)
         return out, stats.as_dict()
 
+    def predict_proba_f64(self, model: LinearModel, batch: Batch, log: bool = False,
+                          out_device_ptr: Optional[int] = None,
+                          want_stats: bool = False) -> Tuple[Optional[np.ndarray], Optional[dict]]:
+        """``predict_proba`` (``log``: ``predict_log_proba``) per row in float64, ``(n_rows, n_classes)``, ``[1 - p, p]``
+        for a binary model: scikit-learn's softmax / expit of the float64 scores :meth:`decision_function` computes from
+        the same rows (DESIGN.md §3.9).  With ``out_device_ptr`` (8-byte aligned) the output is written there and
+        ``None`` is returned."""
+        stats = N.Stats() if want_stats else None
+        with self._lock:
+            if out_device_ptr is not None:
+                st = N.lib().uml_linear_predict_proba_f64(
+                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, int(log), C.byref(stats) if stats else None
+                )
+                self._check(st)
+                return None, stats.as_dict() if stats else None
+            out = np.empty((batch.n_rows, model.n_classes), dtype=np.float64)
+            st = N.lib().uml_linear_predict_proba_f64(
+                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, int(log), C.byref(stats) if stats else None
+            )
+            self._check(st)
+        return out, stats.as_dict() if stats else None
+
+    def predict_proba_f64_host(self, model: LinearModel, features: Any, log: bool = False, chunk_rows: int = 0,
+                               out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, dict]:
+        """Host rows (any order, f32/f64/int) -> float64 probabilities (``log``: their logs) through the chunk pipeline
+        of :meth:`predict_host`, from the caller's own values; shapes as :meth:`predict_proba_f64`."""
+        arr = as_feature_array(features)
+        shape = (arr.shape[0], model.n_classes)
+        if out is None:
+            out = np.empty(shape, dtype=np.float64)
+        elif out.dtype != np.float64 or out.shape != shape or not out.flags.c_contiguous:
+            raise ValueError(f"out must be a C-contiguous float64 array of shape {shape}")
+        stats = N.Stats()
+        with self._lock:
+            st = N.lib().uml_linear_predict_proba_f64_host(
+                self._h,
+                model._h,
+                C.c_void_p(arr.ctypes.data),
+                arr.shape[0],
+                arr.shape[1],
+                arr.strides[0],
+                arr.strides[1],
+                _DTYPES[arr.dtype],
+                out.ctypes.data_as(C.c_void_p),
+                int(log),
+                chunk_rows,
+                C.byref(stats),
+            )
+            self._check(st)
+        return out, stats.as_dict()
+
 
 _default_engine: Optional[Engine] = None
 _default_lock = threading.Lock()

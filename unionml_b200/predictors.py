@@ -269,10 +269,22 @@ def linear_argmax(estimator: Any, features: Any) -> List[float]:
 _SMALL_ROWS = 64
 
 
-def linear_predict_proba(estimator: Any, features: Any) -> np.ndarray:
+def linear_predict_proba(estimator: Any, features: Any, *, dtype=np.float32) -> np.ndarray:
     """``estimator.predict_proba(features)`` on the GPU (``sklearn/linear_model/_logistic.py`` predict_proba: softmax of
-    the decision function, sigmoid columns ``[1 - p, p]`` for a binary model).  fp32 arithmetic: agrees with
-    scikit-learn's float64 probabilities to ~1e-6 absolute (the tests state the tolerance)."""
+    the decision function, sigmoid columns ``[1 - p, p]`` for a binary model).
+
+    ``dtype=np.float32`` (the default): fp32 arithmetic on the staged fp32 rows, agreeing with scikit-learn's float64
+    probabilities to ~1e-6 absolute (the tests state the tolerance).  ``dtype=np.float64``: scikit-learn's formula in
+    float64 on the float64 scores of the caller's own values, through the chunk pipeline (frames larger than HBM
+    included), within the bound of DESIGN.md §3.9.  Any other dtype raises ``ValueError``."""
+    try:
+        dt = None if dtype is None else np.dtype(dtype)  # (np.dtype(None) would be float64)
+    except TypeError:
+        dt = None
+    if dt == np.float64:
+        return _linear_proba_f64(estimator, features, log=False)
+    if dt != np.float32:
+        raise ValueError(f"linear_predict_proba computes float32 or float64 probabilities, not {dtype!r}")
     engine = get_engine()
     dm = device_model(estimator, engine)
     _check_feature_names(estimator, features)
@@ -299,6 +311,25 @@ def linear_decision_function(estimator: Any, features: Any) -> np.ndarray:
     scores, stats = engine.decision_function_host(dm, features)
     _note_ambiguous(stats)
     return scores
+
+
+def linear_predict_log_proba(estimator: Any, features: Any) -> np.ndarray:
+    """``estimator.predict_log_proba(features)`` on the GPU (``np.log(predict_proba)``, float64): the logs of
+    ``linear_predict_proba(estimator, features, dtype=np.float64)``, computed on the device; a probability that rounds to
+    0 gives ``-inf`` as in scikit-learn.  The guards of :func:`linear_argmax` apply."""
+    return _linear_proba_f64(estimator, features, log=True)
+
+
+def _linear_proba_f64(estimator: Any, features: Any, log: bool) -> np.ndarray:
+    """float64 probabilities (or their logs) of the caller's own values through the chunk pipeline, ``(n, n_classes)``
+    (``(n, 2)`` for a binary model), each within the bound of DESIGN.md §3.9 of the exact value."""
+    engine = get_engine()
+    dm = device_model(estimator, engine)
+    _check_feature_names(estimator, features)
+    _check_min_samples(features)
+    proba, stats = engine.predict_proba_f64_host(dm, features, log=log)
+    _note_ambiguous(stats)
+    return proba
 
 
 # ---------------------------------------------------------------------------------------------------------------
