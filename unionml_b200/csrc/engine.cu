@@ -189,17 +189,16 @@ struct uml_engine {
   unsigned long long* d_counters = nullptr;
   StageResult* d_stage = nullptr;
   Scratch<int32_t> d_flag_rows;
-  Scratch<int32_t> d_labels;
-  Scratch<float> d_proba;                // class probabilities bound for host memory (uml_mlp_predict_proba)
-  Scratch<double> d_scores;              // float64 scores / probabilities bound for host memory (linear_f64_resident)
+  Scratch<int32_t> d_labels;             // labels on their way to another output (peer scatter, class values)
+  Scratch<char> d_result;                // outputs of a resident-batch call bound for host memory (predict_resident)
   Scratch<char, 3> d_chunk;              // raw source chunks (staging / predict_host)
   Scratch<float, 3> d_xchunk;            // converted fp32 chunks (predict_host)
-  Scratch<double, 3> d_vchunk;           // class values (predict_host_values) or float64 outputs (f64_out) of a chunk
+  Scratch<char, 3> d_ochunk;             // the output of a chunk (predict_host)
   Scratch<double> d_classes;
   Scratch<double> d_targets;             // uml_topk_count_hits: targets and first-hit counters
   Scratch<unsigned long long> d_hits;
   Scratch<char, 3, true> h_bounce;       // pinned bounce buffers for pageable sources
-  Scratch<char, 3, true> h_result;       // pinned landing slots for labels / values bound for pageable outputs
+  Scratch<char, 3, true> h_result;       // pinned landing slots for chunk outputs bound for pageable memory
   CopyPool* pool = nullptr;
   // online path (B <= kSmallRows): pinned request buffer, its device twin, result slots, cached graphs
   void* h_req = nullptr;
@@ -438,11 +437,10 @@ void uml_engine_destroy(uml_engine* e) {
   cudaFree(e->d_stage);
   e->d_flag_rows.release();
   e->d_labels.release();
-  e->d_proba.release();
-  e->d_scores.release();
+  e->d_result.release();
   e->d_chunk.release();
   e->d_xchunk.release();
-  e->d_vchunk.release();
+  e->d_ochunk.release();
   e->d_classes.release();
   e->d_targets.release();
   e->d_hits.release();
@@ -1114,8 +1112,8 @@ void uml_batch_free(uml_batch* b) {
 // ---------------------------------------------------------------------------------------------------------------
 // predict
 // ---------------------------------------------------------------------------------------------------------------
-// enqueue the scoring of one resident block of rows on e->stream; no host synchronisation.
-// ev_k (optional) brackets the scoring kernel, ev_r the fp64 re-score.  half_map (optional): the rows' compact fp16
+// enqueue the scoring of one resident block of rows on e->stream; no host synchronisation.  timed: ev[2] ends the
+// scoring kernel (the caller brackets the step with ev[1] / ev[3]).  half_map (optional): the rows' compact fp16
 // copy, which the tile kernel then reads; *x_elem_bytes (optional) gets the bytes per feature it read (2 or 4).
 static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch& l, const CUtensorMap* map,
                            const CUtensorMap* half_map, int mode, bool timed, int* launches, int* path,
@@ -1124,7 +1122,6 @@ static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch
   const bool exact = mode == UML_PREDICT_EXACT;
   std::string why;
   const bool tma = map != nullptr && uml::linear_tma_supported(m->dm, &why);
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
   if (tma) {
     NvtxRange r_score("uml:score");
     std::string err;
@@ -1142,30 +1139,25 @@ static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch
       UML_CUDA(e, uml::launch_rescore_f64(m->dm, l, fl, false, e->info.sm_count, e->stream));
       *launches += 1;
     }
-    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
   } else {
     NvtxRange r_score("uml:score_f64_generic");
     UML_CUDA(e, uml::launch_rescore_f64(m->dm, l, fl, true, e->info.sm_count, e->stream));
     *launches += 1;
     *path = 2;
-    if (timed) {
-      UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
-      UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
-    }
+    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
   }
   return UML_OK;
 }
 
 // the MLP counterpart of enqueue_predict: the scoring kernel of `route` (mlp_route), the fp64 re-score of its flagged
 // rows when exact, and for the CUDA-core kernel with peers, the scatter of its labels.  `out` holds the row count and
-// where the labels go.  No host synchronisation; ev[1] / ev[2] bracket the scoring kernel, ev[2] / ev[3] the rest.
+// where the labels go.  No host synchronisation; timed: ev[2] ends the scoring kernel, as in enqueue_predict.
 static int enqueue_mlp(uml_engine* e, const uml::MlpDeviceModel& m, const CUtensorMap& map, const float* x, int64_t ld,
                        const uml::MlpTcLaunch& out, bool exact, int route, bool timed, int* launches, int* path) {
   const FlagList fl = flag_list(e);
   const int sm = e->info.sm_count;
   cudaStream_t s = e->stream;
   *path = route;
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], s));
   if (route == 2) {
     NvtxRange r_score("uml:mlp_score_f64_generic");
     UML_CUDA(e, uml::launch_mlp_rescore_f64(m, x, ld, out.n_rows, out, fl, true, sm, s));
@@ -1194,7 +1186,6 @@ static int enqueue_mlp(uml_engine* e, const uml::MlpDeviceModel& m, const CUtens
       *launches += 1;
     }
   }
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], s));
   return UML_OK;
 }
 
@@ -1229,63 +1220,93 @@ static int finish_stats(uml_engine* e, uml_stats* stats, int64_t n_rows, int lau
   return UML_OK;
 }
 
-// One predict call on a resident batch, linear or MLP.  `model` names the model in the feature-count message
-// ("estimator" as scikit-learn words it, "module" as the torch app does).  prepare() makes the model's host-side
-// choices before the first timed stream operation; score(labels, timed, &launches, &path, &x_elem_bytes) enqueues its
-// scoring step (x_elem_bytes: bytes per feature its kernel read, preset to 4).  labels: host-label scratch or the
-// caller's device vector; nullptr with peers, which each model's step serves.
+// the checks every predict call makes of its mode and of the rows' feature count.  `model` names the model as the
+// message does: "estimator" as scikit-learn words it, "module" as the torch app does.  A call without a mode passes FAST.
+static int check_mode_features(uml_engine* e, int mode, int n_features, int want, const char* model) {
+  if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
+  if (n_features != want)
+    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the %s is expecting %d features as input.", n_features, model,
+             want);
+  return UML_OK;
+}
+
+// What a predict call on a resident batch hands predict_resident besides its steps: its model's shape, its outputs
+// (out[1] is optional: top-k's probabilities) with their bytes per row, in host or device memory, its mode and stats.
+// always_sync: synchronous even with device outputs and no stats, so that NaN / Inf are reported on return.
+// n_peers / label_bytes: the labels' fused exchange (with peers, out[0] is NULL and each model's labels step serves them).
+struct ResidentCall {
+  int n_classes, n_features;
+  const char* model;
+  void* out[2];
+  int64_t row_bytes[2];
+  int on_device, mode;
+  uml_stats* stats;
+  bool always_sync = false;
+  int n_peers = 0, label_bytes = 4;
+};
+
+// One predict call on a resident batch: the checks, device setup, output scratch, events, counters, D2H and stats
+// that every such call shares.  prepare() makes the call's host-side checks and choices before the first timed stream
+// operation; score(out, timed, &launches, &path, &x_elem_bytes) enqueues its own step between ev[1] and ev[3], writing
+// output i to out[i] (the caller's device memory, or scratch bound for host memory) and recording ev[2] after its
+// scoring kernel when timed.  An asynchronous call (device outputs, no stats) returns once the step is enqueued.
 extern "C++" {  // a template cannot have the C linkage of the ABI section around it
 template <class Prepare, class Score>
-static int predict_resident(uml_engine* e, const uml_batch* b, int n_classes, int n_features, const char* model,
-                            int32_t* labels_out, int labels_on_device, int n_peers, int label_bytes, int mode,
-                            uml_stats* stats, Prepare&& prepare, Score&& score) {
+static int predict_resident(uml_engine* e, const uml_batch* b, const ResidentCall& c, Prepare&& prepare, Score&& score) {
   if (!e || !b) return UML_ERR_INVALID;
-  if (!labels_out && b->n_rows > 0 && n_peers == 0) return UML_ERR_INVALID;
-  if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
-  if (n_peers < 0 || n_peers > 8) UML_FAIL(e, UML_ERR_INVALID, "n_peers %d (max 8)", n_peers);
-  if (n_peers > 0 && label_bytes != 1 && label_bytes != 4) UML_FAIL(e, UML_ERR_INVALID, "label_bytes %d", label_bytes);
-  if (n_peers > 0 && label_bytes == 1 && n_classes > 256)
-    UML_FAIL(e, UML_ERR_UNSUPPORTED, "byte labels need n_classes <= 256 (model has %d)", n_classes);
-  if (b->n_features != n_features)
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the %s is expecting %d features as input.", b->n_features, model,
-             n_features);
+  if (!c.out[0] && b->n_rows > 0 && c.n_peers == 0) return UML_ERR_INVALID;
+  if (c.n_peers < 0 || c.n_peers > 8) UML_FAIL(e, UML_ERR_INVALID, "n_peers %d (max 8)", c.n_peers);
+  if (c.n_peers > 0 && c.label_bytes != 1 && c.label_bytes != 4)
+    UML_FAIL(e, UML_ERR_INVALID, "label_bytes %d", c.label_bytes);
+  if (c.n_peers > 0 && c.label_bytes == 1 && c.n_classes > 256)
+    UML_FAIL(e, UML_ERR_UNSUPPORTED, "byte labels need n_classes <= 256 (model has %d)", c.n_classes);
+  int rc;
+  if ((rc = check_mode_features(e, c.mode, b->n_features, c.n_features, c.model)) != UML_OK) return rc;
   UML_CUDA(e, cudaSetDevice(e->device));
   (void)cudaGetLastError();
+  uml_stats* stats = c.stats;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (b->n_rows == 0) return UML_OK;
   const bool timed = stats != nullptr;
-  const bool sync_call = stats || !labels_on_device;
-  int rc;
-  if (mode == UML_PREDICT_EXACT && (rc = grow(e, e->d_flag_rows, b->n_rows)) != UML_OK) return rc;
+  const bool sync_call = stats || !c.on_device || c.always_sync;
+  if (c.mode == UML_PREDICT_EXACT && (rc = grow(e, e->d_flag_rows, b->n_rows)) != UML_OK) return rc;
   if ((rc = prepare()) != UML_OK) return rc;
-  int32_t* d_labels = labels_out;
-  if (!labels_on_device) {
-    if ((rc = grow(e, e->d_labels, b->n_rows)) != UML_OK) return rc;
-    d_labels = e->d_labels.p[0];
+  void* out[2] = {c.out[0], c.out[1]};
+  int64_t d2h = 0;
+  if (!c.on_device) {  // back to back in scratch
+    for (int i = 0; i < 2; ++i) d2h += c.out[i] ? b->n_rows * c.row_bytes[i] : 0;
+    if ((rc = grow(e, e->d_result, d2h)) != UML_OK) return rc;
+    out[0] = e->d_result.p[0];
+    if (c.out[1]) out[1] = e->d_result.p[0] + b->n_rows * c.row_bytes[0];
   }
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
-  // The asynchronous step (device labels, no stats) needs no memset at all: the flag list is handed back empty by the
-  // previous re-score kernel.
+  // The asynchronous step needs no memset at all: the flag list is handed back empty by the previous re-score kernel.
   if (sync_call) UML_CUDA(e, reset_counters(e, e->stream));
-  int launches = 0, path = 0, elem_bytes = 4;
-  if ((rc = score(d_labels, timed, &launches, &path, &elem_bytes)) != UML_OK) return rc;
+  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
+  int launches = 0, path = 0, x_elem_bytes = 0;
+  if ((rc = score(out, timed, &launches, &path, &x_elem_bytes)) != UML_OK) return rc;
+  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
   if (!sync_call) return UML_OK;
-  if (!labels_on_device)
-    UML_CUDA(e, cudaMemcpyAsync(labels_out, d_labels, (size_t)b->n_rows * 4, cudaMemcpyDeviceToHost, e->stream));
+  for (int i = 0; i < 2; ++i)
+    if (!c.on_device && c.out[i])
+      UML_CUDA(e, cudaMemcpyAsync(c.out[i], out[i], (size_t)(b->n_rows * c.row_bytes[i]), cudaMemcpyDeviceToHost,
+                                  e->stream));
   rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
   if (stats) {
-    stats->d2h_bytes = labels_on_device ? 0 : b->n_rows * 4;
-    stats->x_elem_bytes = elem_bytes;
+    stats->d2h_bytes = d2h;
+    stats->x_elem_bytes = x_elem_bytes;
   }
   return rc;
 }
 }  // extern "C++"
 
+static int no_prepare() { return UML_OK; }
+
 static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_batch* b, int32_t* labels_out,
                                    int labels_on_device, void* const* peers, int n_peers, int64_t row_offset,
                                    int label_bytes, int mode, uml_stats* stats) {
   if (!m) return UML_ERR_INVALID;
-  auto score = [&](int32_t* labels, bool timed, int* launches, int* path, int* elem_bytes) {
+  auto score = [&](void* const* out, bool timed, int* launches, int* path, int* elem_bytes) {
     LinearLaunch l{};
     l.x = b->x;
     l.x64 = b->x64;
@@ -1293,7 +1314,7 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
     l.ld64 = b->ld64;
     l.n_rows = b->n_rows;
     uml::LabelTargets& t = l.targets;
-    t.labels = labels;
+    t.labels = static_cast<int32_t*>(out[0]);
     t.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
     t.row_offset = row_offset;
     // fused int32 exchange: entry 0 is this rank's own full-length vector, the local label target.  Byte vectors are
@@ -1303,11 +1324,15 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
     t.n_peers = n_peers - own;
     for (int i = 0; i < t.n_peers; ++i) t.peers[i] = peers[own + i];
     const CUtensorMap* half = b->has_half && compact_rows_enabled() ? &b->half_map : nullptr;
+    *elem_bytes = 4;
     return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, half, mode, timed, launches, path, elem_bytes,
                            b->half_nonneg);
   };
-  return predict_resident(e, b, m->dm.n_classes, m->n_features_in, "estimator", labels_out, labels_on_device, n_peers,
-                          label_bytes, mode, stats, [] { return (int)UML_OK; }, score);
+  ResidentCall c{m->dm.n_classes, m->n_features_in, "estimator", {labels_out, nullptr}, {4, 0}, labels_on_device, mode,
+                 stats};
+  c.n_peers = n_peers;
+  c.label_bytes = label_bytes;
+  return predict_resident(e, b, c, no_prepare, score);
 }
 
 int uml_linear_predict(uml_engine* e, const uml_model* m, const uml_batch* b, int32_t* labels_out,
@@ -1330,28 +1355,18 @@ int uml_labels_take(uml_engine* e, const void* labels_dev, int label_bytes, int6
   if (label_bytes != 1 && label_bytes != 4) UML_FAIL(e, UML_ERR_INVALID, "label_bytes %d", label_bytes);
   UML_CUDA(e, cudaSetDevice(e->device));
   if (n == 0) return UML_OK;
-  double* d_classes = nullptr;
-  double* d_out = nullptr;
-  UML_CUDA(e, cudaMalloc((void**)&d_classes, (size_t)n_classes * 8));
-  cudaError_t ce = cudaMalloc((void**)&d_out, (size_t)n * 8);
-  if (ce != cudaSuccess) {
-    cudaFree(d_classes);
-    UML_FAIL(e, UML_ERR_NOMEM, "uml_labels_take: %s", cudaGetErrorString(ce));
-  }
-  auto done = [&](int rc) {
-    cudaStreamSynchronize(e->stream);
-    cudaFree(d_classes);
-    cudaFree(d_out);
-    return rc;
-  };
-  if ((ce = cudaMemcpyAsync(d_classes, classes_host, (size_t)n_classes * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
-      (ce = uml::launch_labels_take(labels_dev, label_bytes, n, d_classes, n_classes, d_out, e->stream)) != cudaSuccess ||
+  int rc;
+  if ((rc = grow(e, e->d_classes, n_classes)) != UML_OK || (rc = grow(e, e->d_result, n * 8)) != UML_OK) return rc;
+  double* d_out = reinterpret_cast<double*>(e->d_result.p[0]);
+  cudaError_t ce;
+  if ((ce = cudaMemcpyAsync(e->d_classes.p[0], classes_host, (size_t)n_classes * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
+      (ce = uml::launch_labels_take(labels_dev, label_bytes, n, e->d_classes.p[0], n_classes, d_out, e->stream)) != cudaSuccess ||
       (ce = cudaMemcpyAsync(out_host, d_out, (size_t)n * 8, cudaMemcpyDeviceToHost, e->stream)) != cudaSuccess ||
       (ce = cudaStreamSynchronize(e->stream)) != cudaSuccess) {
-    e->last_error = std::string("uml_labels_take: ") + cudaGetErrorString(ce);
-    return done(UML_ERR_CUDA);
+    cudaStreamSynchronize(e->stream);
+    UML_FAIL(e, UML_ERR_CUDA, "uml_labels_take: %s", cudaGetErrorString(ce));
   }
-  return done(UML_OK);
+  return UML_OK;
 }
 
 // number of rows whose predicted class value equals the target (the numerator of accuracy_score in the reference's
@@ -1364,31 +1379,21 @@ int uml_labels_count_equal(uml_engine* e, const void* labels_dev, int label_byte
   UML_CUDA(e, cudaSetDevice(e->device));
   *count_out = 0;
   if (n == 0) return UML_OK;
-  double* d_classes = nullptr;
-  double* d_targets = nullptr;
-  UML_CUDA(e, cudaMalloc((void**)&d_classes, (size_t)n_classes * 8));
-  cudaError_t ce = cudaMalloc((void**)&d_targets, (size_t)n * 8);
-  if (ce != cudaSuccess) {
-    cudaFree(d_classes);
-    UML_FAIL(e, UML_ERR_NOMEM, "uml_labels_count_equal: %s", cudaGetErrorString(ce));
-  }
-  auto done = [&](int rc) {
-    cudaStreamSynchronize(e->stream);
-    cudaFree(d_classes);
-    cudaFree(d_targets);
-    return rc;
-  };
-  if ((ce = cudaMemcpyAsync(d_classes, classes_host, (size_t)n_classes * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
-      (ce = cudaMemcpyAsync(d_targets, targets_host, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
+  int rc;
+  if ((rc = grow(e, e->d_classes, n_classes)) != UML_OK || (rc = grow(e, e->d_targets, n)) != UML_OK) return rc;
+  cudaError_t ce;
+  if ((ce = cudaMemcpyAsync(e->d_classes.p[0], classes_host, (size_t)n_classes * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
+      (ce = cudaMemcpyAsync(e->d_targets.p[0], targets_host, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess ||
       (ce = cudaMemsetAsync(e->d_counters, 0, sizeof(e->h->counters), e->stream)) != cudaSuccess ||
-      (ce = uml::launch_labels_count_equal(labels_dev, label_bytes, n, d_classes, n_classes, d_targets, e->d_counters, e->stream)) != cudaSuccess ||
+      (ce = uml::launch_labels_count_equal(labels_dev, label_bytes, n, e->d_classes.p[0], n_classes, e->d_targets.p[0],
+                                           e->d_counters, e->stream)) != cudaSuccess ||
       (ce = cudaMemcpyAsync(e->h->counters, e->d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream)) != cudaSuccess ||
       (ce = cudaStreamSynchronize(e->stream)) != cudaSuccess) {
-    e->last_error = std::string("uml_labels_count_equal: ") + cudaGetErrorString(ce);
-    return done(UML_ERR_CUDA);
+    cudaStreamSynchronize(e->stream);
+    UML_FAIL(e, UML_ERR_CUDA, "uml_labels_count_equal: %s", cudaGetErrorString(ce));
   }
   *count_out = (int64_t)e->h->counters[0];
-  return done(UML_OK);
+  return UML_OK;
 }
 
 // top-k hit counts of the quickdraw template's accuracy(output, target, topk) (quickdraw/model.py:20-27):
@@ -1454,11 +1459,12 @@ static bool host_sample_is_tf32(const void* host, const SrcLayout& L, int64_t n_
 // B <= kSmallRows: request block -> pinned (device-mapped) buffer -> one small-batch kernel (replayed as a CUDA graph)
 // -> labels written straight into pinned host memory.  The kernel scores in fp64 (linear_small_kernel from the
 // caller's own values, mlp_small_kernel from their fp32 cast), so the result is the exact-mode result for either mode.
-// `launch(view, stream)` enqueues that kernel on the request block; model_uid keys its cached graphs.
-using SmallLaunch = std::function<cudaError_t(const uml::SrcView&, cudaStream_t)>;
+// `launch(view, rows, stream)` enqueues that kernel on the request block; model_uid keys its cached graphs.  out: the
+// int32 labels, or with classes, classes[label] as float64.
+using SmallLaunch = std::function<cudaError_t(const uml::SrcView&, int, cudaStream_t)>;
 static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaunch& launch, const void* host_ptr,
-                              int n_rows, int F, const SrcLayout& L, int src_dtype, int32_t* labels_out,
-                              double* values_out, const double* classes, int n_classes, uml_stats* stats) {
+                              int n_rows, int F, const SrcLayout& L, int src_dtype, void* out, const double* classes,
+                              int n_classes, uml_stats* stats) {
   NvtxRange r_all("uml:predict_host_small");
   const size_t width = (size_t)F * L.elem;
   const size_t bytes = width * (size_t)n_rows;
@@ -1495,7 +1501,7 @@ static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaun
     }
   }
   uml::SrcView view{e->d_req, src_dtype, (long long)F, 1};
-  auto enqueue = [&](cudaStream_t s) -> cudaError_t { return launch(view, s); };
+  auto enqueue = [&](cudaStream_t s) -> cudaError_t { return launch(view, n_rows, s); };
   static const bool no_graph = getenv("UML_B200_NO_GRAPH") != nullptr;
   bool launched = false;
   if (e->small_graph_ok && !no_graph) {
@@ -1539,8 +1545,8 @@ static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaun
   int64_t n_bad = 0, n_amb = 0;
   for (int r = 0; r < n_rows; ++r) {
     const uml::SmallResult& q = e->h->small[r];
-    if (labels_out) labels_out[r] = q.label;
-    if (values_out) values_out[r] = (q.label >= 0 && q.label < n_classes) ? classes[q.label] : NAN;
+    if (classes) static_cast<double*>(out)[r] = (q.label >= 0 && q.label < n_classes) ? classes[q.label] : NAN;
+    else static_cast<int32_t*>(out)[r] = q.label;
     n_bad += q.status & 1;
     n_amb += (q.status >> 1) & 1;
   }
@@ -1557,45 +1563,50 @@ static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaun
   return UML_OK;
 }
 
-static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows, int n_features,
-                             int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out,
-                             double* values_out, const double* classes, int n_classes, int mode, int64_t chunk_rows,
-                             uml_stats* stats, std::atomic<int64_t>* progress = nullptr, const uml_mlp* mlp = nullptr,
-                             double* f64_out = nullptr, int f64_kind = uml::kF64Scores) {
-  // exactly one of m (linear classifier) and mlp (2-layer MLP) scores the chunks.  f64_out (linear only, instead of
-  // labels / values): the float64 scores, probabilities or log-probabilities (f64_kind), n_rows x linear_f64_width
-  // row-major
-  if (!e || (!m && !mlp) || (!host_ptr && n_rows > 0) || (!labels_out && !values_out && !f64_out && n_rows > 0) ||
-      n_rows < 0 || n_features < 1 || (f64_out && !m))
-    return UML_ERR_INVALID;
-  if (values_out && (!classes || n_classes < 1)) return UML_ERR_INVALID;
-  if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
-  if (mlp) {
-    if (n_features != mlp->dm.n_in)
-      UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the module is expecting %d features as input.", n_features,
-               mlp->dm.n_in);
-  } else if (n_features != m->n_features_in) {
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the estimator is expecting %d features as input.", n_features,
-             m->n_features_in);
-  }
+// One chunk of host rows as the pipeline hands it to a score step
+struct Chunk {
+  float* x;          // the fp32 rows (staged and checked, unless the step reads the raw chunk)
+  int64_t ld, rows;
+  uml::SrcView src;  // the caller's own values as they crossed PCIe (a float64 chunk that travelled as fp32 was checked
+                     // lossless by the gather threads); rows already in the resident layout: x itself
+  std::function<bool()> tf32;  // a host-side guess at whether the rows are tf32 values (MLP kernel choice)
+};
+
+// What a call through the chunk pipeline computes: score(chunk, out, &launches, &path) enqueues it on e->stream and
+// writes chunk.rows x row_bytes to the device buffer `out`.  n_features / model: as for check_mode_features.
+struct ChunkStep {
+  int n_features;
+  const char* model;
+  int64_t row_bytes;
+  bool raw;  // reads chunk.src only: no staging kernel or finite scan (the float64 outputs check finiteness themselves)
+  std::function<int(const Chunk&, void*, int*, int*)> score;
+  std::function<int(int64_t)> prepare;  // optional, given chunk_rows once the pipeline's scratch exists
+  // the <= kSmallRows route, none without a kernel: the model uid that keys its graphs, and the classes it writes
+  // as float64 in place of the label (class values)
+  SmallLaunch small;
+  uint64_t small_uid = 0;
+  const double* classes = nullptr;
+  int n_classes = 0;
+};
+
+// host rows -> `out` (host memory, n_rows x step.row_bytes) in chunks: gather / H2D on the copy stream, staging, the
+// step and the D2H on e->stream, three chunks in flight.  progress: the asynchronous call's published row count
+static int predict_host_impl(uml_engine* e, const ChunkStep& step, const void* host_ptr, int64_t n_rows, int n_features,
+                             int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, void* out, int mode,
+                             int64_t chunk_rows, uml_stats* stats, std::atomic<int64_t>* progress = nullptr) {
+  if (!e || (!host_ptr && n_rows > 0) || (!out && n_rows > 0) || n_rows < 0 || n_features < 1) return UML_ERR_INVALID;
+  int rc;
+  if ((rc = check_mode_features(e, mode, n_features, step.n_features, step.model)) != UML_OK) return rc;
   UML_CUDA(e, cudaSetDevice(e->device));
   (void)cudaGetLastError();
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n_rows == 0) return UML_OK;
   SrcLayout L{};
-  int rc = classify_layout(e, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, &L);
-  if (rc != UML_OK) return rc;
+  if ((rc = classify_layout(e, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, &L)) != UML_OK) return rc;
   const int F = n_features;
-  // an MLP whose weights and strips do not fit one SM's shared memory keeps the chunk pipeline, and so do the float64
-  // outputs
-  if (n_rows <= kSmallRows && (int64_t)F * L.elem * n_rows <= kSmallBytes && (!mlp || mlp->small_smem > 0) && !f64_out) {
-    const int rows = (int)n_rows;
-    const SmallLaunch launch = [&](const uml::SrcView& v, cudaStream_t s) {
-      return mlp ? uml::launch_mlp_small(mlp->dm, v, rows, e->d_small, mlp->small_smem, s)
-                 : uml::launch_linear_small(m->dm, v, rows, e->d_small, s);
-    };
-    rc = predict_host_small(e, mlp ? mlp->uid : m->uid, launch, host_ptr, rows, F, L, src_dtype, labels_out, values_out,
-                            classes, n_classes, stats);
+  if (step.small && n_rows <= kSmallRows && (int64_t)F * L.elem * n_rows <= kSmallBytes) {
+    rc = predict_host_small(e, step.small_uid, step.small, host_ptr, (int)n_rows, F, L, src_dtype, out, step.classes,
+                            step.n_classes, stats);
     if (progress && rc == UML_OK) progress->store(n_rows);
     return rc;
   }
@@ -1604,9 +1615,9 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   const int64_t ld = (F + 3) / 4 * 4;
   const bool exact = mode == UML_PREDICT_EXACT;
   const int64_t row_bytes = (int64_t)F * L.elem;
-  const int n_f64 = f64_out ? uml::linear_f64_width(m->dm, f64_kind) : 0;  // doubles per row of f64_out
+  const int64_t out_bytes = step.row_bytes;
   if (chunk_rows <= 0)
-    chunk_rows = std::max<int64_t>(4096, (32ll << 20) / std::max<int64_t>({ld * 4, row_bytes, 8ll * n_f64}));
+    chunk_rows = std::max<int64_t>(4096, (32ll << 20) / std::max<int64_t>({ld * 4, row_bytes, out_bytes}));
   chunk_rows = std::min<int64_t>((chunk_rows + 127) / 128 * 128, (n_rows + 127) / 128 * 128);
   const bool direct = !L.feature_major && src_dtype == UML_F32 && L.pitch_elems == ld;
   // pageable sources of any size worth the trouble go through pinned bounce buffers filled by the copy pool
@@ -1617,19 +1628,14 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   // bytes of one row as it travels: `direct` rows keep their padding up to ld
   const int64_t wire_row_bytes = direct ? ld * 4 : row_bytes;
   if (bounce && (rc = grow_bounce(e, chunk_rows * wire_row_bytes)) != UML_OK) return rc;
-  if ((values_out || f64_out) && (rc = grow(e, e->d_vchunk, chunk_rows * std::max(1, n_f64))) != UML_OK) return rc;
-  if (values_out && (rc = grow(e, e->d_classes, n_classes)) != UML_OK) return rc;
-  if ((rc = grow(e, e->d_labels, 3 * chunk_rows)) != UML_OK) return rc;
+  if ((rc = grow(e, e->d_ochunk, chunk_rows * out_bytes)) != UML_OK) return rc;
   if (exact && (rc = grow(e, e->d_flag_rows, chunk_rows)) != UML_OK) return rc;
   // A device-to-host copy into PAGEABLE memory blocks the calling thread until the chunk's whole pipeline has drained,
   // which would serialise gather / H2D / scoring.  Pageable outputs therefore land in pinned slots first and are
   // copied out by the host when the slot comes round again (three chunks later) or at the end.
   // (the asynchronous variant always does: the flush is also where a finished prefix is published to the poller)
-  const bool result_bounce = progress != nullptr || (labels_out && !host_ptr_is_pinned(labels_out)) ||
-                             (values_out && !host_ptr_is_pinned(values_out)) ||
-                             (f64_out && !host_ptr_is_pinned(f64_out));
-  // a slot holds a chunk's values (8 B per row) and labels (4 B), or its float64 outputs (8 B per column)
-  if (result_bounce && (rc = grow(e, e->h_result, chunk_rows * (f64_out ? 8 * n_f64 : 12))) != UML_OK) return rc;
+  const bool result_bounce = progress != nullptr || !host_ptr_is_pinned(out);
+  if (result_bounce && (rc = grow(e, e->h_result, chunk_rows * out_bytes)) != UML_OK) return rc;
   struct Pending {
     int64_t r0 = 0, rows = 0;
     bool live = false;
@@ -1638,10 +1644,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     if (!pending[sl].live) return cudaSuccess;
     cudaError_t fe = cudaEventSynchronize(e->chunk_ev[3 + sl]);  // recorded after the slot's D2H copies
     if (fe != cudaSuccess) return fe;
-    const char* base = e->h_result.p[sl];
-    if (values_out) memcpy(values_out + pending[sl].r0, base, (size_t)pending[sl].rows * 8);
-    if (f64_out) memcpy(f64_out + pending[sl].r0 * n_f64, base, (size_t)pending[sl].rows * n_f64 * 8);
-    if (labels_out) memcpy(labels_out + pending[sl].r0, base + (size_t)chunk_rows * 8, (size_t)pending[sl].rows * 4);
+    memcpy(static_cast<char*>(out) + pending[sl].r0 * out_bytes, e->h_result.p[sl], (size_t)(pending[sl].rows * out_bytes));
     pending[sl].live = false;
     if (progress) progress->store(pending[sl].r0 + pending[sl].rows, std::memory_order_release);  // slots flush in row order
     return cudaSuccess;
@@ -1650,7 +1653,9 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   // MLP: the tensor cores' tf32 question is answered by a host-side sample of the first rows (rows that are not tf32
   // values are caught in the kernel and re-scored, so a wrong guess costs time, never labels); taken once
   int sample_tf32 = -1;
-  auto tf32 = [&] {
+  Chunk c{};
+  c.ld = ld;
+  c.tf32 = [&] {
     if (sample_tf32 < 0) sample_tf32 = host_sample_is_tf32(host_ptr, L, n_rows, F, src_dtype) ? 1 : 0;
     return sample_tf32 == 1;
   };
@@ -1660,8 +1665,7 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   if (timed) UML_CUDA_DRAIN(e, cudaEventRecord(e->ev[0], cs));
   UML_CUDA_DRAIN(e, reset_counters(e, cs));
   UML_CUDA_DRAIN(e, cudaMemsetAsync(e->d_stage, 0, sizeof(StageResult), cs));
-  if (values_out)
-    UML_CUDA_DRAIN(e, cudaMemcpyAsync(e->d_classes.p[0], classes, (size_t)n_classes * 8, cudaMemcpyHostToDevice, cs));
+  if (step.prepare && (rc = step.prepare(chunk_rows)) != UML_OK) return rc;
   UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[6], cs));
   UML_CUDA_DRAIN(e, cudaStreamWaitEvent(e->copy_stream, e->chunk_ev[6], 0));
   int launches = 0, path = 0;
@@ -1752,86 +1756,33 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
     UML_CUDA_DRAIN(e, cudaEventRecord(e->chunk_ev[slot], e->copy_stream));
     UML_CUDA_DRAIN(e, cudaStreamWaitEvent(cs, e->chunk_ev[slot], 0));
     if (tli >= 0) cudaEventRecord(tl[tli][2], cs);
-    // (2) transpose / down-cast (+ finiteness) on the compute stream; not for the float64 outputs: their kernel reads the
-    // chunk as it arrived and checks finiteness itself
-    if (!direct && !f64_out) {
+    // (2) transpose / down-cast (+ finiteness) on the compute stream; not for a step that reads the chunk as it arrived
+    if (!direct && !step.raw) {
       NvtxRange r_stage("uml:stage_convert");
       UML_CUDA_DRAIN(e, uml::launch_stage_convert(raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major,
                                                   L.feature_major ? rows : F, rows, F, xc, ld, nullptr, 0, e->d_stage,
                                                   true, cs));
       launches += 1;
-    } else if (!exact && !f64_out) {
+    } else if (!exact && !step.raw) {
       UML_CUDA_DRAIN(e, uml::launch_finite_scan(xc, ld, rows, F, e->d_stage, cs));
       launches += 1;
     }
     // (3) score
-    LinearLaunch l{};
-    l.x = xc;
-    l.ld = ld;
-    l.n_rows = rows;
-    l.targets.labels = e->d_labels.p[0] + (int64_t)slot * chunk_rows;
-    if (f64_out) {
-      // float64 scores (or probabilities) from the chunk as it crossed PCIe: the caller's own values (a float64 chunk
-      // that travelled as fp32 was checked lossless by the gather threads)
-      NvtxRange r_score("uml:scores_f64");
-      uml::SrcView v{raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major ? 1 : F, L.feature_major ? rows : 1};
-      if (direct) v = uml::SrcView{xc, UML_F32, ld, 1};
-      const cudaError_t ce = uml::launch_linear_scores_f64(m->dm, v, rows, e->d_vchunk.p[slot], e->d_counters + uml::kCounterNonfinite,
-                                                           e->info.sm_count, cs, f64_kind);
-      if (ce != cudaSuccess) {
-        e->last_error = std::string("linear_scores_f64 launch: ") + cudaGetErrorString(ce);
-        rc = UML_ERR_CUDA;
-      }
-      launches += 1;
-      path = f64_path(f64_kind);
-    } else {
-      CUtensorMap map;  // the MLP kernels' boxes, or the linear tile kernel's
-      bool has_map = encode_map(e, &map, xc, rows, F, ld, mlp ? uml::kTileRows : linear_box_rows_for(F)) == UML_OK;
-      if (!mlp && exact && !direct && !chunk_narrow && lossy_capable(src_dtype)) {  // (the reference MLP predictor casts
-        // to float32; a chunk that travelled as fp32 was checked lossless on the host: its fp32 rows ARE the caller's
-        // values) flagged rows are re-scored from the caller's own values (the raw chunk is still resident): float64 /
-        // int features that do not survive the fp32 down-cast still get sklearn's float64 labels (_base.py:366-396)
-        l.src.base = raw;
-        l.src.dtype = src_dtype;
-        l.src.row_stride = L.feature_major ? 1 : F;
-        l.src.col_stride = L.feature_major ? rows : 1;
-      }
-      if (mlp) {
-        uml::MlpTcLaunch out{};
-        out.n_rows = rows;
-        out.targets.labels = l.targets.labels;
-        rc = enqueue_mlp(e, mlp->dm, map, xc, ld, out, exact, mlp_route(mlp->dm, has_map, false, tf32), false, &launches,
-                         &path);
-      } else {
-        rc = enqueue_predict(e, m, l, has_map ? &map : nullptr, nullptr, mode, false, &launches, &path);
-      }
-    }
-    if (rc != UML_OK) {
+    c.x = xc;
+    c.rows = rows;
+    c.src = direct ? uml::SrcView{xc, UML_F32, ld, 1}
+                   : uml::SrcView{raw, chunk_narrow ? (int)UML_F32 : src_dtype, L.feature_major ? 1 : F,
+                                  L.feature_major ? rows : 1};
+    if ((rc = step.score(c, e->d_ochunk.p[slot], &launches, &path)) != UML_OK) {
       cudaStreamSynchronize(cs);
       cudaStreamSynchronize(e->copy_stream);
       return rc;
     }
-    // (4) labels (or class values, or the float64 outputs) back
-    char* land = result_bounce ? e->h_result.p[slot] : nullptr;
-    if (f64_out) {
-      const size_t bytes = (size_t)rows * n_f64 * 8;
-      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)land : (void*)(f64_out + r0 * n_f64), e->d_vchunk.p[slot],
-                                        bytes, cudaMemcpyDeviceToHost, cs));
-      d2h += (int64_t)bytes;
-    }
-    if (values_out) {
-      UML_CUDA_DRAIN(e, uml::launch_labels_take(l.targets.labels, 4, rows, e->d_classes.p[0], n_classes, e->d_vchunk.p[slot],
-                                                cs));
-      launches += 1;
-      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)land : (void*)(values_out + r0), e->d_vchunk.p[slot],
-                                        (size_t)rows * 8, cudaMemcpyDeviceToHost, cs));
-      d2h += rows * 8;
-    }
-    if (labels_out) {
-      UML_CUDA_DRAIN(e, cudaMemcpyAsync(land ? (void*)(land + (size_t)chunk_rows * 8) : (void*)(labels_out + r0), l.targets.labels,
-                                        (size_t)rows * 4, cudaMemcpyDeviceToHost, cs));
-      d2h += rows * 4;
-    }
+    // (4) the output back
+    const int64_t bytes = rows * out_bytes;
+    UML_CUDA_DRAIN(e, cudaMemcpyAsync(result_bounce ? (void*)e->h_result.p[slot] : static_cast<char*>(out) + r0 * out_bytes,
+                                      e->d_ochunk.p[slot], (size_t)bytes, cudaMemcpyDeviceToHost, cs));
+    d2h += bytes;
     if (result_bounce) {
       pending[slot].r0 = r0;
       pending[slot].rows = rows;
@@ -1878,31 +1829,115 @@ static int predict_host_impl(uml_engine* e, const uml_model* m, const void* host
   return rc;
 }
 
+// The chunk pipeline's steps.  They capture by value: an asynchronous call runs its step on the library thread after
+// the entry point has returned.
+static ChunkStep linear_labels_step(uml_engine* e, const uml_model* m, int mode) {
+  ChunkStep s{m->n_features_in, "estimator", 4, false};
+  s.score = [=](const Chunk& c, void* out, int* launches, int* path) {
+    LinearLaunch l{};
+    l.x = c.x;
+    l.ld = c.ld;
+    l.n_rows = c.rows;
+    l.targets.labels = static_cast<int32_t*>(out);
+    // (the reference MLP predictor casts to float32; a chunk that travelled as fp32 was checked lossless on the host: its
+    // fp32 rows ARE the caller's values) flagged rows are re-scored from the caller's own values (the raw chunk is still
+    // resident): float64 / int features that do not survive the fp32 down-cast still get sklearn's float64 labels
+    // (_base.py:366-396)
+    if (mode == UML_PREDICT_EXACT && lossy_capable(c.src.dtype)) l.src = c.src;
+    CUtensorMap map;
+    const bool has_map = encode_map(e, &map, c.x, c.rows, m->n_features_in, c.ld, linear_box_rows_for(m->n_features_in)) == UML_OK;
+    return enqueue_predict(e, m, l, has_map ? &map : nullptr, nullptr, mode, false, launches, path);
+  };
+  s.small = [=](const uml::SrcView& v, int rows, cudaStream_t st) {
+    return uml::launch_linear_small(m->dm, v, rows, e->d_small, st);
+  };
+  s.small_uid = m->uid;
+  return s;
+}
+
+// the labels, then classes[label] as float64 on the device
+static ChunkStep linear_values_step(uml_engine* e, const uml_model* m, int mode, const double* classes, int n_classes) {
+  ChunkStep s = linear_labels_step(e, m, mode);
+  s.row_bytes = 8;
+  s.classes = classes;
+  s.n_classes = n_classes;
+  s.prepare = [=](int64_t chunk_rows) -> int {
+    int rc;
+    if ((rc = grow(e, e->d_labels, chunk_rows)) != UML_OK || (rc = grow(e, e->d_classes, n_classes)) != UML_OK) return rc;
+    UML_CUDA(e, cudaMemcpyAsync(e->d_classes.p[0], classes, (size_t)n_classes * 8, cudaMemcpyHostToDevice, e->stream));
+    return UML_OK;
+  };
+  s.score = [=, labels = s.score](const Chunk& c, void* out, int* launches, int* path) -> int {
+    const int rc = labels(c, e->d_labels.p[0], launches, path);
+    if (rc != UML_OK) return rc;
+    UML_CUDA(e, uml::launch_labels_take(e->d_labels.p[0], 4, c.rows, e->d_classes.p[0], n_classes,
+                                        static_cast<double*>(out), e->stream));
+    *launches += 1;
+    return UML_OK;
+  };
+  return s;
+}
+
+// float64 scores, probabilities or log-probabilities (kind) from the chunk as it crossed PCIe
+static ChunkStep linear_f64_step(uml_engine* e, const uml_model* m, int kind) {
+  ChunkStep s{m->n_features_in, "estimator", 8ll * uml::linear_f64_width(m->dm, kind), true};
+  s.score = [=](const Chunk& c, void* out, int* launches, int* path) -> int {
+    NvtxRange r_score("uml:scores_f64");
+    UML_CUDA(e, uml::launch_linear_scores_f64(m->dm, c.src, c.rows, static_cast<double*>(out),
+                                              e->d_counters + uml::kCounterNonfinite, e->info.sm_count, e->stream, kind));
+    *launches += 1;
+    *path = f64_path(kind);
+    return UML_OK;
+  };
+  return s;
+}
+
+// an MLP whose weights and strips do not fit one SM's shared memory has no small-batch kernel
+static ChunkStep mlp_labels_step(uml_engine* e, const uml_mlp* m, int mode) {
+  ChunkStep s{m->dm.n_in, "module", 4, false};
+  s.score = [=](const Chunk& c, void* out, int* launches, int* path) {
+    CUtensorMap map;
+    const bool has_map = encode_map(e, &map, c.x, c.rows, m->dm.n_in, c.ld) == UML_OK;
+    uml::MlpTcLaunch o{};
+    o.n_rows = c.rows;
+    o.targets.labels = static_cast<int32_t*>(out);
+    return enqueue_mlp(e, m->dm, map, c.x, c.ld, o, mode == UML_PREDICT_EXACT, mlp_route(m->dm, has_map, false, c.tf32),
+                       false, launches, path);
+  };
+  if (m->small_smem > 0) {
+    s.small = [=](const uml::SrcView& v, int rows, cudaStream_t st) {
+      return uml::launch_mlp_small(m->dm, v, rows, e->d_small, m->small_smem, st);
+    };
+    s.small_uid = m->uid;
+  }
+  return s;
+}
+
 int uml_linear_predict_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows, int n_features,
                             int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out,
                             int mode, int64_t chunk_rows, uml_stats* stats) {
-  if (!labels_out && n_rows > 0) return UML_ERR_INVALID;
-  return predict_host_impl(e, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, labels_out,
-                           nullptr, nullptr, 0, mode, chunk_rows, stats);
+  if (!m) return UML_ERR_INVALID;
+  return predict_host_impl(e, linear_labels_step(e, m, mode), host_ptr, n_rows, n_features, row_stride_bytes,
+                           col_stride_bytes, src_dtype, labels_out, mode, chunk_rows, stats);
 }
 
 int uml_linear_predict_host_values(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows,
                                    int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype,
                                    const double* classes_host, int n_classes, double* values_out, int mode,
                                    int64_t chunk_rows, uml_stats* stats) {
-  if ((!values_out && n_rows > 0) || !classes_host || n_classes < 1) return UML_ERR_INVALID;
-  if (m && n_classes < m->dm.n_classes) UML_FAIL(e, UML_ERR_INVALID, "classes_ has %d entries, the model scores %d classes", n_classes, m->dm.n_classes);
-  return predict_host_impl(e, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, nullptr,
-                           values_out, classes_host, n_classes, mode, chunk_rows, stats);
+  if (!m || (!values_out && n_rows > 0) || !classes_host || n_classes < 1) return UML_ERR_INVALID;
+  if (n_classes < m->dm.n_classes) UML_FAIL(e, UML_ERR_INVALID, "classes_ has %d entries, the model scores %d classes", n_classes, m->dm.n_classes);
+  return predict_host_impl(e, linear_values_step(e, m, mode, classes_host, n_classes), host_ptr, n_rows, n_features,
+                           row_stride_bytes, col_stride_bytes, src_dtype, values_out, mode, chunk_rows, stats);
 }
 
 // asynchronous variant: the whole pipeline runs on a library thread so that the caller (Python building the
 // List[float] of the predictor contract) can consume labels_out[0, rows_done) while the rest of the batch is still
 // crossing PCIe.  One call in flight per engine; no other call on the engine until _finish.
-static int async_begin(uml_engine* e, const uml_model* m, const uml_mlp* mlp, const void* host_ptr, int64_t n_rows,
-                       int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype,
-                       int32_t* labels_out, int mode, int64_t chunk_rows) {
-  if (!e || (!m && !mlp) || (!labels_out && n_rows > 0)) return UML_ERR_INVALID;
+static int async_begin(uml_engine* e, const ChunkStep& step, const void* host_ptr, int64_t n_rows, int n_features,
+                       int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out, int mode,
+                       int64_t chunk_rows) {
+  if (!e || (!labels_out && n_rows > 0)) return UML_ERR_INVALID;
   if (!e->async_finished.load() || e->async_thread.joinable())
     UML_FAIL(e, UML_ERR_INVALID, "an asynchronous call is already in flight on this engine (call uml_async_finish first)");
   e->async_rows_done.store(0);
@@ -1910,9 +1945,8 @@ static int async_begin(uml_engine* e, const uml_model* m, const uml_mlp* mlp, co
   e->async_status = UML_OK;
   memset(&e->async_stats, 0, sizeof(e->async_stats));
   e->async_thread = std::thread([=]() {
-    e->async_status = predict_host_impl(e, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype,
-                                        labels_out, nullptr, nullptr, 0, mode, chunk_rows, &e->async_stats,
-                                        &e->async_rows_done, mlp);
+    e->async_status = predict_host_impl(e, step, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes,
+                                        src_dtype, labels_out, mode, chunk_rows, &e->async_stats, &e->async_rows_done);
     e->async_finished.store(1, std::memory_order_release);
   });
   return UML_OK;
@@ -1922,8 +1956,8 @@ int uml_linear_predict_host_begin(uml_engine* e, const uml_model* m, const void*
                                   int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out,
                                   int mode, int64_t chunk_rows) {
   if (!m) return UML_ERR_INVALID;
-  return async_begin(e, m, nullptr, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, labels_out,
-                     mode, chunk_rows);
+  return async_begin(e, linear_labels_step(e, m, mode), host_ptr, n_rows, n_features, row_stride_bytes,
+                     col_stride_bytes, src_dtype, labels_out, mode, chunk_rows);
 }
 
 // the MLP predictor through the same chunk pipeline, or for B <= kSmallRows the same online route (mlp_small_kernel):
@@ -1932,17 +1966,17 @@ int uml_linear_predict_host_begin(uml_engine* e, const uml_model* m, const void*
 int uml_mlp_predict_host(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows, int n_features,
                          int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out, int mode,
                          int64_t chunk_rows, uml_stats* stats) {
-  if (!e || !m || (!labels_out && n_rows > 0)) return UML_ERR_INVALID;
-  return predict_host_impl(e, nullptr, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype,
-                           labels_out, nullptr, nullptr, 0, mode, chunk_rows, stats, nullptr, m);
+  if (!m) return UML_ERR_INVALID;
+  return predict_host_impl(e, mlp_labels_step(e, m, mode), host_ptr, n_rows, n_features, row_stride_bytes,
+                           col_stride_bytes, src_dtype, labels_out, mode, chunk_rows, stats);
 }
 
 int uml_mlp_predict_host_begin(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows, int n_features,
                                int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out,
                                int mode, int64_t chunk_rows) {
   if (!m) return UML_ERR_INVALID;
-  return async_begin(e, nullptr, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, labels_out,
-                     mode, chunk_rows);
+  return async_begin(e, mlp_labels_step(e, m, mode), host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes,
+                     src_dtype, labels_out, mode, chunk_rows);
 }
 
 int uml_async_poll(uml_engine* e, int64_t* rows_done, int* finished) {
@@ -1961,28 +1995,17 @@ int uml_async_finish(uml_engine* e, uml_stats* stats) {
 }
 
 int uml_linear_predict_proba(uml_engine* e, const uml_model* m, const uml_batch* b, float* proba_out, int proba_on_device) {
-  if (!e || !m || !b || (!proba_out && b->n_rows > 0)) return UML_ERR_INVALID;
-  if (b->n_features != m->n_features_in)
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the estimator is expecting %d features as input.",
-             b->n_features, m->n_features_in);
-  UML_CUDA(e, cudaSetDevice(e->device));
-  (void)cudaGetLastError();
-  if (b->n_rows == 0) return UML_OK;
+  if (!m) return UML_ERR_INVALID;
   NvtxRange r_all("uml:predict_proba");
-  const int C = m->dm.n_classes;
-  float* d_out = proba_out;
-  if (!proba_on_device) UML_CUDA(e, cudaMalloc((void**)&d_out, (size_t)b->n_rows * C * 4));
-  cudaError_t ce = uml::launch_linear_proba(m->dm, b->x, b->ld, b->n_rows, d_out, e->info.sm_count, e->stream);
-  if (ce == cudaSuccess && !proba_on_device) {
-    ce = cudaMemcpyAsync(proba_out, d_out, (size_t)b->n_rows * C * 4, cudaMemcpyDeviceToHost, e->stream);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
-  }
-  if (!proba_on_device) {
-    cudaStreamSynchronize(e->stream);
-    cudaFree(d_out);
-  }
-  if (ce != cudaSuccess) UML_FAIL(e, UML_ERR_CUDA, "uml_linear_predict_proba: %s", cudaGetErrorString(ce));
-  return UML_OK;
+  auto score = [&](void* const* out, bool, int* launches, int*, int*) -> int {
+    UML_CUDA(e, uml::launch_linear_proba(m->dm, b->x, b->ld, b->n_rows, static_cast<float*>(out[0]), e->info.sm_count,
+                                         e->stream));
+    *launches = 1;
+    return UML_OK;
+  };
+  return predict_resident(e, b, {m->dm.n_classes, m->n_features_in, "estimator", {proba_out, nullptr},
+                                 {4ll * m->dm.n_classes, 0}, proba_on_device, UML_PREDICT_FAST, nullptr},
+                          no_prepare, score);
 }
 
 // float64 decision_function scores of a resident batch (sklearn/linear_model/_base.py:366-396), or their probabilities /
@@ -1991,39 +2014,27 @@ int uml_linear_predict_proba(uml_engine* e, const uml_model* m, const uml_batch*
 // and NaN / Inf reported, when it returns.
 static int linear_f64_resident(uml_engine* e, const uml_model* m, const uml_batch* b, double* out, int on_device,
                                int kind, uml_stats* stats) {
-  if (!e || !m || !b || (!out && b->n_rows > 0)) return UML_ERR_INVALID;
-  if (b->n_features != m->n_features_in)
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the estimator is expecting %d features as input.",
-             b->n_features, m->n_features_in);
-  UML_CUDA(e, cudaSetDevice(e->device));
-  (void)cudaGetLastError();
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (b->n_rows == 0) return UML_OK;
-  if (!b->x64 && !b->lossless)
-    UML_FAIL(e, UML_ERR_UNSUPPORTED, "the batch's fp32 rows are a lossy cast of the caller's values and it kept no "
-                                     "float64 copy: stage it with UML_STAGE_KEEP_F64 for its float64 %s",
-             kind == uml::kF64Scores ? "scores" : "probabilities");
-  const int64_t n_doubles = b->n_rows * uml::linear_f64_width(m->dm, kind);
-  double* d_out = out;
-  int rc;
-  if (!on_device) {
-    if ((rc = grow(e, e->d_scores, n_doubles)) != UML_OK) return rc;
-    d_out = e->d_scores.p[0];
-  }
-  const bool timed = stats != nullptr;
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
-  UML_CUDA(e, reset_counters(e, e->stream));
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
-  const uml::SrcView src = b->x64 ? uml::SrcView{b->x64, UML_F64, b->ld64, 1} : uml::SrcView{b->x, UML_F32, b->ld, 1};
-  UML_CUDA(e, uml::launch_linear_scores_f64(m->dm, src, b->n_rows, d_out, e->d_counters + uml::kCounterNonfinite, e->info.sm_count, e->stream, kind));
-  if (timed) {
-    UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
-    UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
-  }
-  if (!on_device) UML_CUDA(e, cudaMemcpyAsync(out, d_out, (size_t)n_doubles * 8, cudaMemcpyDeviceToHost, e->stream));
-  rc = finish_stats(e, stats, b->n_rows, 1, f64_path(kind), timed);
-  if (stats) stats->d2h_bytes = on_device ? 0 : n_doubles * 8;
-  return rc;
+  if (!m) return UML_ERR_INVALID;
+  auto prepare = [&]() -> int {
+    if (!b->x64 && !b->lossless)
+      UML_FAIL(e, UML_ERR_UNSUPPORTED, "the batch's fp32 rows are a lossy cast of the caller's values and it kept no "
+                                       "float64 copy: stage it with UML_STAGE_KEEP_F64 for its float64 %s",
+               kind == uml::kF64Scores ? "scores" : "probabilities");
+    return UML_OK;
+  };
+  auto score = [&](void* const* o, bool timed, int* launches, int* path, int*) -> int {
+    const uml::SrcView src = b->x64 ? uml::SrcView{b->x64, UML_F64, b->ld64, 1} : uml::SrcView{b->x, UML_F32, b->ld, 1};
+    UML_CUDA(e, uml::launch_linear_scores_f64(m->dm, src, b->n_rows, static_cast<double*>(o[0]),
+                                              e->d_counters + uml::kCounterNonfinite, e->info.sm_count, e->stream, kind));
+    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
+    *launches = 1;
+    *path = f64_path(kind);
+    return UML_OK;
+  };
+  ResidentCall c{m->dm.n_classes, m->n_features_in, "estimator", {out, nullptr},
+                 {8ll * uml::linear_f64_width(m->dm, kind), 0}, on_device, UML_PREDICT_FAST, stats};
+  c.always_sync = true;
+  return predict_resident(e, b, c, prepare, score);
 }
 
 int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_batch* b, double* scores_out,
@@ -2036,10 +2047,10 @@ int uml_linear_decision_function(uml_engine* e, const uml_model* m, const uml_ba
 int uml_linear_decision_function_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows,
                                       int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype,
                                       double* scores_out, int64_t chunk_rows, uml_stats* stats) {
-  if (!e || !m || (!scores_out && n_rows > 0)) return UML_ERR_INVALID;
+  if (!m) return UML_ERR_INVALID;
   NvtxRange r_all("uml:decision_function");
-  return predict_host_impl(e, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, nullptr,
-                           nullptr, nullptr, 0, UML_PREDICT_FAST, chunk_rows, stats, nullptr, nullptr, scores_out);
+  return predict_host_impl(e, linear_f64_step(e, m, uml::kF64Scores), host_ptr, n_rows, n_features, row_stride_bytes,
+                           col_stride_bytes, src_dtype, scores_out, UML_PREDICT_FAST, chunk_rows, stats);
 }
 
 // float64 probabilities (LogisticRegression.predict_proba) or their logs (predict_log_proba) of a resident batch, from
@@ -2054,11 +2065,11 @@ int uml_linear_predict_proba_f64(uml_engine* e, const uml_model* m, const uml_ba
 int uml_linear_predict_proba_f64_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows,
                                       int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype,
                                       double* proba_out, int log_proba, int64_t chunk_rows, uml_stats* stats) {
-  if (!e || !m || (!proba_out && n_rows > 0)) return UML_ERR_INVALID;
+  if (!m) return UML_ERR_INVALID;
   NvtxRange r_all("uml:predict_proba_f64");
-  return predict_host_impl(e, m, host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, nullptr,
-                           nullptr, nullptr, 0, UML_PREDICT_FAST, chunk_rows, stats, nullptr, nullptr, proba_out,
-                           log_proba ? uml::kF64LogProba : uml::kF64Proba);
+  return predict_host_impl(e, linear_f64_step(e, m, log_proba ? uml::kF64LogProba : uml::kF64Proba), host_ptr, n_rows,
+                           n_features, row_stride_bytes, col_stride_bytes, src_dtype, proba_out, UML_PREDICT_FAST,
+                           chunk_rows, stats);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2210,19 +2221,22 @@ static int mlp_predict_resident(uml_engine* e, const uml_mlp* m, const uml_batch
     // scratch for the CUDA-core kernel's labels on their way to the peers (enqueue_mlp)
     return route == 3 && n_peers > 0 ? grow(e, e->d_labels, b->n_rows) : (int)UML_OK;
   };
-  auto score = [&](int32_t* labels, bool timed, int* launches, int* path, int*) {  // the MLP kernels read fp32 rows
-    uml::MlpTcLaunch out{};
-    out.n_rows = b->n_rows;
-    uml::LabelTargets& t = out.targets;
-    t.labels = labels;
+  auto score = [&](void* const* out, bool timed, int* launches, int* path, int* elem_bytes) {
+    uml::MlpTcLaunch o{};
+    o.n_rows = b->n_rows;
+    uml::LabelTargets& t = o.targets;
+    t.labels = static_cast<int32_t*>(out[0]);
     t.row_offset = row_offset;
     t.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
     t.n_peers = n_peers;  // every peer vector, this rank's own included
     for (int i = 0; i < n_peers; ++i) t.peers[i] = peers[i];
-    return enqueue_mlp(e, m->dm, b->map, b->x, b->ld, out, mode == UML_PREDICT_EXACT, route, timed, launches, path);
+    *elem_bytes = 4;  // the MLP kernels read fp32 rows
+    return enqueue_mlp(e, m->dm, b->map, b->x, b->ld, o, mode == UML_PREDICT_EXACT, route, timed, launches, path);
   };
-  return predict_resident(e, b, m->dm.n_classes, m->dm.n_in, "module", labels_out, labels_on_device, n_peers,
-                          label_bytes, mode, stats, prepare, score);
+  ResidentCall c{m->dm.n_classes, m->dm.n_in, "module", {labels_out, nullptr}, {4, 0}, labels_on_device, mode, stats};
+  c.n_peers = n_peers;
+  c.label_bytes = label_bytes;
+  return predict_resident(e, b, c, prepare, score);
 }
 
 int uml_mlp_predict(uml_engine* e, const uml_mlp* m, const uml_batch* b, int32_t* labels_out, int labels_on_device,
@@ -2238,125 +2252,83 @@ int uml_mlp_predict_peers(uml_engine* e, const uml_mlp* m, const uml_batch* b, v
 
 int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, float* proba_out, int proba_on_device,
                           uml_stats* stats) {
-  if (!e || !m || !b || (!proba_out && b->n_rows > 0)) return UML_ERR_INVALID;
-  if (b->n_features != m->dm.n_in)
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the module is expecting %d features as input.", b->n_features,
-             m->dm.n_in);
-  UML_CUDA(e, cudaSetDevice(e->device));
-  (void)cudaGetLastError();
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (b->n_rows == 0) return UML_OK;
+  if (!m) return UML_ERR_INVALID;
   NvtxRange r_all("uml:mlp_proba");
-  const int path = mlp_route(m->dm, b->has_map, true, [&] { return batch_tf32_exact(e, b) == 1; });
-  const int64_t n_floats = b->n_rows * m->dm.n_classes;
-  float* d_out = proba_out;
-  int rc;
-  if (!proba_on_device) {
-    if ((rc = grow(e, e->d_proba, n_floats)) != UML_OK) return rc;
-    d_out = e->d_proba.p[0];
-  }
-  const bool timed = stats != nullptr;
-  if (timed) {
-    UML_CUDA(e, cudaMemsetAsync(e->d_counters, 0, sizeof(e->h->counters), e->stream));
-    UML_CUDA(e, cudaEventRecord(e->ev[0], e->stream));
-    UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
-  }
-  if (path == 5) {
-    uml::MlpTcLaunch out{};
-    out.n_rows = b->n_rows;
-    out.proba = d_out;
-    UML_CUDA(e, uml::launch_mlp_tc_proba(b->map, m->dm, out, e->info.sm_count, e->stream));
-  } else if (path == 3) {  // (no labels, so no flag list)
-    UML_CUDA(e, uml::launch_mlp_tma(b->map, m->dm, b->x, b->n_rows, nullptr, false, {}, e->info.sm_count, e->stream,
-                                    d_out));
-  } else {
-    UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, b->x, b->ld, b->n_rows, d_out, e->info.sm_count, e->stream));
-  }
-  if (timed) {
-    UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
-    UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
-  }
-  if (!proba_on_device)
-    UML_CUDA(e, cudaMemcpyAsync(proba_out, d_out, (size_t)n_floats * 4, cudaMemcpyDeviceToHost, e->stream));
-  if (timed) {
-    rc = finish_stats(e, stats, b->n_rows, 1, path, true);
-    stats->d2h_bytes = proba_on_device ? 0 : n_floats * 4;
-    return rc;
-  }
-  if (!proba_on_device) UML_CUDA(e, cudaStreamSynchronize(e->stream));
-  return UML_OK;
+  int route = 2;
+  auto prepare = [&] {
+    route = mlp_route(m->dm, b->has_map, true, [&] { return batch_tf32_exact(e, b) == 1; });
+    return (int)UML_OK;
+  };
+  auto score = [&](void* const* out, bool timed, int* launches, int* path, int*) -> int {
+    float* proba = static_cast<float*>(out[0]);
+    if (route == 5) {
+      uml::MlpTcLaunch o{};
+      o.n_rows = b->n_rows;
+      o.proba = proba;
+      UML_CUDA(e, uml::launch_mlp_tc_proba(b->map, m->dm, o, e->info.sm_count, e->stream));
+    } else if (route == 3) {  // (no labels, so no flag list)
+      UML_CUDA(e, uml::launch_mlp_tma(b->map, m->dm, b->x, b->n_rows, nullptr, false, {}, e->info.sm_count, e->stream,
+                                      proba));
+    } else {
+      UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, b->x, b->ld, b->n_rows, proba, e->info.sm_count, e->stream));
+    }
+    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
+    *launches = 1;
+    *path = route;
+    return UML_OK;
+  };
+  return predict_resident(e, b, {m->dm.n_classes, m->dm.n_in, "module", {proba_out, nullptr}, {4ll * m->dm.n_classes, 0},
+                                 proba_on_device, UML_PREDICT_FAST, stats},
+                          prepare, score);
 }
 
 int uml_mlp_predict_topk(uml_engine* e, const uml_mlp* m, const uml_batch* b, int k, int32_t* idx_out, float* proba_out,
                          int out_on_device, int mode, uml_stats* stats) {
-  if (!e || !m || !b || (!idx_out && b->n_rows > 0)) return UML_ERR_INVALID;
+  if (!e || !m) return UML_ERR_INVALID;
   const int C = m->dm.n_classes;
   if (k < 1 || k > C) UML_FAIL(e, UML_ERR_INVALID, "k = %d: the module has %d classes (need 1 <= k <= %d)", k, C, C);
-  if (mode != UML_PREDICT_FAST && mode != UML_PREDICT_EXACT) UML_FAIL(e, UML_ERR_INVALID, "mode %d", mode);
-  if (b->n_features != m->dm.n_in)
-    UML_FAIL(e, UML_ERR_SHAPE, "X has %d features, but the module is expecting %d features as input.", b->n_features,
-             m->dm.n_in);
-  UML_CUDA(e, cudaSetDevice(e->device));
-  (void)cudaGetLastError();
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (b->n_rows == 0) return UML_OK;
   NvtxRange r_all("uml:mlp_topk");
-  const bool exact = mode == UML_PREDICT_EXACT;
-  // k beyond what the tile kernels select in registers: the float64 kernel serves every row
-  const int path = k > uml::kMlpTopkMax ? 2 : mlp_route(m->dm, b->has_map, false, [&] { return batch_tf32_exact(e, b) == 1; }, true);
-  const int64_t n_out = b->n_rows * k;
-  int32_t* d_idx = idx_out;
-  float* d_proba = proba_out;
-  int rc;
-  if (exact && path != 2 && (rc = grow(e, e->d_flag_rows, b->n_rows)) != UML_OK) return rc;
-  if (!out_on_device) {
-    if ((rc = grow(e, e->d_labels, n_out)) != UML_OK) return rc;
-    d_idx = e->d_labels.p[0];
-    if (proba_out) {
-      if ((rc = grow(e, e->d_proba, n_out)) != UML_OK) return rc;
-      d_proba = e->d_proba.p[0];
+  int route = 2;
+  auto prepare = [&] {
+    // k beyond what the tile kernels select in registers: the float64 kernel serves every row
+    if (k <= uml::kMlpTopkMax) route = mlp_route(m->dm, b->has_map, false, [&] { return batch_tf32_exact(e, b) == 1; }, true);
+    return (int)UML_OK;
+  };
+  auto score = [&](void* const* out, bool timed, int* launches, int* path, int*) -> int {
+    int32_t* idx = static_cast<int32_t*>(out[0]);
+    float* proba = static_cast<float*>(out[1]);
+    const bool exact = mode == UML_PREDICT_EXACT;
+    const FlagList fl = flag_list(e);
+    const int sm = e->info.sm_count;
+    cudaStream_t s = e->stream;
+    *launches = 1;
+    *path = route;
+    if (route == 2) {
+      UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, b->x, b->ld, b->n_rows, k, idx, proba, fl, true, sm, s));
+      if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
+      return UML_OK;
     }
-  }
-  const FlagList fl = flag_list(e);
-  const int sm = e->info.sm_count;
-  cudaStream_t s = e->stream;
-  const bool timed = stats != nullptr;
-  const bool sync_call = timed || !out_on_device;
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[0], s));
-  // as for the labels: an asynchronous call finds the flag list handed back empty by the previous re-score
-  if (sync_call) UML_CUDA(e, reset_counters(e, s));
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], s));
-  int launches = 1;
-  if (path == 2) {
-    UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, b->x, b->ld, b->n_rows, k, d_idx, d_proba, fl, true, sm, s));
-    if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
-  } else {
-    if (path == 5) {
-      uml::MlpTcLaunch out{};
-      out.n_rows = b->n_rows;
-      out.topk_idx = d_idx;
-      out.topk_proba = d_proba;
-      out.topk_k = k;
-      UML_CUDA(e, uml::launch_mlp_tc_topk(b->map, m->dm, out, exact, fl, sm, s));
+    if (route == 5) {
+      uml::MlpTcLaunch o{};
+      o.n_rows = b->n_rows;
+      o.topk_idx = idx;
+      o.topk_proba = proba;
+      o.topk_k = k;
+      UML_CUDA(e, uml::launch_mlp_tc_topk(b->map, m->dm, o, exact, fl, sm, s));
     } else {
-      UML_CUDA(e, uml::launch_mlp_tma_topk(b->map, m->dm, b->n_rows, k, d_idx, d_proba, exact, fl, sm, s));
+      UML_CUDA(e, uml::launch_mlp_tma_topk(b->map, m->dm, b->n_rows, k, idx, proba, exact, fl, sm, s));
     }
     if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], s));
     if (exact) {
       NvtxRange r_rescore("uml:mlp_topk_f64");
-      UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, b->x, b->ld, b->n_rows, k, d_idx, d_proba, fl, false, sm, s));
-      ++launches;
+      UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, b->x, b->ld, b->n_rows, k, idx, proba, fl, false, sm, s));
+      ++*launches;
     }
-  }
-  if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], s));
-  if (!sync_call) return UML_OK;
-  if (!out_on_device) {
-    UML_CUDA(e, cudaMemcpyAsync(idx_out, d_idx, (size_t)n_out * 4, cudaMemcpyDeviceToHost, s));
-    if (proba_out) UML_CUDA(e, cudaMemcpyAsync(proba_out, d_proba, (size_t)n_out * 4, cudaMemcpyDeviceToHost, s));
-  }
-  rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
-  if (stats) stats->d2h_bytes = out_on_device ? 0 : n_out * 4 * (proba_out ? 2 : 1);
-  return rc;
+    return UML_OK;
+  };
+  return predict_resident(e, b, {C, m->dm.n_in, "module", {idx_out, proba_out}, {4ll * k, 4ll * k}, out_on_device, mode,
+                                 stats},
+                          prepare, score);
 }
 
 }  // extern "C"

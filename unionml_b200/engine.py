@@ -42,6 +42,10 @@ def _raise(status: int, message: str):
     raise EngineError(status, message)
 
 
+def _mode(exact: bool) -> int:
+    return N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
+
+
 def as_feature_array(features: Any) -> np.ndarray:
     """Borrow ``features`` as a 2-D ndarray in a dtype the staging kernels take, without copying when possible.
 
@@ -188,6 +192,41 @@ class Engine:
         if status != N.UML_OK:
             _raise(status, (N.lib().uml_last_error(self._h) or b"").decode())
 
+    def _resident(self, fn, model, batch: Batch, outs, device_ptrs, before=(), after=(), want_stats=False,
+                  takes_stats=True):
+        """One predict call on a resident batch: ``fn(engine, model, batch, *before, *outputs, on_device, *after,
+        stats)``.  ``outs``: ``(shape, dtype)`` of each host output to allocate, ``None`` for one not asked for.  When
+        ``device_ptrs[0]`` is not ``None`` the outputs go to ``device_ptrs`` instead and ``None`` stands in for each
+        array."""
+        stats = N.Stats() if want_stats else None
+        on_device = device_ptrs[0] is not None
+        if on_device:
+            arrays = [None] * len(outs)
+            ptrs = [None if p is None else C.c_void_p(p) for p in device_ptrs]
+        else:
+            arrays = [None if o is None else np.empty(o[0], dtype=o[1]) for o in outs]
+            ptrs = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrays]
+        tail = (C.byref(stats) if stats else None,) if takes_stats else ()
+        with self._lock:
+            # under the lock: uml_last_error is per engine, another thread's call may overwrite it
+            self._check(fn(self._h, model._h, batch._h, *before, *ptrs, int(on_device), *after, *tail))
+        return arrays, stats.as_dict() if stats else None
+
+    @staticmethod
+    def _host_rows(features: Any):
+        """``features`` as :func:`as_feature_array` borrows them, and the six ABI arguments that describe them: pointer,
+        rows, features, row and column strides in bytes, dtype."""
+        arr = as_feature_array(features)
+        return arr, (C.c_void_p(arr.ctypes.data), arr.shape[0], arr.shape[1], arr.strides[0], arr.strides[1],
+                     _DTYPES[arr.dtype])
+
+    def _predict_rows(self, fn, model, rows: tuple, *args) -> dict:
+        """One call through the chunk pipeline: ``fn(engine, model, *rows, *args, stats)``; returns the stats dict."""
+        stats = N.Stats()
+        with self._lock:
+            self._check(fn(self._h, model._h, *rows, *args, C.byref(stats)))
+        return stats.as_dict()
+
     def set_stream(self, cuda_stream: Optional[int]) -> None:
         """Run on the caller's stream (e.g. ``torch.cuda.current_stream().cuda_stream``); ``None`` = engine stream."""
         self._check(N.lib().uml_engine_set_stream(self._h, C.c_void_p(cuda_stream or 0)))
@@ -264,40 +303,18 @@ class Engine:
     def predict_mlp(self, model: MlpModel, batch: Batch, exact: bool = True, out_device_ptr: Optional[int] = None,
                     want_stats: bool = True) -> Tuple[Optional[np.ndarray], Optional[dict]]:
         """Argmax class index per row of ``softmax(W2 relu(W1 x + b1) + b2)``."""
-        mode = N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
-        stats = N.Stats() if want_stats else None
-        with self._lock:
-            if out_device_ptr is not None:
-                st = N.lib().uml_mlp_predict(
-                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, mode, C.byref(stats) if stats else None
-                )
-                self._check(st)
-                return None, stats.as_dict() if stats else None
-            out = np.empty(batch.n_rows, dtype=np.int32)
-            st = N.lib().uml_mlp_predict(
-                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, mode, C.byref(stats) if stats else None
-            )
-            self._check(st)  # under the lock: uml_last_error is per engine, another thread's call may overwrite it
-        return out, stats.as_dict() if stats else None
+        (out,), stats = self._resident(N.lib().uml_mlp_predict, model, batch, [(batch.n_rows, np.int32)],
+                                       [out_device_ptr], after=(_mode(exact),), want_stats=want_stats)
+        return out, stats
 
     def predict_mlp_proba(self, model: MlpModel, batch: Batch, out_device_ptr: Optional[int] = None,
                           want_stats: bool = False) -> Tuple[Optional[np.ndarray], Optional[dict]]:
         """``softmax(W2 relu(W1 x + b1) + b2)`` per row (fp32), ``(n_rows, n_classes)``: what the torch quickstart's
         ``PytorchModel.forward`` returns.  With ``out_device_ptr`` the rows are written there and ``None`` is returned."""
-        stats = N.Stats() if want_stats else None
-        with self._lock:
-            if out_device_ptr is not None:
-                st = N.lib().uml_mlp_predict_proba(
-                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, C.byref(stats) if stats else None
-                )
-                self._check(st)
-                return None, stats.as_dict() if stats else None
-            out = np.empty((batch.n_rows, model.n_classes), dtype=np.float32)
-            st = N.lib().uml_mlp_predict_proba(
-                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, C.byref(stats) if stats else None
-            )
-            self._check(st)
-        return out, stats.as_dict() if stats else None
+        (out,), stats = self._resident(N.lib().uml_mlp_predict_proba, model, batch,
+                                       [((batch.n_rows, model.n_classes), np.float32)],
+                                       [out_device_ptr], want_stats=want_stats)
+        return out, stats
 
     def predict_mlp_topk(self, model: MlpModel, batch: Batch, k: int, exact: bool = True, want_proba: bool = True,
                          idx_device_ptr: Optional[int] = None, proba_device_ptr: Optional[int] = None,
@@ -307,26 +324,14 @@ class Engine:
         mode.  ``exact``: the indices of the float64 network (rows the fp32 rank guard cannot certify are re-scored in
         float64).  With ``idx_device_ptr`` (and ``proba_device_ptr`` when ``want_proba``) the results are written to
         device memory and ``None`` is returned in their place."""
-        mode = N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
-        stats = N.Stats() if want_stats else None
-        on_device = idx_device_ptr is not None
-        if on_device and want_proba and proba_device_ptr is None:
+        if idx_device_ptr is not None and want_proba and proba_device_ptr is None:
             raise ValueError("want_proba with device outputs needs proba_device_ptr")
-        with self._lock:
-            if on_device:
-                idx_p, proba_p = C.c_void_p(idx_device_ptr), C.c_void_p(proba_device_ptr) if want_proba else None
-                idx = proba = None
-            else:
-                idx = np.empty((batch.n_rows, max(int(k), 0)), dtype=np.int32)
-                proba = np.empty((batch.n_rows, max(int(k), 0)), dtype=np.float32) if want_proba else None
-                idx_p = idx.ctypes.data_as(C.c_void_p)
-                proba_p = None if proba is None else proba.ctypes.data_as(C.c_void_p)
-            st = N.lib().uml_mlp_predict_topk(
-                self._h, model._h, batch._h, int(k), idx_p, proba_p, 1 if on_device else 0, mode,
-                C.byref(stats) if stats else None
-            )
-            self._check(st)
-        return idx, proba, stats.as_dict() if stats else None
+        shape = (batch.n_rows, max(int(k), 0))
+        (idx, proba), stats = self._resident(
+            N.lib().uml_mlp_predict_topk, model, batch, [(shape, np.int32), (shape, np.float32) if want_proba else None],
+            [idx_device_ptr, proba_device_ptr if want_proba else None],
+            before=(int(k),), after=(_mode(exact),), want_stats=want_stats)
+        return idx, proba, stats
 
     def count_topk_hits(self, idx_ptr: int, k: int, n: int, classes, targets) -> np.ndarray:
         """``hits[j]`` = rows whose target is ``classes[idx[row, j']]`` for some ``j' <= j`` (int64, length ``k``), from
@@ -346,34 +351,23 @@ class Engine:
     def predict_mlp_peers(self, model: MlpModel, batch: Batch, peer_ptrs, row_offset: int, exact: bool = True,
                           want_stats: bool = False, label_bytes: int = 4) -> Optional[dict]:
         """Fused compute + all-gather for the MLP predictor (same contract as :meth:`predict_peers`)."""
-        mode = N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
         arr = (C.c_void_p * len(peer_ptrs))(*[C.c_void_p(p) for p in peer_ptrs])
         stats = N.Stats() if want_stats else None
         with self._lock:
             st = N.lib().uml_mlp_predict_peers(
-                self._h, model._h, batch._h, arr, len(peer_ptrs), row_offset, label_bytes, mode, C.byref(stats) if stats else None
+                self._h, model._h, batch._h, arr, len(peer_ptrs), row_offset, label_bytes, _mode(exact),
+                C.byref(stats) if stats else None
             )
             self._check(st)
         return stats.as_dict() if stats else None
 
     def stage(self, features: Any, keep_f64: bool = True, check_finite: bool = True) -> Batch:
         """Host rows (ndarray / DataFrame, any order, f32/f64/int) -> device fp32 row-major, converted on the GPU."""
-        arr = as_feature_array(features)
+        _, rows = self._host_rows(features)
         flags = (N.UML_STAGE_KEEP_F64 if keep_f64 else 0) | (0 if check_finite else N.UML_STAGE_SKIP_FINITE_CHECK)
         h = C.c_void_p()
         with self._lock:
-            st = N.lib().uml_stage_rows(
-                self._h,
-                C.byref(h),
-                C.c_void_p(arr.ctypes.data),
-                arr.shape[0],
-                arr.shape[1],
-                arr.strides[0],
-                arr.strides[1],
-                _DTYPES[arr.dtype],
-                flags,
-            )
-            self._check(st)
+            self._check(N.lib().uml_stage_rows(self._h, C.byref(h), *rows, flags))
         return Batch(self, h.value)
 
     def wrap_device(self, device_ptr: int, n_rows: int, n_features: int, ld: Optional[int] = None, keepalive: Any = None) -> Batch:
@@ -396,31 +390,19 @@ class Engine:
         want_stats: bool = True,
     ) -> Tuple[Optional[np.ndarray], Optional[dict]]:
         """Class *indices* per row.  Host result (int32 ndarray) unless ``out_device_ptr`` is given."""
-        mode = N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
-        stats = N.Stats() if want_stats else None
-        with self._lock:
-            if out_device_ptr is not None:
-                st = N.lib().uml_linear_predict(
-                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, mode, C.byref(stats) if stats else None
-                )
-                self._check(st)
-                return None, stats.as_dict() if stats else None
-            out = np.empty(batch.n_rows, dtype=np.int32)
-            st = N.lib().uml_linear_predict(
-                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, mode, C.byref(stats) if stats else None
-            )
-            self._check(st)
-        return out, stats.as_dict() if stats else None
+        (out,), stats = self._resident(N.lib().uml_linear_predict, model, batch, [(batch.n_rows, np.int32)],
+                                       [out_device_ptr], after=(_mode(exact),), want_stats=want_stats)
+        return out, stats
 
     def predict_peers(self, model: LinearModel, batch: Batch, peer_ptrs, row_offset: int, exact: bool = True,
                       want_stats: bool = False, label_bytes: int = 4) -> Optional[dict]:
         """Fused compute + all-gather: labels are stored into every peer's vector from the kernel epilogue."""
-        mode = N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
         arr = (C.c_void_p * len(peer_ptrs))(*[C.c_void_p(p) for p in peer_ptrs])
         stats = N.Stats() if want_stats else None
         with self._lock:
             st = N.lib().uml_linear_predict_peers(
-                self._h, model._h, batch._h, arr, len(peer_ptrs), row_offset, label_bytes, mode, C.byref(stats) if stats else None
+                self._h, model._h, batch._h, arr, len(peer_ptrs), row_offset, label_bytes, _mode(exact),
+                C.byref(stats) if stats else None
             )
             self._check(st)
         return stats.as_dict() if stats else None
@@ -466,58 +448,26 @@ class Engine:
         chunk_rows: int = 0,
     ) -> Tuple[np.ndarray, dict]:
         """Host rows -> host labels in one pipelined call (chunked H2D / convert / score / D2H)."""
-        arr = as_feature_array(features)
+        arr, rows = self._host_rows(features)
         if out is None:
             out = np.empty(arr.shape[0], dtype=np.int32)
         elif out.dtype != np.int32 or out.shape != (arr.shape[0],) or not out.flags.c_contiguous:
             raise ValueError("out must be a C-contiguous int32 vector of length n_rows")
-        stats = N.Stats()
-        with self._lock:
-            st = N.lib().uml_linear_predict_host(
-                self._h,
-                model._h,
-                C.c_void_p(arr.ctypes.data),
-                arr.shape[0],
-                arr.shape[1],
-                arr.strides[0],
-                arr.strides[1],
-                _DTYPES[arr.dtype],
-                out.ctypes.data_as(C.c_void_p),
-                N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST,
-                chunk_rows,
-                C.byref(stats),
-            )
-            self._check(st)
-        return out, stats.as_dict()
+        stats = self._predict_rows(N.lib().uml_linear_predict_host, model, rows, out.ctypes.data_as(C.c_void_p),
+                                   _mode(exact), chunk_rows)
+        return out, stats
 
     def predict_host_values(self, model: LinearModel, features: Any, classes, exact: bool = True,
                             chunk_rows: int = 0) -> Tuple[np.ndarray, dict]:
         """Host rows -> ``classes_[argmax]`` as a float64 host vector: the pipelined call with ``classes_.take`` and the
         float conversion of the canonical predictor (``README.md:92``) done on the device, chunk by chunk."""
-        arr = as_feature_array(features)
+        arr, rows = self._host_rows(features)
         if not (isinstance(classes, np.ndarray) and classes.dtype == np.float64 and classes.flags.c_contiguous):
             classes = np.ascontiguousarray(classes, dtype=np.float64)
         out = np.empty(arr.shape[0], dtype=np.float64)
-        stats = N.Stats()
-        with self._lock:
-            st = N.lib().uml_linear_predict_host_values(
-                self._h,
-                model._h,
-                C.c_void_p(arr.ctypes.data),
-                arr.shape[0],
-                arr.shape[1],
-                arr.strides[0],
-                arr.strides[1],
-                _DTYPES[arr.dtype],
-                classes.ctypes.data_as(C.c_void_p),
-                len(classes),
-                out.ctypes.data_as(C.c_void_p),
-                N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST,
-                chunk_rows,
-                C.byref(stats),
-            )
-            self._check(st)
-        return out, stats.as_dict()
+        stats = self._predict_rows(N.lib().uml_linear_predict_host_values, model, rows, classes.ctypes.data_as(C.c_void_p),
+                                   len(classes), out.ctypes.data_as(C.c_void_p), _mode(exact), chunk_rows)
+        return out, stats
 
     def predict_mlp_host(self, model: MlpModel, features: Any, exact: bool = True, chunk_rows: int = 0,
                          out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, dict]:
@@ -526,18 +476,12 @@ class Engine:
         reads the request from pinned host memory, replayed as a CUDA graph (stats ``path`` 4, exact labels in either
         mode).  Larger batches, or a model too large for that kernel's shared memory: the chunk pipeline (pinned bounce
         buffers, GPU down-cast, scoring kernel, fp64 re-score)."""
-        arr = as_feature_array(features)
+        arr, rows = self._host_rows(features)
         if out is None:
             out = np.empty(arr.shape[0], dtype=np.int32)
-        stats = N.Stats()
-        with self._lock:
-            st = N.lib().uml_mlp_predict_host(
-                self._h, model._h, C.c_void_p(arr.ctypes.data), arr.shape[0], arr.shape[1], arr.strides[0], arr.strides[1],
-                _DTYPES[arr.dtype], out.ctypes.data_as(C.c_void_p), N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST,
-                chunk_rows, C.byref(stats),
-            )
-            self._check(st)
-        return out, stats.as_dict()
+        stats = self._predict_rows(N.lib().uml_mlp_predict_host, model, rows, out.ctypes.data_as(C.c_void_p),
+                                   _mode(exact), chunk_rows)
+        return out, stats
 
     def predict_host_list(self, model, features: Any, table: list, exact: bool = True, chunk_rows: int = 0,
                           asynchronous: Optional[bool] = None) -> Tuple[list, dict]:
@@ -549,13 +493,12 @@ class Engine:
         the finished prefix is filled into the list while the rest of the batch is still in flight."""
         import time
 
-        arr = as_feature_array(features)
+        arr, rows = self._host_rows(features)
         is_mlp = isinstance(model, MlpModel)
         n = arr.shape[0]
         labels = np.empty(n, dtype=np.int32)
         helper = N.pylist()
         lib = N.lib()
-        mode = N.UML_PREDICT_EXACT if exact else N.UML_PREDICT_FAST
         if asynchronous is None:
             asynchronous = n >= 1_000_000
         stats = N.Stats()
@@ -577,8 +520,7 @@ class Engine:
         begin = lib.uml_mlp_predict_host_begin if is_mlp else lib.uml_linear_predict_host_begin
         with self._lock:
             t0 = time.perf_counter()
-            st = begin(self._h, model._h, C.c_void_p(arr.ctypes.data), n, arr.shape[1], arr.strides[0], arr.strides[1],
-                       _DTYPES[arr.dtype], labels.ctypes.data_as(C.c_void_p), mode, chunk_rows)
+            st = begin(self._h, model._h, *rows, labels.ctypes.data_as(C.c_void_p), _mode(exact), chunk_rows)
             self._check(st)
             done, rows_done, finished = 0, C.c_int64(), C.c_int()
             t_pipeline = t_list = 0.0
@@ -611,12 +553,9 @@ class Engine:
 
     def predict_proba(self, model: LinearModel, batch: Batch, out_device_ptr: Optional[int] = None) -> Optional[np.ndarray]:
         """``softmax(X @ coef_.T + intercept_)`` per row (fp32), ``(n_rows, n_classes)``; ``[1 - p, p]`` for a binary model."""
-        with self._lock:
-            if out_device_ptr is not None:
-                self._check(N.lib().uml_linear_predict_proba(self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1))
-                return None
-            out = np.empty((batch.n_rows, model.n_classes), dtype=np.float32)
-            self._check(N.lib().uml_linear_predict_proba(self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0))
+        (out,), _ = self._resident(N.lib().uml_linear_predict_proba, model, batch,
+                                   [((batch.n_rows, model.n_classes), np.float32)],
+                                   [out_device_ptr], takes_stats=False)
         return out
 
     @staticmethod
@@ -629,48 +568,24 @@ class Engine:
         for a binary model, else ``(n_rows, n_classes)``.  Scored from the batch's float64 copy when it has one
         (``stage(keep_f64=True)``), else from its fp32 rows, which must then be the caller's values.  With
         ``out_device_ptr`` (8-byte aligned) the scores are written there and ``None`` is returned."""
-        stats = N.Stats() if want_stats else None
-        with self._lock:
-            if out_device_ptr is not None:
-                st = N.lib().uml_linear_decision_function(
-                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, C.byref(stats) if stats else None
-                )
-                self._check(st)
-                return None, stats.as_dict() if stats else None
-            out = np.empty(self._scores_shape(model, batch.n_rows), dtype=np.float64)
-            st = N.lib().uml_linear_decision_function(
-                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, C.byref(stats) if stats else None
-            )
-            self._check(st)
-        return out, stats.as_dict() if stats else None
+        (out,), stats = self._resident(N.lib().uml_linear_decision_function, model, batch,
+                                       [(self._scores_shape(model, batch.n_rows), np.float64)],
+                                       [out_device_ptr], want_stats=want_stats)
+        return out, stats
 
     def decision_function_host(self, model: LinearModel, features: Any, chunk_rows: int = 0,
                                out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, dict]:
         """Host rows (any order, f32/f64/int) -> float64 scores through the chunk pipeline of :meth:`predict_host`,
         from the caller's own values; shapes as :meth:`decision_function`."""
-        arr = as_feature_array(features)
+        arr, rows = self._host_rows(features)
         shape = self._scores_shape(model, arr.shape[0])
         if out is None:
             out = np.empty(shape, dtype=np.float64)
         elif out.dtype != np.float64 or out.shape != shape or not out.flags.c_contiguous:
             raise ValueError(f"out must be a C-contiguous float64 array of shape {shape}")
-        stats = N.Stats()
-        with self._lock:
-            st = N.lib().uml_linear_decision_function_host(
-                self._h,
-                model._h,
-                C.c_void_p(arr.ctypes.data),
-                arr.shape[0],
-                arr.shape[1],
-                arr.strides[0],
-                arr.strides[1],
-                _DTYPES[arr.dtype],
-                out.ctypes.data_as(C.c_void_p),
-                chunk_rows,
-                C.byref(stats),
-            )
-            self._check(st)
-        return out, stats.as_dict()
+        stats = self._predict_rows(N.lib().uml_linear_decision_function_host, model, rows, out.ctypes.data_as(C.c_void_p),
+                                   chunk_rows)
+        return out, stats
 
     def predict_proba_f64(self, model: LinearModel, batch: Batch, log: bool = False,
                           out_device_ptr: Optional[int] = None,
@@ -679,49 +594,25 @@ class Engine:
         for a binary model: scikit-learn's softmax / expit of the float64 scores :meth:`decision_function` computes from
         the same rows (DESIGN.md §3.9).  With ``out_device_ptr`` (8-byte aligned) the output is written there and
         ``None`` is returned."""
-        stats = N.Stats() if want_stats else None
-        with self._lock:
-            if out_device_ptr is not None:
-                st = N.lib().uml_linear_predict_proba_f64(
-                    self._h, model._h, batch._h, C.c_void_p(out_device_ptr), 1, int(log), C.byref(stats) if stats else None
-                )
-                self._check(st)
-                return None, stats.as_dict() if stats else None
-            out = np.empty((batch.n_rows, model.n_classes), dtype=np.float64)
-            st = N.lib().uml_linear_predict_proba_f64(
-                self._h, model._h, batch._h, out.ctypes.data_as(C.c_void_p), 0, int(log), C.byref(stats) if stats else None
-            )
-            self._check(st)
-        return out, stats.as_dict() if stats else None
+        (out,), stats = self._resident(N.lib().uml_linear_predict_proba_f64, model, batch,
+                                       [((batch.n_rows, model.n_classes), np.float64)],
+                                       [out_device_ptr], after=(int(log),),
+                                       want_stats=want_stats)
+        return out, stats
 
     def predict_proba_f64_host(self, model: LinearModel, features: Any, log: bool = False, chunk_rows: int = 0,
                                out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, dict]:
         """Host rows (any order, f32/f64/int) -> float64 probabilities (``log``: their logs) through the chunk pipeline
         of :meth:`predict_host`, from the caller's own values; shapes as :meth:`predict_proba_f64`."""
-        arr = as_feature_array(features)
+        arr, rows = self._host_rows(features)
         shape = (arr.shape[0], model.n_classes)
         if out is None:
             out = np.empty(shape, dtype=np.float64)
         elif out.dtype != np.float64 or out.shape != shape or not out.flags.c_contiguous:
             raise ValueError(f"out must be a C-contiguous float64 array of shape {shape}")
-        stats = N.Stats()
-        with self._lock:
-            st = N.lib().uml_linear_predict_proba_f64_host(
-                self._h,
-                model._h,
-                C.c_void_p(arr.ctypes.data),
-                arr.shape[0],
-                arr.shape[1],
-                arr.strides[0],
-                arr.strides[1],
-                _DTYPES[arr.dtype],
-                out.ctypes.data_as(C.c_void_p),
-                int(log),
-                chunk_rows,
-                C.byref(stats),
-            )
-            self._check(st)
-        return out, stats.as_dict()
+        stats = self._predict_rows(N.lib().uml_linear_predict_proba_f64_host, model, rows,
+                                   out.ctypes.data_as(C.c_void_p), int(log), chunk_rows)
+        return out, stats
 
 
 _default_engine: Optional[Engine] = None
