@@ -268,6 +268,25 @@ UML_API int uml_mlp_predict_host(uml_engine* e, const uml_mlp* m, const void* ho
 UML_API int uml_mlp_predict_host_begin(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows, int n_features,
                                int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out,
                                int mode, int64_t chunk_rows);
+/* uml_mlp_predict_proba and uml_mlp_predict_topk from HOST rows of any layout and dtype uml_mlp_predict_host takes.
+ * proba_out: n_rows x n_out fp32.  out: n_rows records of 2k 32-bit words, k int32 class indices then their k fp32
+ * probabilities.  Host memory, pageable or pinned.  1 <= k <= n_out, else UML_ERR_INVALID; NaN/Inf in the fp32
+ * features (a finite float64 beyond the fp32 range included) is UML_ERR_NONFINITE; a wrong feature count UML_ERR_SHAPE.
+ *  - More than 64 rows: the chunk pipeline, which picks the kernel of every chunk from the first 2048 rows, as for
+ *    labels.  When every row is a tf32 value, or none is, the result has the bits of the resident call
+ *    (uml_mlp_predict_proba / uml_mlp_predict_topk in the same mode) on the same rows.  Otherwise, when the tensor
+ *    cores were picked, the rows that are not tf32 values get the float64 route's values (stats n_flagged counts them).
+ *  - Up to 64 rows whose raw block fits 256 KiB: the online route of uml_mlp_predict_host (stats path 4, one kernel
+ *    replayed as a CUDA graph): the float64 route's values in either mode, so a row's probabilities can differ in the
+ *    last bits between a small and a large request, as its label can in FAST mode.  Top-k rows whose consecutive
+ *    ranks 0 .. min(k, n_out - 1) are not separated by the fp64 bound count in stats n_ambiguous.  A model too large for
+ *    the kernel (its labels' shared memory plus a 4-row logits strip per warp) keeps the pipeline. */
+UML_API int uml_mlp_predict_proba_host(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows,
+                                       int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype,
+                                       float* proba_out, int64_t chunk_rows, uml_stats* stats);
+UML_API int uml_mlp_predict_topk_host(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows,
+                                      int n_features, int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype,
+                                      int k, int32_t* out, int mode, int64_t chunk_rows, uml_stats* stats);
 /* fused compute + collective for the MLP predictor: same contract as uml_linear_predict_peers (labels of this rank's
  * rows are stored into every entry of peer_labels at row_offset from the kernel epilogue; int32 or uint8 vectors).
  * Batches whose features are tf32 values (integer / pixel domains) run layer 1 on the tensor cores (wgmma, stats

@@ -108,4 +108,16 @@ for log in (False, True):
     eng.predict_proba_f64_host(m784, X784, log=log, chunk_rows=2048)
 pf = eng.device_alloc(8 * (10 * b64.n_rows + 2))
 eng.predict_proba_f64(m, b64, out_device_ptr=pf.ptr + 8, want_stats=True)
+# MLP probabilities and top-k from host rows: the online kernel's two record forms (1 and 32 rows, capture then replay,
+# k = 3 and k = C), and a mixed frame through the pipeline - integer rows first, so the tensor cores are picked and flag
+# the later general-float rows for the flagged-row float64 probabilities and top-k
+for rows in (1, 32):
+    for _ in range(2):
+        eng.predict_mlp_proba_host(mlp, Xf[:rows])
+        eng.predict_mlp_topk_host(mlp, Xf[:rows], 3)
+        eng.predict_mlp_topk_host(mlp, Xf[:rows], 10, exact=False)
+mixed = np.concatenate([X[:4096].astype(np.float64), Xf[:3_001]])
+eng.predict_mlp_proba_host(mlp, mixed, chunk_rows=2048)
+for exact in (True, False):
+    eng.predict_mlp_topk_host(mlp, mixed, 3, exact=exact, chunk_rows=2048)
 print("sanitizer driver ok")

@@ -117,6 +117,15 @@ SIGNATURES = {
         C.c_int,
         [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, _P, C.c_int, C.c_int64, C.POINTER(Stats)],
     ),
+    "uml_mlp_predict_proba_host": (
+        C.c_int,
+        [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, _P, C.c_int64, C.POINTER(Stats)],
+    ),
+    "uml_mlp_predict_topk_host": (
+        C.c_int,
+        [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int, _P, C.c_int, C.c_int64,
+         C.POINTER(Stats)],
+    ),
     "uml_mlp_predict_host_begin": (
         C.c_int,
         [_P, _P, _P, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, _P, C.c_int, C.c_int64],

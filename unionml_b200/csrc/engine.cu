@@ -154,9 +154,10 @@ class CopyPool {
   bool stop_ = false;
 };
 
-struct SmallGraph {  // one captured small-batch kernel (linear or MLP) per (model, rows, features, dtype)
+struct SmallGraph {  // one captured small-batch kernel (linear or MLP) per (model, rows, features, dtype, output, k)
   uint64_t model_uid = 0;
   int n_rows = 0, n_features = 0, dtype = 0;
+  int kind = 0, k = 0;  // uml::SmallOutput and the top-k width: a model's labels, probabilities and top-k differ
   cudaGraphExec_t exec = nullptr;
   uint64_t last_use = 0;
 };
@@ -258,6 +259,11 @@ struct uml_mlp {
   uml_engine* e = nullptr;
   uint64_t uid = 0;  // keys the cached small-batch graphs (from the same counter as uml_model::uid)
   size_t small_smem = 0;  // dynamic shared memory of mlp_small_kernel; 0: too large, batches keep the chunk pipeline
+  size_t small_rec_smem = 0;  // ... of its probability / top-k forms (a logits strip more); 0: those keep the pipeline
+  // where those forms write their records: mapped pinned memory for kSmallRows x C x 8 bytes, allocated at the model's
+  // first such request and kept, so that the graphs captured with it stay valid
+  void* h_rec = nullptr;
+  void* d_rec = nullptr;
   uml::MlpDeviceModel dm{};
   float* d_w1t = nullptr;
   float* d_b1 = nullptr;
@@ -1456,15 +1462,44 @@ static bool host_sample_is_tf32(const void* host, const SrcLayout& L, int64_t n_
   return true;
 }
 
+using SmallLaunch = std::function<cudaError_t(const uml::SrcView&, int, cudaStream_t)>;
+
+// One chunk of host rows as the pipeline hands it to a score step
+struct Chunk {
+  float* x;          // the fp32 rows (staged and checked, unless the step reads the raw chunk)
+  int64_t ld, rows;
+  uml::SrcView src;  // the caller's own values as they crossed PCIe (a float64 chunk that travelled as fp32 was checked
+                     // lossless by the gather threads); rows already in the resident layout: x itself
+  std::function<bool()> tf32;  // a host-side guess at whether the rows are tf32 values (MLP kernel choice)
+};
+
+// What a call through the chunk pipeline computes: score(chunk, out, &launches, &path) enqueues it on e->stream and
+// writes chunk.rows x row_bytes to the device buffer `out`.  n_features / model: as for check_mode_features.
+struct ChunkStep {
+  int n_features;
+  const char* model;
+  int64_t row_bytes;
+  bool raw;  // reads chunk.src only: no staging kernel or finite scan (the float64 outputs check finiteness themselves)
+  std::function<int(const Chunk&, void*, int*, int*)> score;
+  std::function<int(int64_t)> prepare;  // optional, given chunk_rows once the pipeline's scratch exists
+  // the <= kSmallRows route, none without a kernel: the model uid that keys its graphs, and the classes it writes
+  // as float64 in place of the label (class values).  small_rec: the host view of the records the kernel writes in
+  // place of labels (row_bytes each; kind / k key its graphs), nullptr for labels
+  SmallLaunch small;
+  uint64_t small_uid = 0;
+  const double* classes = nullptr;
+  int n_classes = 0;
+  const void* small_rec = nullptr;
+  int small_kind = uml::kSmallLabels, small_k = 0;
+};
+
 // B <= kSmallRows: request block -> pinned (device-mapped) buffer -> one small-batch kernel (replayed as a CUDA graph)
 // -> labels written straight into pinned host memory.  The kernel scores in fp64 (linear_small_kernel from the
 // caller's own values, mlp_small_kernel from their fp32 cast), so the result is the exact-mode result for either mode.
-// `launch(view, rows, stream)` enqueues that kernel on the request block; model_uid keys its cached graphs.  out: the
-// int32 labels, or with classes, classes[label] as float64.
-using SmallLaunch = std::function<cudaError_t(const uml::SrcView&, int, cudaStream_t)>;
-static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaunch& launch, const void* host_ptr,
-                              int n_rows, int F, const SrcLayout& L, int src_dtype, void* out, const double* classes,
-                              int n_classes, uml_stats* stats) {
+// step.small(view, rows, stream) enqueues that kernel on the request block; step.small_uid keys its cached graphs.
+// out: the int32 labels, with step.classes classes[label] as float64, or with step.small_rec the kernel's records.
+static int predict_host_small(uml_engine* e, const ChunkStep& step, const void* host_ptr, int n_rows, int F,
+                              const SrcLayout& L, int src_dtype, void* out, uml_stats* stats) {
   NvtxRange r_all("uml:predict_host_small");
   const size_t width = (size_t)F * L.elem;
   const size_t bytes = width * (size_t)n_rows;
@@ -1501,13 +1536,16 @@ static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaun
     }
   }
   uml::SrcView view{e->d_req, src_dtype, (long long)F, 1};
-  auto enqueue = [&](cudaStream_t s) -> cudaError_t { return launch(view, n_rows, s); };
+  auto enqueue = [&](cudaStream_t s) -> cudaError_t { return step.small(view, n_rows, s); };
+  const uint64_t model_uid = step.small_uid;
   static const bool no_graph = getenv("UML_B200_NO_GRAPH") != nullptr;
   bool launched = false;
   if (e->small_graph_ok && !no_graph) {
     SmallGraph* hit = nullptr;
     for (auto& g : e->small_graphs)
-      if (g.model_uid == model_uid && g.n_rows == n_rows && g.n_features == F && g.dtype == src_dtype) hit = &g;
+      if (g.model_uid == model_uid && g.n_rows == n_rows && g.n_features == F && g.dtype == src_dtype &&
+          g.kind == step.small_kind && g.k == step.small_k)
+        hit = &g;
     if (!hit) {
       cudaGraph_t graph = nullptr;
       cudaGraphExec_t exec = nullptr;
@@ -1530,7 +1568,7 @@ static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaun
           cudaGraphExecDestroy(e->small_graphs[lru].exec);
           e->small_graphs.erase(e->small_graphs.begin() + (long)lru);
         }
-        e->small_graphs.push_back({model_uid, n_rows, F, src_dtype, exec, 0});
+        e->small_graphs.push_back({model_uid, n_rows, F, src_dtype, step.small_kind, step.small_k, exec, 0});
         hit = &e->small_graphs.back();
       }
     }
@@ -1543,10 +1581,14 @@ static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaun
   if (!launched) UML_CUDA(e, enqueue(e->stream));
   UML_CUDA(e, cudaStreamSynchronize(e->stream));
   int64_t n_bad = 0, n_amb = 0;
+  const double* classes = step.classes;
+  if (step.small_rec) memcpy(out, step.small_rec, (size_t)(n_rows * step.row_bytes));
   for (int r = 0; r < n_rows; ++r) {
     const uml::SmallResult& q = e->h->small[r];
-    if (classes) static_cast<double*>(out)[r] = (q.label >= 0 && q.label < n_classes) ? classes[q.label] : NAN;
-    else static_cast<int32_t*>(out)[r] = q.label;
+    if (!step.small_rec && classes)
+      static_cast<double*>(out)[r] = (q.label >= 0 && q.label < step.n_classes) ? classes[q.label] : NAN;
+    else if (!step.small_rec)
+      static_cast<int32_t*>(out)[r] = q.label;
     n_bad += q.status & 1;
     n_amb += (q.status >> 1) & 1;
   }
@@ -1557,37 +1599,11 @@ static int predict_host_small(uml_engine* e, uint64_t model_uid, const SmallLaun
     stats->kernel_launches = 1;
     stats->path = 4;
     stats->h2d_bytes = (int64_t)bytes;  // read by the kernel over PCIe (zero-copy), not by a copy engine
-    stats->d2h_bytes = (int64_t)sizeof(uml::SmallResult) * n_rows;
+    stats->d2h_bytes = (int64_t)sizeof(uml::SmallResult) * n_rows + (step.small_rec ? n_rows * step.row_bytes : 0);
   }
   if (n_bad > 0) UML_FAIL(e, UML_ERR_NONFINITE, "Input X contains NaN or infinity.");
   return UML_OK;
 }
-
-// One chunk of host rows as the pipeline hands it to a score step
-struct Chunk {
-  float* x;          // the fp32 rows (staged and checked, unless the step reads the raw chunk)
-  int64_t ld, rows;
-  uml::SrcView src;  // the caller's own values as they crossed PCIe (a float64 chunk that travelled as fp32 was checked
-                     // lossless by the gather threads); rows already in the resident layout: x itself
-  std::function<bool()> tf32;  // a host-side guess at whether the rows are tf32 values (MLP kernel choice)
-};
-
-// What a call through the chunk pipeline computes: score(chunk, out, &launches, &path) enqueues it on e->stream and
-// writes chunk.rows x row_bytes to the device buffer `out`.  n_features / model: as for check_mode_features.
-struct ChunkStep {
-  int n_features;
-  const char* model;
-  int64_t row_bytes;
-  bool raw;  // reads chunk.src only: no staging kernel or finite scan (the float64 outputs check finiteness themselves)
-  std::function<int(const Chunk&, void*, int*, int*)> score;
-  std::function<int(int64_t)> prepare;  // optional, given chunk_rows once the pipeline's scratch exists
-  // the <= kSmallRows route, none without a kernel: the model uid that keys its graphs, and the classes it writes
-  // as float64 in place of the label (class values)
-  SmallLaunch small;
-  uint64_t small_uid = 0;
-  const double* classes = nullptr;
-  int n_classes = 0;
-};
 
 // host rows -> `out` (host memory, n_rows x step.row_bytes) in chunks: gather / H2D on the copy stream, staging, the
 // step and the D2H on e->stream, three chunks in flight.  progress: the asynchronous call's published row count
@@ -1605,8 +1621,7 @@ static int predict_host_impl(uml_engine* e, const ChunkStep& step, const void* h
   if ((rc = classify_layout(e, n_rows, n_features, row_stride_bytes, col_stride_bytes, src_dtype, &L)) != UML_OK) return rc;
   const int F = n_features;
   if (step.small && n_rows <= kSmallRows && (int64_t)F * L.elem * n_rows <= kSmallBytes) {
-    rc = predict_host_small(e, step.small_uid, step.small, host_ptr, (int)n_rows, F, L, src_dtype, out, step.classes,
-                            step.n_classes, stats);
+    rc = predict_host_small(e, step, host_ptr, (int)n_rows, F, L, src_dtype, out, stats);
     if (progress && rc == UML_OK) progress->store(n_rows);
     return rc;
   }
@@ -1913,6 +1928,118 @@ static ChunkStep mlp_labels_step(uml_engine* e, const uml_mlp* m, int mode) {
   return s;
 }
 
+// The probability and top-k steps have no re-score that would find a finite float64 beyond the fp32 range (the staging
+// kernel checks the caller's values, and the fp32 cast of such a value is inf): a chunk that crossed PCIe as float64
+// has its fp32 rows scanned for NaN / Inf, as the reference's cast makes them.
+static int mlp_scan_f64_chunk(uml_engine* e, const uml_mlp* m, const Chunk& c, int* launches) {
+  if (c.src.dtype != UML_F64) return UML_OK;
+  UML_CUDA(e, uml::launch_finite_scan(c.x, c.ld, c.rows, m->dm.n_in, e->d_stage, e->stream));
+  *launches += 1;
+  return UML_OK;
+}
+
+// the <= kSmallRows form of a probability / top-k step: mlp_small_kernel's record form into the model's mapped buffer
+static void mlp_small_records(uml_engine* e, const uml_mlp* m, ChunkStep& s, int kind, int k) {
+  if (m->small_rec_smem == 0 || !m->h_rec) return;
+  s.small = [=](const uml::SrcView& v, int rows, cudaStream_t st) {
+    return uml::launch_mlp_small(m->dm, v, rows, e->d_small, m->small_rec_smem, st, kind, k, m->d_rec);
+  };
+  s.small_uid = m->uid;
+  s.small_rec = m->h_rec;
+  s.small_kind = kind;
+  s.small_k = k;
+}
+
+// class probabilities: the kernel mlp_route picks from the chunk's tf32 guess.  Behind the tensor cores, the float64
+// probabilities of the rows they flagged (not tf32 values) overwrite theirs.
+static ChunkStep mlp_proba_step(uml_engine* e, const uml_mlp* m) {
+  ChunkStep s{m->dm.n_in, "module", 4ll * m->dm.n_classes, false};
+  s.prepare = [=](int64_t chunk_rows) { return grow(e, e->d_flag_rows, chunk_rows); };
+  s.score = [=](const Chunk& c, void* out, int* launches, int* path) -> int {
+    int rc;
+    if ((rc = mlp_scan_f64_chunk(e, m, c, launches)) != UML_OK) return rc;
+    CUtensorMap map;
+    const bool has_map = encode_map(e, &map, c.x, c.rows, m->dm.n_in, c.ld) == UML_OK;
+    const int route = mlp_route(m->dm, has_map, true, c.tf32);
+    float* proba = static_cast<float*>(out);
+    const int sm = e->info.sm_count;
+    if (route == 5) {
+      uml::MlpTcLaunch o{};
+      o.n_rows = c.rows;
+      o.proba = proba;
+      UML_CUDA(e, uml::launch_mlp_tc_proba(map, m->dm, o, flag_list(e), sm, e->stream));
+      UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, c.x, c.ld, c.rows, proba, flag_list(e), false, sm, e->stream));
+      *launches += 2;
+    } else if (route == 3) {
+      UML_CUDA(e, uml::launch_mlp_tma(map, m->dm, c.x, c.rows, nullptr, false, {}, sm, e->stream, proba));
+      *launches += 1;
+    } else {
+      UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, c.x, c.ld, c.rows, proba, {}, true, sm, e->stream));
+      *launches += 1;
+    }
+    *path = route;
+    return UML_OK;
+  };
+  mlp_small_records(e, m, s, uml::kSmallProba, 0);
+  return s;
+}
+
+// top-k: routed as uml_mlp_predict_topk, with the chunk's tf32 guess.  Behind a tensor-core or EXACT launch, the float64
+// top-k of the flagged rows.  The kernels write [rows][k] index and probability planes to scratch; two strided copies
+// lay them into the pipeline's one output, a record of k int32 indices then k fp32 probabilities per row.
+static ChunkStep mlp_topk_step(uml_engine* e, const uml_mlp* m, int k, int mode) {
+  ChunkStep s{m->dm.n_in, "module", 8ll * k, false};
+  s.prepare = [=](int64_t chunk_rows) {
+    int rc;
+    if ((rc = grow(e, e->d_flag_rows, chunk_rows)) != UML_OK) return rc;
+    return grow(e, e->d_labels, 2 * k * chunk_rows);
+  };
+  s.score = [=](const Chunk& c, void* out, int* launches, int* path) -> int {
+    int rc;
+    if ((rc = mlp_scan_f64_chunk(e, m, c, launches)) != UML_OK) return rc;
+    const bool exact = mode == UML_PREDICT_EXACT;
+    CUtensorMap map;
+    int route = 2;
+    if (k <= uml::kMlpTopkMax) {
+      const bool has_map = encode_map(e, &map, c.x, c.rows, m->dm.n_in, c.ld) == UML_OK;
+      route = mlp_route(m->dm, has_map, false, c.tf32, true);
+    }
+    int32_t* idx = e->d_labels.p[0];
+    float* proba = reinterpret_cast<float*>(idx + k * c.rows);
+    const FlagList fl = flag_list(e);
+    const int sm = e->info.sm_count;
+    cudaStream_t st = e->stream;
+    if (route == 2) {
+      UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, c.x, c.ld, c.rows, k, idx, proba, fl, true, sm, st));
+      *launches += 1;
+    } else {
+      if (route == 5) {
+        uml::MlpTcLaunch o{};
+        o.n_rows = c.rows;
+        o.topk_idx = idx;
+        o.topk_proba = proba;
+        o.topk_k = k;
+        UML_CUDA(e, uml::launch_mlp_tc_topk(map, m->dm, o, exact, fl, sm, st));
+      } else {
+        UML_CUDA(e, uml::launch_mlp_tma_topk(map, m->dm, c.rows, k, idx, proba, exact, fl, sm, st));
+      }
+      *launches += 1;
+      if (exact || route == 5) {
+        UML_CUDA(e, uml::launch_mlp_topk_f64(m->dm, c.x, c.ld, c.rows, k, idx, proba, fl, false, sm, st));
+        *launches += 1;
+      }
+    }
+    const size_t plane = 4ull * k;
+    UML_CUDA(e, cudaMemcpy2DAsync(out, 2 * plane, idx, plane, plane, (size_t)c.rows, cudaMemcpyDeviceToDevice, st));
+    UML_CUDA(e, cudaMemcpy2DAsync(static_cast<char*>(out) + plane, 2 * plane, proba, plane, plane, (size_t)c.rows,
+                                  cudaMemcpyDeviceToDevice, st));
+    *path = route;
+    return UML_OK;
+  };
+  mlp_small_records(e, m, s, uml::kSmallTopk, k);
+  return s;
+}
+
 int uml_linear_predict_host(uml_engine* e, const uml_model* m, const void* host_ptr, int64_t n_rows, int n_features,
                             int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int32_t* labels_out,
                             int mode, int64_t chunk_rows, uml_stats* stats) {
@@ -1977,6 +2104,38 @@ int uml_mlp_predict_host_begin(uml_engine* e, const uml_mlp* m, const void* host
   if (!m) return UML_ERR_INVALID;
   return async_begin(e, mlp_labels_step(e, m, mode), host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes,
                      src_dtype, labels_out, mode, chunk_rows);
+}
+
+// the online route's record buffer of a model (uml_mlp::h_rec), made at its first request that can take the route
+static int mlp_reserve_records(uml_engine* e, const uml_mlp* m, int64_t n_rows) {
+  if (n_rows > kSmallRows || m->small_rec_smem == 0 || m->h_rec) return UML_OK;
+  uml_mlp* mm = const_cast<uml_mlp*>(m);  // the handle is logically const for the caller
+  UML_CUDA(e, cudaSetDevice(e->device));
+  UML_CUDA(e, cudaHostAlloc(&mm->h_rec, (size_t)kSmallRows * m->dm.n_classes * 8, cudaHostAllocMapped));
+  UML_CUDA(e, cudaHostGetDevicePointer(&mm->d_rec, mm->h_rec, 0));
+  return UML_OK;
+}
+
+int uml_mlp_predict_proba_host(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows, int n_features,
+                               int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, float* proba_out,
+                               int64_t chunk_rows, uml_stats* stats) {
+  if (!e || !m) return UML_ERR_INVALID;
+  int rc;
+  if ((rc = mlp_reserve_records(e, m, n_rows)) != UML_OK) return rc;
+  return predict_host_impl(e, mlp_proba_step(e, m), host_ptr, n_rows, n_features, row_stride_bytes, col_stride_bytes,
+                           src_dtype, proba_out, UML_PREDICT_FAST, chunk_rows, stats);
+}
+
+int uml_mlp_predict_topk_host(uml_engine* e, const uml_mlp* m, const void* host_ptr, int64_t n_rows, int n_features,
+                              int64_t row_stride_bytes, int64_t col_stride_bytes, int src_dtype, int k, int32_t* out,
+                              int mode, int64_t chunk_rows, uml_stats* stats) {
+  if (!e || !m) return UML_ERR_INVALID;
+  const int C = m->dm.n_classes;
+  if (k < 1 || k > C) UML_FAIL(e, UML_ERR_INVALID, "k = %d: the module has %d classes (need 1 <= k <= %d)", k, C, C);
+  int rc;
+  if ((rc = mlp_reserve_records(e, m, n_rows)) != UML_OK) return rc;
+  return predict_host_impl(e, mlp_topk_step(e, m, k, mode), host_ptr, n_rows, n_features, row_stride_bytes,
+                           col_stride_bytes, src_dtype, out, mode, chunk_rows, stats);
 }
 
 int uml_async_poll(uml_engine* e, int64_t* rows_done, int* finished) {
@@ -2174,7 +2333,9 @@ int uml_mlp_load(uml_engine* e, uml_mlp** out, const float* w1, const float* b1,
   m->uid = g_model_uid.fetch_add(1);
   // the online kernel's shared-memory limit is set here, not where its launch is captured into a graph
   m->small_smem = uml::mlp_small_smem_bytes(F, H, C);
-  if (m->small_smem > 0 && (ce = uml::mlp_small_reserve(m->small_smem)) != cudaSuccess) {
+  m->small_rec_smem = uml::mlp_small_smem_bytes(F, H, C, true);
+  if ((m->small_smem > 0 && (ce = uml::mlp_small_reserve(m->small_smem)) != cudaSuccess) ||
+      (m->small_rec_smem > 0 && (ce = uml::mlp_small_reserve(m->small_rec_smem, true)) != cudaSuccess)) {
     e->last_error = std::string("uml_mlp_load: ") + cudaGetErrorString(ce);
     uml_mlp_free(m);
     return UML_ERR_CUDA;
@@ -2192,6 +2353,7 @@ void uml_mlp_free(uml_mlp* m) {
   cudaFree(m->d_b2);
   cudaFree(m->d_w64);
   cudaFree(m->d_w1_tiles);
+  if (m->h_rec) cudaFreeHost(m->h_rec);  // no graph replays it: the graphs are keyed by this model's uid
   delete m;
 }
 
@@ -2265,12 +2427,13 @@ int uml_mlp_predict_proba(uml_engine* e, const uml_mlp* m, const uml_batch* b, f
       uml::MlpTcLaunch o{};
       o.n_rows = b->n_rows;
       o.proba = proba;
-      UML_CUDA(e, uml::launch_mlp_tc_proba(b->map, m->dm, o, e->info.sm_count, e->stream));
+      // (every row is a tf32 value, or mlp_route would not have picked the tensor cores: no flag list)
+      UML_CUDA(e, uml::launch_mlp_tc_proba(b->map, m->dm, o, {}, e->info.sm_count, e->stream));
     } else if (route == 3) {  // (no labels, so no flag list)
       UML_CUDA(e, uml::launch_mlp_tma(b->map, m->dm, b->x, b->n_rows, nullptr, false, {}, e->info.sm_count, e->stream,
                                       proba));
     } else {
-      UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, b->x, b->ld, b->n_rows, proba, e->info.sm_count, e->stream));
+      UML_CUDA(e, uml::launch_mlp_proba_f64(m->dm, b->x, b->ld, b->n_rows, proba, {}, true, e->info.sm_count, e->stream));
     }
     if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
     *launches = 1;
@@ -2314,7 +2477,9 @@ int uml_mlp_predict_topk(uml_engine* e, const uml_mlp* m, const uml_batch* b, in
       o.topk_idx = idx;
       o.topk_proba = proba;
       o.topk_k = k;
-      UML_CUDA(e, uml::launch_mlp_tc_topk(b->map, m->dm, o, exact, fl, sm, s));
+      // FAST: no flag list, so that no row waits for a float64 pass this call does not make (a batch routed here is
+      // all tf32 values, unless UML_B200_MLP_TC=1 forces the route)
+      UML_CUDA(e, uml::launch_mlp_tc_topk(b->map, m->dm, o, exact, exact ? fl : FlagList{}, sm, s));
     } else {
       UML_CUDA(e, uml::launch_mlp_tma_topk(b->map, m->dm, b->n_rows, k, idx, proba, exact, fl, sm, s));
     }

@@ -15,8 +15,10 @@
 //  * mlp_topk_f64_kernel: the fp64 top-k of those flagged rows, or of every row for shapes / k no tile kernel takes.
 //  * mlp_rescore_f64_kernel: warp per row, lane per hidden unit, fp64; flagged rows of EXACT mode, or every row for
 //    shapes the tile kernel is not instantiated for.
-//  * mlp_proba_f64_kernel: class probabilities for those shapes - the same fp64 scorer, then a float64 softmax.
-//  * mlp_small_kernel: the online path (B <= 64 rows): the same fp64 scorer on the request block in pinned host memory.
+//  * mlp_proba_f64_kernel: class probabilities for those shapes - the same fp64 scorer, then a float64 softmax - or
+//    for the rows a tensor-core PROBA launch flagged as not tf32 values.
+//  * mlp_small_kernel: the online path (B <= 64 rows): the same fp64 scorer on the request block in pinned host memory,
+//    writing labels, class probabilities or top-k records.
 //
 // This is CUDA-core fp32 (FFMA): 4 736 flop/row puts the HBM roofline (25 G rows/s) above the FFMA peak, so this kernel
 // is FMA-pipe bound (~0.66 ms per 10M rows at 1.9 GHz).  It serves batches whose features are NOT tf32 values (general
@@ -387,9 +389,51 @@ __global__ void __launch_bounds__(256) mlp_rescore_f64_kernel(const MlpRescorePa
   flag_list_hand_back(p);
 }
 
-// class probabilities for shapes no tile kernel takes: the logits of the fp64 scorer above (mlp_rs_rows), a float64
-// softmax, each probability rounded once to fp32.  A warp scores kMlpRsRows consecutive rows per pass; lane per class,
-// so each row's C floats leave as consecutive stores.
+// One row's float64 outputs from the logits a pass of the fp64 scorer left in its strip (logit c at zr[c R]): the
+// softmax (max, exp(z - m), lane sum, true division), each probability rounded once to fp32, and for top-k each class's
+// rank in the stable descending order (the logits above it, and equal logits of lower index) - no sort, any k <= C.
+// proba: the row's C probabilities by class, or nullptr.  k > 0: idx / kproba receive slot `rank` of a class of rank < k
+// (kproba may be nullptr).  Returns, in every lane, whether a consecutive gap among ranks 0 .. min(k, C - 1) is within
+// twice err (the labels' top-2 margin rule).  Every float64 probability and top-k of the MLP leaves through this one
+// routine (mlp_proba_f64_kernel, mlp_topk_f64_kernel, mlp_small_kernel), so their bits agree by construction.
+__device__ __noinline__ bool mlp_f64_row_outputs(const double* zr, int R, int C, int lane, float* proba, int k,
+                                                 int32_t* idx, float* kproba, double err) {
+  double m = -INFINITY;
+  for (int c = lane; c < C; c += 32) m = fmax(m, zr[c * R]);
+  m = warp_max(m, 1);
+  double s = 0.0;
+  for (int c = lane; c < C; c += 32) s += exp(zr[c * R] - m);
+  s = warp_sum(s);
+  const int kk = min(k, C - 1);
+  bool ambiguous = false;
+  for (int c = lane; c < C; c += 32) {
+    const double zc = zr[c * R];
+    const float pc = proba || kproba ? static_cast<float>(exp(zc - m) / s) : 0.f;
+    if (proba) proba[c] = pc;
+    if (k > 0) {
+      int rank = 0;
+      double above = INFINITY;  // the smallest logit ranked above c: its neighbour one rank up
+      for (int o = 0; o < C; ++o) {
+        const double zo = zr[o * R];
+        if (zo > zc || (zo == zc && o < c)) {
+          ++rank;
+          above = fmin(above, zo);
+        }
+      }
+      if (rank < k) {
+        idx[rank] = c;
+        if (kproba) kproba[rank] = pc;
+      }
+      if (rank >= 1 && rank <= kk && !((above - zc) > 2.0 * err)) ambiguous = true;
+    }
+  }
+  return __any_sync(0xffffffffu, ambiguous);
+}
+
+// class probabilities for shapes no tile kernel takes: the logits of the fp64 scorer above (mlp_rs_rows), then
+// mlp_f64_row_outputs.  A warp scores kMlpRsRows rows per pass; lane per class, so each row's C floats leave as
+// consecutive stores.  Every row (all_rows), or the rows on the flag list: those the tensor-core PROBA kernel in front of
+// this launch scored from features that are not tf32 values, whose probabilities this overwrites.
 struct MlpProbaF64Params {
   const float* x;
   long long ld;
@@ -397,6 +441,11 @@ struct MlpProbaF64Params {
   const double* pack;
   int F, H, C;
   float* proba;
+  const int* flag_count;
+  const int32_t* flag_rows;
+  int flag_cap;
+  int all_rows;
+  unsigned long long* counters;
 };
 
 __global__ void __launch_bounds__(256) mlp_proba_f64_kernel(const MlpProbaF64Params p) {
@@ -410,33 +459,33 @@ __global__ void __launch_bounds__(256) mlp_proba_f64_kernel(const MlpProbaF64Par
   __syncthreads();
   mlp_rs_finish_stage(view);
 
+  pdl_wait_for_predecessor();  // flagged mode: the flag list and outputs of the tile kernel this launch depends on
   const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps_total = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
-  for (long long i = warp_global * R; i < p.n_rows; i += warps_total * R) {
+  const long long n = flag_list_rows(p);
+  for (long long i = warp_global * R; i < n; i += warps_total * R) {
+    long long row[R];
     const float* xr[R];
 #pragma unroll
-    for (int r = 0; r < R; ++r) xr[r] = p.x + (i + r < p.n_rows ? i + r : i) * p.ld;  // unused slots repeat row i
+    for (int r = 0; r < R; ++r) {
+      const long long j = i + r < n ? i + r : i;  // unused slots repeat the first row (result ignored)
+      row[r] = p.all_rows ? j : static_cast<long long>(p.flag_rows[j]);
+      xr[r] = p.x + row[r] * p.ld;
+    }
     MlpRowResult res[R];
     mlp_rs_rows<R, true>(view, xr, xs, hv, lane, res, zs);
-    for (int r = 0; r < R && i + r < p.n_rows; ++r) {
-      double m = -INFINITY;
-      for (int c = lane; c < p.C; c += 32) m = fmax(m, zs[c * R + r]);
-      m = warp_max(m, 1);
-      double s = 0.0;
-      for (int c = lane; c < p.C; c += 32) s += exp(zs[c * R + r] - m);
-      s = warp_sum(s);
-      float* out = p.proba + (i + r) * p.C;
-      for (int c = lane; c < p.C; c += 32) out[c] = static_cast<float>(exp(zs[c * R + r] - m) / s);
+    for (int r = 0; r < R && i + r < n; ++r) {
+      mlp_f64_row_outputs(zs + r, R, p.C, lane, p.proba + row[r] * p.C, 0, nullptr, nullptr, 0.0);
+      if (!p.all_rows && lane == 0) count_rescored_row(p, res[r].bad, false);
     }
     __syncwarp();  // the strip is rewritten by the next pass
   }
+  if (!p.all_rows) flag_list_hand_back(p);
 }
 
-// top-k of the float64 network: the flagged rows of a TOPK tile kernel in EXACT mode, or every row for a shape or k no
-// tile kernel takes.  The fp64 scorer above (logits kept), then per row and lane per class: the class's rank in the
-// stable descending order (the logits above it, and equal logits of lower index) - no sort, any k <= C.  A class of
-// rank r < k writes slot r of its row's indices and, when requested, the float64 softmax of mlp_proba_f64_kernel
-// rounded once to fp32.  A row where a consecutive gap among ranks 0 .. min(k, C - 1) is within twice the fp64 logit
+// top-k of the float64 network: the flagged rows of a TOPK tile kernel (EXACT mode, or rows that are not tf32 values),
+// or every row for a shape or k no tile kernel takes.  The fp64 scorer above (logits and their bound kept), then
+// mlp_f64_row_outputs: a row where a consecutive gap among ranks 0 .. min(k, C - 1) is within twice the fp64 logit
 // bound counts as ambiguous, as the labels' top-2 margin does.
 struct MlpTopkF64Params {
   const float* x;
@@ -469,7 +518,7 @@ __global__ void __launch_bounds__(256) mlp_topk_f64_kernel(const MlpTopkF64Param
   const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long warps_total = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
   const long long n = flag_list_rows(p);
-  const int C = p.C, k = p.k, kk = min(p.k, p.C - 1);
+  const int k = p.k;
   for (long long i = warp_global * R; i < n; i += warps_total * R) {
     long long row[R];
     const float* xr[R];
@@ -483,34 +532,9 @@ __global__ void __launch_bounds__(256) mlp_topk_f64_kernel(const MlpTopkF64Param
     double err[R];
     mlp_rs_rows<R, true, true>(view, xr, xs, hv, lane, res, zs, err);
     for (int r = 0; r < R && i + r < n; ++r) {
-      const double* zr = zs + r;  // logit c at zr[c R]
-      const long long out_row = p.all_rows ? i + r : static_cast<long long>(p.flag_rows[i + r]);
-      double m = -INFINITY;
-      for (int c = lane; c < C; c += 32) m = fmax(m, zr[c * R]);
-      m = warp_max(m, 1);
-      double s = 0.0;
-      for (int c = lane; c < C; c += 32) s += exp(zr[c * R] - m);
-      s = warp_sum(s);
-      bool ambiguous = false;
-      for (int c = lane; c < C; c += 32) {
-        const double zc = zr[c * R];
-        int rank = 0;
-        double above = INFINITY;  // the smallest logit ranked above c: its neighbour one rank up
-        for (int o = 0; o < C; ++o) {
-          const double zo = zr[o * R];
-          if (zo > zc || (zo == zc && o < c)) {
-            ++rank;
-            above = fmin(above, zo);
-          }
-        }
-        if (rank < k) {
-          const long long at = out_row * k + rank;
-          p.idx[at] = c;
-          if (p.proba) p.proba[at] = static_cast<float>(exp(zc - m) / s);
-        }
-        if (rank >= 1 && rank <= kk && !((above - zc) > 2.0 * err[r])) ambiguous = true;
-      }
-      ambiguous = __any_sync(0xffffffffu, ambiguous);
+      const long long at = (p.all_rows ? i + r : static_cast<long long>(p.flag_rows[i + r])) * k;
+      const bool ambiguous = mlp_f64_row_outputs(zs + r, R, p.C, lane, nullptr, k, p.idx + at,
+                                                 p.proba ? p.proba + at : nullptr, err[r]);
       if (lane == 0) count_rescored_row(p, res[r].bad, ambiguous);
     }
     __syncwarp();  // the strip is rewritten by the next pass
@@ -523,6 +547,9 @@ __global__ void __launch_bounds__(256) mlp_topk_f64_kernel(const MlpTopkF64Param
 // guard, exact by construction.  Each warp casts its four rows to fp32 as the staging kernels do (convert_one: the
 // value as double, then to float), so this route scores the same fp32 features as the chunk pipeline and as the
 // reference predictor (`torch.from_numpy(values).float()`), into an fp32 strip in its own shared memory.
+// OUT (kSmallLabels / kSmallProba / kSmallTopk): what it writes besides each row's status - the label, or through
+// mlp_f64_row_outputs the row's record in p.rec: C fp32 probabilities, or k int32 class indices then their k fp32
+// probabilities.  The record forms keep the pass's logits in a further C x 4 doubles of the warp's strip.
 struct MlpSmallParams {
   SrcView src;
   int n_rows;
@@ -531,13 +558,22 @@ struct MlpSmallParams {
   SmallResult* out;
 };
 
-__global__ void __launch_bounds__(256) mlp_small_kernel(const MlpSmallParams p) {
+struct MlpSmallRecParams : MlpSmallParams {
+  void* rec;  // [n_rows][C] fp32, or [n_rows][2k] words
+  int k;
+};
+
+template <int OUT, class Params>
+__global__ void __launch_bounds__(256) mlp_small_kernel(const Params p) {
   extern __shared__ __align__(16) double rs_smem[];
   constexpr int R = kMlpRsRows;
+  constexpr bool kRec = OUT != kSmallLabels;
   MlpRsView view = mlp_rs_stage(rs_smem, p.pack, p.F, p.H, p.C);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  // per warp: the scorer's strip, then the four rows as fp32 (F x R doubles hold 2 F x R floats: room to spare)
-  double* xs = rs_smem + mlp_rs_weight_doubles(p.F, p.H, p.C) + warp * (mlp_rs_strip_doubles(p.F, p.H, R) + 2 * p.F);
+  // per warp: the scorer's strip, then the four rows as fp32 (F x R doubles hold 2 F x R floats: room to spare), then
+  // (records) the logits
+  double* xs = rs_smem + mlp_rs_weight_doubles(p.F, p.H, p.C) +
+               warp * (mlp_rs_strip_doubles(p.F, p.H, R) + 2 * p.F + (kRec ? p.C * R : 0));
   double* hv = xs + p.F * R;
   float* x32 = reinterpret_cast<float*>(hv + p.H * R);
   __syncthreads();
@@ -567,38 +603,67 @@ __global__ void __launch_bounds__(256) mlp_small_kernel(const MlpSmallParams p) 
   for (int r = 0; r < R; ++r) xr[r] = x32 + r * p.F;
   __syncwarp();
   MlpRowResult res[R];
-  mlp_rs_rows<R>(view, xr, xs, hv, lane, res);
+  if constexpr (!kRec) {
+    mlp_rs_rows<R>(view, xr, xs, hv, lane, res);
+  } else {
+    double* zs = xs + mlp_rs_strip_doubles(p.F, p.H, R) + 2 * p.F;  // the pass's logits, [c][R]
+    double err[R];
+    mlp_rs_rows<R, true, true>(view, xr, xs, hv, lane, res, zs, err);
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (i + r >= p.n_rows) continue;  // (unrolled: res[] stays in registers)
+      if constexpr (OUT == kSmallProba) {
+        mlp_f64_row_outputs(zs + r, R, p.C, lane, static_cast<float*>(p.rec) + static_cast<long long>(i + r) * p.C, 0,
+                            nullptr, nullptr, 0.0);
+      } else {
+        int32_t* at = static_cast<int32_t*>(p.rec) + static_cast<long long>(i + r) * 2 * p.k;
+        // top-k rows are ambiguous by the rank rule of mlp_topk_f64_kernel, not by the labels' top-2 margin
+        res[r].ambiguous = mlp_f64_row_outputs(zs + r, R, p.C, lane, nullptr, p.k, at, reinterpret_cast<float*>(at + p.k),
+                                               err[r]);
+      }
+    }
+  }
   if (lane < R && i + lane < p.n_rows) {
     MlpRowResult mine = res[0];
 #pragma unroll
     for (int r = 1; r < R; ++r)
       if (lane == r) mine = res[r];
     p.out[i + lane].label = mine.idx;
-    p.out[i + lane].status = (mine.bad ? 1 : 0) | (mine.ambiguous ? 2 : 0);
+    // (probabilities have no ranks to be ambiguous about)
+    p.out[i + lane].status = (mine.bad ? 1 : 0) | (mine.ambiguous && OUT != kSmallProba ? 2 : 0);
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-size_t mlp_small_smem_bytes(int n_in, int n_hidden, int n_classes) {
-  const size_t per_warp = mlp_rs_strip_doubles(n_in, n_hidden, kMlpRsRows) + 2 * static_cast<size_t>(n_in);
+size_t mlp_small_smem_bytes(int n_in, int n_hidden, int n_classes, bool records) {
+  const size_t per_warp = mlp_rs_strip_doubles(n_in, n_hidden, kMlpRsRows) + 2 * static_cast<size_t>(n_in) +
+                          (records ? static_cast<size_t>(n_classes) * kMlpRsRows : 0);
   const size_t smem = (mlp_rs_weight_doubles(n_in, n_hidden, n_classes) + 8 * per_warp) * sizeof(double);
   return smem > static_cast<size_t>(kMaxSmemBytes) ? 0 : smem;
 }
 
-cudaError_t mlp_small_reserve(size_t smem) {
+template <int OUT, class Params>
+static cudaError_t mlp_small_reserve_one(size_t smem) {
   static size_t configured = 0;
   if (smem <= configured) return cudaSuccess;
-  cudaError_t err = cudaFuncSetAttribute(mlp_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  cudaError_t err = cudaFuncSetAttribute(mlp_small_kernel<OUT, Params>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         static_cast<int>(smem));
   if (err == cudaSuccess) configured = smem;
   return err;
 }
 
+cudaError_t mlp_small_reserve(size_t smem, bool records) {
+  if (!records) return mlp_small_reserve_one<kSmallLabels, MlpSmallParams>(smem);
+  const cudaError_t err = mlp_small_reserve_one<kSmallProba, MlpSmallRecParams>(smem);
+  return err != cudaSuccess ? err : mlp_small_reserve_one<kSmallTopk, MlpSmallRecParams>(smem);
+}
+
 cudaError_t launch_mlp_small(const MlpDeviceModel& m, const SrcView& src, int n_rows, SmallResult* out, size_t smem,
-                             cudaStream_t stream) {
+                             cudaStream_t stream, int kind, int k, void* rec) {
   if (n_rows <= 0) return cudaSuccess;
-  MlpSmallParams p{};
+  MlpSmallRecParams p{};
   p.src = src;
   p.n_rows = n_rows;
   p.pack = m.rs_pack;
@@ -606,8 +671,13 @@ cudaError_t launch_mlp_small(const MlpDeviceModel& m, const SrcView& src, int n_
   p.H = m.n_hidden;
   p.C = m.n_classes;
   p.out = out;
+  p.rec = rec;
+  p.k = k;
   constexpr int rows_per_block = 8 * kMlpRsRows;
-  mlp_small_kernel<<<(n_rows + rows_per_block - 1) / rows_per_block, 256, smem, stream>>>(p);
+  const int grid = (n_rows + rows_per_block - 1) / rows_per_block;
+  if (kind == kSmallProba) mlp_small_kernel<kSmallProba><<<grid, 256, smem, stream>>>(p);
+  else if (kind == kSmallTopk) mlp_small_kernel<kSmallTopk><<<grid, 256, smem, stream>>>(p);
+  else mlp_small_kernel<kSmallLabels><<<grid, 256, smem, stream>>>(static_cast<const MlpSmallParams&>(p));
   return cudaGetLastError();
 }
 
@@ -751,7 +821,7 @@ cudaError_t launch_mlp_rescore_f64(const MlpDeviceModel& m, const float* x, int6
 }
 
 cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, float* proba,
-                                 int sm_count, cudaStream_t stream) {
+                                 const FlagList& flags, bool all_rows, int sm_count, cudaStream_t stream) {
   if (n_rows <= 0) return cudaSuccess;
   MlpProbaF64Params p{};
   p.x = x;
@@ -762,6 +832,11 @@ cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_
   p.H = m.n_hidden;
   p.C = m.n_classes;
   p.proba = proba;
+  p.flag_count = flags.count;
+  p.flag_rows = flags.rows;
+  p.flag_cap = flags.capacity;
+  p.all_rows = all_rows ? 1 : 0;
+  p.counters = flags.counters;
   // the re-score kernel's shared memory plus C x kMlpRsRows logits per warp
   const size_t strip = mlp_rs_strip_doubles(m.n_in, m.n_hidden, kMlpRsRows) + static_cast<size_t>(m.n_classes) * kMlpRsRows;
   const size_t smem = (mlp_rs_weight_doubles(m.n_in, m.n_hidden, m.n_classes) + 8 * strip) * sizeof(double);
@@ -774,8 +849,14 @@ cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_
   }
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mlp_proba_f64_kernel, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  const long long blocks = std::min<long long>(static_cast<long long>(sm_count) * per_sm, (n_rows + 8 * kMlpRsRows - 1) / (8 * kMlpRsRows));
-  mlp_proba_f64_kernel<<<static_cast<int>(std::max<long long>(1, blocks)), 256, smem, stream>>>(p);
+  long long blocks = static_cast<long long>(sm_count) * per_sm;  // persistent: every resident warp loops over rows
+  if (all_rows) {
+    blocks = std::min<long long>(blocks, (n_rows + 8 * kMlpRsRows - 1) / (8 * kMlpRsRows));
+    mlp_proba_f64_kernel<<<static_cast<int>(std::max<long long>(1, blocks)), 256, smem, stream>>>(p);
+    return cudaGetLastError();
+  }
+  cudaError_t lerr = launch_dependent(mlp_proba_f64_kernel, static_cast<int>(std::max<long long>(1, blocks)), 256, smem, stream, p);
+  if (lerr != cudaSuccess) return lerr;
   return cudaGetLastError();
 }
 

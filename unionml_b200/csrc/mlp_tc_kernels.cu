@@ -12,7 +12,9 @@
 //   * X: this kernel is dispatched for batches whose features ARE tf32 values (low 13 mantissa bits zero - integer /
 //     pixel domains such as the reference's digits and MNIST frames; the staging pass records it).  Every row is
 //     re-checked here (scan warps OR the low bits): a row that is not tf32-exact gets A1 = +inf and is therefore
-//     flagged for the fp64 re-score, so the answer is right for any input - only slower.
+//     flagged for the fp64 re-score, so the answer is right for any input - only slower.  The PROBA form, and the
+//     TOPK form in FAST mode, flag such rows too when the launch has a flag list (the chunk pipeline, whose kernel
+//     choice is a guess from the first rows), and the float64 kernels behind them overwrite those rows.
 //   * W1: split on the host as w = hi + lo + r with hi, lo tf32 (round to nearest) and |r| <= 2^-22 |w|; B holds
 //     [hi | lo] as 2H columns, so ONE MMA per K step yields main = x.hi and small = x.lo in separate accumulator
 //     columns (the small terms never lose bits against the large accumulator), summed in fp32 in the epilogue.
@@ -84,7 +86,9 @@ struct MlpTcParams {
 // (l / 4) holds rows 16 wq + l / 4 (+ 8) of both 64-row halves, and lane l % 4 keeps the (half, +8) pair it names
 __device__ __forceinline__ int tc_row_of_lane(int wq, int l) { return 64 * ((l & 3) >> 1) + 16 * wq + (l >> 2) + 8 * (l & 1); }
 
-template <int H, int C, bool EXACT, bool PROBA, bool TOPK = false>
+// FLAG_TF32 (PROBA, and TOPK in FAST mode): rows that are not tf32 values go onto the flag list (a template argument,
+// not a runtime test of the list: the forms without it keep their code and their measured time)
+template <int H, int C, bool EXACT, bool PROBA, bool TOPK = false, bool FLAG_TF32 = false>
 __global__ void __launch_bounds__(kTcRegBudgetThreads, 1)
 mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ MlpTcParams<H, C> p) {
   constexpr int N = 2 * H;     // accumulator columns per row: [main | small]
@@ -284,6 +288,12 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
         for (int h = 0; h < 2; ++h)
           mlp_proba_store_run<C, 16>(strip + 16 * h * C, p.proba, tile * kTileRows + 64 * h + 16 * wq, p.n_rows, lane);
         __syncwarp();  // the strip is rewritten by this warp's next tile
+        // given a flag list: a row that is not a tf32 value (A1 = +inf) was scored from truncated features, and the
+        // float64 probabilities behind this launch replace its values
+        if constexpr (FLAG_TF32) {
+          const long long row = tile * kTileRows + row_in_tile;
+          flag_rows_warp(row < p.n_rows && isinf(a1), row, p, lane);
+        }
         continue;
       }
       if constexpr (TOPK) {
@@ -325,6 +335,10 @@ mlp_argmax_tc_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
           const float err = p.e1_scale * a1 + p.e2_scale * z[C];
           const bool certain = mlp_topk_certain<M>(v, min(k, C - 1), 2.0f * err);
           flag_rows_warp(row < p.n_rows && !certain, row, p, lane);
+        }
+        if constexpr (!EXACT && FLAG_TF32) {  // only the rows that are not tf32 values (EXACT flags them through err = inf)
+          const long long row = tile * kTileRows + row_in_tile;
+          flag_rows_warp(row < p.n_rows && isinf(a1), row, p, lane);
         }
         continue;
       }
@@ -424,7 +438,7 @@ bool mlp_tc_supported(const MlpDeviceModel& m, std::string* why, bool topk) {
   return mlp_tc_fixed_smem(m, false, topk) + 6 * static_cast<size_t>(kStageBytes) <= static_cast<size_t>(kMaxSmemBytes);
 }
 
-template <int H, int C, bool EXACT, bool PROBA = false, bool TOPK = false>
+template <int H, int C, bool EXACT, bool PROBA = false, bool TOPK = false, bool FLAG_TF32 = false>
 static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l,
                                      const FlagList& flags, int sm_count, cudaStream_t stream) {
   using Params = MlpTcParams<H, C>;
@@ -486,7 +500,7 @@ static cudaError_t mlp_tc_launch_one(const CUtensorMap& xmap, const MlpDeviceMod
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
   const size_t smem = fixed + static_cast<size_t>(stages) * kStageBytes;
-  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, PROBA, TOPK>;
+  auto kern = mlp_argmax_tc_kernel<H, C, EXACT, PROBA, TOPK, FLAG_TF32>;
   static size_t configured = 0;
   if (smem > configured) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -510,12 +524,13 @@ cudaError_t launch_mlp_tc(const CUtensorMap& xmap, const MlpDeviceModel& m, cons
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, int sm_count,
-                                cudaStream_t stream) {
+cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l,
+                                const FlagList& flags, int sm_count, cudaStream_t stream) {
   if (l.n_rows <= 0) return cudaSuccess;
-  const FlagList none{};
-#define UML_TC_CASE(HH, CC) \
-  if (m.n_hidden == HH && m.n_classes == CC) return mlp_tc_launch_one<HH, CC, false, true>(xmap, m, l, none, sm_count, stream);
+#define UML_TC_CASE(HH, CC)                                                                                  \
+  if (m.n_hidden == HH && m.n_classes == CC)                                                                 \
+    return flags.count ? mlp_tc_launch_one<HH, CC, false, true, false, true>(xmap, m, l, flags, sm_count, stream) \
+                       : mlp_tc_launch_one<HH, CC, false, true>(xmap, m, l, flags, sm_count, stream);
   UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
 #undef UML_TC_CASE
   return cudaErrorInvalidValue;
@@ -527,8 +542,9 @@ cudaError_t launch_mlp_tc_topk(const CUtensorMap& xmap, const MlpDeviceModel& m,
   if (l.topk_k < 1 || l.topk_k > std::min(m.n_classes, kMlpTopkMax)) return cudaErrorInvalidValue;
 #define UML_TC_CASE(HH, CC)                                                                                  \
   if (m.n_hidden == HH && m.n_classes == CC)                                                                 \
-    return exact ? mlp_tc_launch_one<HH, CC, true, false, true>(xmap, m, l, flags, sm_count, stream)         \
-                 : mlp_tc_launch_one<HH, CC, false, false, true>(xmap, m, l, flags, sm_count, stream);
+    return exact         ? mlp_tc_launch_one<HH, CC, true, false, true>(xmap, m, l, flags, sm_count, stream)        \
+           : flags.count ? mlp_tc_launch_one<HH, CC, false, false, true, true>(xmap, m, l, flags, sm_count, stream) \
+                         : mlp_tc_launch_one<HH, CC, false, false, true>(xmap, m, l, flags, sm_count, stream);
   UML_TC_CASE(32, 10) UML_TC_CASE(32, 2) UML_TC_CASE(32, 3) UML_TC_CASE(16, 10) UML_TC_CASE(16, 2) UML_TC_CASE(16, 3)
 #undef UML_TC_CASE
   return cudaErrorInvalidValue;

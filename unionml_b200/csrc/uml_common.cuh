@@ -264,14 +264,17 @@ std::vector<float> mlp_tc_build_w1_tiles(const float* w1, int H, int F, int f_pa
 cudaError_t launch_mlp_tc(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
                           const FlagList& flags, int sm_count, cudaStream_t stream);
 // class probabilities softmax(logits) of every row into l.proba: tensor-core kernel (rows that are tf32 values), and
-// the fp64 scorer with a float64 softmax for shapes no tile kernel takes
-cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, int sm_count,
-                                cudaStream_t stream);
+// the fp64 scorer with a float64 softmax for shapes no tile kernel takes (all_rows).  Given a flag list, the
+// tensor-core kernel puts the rows that are not tf32 values on it, and launch_mlp_proba_f64 without all_rows behind it
+// overwrites their probabilities with the float64 route's.  No flag list: the caller knows every row is a tf32 value.
+cudaError_t launch_mlp_tc_proba(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l,
+                                const FlagList& flags, int sm_count, cudaStream_t stream);
 cudaError_t launch_mlp_proba_f64(const MlpDeviceModel& m, const float* x, int64_t ld, int64_t n_rows, float* proba,
-                                 int sm_count, cudaStream_t stream);
+                                 const FlagList& flags, bool all_rows, int sm_count, cudaStream_t stream);
 // top-k class indices [n_rows][k] (and probabilities, proba != nullptr) of every row, 1 <= k <= min(C, kMlpTopkMax):
 // the tile kernels' top-k forms.  exact: rows the rank guard cannot certify go to the flag list; the caller launches
-// launch_mlp_topk_f64 (all_rows = false) behind them.  launch_mlp_topk_f64 with all_rows: any shape and any k <= C.
+// launch_mlp_topk_f64 (all_rows = false) behind them.  The tensor-core form in FAST mode, given a flag list, puts the
+// rows that are not tf32 values on it (no flag list: the caller knows there are none).  launch_mlp_topk_f64 with all_rows: any shape and any k <= C.
 cudaError_t launch_mlp_tc_topk(const CUtensorMap& xmap, const MlpDeviceModel& m, const MlpTcLaunch& l, bool exact,
                                const FlagList& flags, int sm_count, cudaStream_t stream);
 cudaError_t launch_mlp_tma_topk(const CUtensorMap& xmap, const MlpDeviceModel& m, int64_t n_rows, int k, int32_t* idx,
@@ -285,11 +288,15 @@ cudaError_t launch_topk_first_hits(const int32_t* idx, int k, int64_t n, const d
 // small-batch kernel of the online path (B <= 64): four rows per warp through the fp64 scorer, the features read
 // straight from the raw source view and cast to fp32 as the staging kernels cast them.  mlp_small_smem_bytes: its
 // dynamic shared memory for the model's shape, 0 when that exceeds one SM; mlp_small_reserve sets the kernel's
-// shared-memory limit (call it before a launch is captured into a graph)
-size_t mlp_small_smem_bytes(int n_in, int n_hidden, int n_classes);
-cudaError_t mlp_small_reserve(size_t smem);
+// shared-memory limit (call it before a launch is captured into a graph).  kind: kSmallLabels writes out[].label;
+// kSmallProba / kSmallTopk also write one record per row to rec (C fp32 probabilities, or k int32 class indices then
+// their k fp32 probabilities), from the float64 softmax and ranks of mlp_topk_f64_kernel, and need the larger shared
+// memory of records = true.  Every kind writes out[].status; top-k sets its bit 1 by the rank rule of that kernel.
+enum SmallOutput { kSmallLabels = 0, kSmallProba = 1, kSmallTopk = 2 };
+size_t mlp_small_smem_bytes(int n_in, int n_hidden, int n_classes, bool records = false);
+cudaError_t mlp_small_reserve(size_t smem, bool records = false);
 cudaError_t launch_mlp_small(const MlpDeviceModel& m, const SrcView& src, int n_rows, SmallResult* out, size_t smem,
-                             cudaStream_t stream);
+                             cudaStream_t stream, int kind = kSmallLabels, int k = 0, void* rec = nullptr);
 // int32 labels (device) -> every target vector of a fused exchange (int32 or uint8 wire), for kernels without peer stores
 cudaError_t launch_labels_scatter(const int32_t* labels, int64_t n, const LabelTargets& out, int sm_count,
                                   cudaStream_t stream);

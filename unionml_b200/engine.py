@@ -483,6 +483,28 @@ class Engine:
                                    _mode(exact), chunk_rows)
         return out, stats
 
+    def predict_mlp_proba_host(self, model: MlpModel, features: Any, chunk_rows: int = 0) -> Tuple[np.ndarray, dict]:
+        """Host rows -> :meth:`predict_mlp_proba`'s class probabilities ``(n_rows, n_classes)`` fp32.  Larger batches
+        take the chunk pipeline (the resident call's bits when every row, or no row, is a tf32 value; otherwise rows
+        that are not tf32 values get the float64 route's values); up to 64 rows the online route of
+        :meth:`predict_mlp_host` (the float64 route's values, stats ``path`` 4)."""
+        arr, rows = self._host_rows(features)
+        out = np.empty((arr.shape[0], model.n_classes), dtype=np.float32)
+        stats = self._predict_rows(N.lib().uml_mlp_predict_proba_host, model, rows, out.ctypes.data_as(C.c_void_p),
+                                   chunk_rows)
+        return out, stats
+
+    def predict_mlp_topk_host(self, model: MlpModel, features: Any, k: int, exact: bool = True,
+                              chunk_rows: int = 0) -> Tuple[np.ndarray, np.ndarray, dict]:
+        """Host rows -> :meth:`predict_mlp_topk`'s ``(indices int32 (n, k), probabilities float32 (n, k), stats)``,
+        through the routes of :meth:`predict_mlp_proba_host` (up to 64 rows: the float64 ranks in either mode)."""
+        arr, rows = self._host_rows(features)
+        k = int(k)
+        rec = np.empty((arr.shape[0], 2 * max(k, 0)), dtype=np.int32)  # per row: k indices, then k fp32 probabilities
+        stats = self._predict_rows(N.lib().uml_mlp_predict_topk_host, model, rows, k, rec.ctypes.data_as(C.c_void_p),
+                                   _mode(exact), chunk_rows)
+        return rec[:, :k].copy(), rec[:, k:].view(np.float32).copy(), stats
+
     def predict_host_list(self, model, features: Any, table: list, exact: bool = True, chunk_rows: int = 0,
                           asynchronous: Optional[bool] = None) -> Tuple[list, dict]:
         """The predictor contract in one call: host rows -> ``[table[label] for label in labels]`` as a Python list.

@@ -390,17 +390,14 @@ def mlp_predict_proba(module: Any, features: Any) -> np.ndarray:
     """``module(process_features(features))`` of the torch quickstart on the GPU: class probabilities, an
     ``(n_rows, n_out)`` float32 ndarray.  The result is ``softmax`` of the module's ``Linear -> ReLU -> Linear`` stack,
     whatever its ``forward`` does.  Features are cast to float32 as ``process_features`` does; NaN/Inf or a wrong
-    feature count raise ``ValueError``.  The frame is staged on the device in one piece (no chunk pipeline)."""
+    feature count raise ``ValueError``.  Frames of any size stream through the chunk pipeline; requests of up to 64
+    rows take the online route, one float64 kernel replayed as a CUDA graph."""
     engine = get_engine()
     dm = device_mlp(module, engine)
     arr = features.to_numpy() if hasattr(features, "to_numpy") else np.asarray(features)
     _check_min_samples(arr)
-    batch = engine.stage(arr, keep_f64=False)
-    try:
-        out, _ = engine.predict_mlp_proba(dm, batch)
-        return out
-    finally:
-        batch.free()
+    out, _ = engine.predict_mlp_proba_host(dm, arr)
+    return out
 
 
 def _check_topk(k, n_classes: int) -> int:
@@ -414,17 +411,14 @@ def mlp_predict_topk(module: Any, features: Any, k: int = 3) -> tuple:
     ``(values, indices)``, the ``k`` largest class probabilities per row as a float32 ``(n, k)`` ndarray and their
     class indices as int64 ``(n, k)``, in descending order.  Probabilities are those of :func:`mlp_predict_proba`;
     the indices are the float64 network's ranks (``UNIONML_B200_MODE=fast``: the fp32 kernel's), ties to the lower
-    class index.  The guards of :func:`mlp_predict_proba` apply; ``k`` outside ``1 .. n_out`` raises ``ValueError``."""
+    class index; requests of up to 64 rows get the float64 ranks and probabilities in either mode.  The guards and
+    routes of :func:`mlp_predict_proba` apply; ``k`` outside ``1 .. n_out`` raises ``ValueError``."""
     engine = get_engine()
     dm = device_mlp(module, engine)
     k = _check_topk(k, dm.n_classes)
     arr = features.to_numpy() if hasattr(features, "to_numpy") else np.asarray(features)
     _check_min_samples(arr)
-    batch = engine.stage(arr, keep_f64=False)
-    try:
-        idx, proba, stats = engine.predict_mlp_topk(dm, batch, k, exact=_exact_default())
-    finally:
-        batch.free()
+    idx, proba, stats = engine.predict_mlp_topk_host(dm, arr, k, exact=_exact_default())
     _note_ambiguous(stats)
     return proba, idx.astype(np.int64)
 
