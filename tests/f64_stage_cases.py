@@ -99,20 +99,121 @@ def exact_linear(X, coef, intercept):
     return np.array(labels, np.int32), np.array(margins)
 
 
+def _exact_mlp_logits(row, w1, b1, w2, b2):
+    """Exact logits of one fp32 row, in Fractions (ReLU is exact); zero features and zero weights are skipped."""
+    xs = [(f, Fraction(float(v))) for f, v in enumerate(row) if v != 0]
+    h = [max(Fraction(float(b1[n])) + sum((v * Fraction(float(w1[n, f])) for f, v in xs if w1[n, f]), Fraction(0)),
+             Fraction(0)) for n in range(w1.shape[0])]
+    return [Fraction(float(b2[c])) + sum((h[n] * Fraction(float(w2[c, n])) for n in range(len(h)) if h[n]), Fraction(0))
+            for c in range(w2.shape[0])]
+
+
 def exact_mlp(X, w1, b1, w2, b2):
     """The float64 network on fp32 x and weights, in Fractions (ReLU is exact)."""
     w1, b1, w2, b2 = (np.asarray(a, np.float32) for a in (w1, b1, w2, b2))
     labels, margins = [], []
     for row in np.asarray(X, np.float32):
-        xs = [(f, Fraction(float(v))) for f, v in enumerate(row) if v != 0]
-        h = [max(Fraction(float(b1[n])) + sum((v * Fraction(float(w1[n, f])) for f, v in xs), Fraction(0)), Fraction(0))
-             for n in range(w1.shape[0])]
-        z = [Fraction(float(b2[c])) + sum((h[n] * Fraction(float(w2[c, n])) for n in range(len(h)) if h[n]), Fraction(0))
-             for c in range(w2.shape[0])]
-        lab, m = label_margin(z)
+        lab, m = label_margin(_exact_mlp_logits(row, w1, b1, w2, b2))
         labels.append(lab)
         margins.append(float(m))
     return np.array(labels, np.int32), np.array(margins)
+
+
+def topk_gap(z, k):
+    """(stable descending top k, smallest consecutive gap among ranks 1 .. min(k, C - 1) + 1) of one row's logits: ties
+    go to the lower class index, as np.argsort(-z, kind="stable") orders them."""
+    order = sorted(range(len(z)), key=lambda c: (-z[c], c))
+    kk = min(k, len(z) - 1)
+    return order[:k], min(z[order[r]] - z[order[r + 1]] for r in range(kk))
+
+
+def mlp_f64_bound(X, w1, b1, w2, b2):
+    """Per row, a bound on the error of any float64 evaluation of any one logit (any summation order): a dot product of
+    n terms errs by at most (n + 1) u times its absolute sum; each hidden unit's error is carried through |W2| (ReLU is
+    1-Lipschitz).  Per unit and class rather than through the largest weights, so that a huge weight on a unit a row
+    leaves at zero does not send every row to Fractions."""
+    x = np.asarray(X, np.float32).astype(np.float64)
+    w1, b1, w2, b2 = (np.asarray(a, np.float32).astype(np.float64) for a in (w1, b1, w2, b2))
+    F, H = x.shape[1], w1.shape[0]
+    e1 = (F + 4) * U * (np.abs(x) @ np.abs(w1).T + np.abs(b1))  # (n, H)
+    carried = e1 @ np.abs(w2).T  # (n, C)
+    h = np.maximum(x @ w1.T + b1, 0.0)
+    a2 = h @ np.abs(w2).T + np.abs(b2) + carried
+    return (carried + (H + 4) * U * a2).max(axis=1) * (1 + 2.0**-20)
+
+
+def exact_mlp_topk(X, w1, b1, w2, b2, k):
+    """Exact top-k of the float64 network on fp32 x and weights: (indices (n, k) int32, gaps (n,) float64), the gap
+    being the smallest exact consecutive gap among ranks 1 .. min(k, C - 1) + 1.  Rows whose float64 gaps all sit
+    beyond four times float64's own error bound keep the float64 order (their gap is the float64 one, within that
+    bound of the exact gap); the others, exact ties included, are recomputed in Fractions."""
+    X = np.asarray(X, np.float32)
+    w1, b1, w2, b2 = (np.asarray(a, np.float32) for a in (w1, b1, w2, b2))
+    C = w2.shape[0]
+    kk = min(k, C - 1)
+    x = X.astype(np.float64)
+    z = np.maximum(x @ w1.T.astype(np.float64) + b1, 0.0) @ w2.T.astype(np.float64) + b2
+    order = np.argsort(-z, axis=1, kind="stable")
+    zs = np.take_along_axis(z, order, axis=1)
+    gap = (zs[:, :kk] - zs[:, 1 : kk + 1]).min(axis=1)
+    idx = order[:, :k].astype(np.int32)
+    for i in np.flatnonzero(~(gap > 4 * mlp_f64_bound(X, w1, b1, w2, b2))):
+        top, g = topk_gap(_exact_mlp_logits(X[i], w1, b1, w2, b2), k)
+        idx[i], gap[i] = top, float(g)
+    return idx, gap
+
+
+def tf32(v):
+    """fp32 values with the low 13 mantissa bits cleared (tf32 values: the tensor-core kernel scores them itself)."""
+    return (np.asarray(v, np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+
+
+RANK_LADDER = (0.6, 0.75, 0.9, 1.3, 1.6, 3.0)  # float64 is exact on these rows: below beta counted, above certified
+RANK_TIE_LADDER = (0.0, 0.1, 0.5, 3.0, 10.0)
+
+
+def mlp_rank_case(F, H, C, r, tie=False, big=False, seed=0):
+    """A network and rows whose logits are D = 64 c0 apart but for one planted pair at ranks r, r + 1 (1-based), set
+    on the ladder of beta (mlp_beta).  Hidden unit 0 = x0 - x1 + x2 with x0 = x1 = 2^20 (big: 2^50, integer rows); it
+    cancels, so herr w2sum dominates beta while float64 is exact.  Class a gets logit h0 = x2, class b the bias c0 =
+    16 beta (rounded to a power of 2); the classes above the pair c0 + j D, those below c0 - j D.  x2 = c0 +- f beta,
+    so a sits above b (+) or below it (-).  tie: class t copies a (weights and bias), so a and t tie exactly on every
+    row and the group a, t, b takes ranks r .. r + 2.  Returns (w1, b1, w2, b2), X (fp32, tf32 values), the factors f
+    (signed), beta and (a, b, t)."""
+    rng = np.random.default_rng(seed)
+    n_pair = 3 if tie else 2
+    assert r + n_pair - 1 <= C and F >= 3 and H >= 1
+    perm = rng.permutation(C)
+    above, group, below = perm[: r - 1], perm[r - 1 : r - 1 + n_pair], perm[r - 1 + n_pair :]
+    a, b = int(group[0]), int(group[-1])
+    t = int(group[1]) if tie else -1
+    w1 = np.zeros((H, F), np.float32)
+    w1[0, :3] = [1.0, -1.0, 1.0]
+    b1 = np.zeros(H, np.float32)
+    w2 = np.zeros((C, H), np.float32)
+    w2[a, 0] = 1.0
+    if tie:
+        w2[t, 0] = 1.0
+    x0 = np.zeros(F, np.float32)
+    x0[:2] = 2.0**50 if big else 2.0**20
+    b2 = np.zeros(C, np.float32)
+    beta = float(mlp_beta(x0[None, :], w1, b1, w2, b2)[0])
+    c0 = 2.0 ** np.ceil(np.log2(16 * beta))
+    D = 64 * c0
+    b2[b] = c0
+    for j, c in enumerate(above[::-1], 1):
+        b2[c] = c0 + j * D
+    for j, c in enumerate(below, 1):
+        b2[c] = c0 - j * D
+    rows, fs = [], []
+    for f in RANK_TIE_LADDER if tie else RANK_LADDER:
+        for sign in (1, -1) if f else (1,):
+            x = x0.copy()
+            v = c0 + sign * f * beta
+            x[2] = tf32(np.rint(v) if big else v)
+            rows.append(x)
+            fs.append(sign * f)
+    return (w1, b1, w2, b2), np.array(rows, np.float32), np.array(fs), beta, (a, b, t)
 
 
 def rungs(margin, beta):

@@ -120,3 +120,79 @@ def test_mlp_beta_is_dominated_by_cancelling_hidden_unit():
     assert herr_part < beta < 1.01 * herr_part
     want, margin = K.exact_mlp(x, w1, b1, w2, b2)
     assert want[0] in (0, 1) and margin[0] == 0  # h0 = 2^-25 = b2_1: an exact tie, class 0 first
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# top-k: the exact reference of the MLP ranks and the rank ladder of tests/test_gpu_mlp_topk_exactness.py
+# ---------------------------------------------------------------------------------------------------------------
+def test_topk_gap_orders_ties_by_lower_index():
+    z = [Fraction(1), Fraction(3), Fraction(1), Fraction(3), Fraction(-2)]
+    assert K.topk_gap(z, 1) == ([1], 0)  # 1 and 3 tie at the top: the lower index first, gap 0
+    assert K.topk_gap(z, 3) == ([1, 3, 0], 0)
+    assert K.topk_gap([Fraction(5), Fraction(1), Fraction(0)], 3) == ([0, 1, 2], 1)  # k == C: the gaps of ranks 1 .. C
+    assert K.topk_gap([Fraction(5), Fraction(1), Fraction(0)], 1) == ([0], 4)
+    assert list(np.argsort(-np.array([1.0, 3.0, 1.0, 3.0, -2.0]), kind="stable")) == [1, 3, 0, 2, 4]
+
+
+@pytest.mark.parametrize("F,H,C,r,tie,big", [(64, 32, 10, 1, False, False), (64, 32, 10, 4, True, False),
+                                             (50, 16, 3, 2, False, False), (32, 16, 3, 1, True, False),
+                                             (40, 24, 5, 3, False, True), (128, 32, 10, 9, False, False)])
+def test_mlp_rank_case_plants_the_gap_at_rank_r(F, H, C, r, tie, big):
+    net, X, fs, beta, (a, b, t) = K.mlp_rank_case(F, H, C, r, tie=tie, big=big, seed=F + r)
+    assert not (X.view(np.uint32) & np.uint32(0x1FFF)).any()  # tf32 values
+    if big:
+        assert (X == np.rint(X)).all()  # integer rows: an int64 frame holds them exactly
+    for k in range(1, C + 1):
+        idx, gap = K.exact_mlp_topk(X, *net, k)
+        ex = [K.topk_gap(K._exact_mlp_logits(x, *net), k) for x in X]  # Fractions on every row
+        assert [list(i) for i in idx] == [e[0] for e in ex]
+        np.testing.assert_array_equal(gap, [float(e[1]) for e in ex])
+        if k < r:  # the planted boundary lies beyond rank k + 1: only the wide gaps count
+            assert (gap > 32 * beta).all(), (k, gap / beta)
+            continue
+        ratio = gap / beta
+        if tie:  # a and its copy t tie exactly (below b on the - rows); the lower index of the two comes first
+            assert (gap[(fs >= 0) | (k > r)] == 0).all()
+            np.testing.assert_allclose(ratio[(fs < 0) & (k == r)], -fs[(fs < 0) & (k == r)], atol=0.02)
+            lo, hi = min(a, t), max(a, t)
+            for row in idx:
+                row = list(row)
+                assert hi not in row or row.index(lo) < row.index(hi)
+        else:
+            # float64 is exact and x2 is a tf32 value: each gap lands within 2 % of beta of its rung
+            np.testing.assert_allclose(ratio, np.abs(fs), atol=0.02)
+            # a above b on the + rows, below it on the - rows, at ranks r and r + 1
+            top = np.where(fs > 0, a, b)
+            if k >= r:
+                assert (idx[:, r - 1] == top).all()
+            if k > r:
+                assert (idx[:, r] == np.where(fs > 0, b, a)).all()
+    if not tie:  # both rungs of the bound factor are there, on both sides of beta
+        assert (np.abs(fs) < 1).sum() >= 4 and (np.abs(fs) > 1).sum() >= 4
+
+
+def test_exact_mlp_topk_uses_float64_only_where_it_is_sure():
+    """Random rows plus rows whose logits tie in float64 but not exactly: the mixed sweep equals Fractions on every row."""
+    rng = np.random.default_rng(6)
+    F, H, C = 12, 8, 6
+    w1 = K.spread64(rng, (H, F), -6, 6).astype(np.float32)
+    b1 = K.spread64(rng, H, -6, 6).astype(np.float32)
+    w2 = K.spread64(rng, (C, H), -6, 6).astype(np.float32)
+    b2 = K.spread64(rng, C, -6, 6).astype(np.float32)
+    w2[4], b2[4] = w2[1], b2[1]  # class 4 ties class 1 exactly
+    # class 5 = h0 + 2^-40 against class 2 = h0: a gap far below float64's resolution of h0 ~ 2^40
+    w1[0] = 0
+    w1[0, 0] = 1.0
+    w2[5], w2[2] = 0, 0
+    w2[5, 0], w2[2, 0] = 1.0, 1.0
+    b2[5], b2[2] = 2.0**-40, 0.0
+    X = K.spread64(rng, (40, F), -6, 6).astype(np.float32)
+    X[:20, 0] = 2.0**40
+    for k in (1, 3, 6):
+        idx, gap = K.exact_mlp_topk(X, w1, b1, w2, b2, k)
+        ex = [K.topk_gap(K._exact_mlp_logits(x, w1, b1, w2, b2), k) for x in X]
+        assert [list(i) for i in idx] == [e[0] for e in ex]
+        bound = K.mlp_f64_bound(X, w1, b1, w2, b2)
+        assert np.all(np.abs(gap - np.array([float(e[1]) for e in ex])) <= 2 * bound)
+    z = X[:20].astype(np.float64)[:, 0]
+    assert ((z + 2.0**-40) == z).all()  # float64 alone could not order classes 5 and 2 on these rows
