@@ -78,8 +78,13 @@ typedef struct uml_stats {
                               (<= 64 rows: zero-copy request buffer, one kernel replayed as a CUDA graph), 6 = float64
                               decision_function scores kernel, 7 = float64 probabilities (the same kernel with the
                               softmax / sigmoid epilogue: predict_proba, predict_log_proba)                               */
-  int32_t x_elem_bytes;    /* predict calls on a resident batch: bytes per feature of the rows the scoring kernel read -
-                              2 = the batch's compact fp16 copy (linear tile kernel), 4 = its fp32 rows; 0 otherwise    */
+  int32_t x_elem_bytes;    /* predict calls on a resident batch: bytes per feature of the values the scoring kernel
+                              multiplied - 2 = fp16 values, read from the batch's compact fp16 copy or, by the linear
+                              tile kernel's tensor-core schedule, from its byte copy (widened to the same fp16
+                              values), 4 = its fp32 rows; 0 otherwise                                                  */
+  int32_t x_read_bytes;    /* the same calls: bytes per feature of the rows the scoring kernel read - 1 = the batch's
+                              byte copy, 2 = its fp16 copy, 4 = its fp32 rows; 0 otherwise (fills the struct's former
+                              tail padding: its size and the offsets of the fields above are unchanged)                */
 } uml_stats;
 
 typedef struct uml_device_info {

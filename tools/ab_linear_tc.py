@@ -1,10 +1,12 @@
 #!/usr/bin/env python
-"""A/B of the two fp16 schedules of the linear tile kernel on bench.py's cfg 2 batch: the tensor-core schedule
-(UML_B200_LINEAR_TC=1, which fails unless it runs) against the CUDA-core one (UML_B200_LINEAR_TC=0).
+"""A/B of the linear tile kernel's schedules on bench.py's cfg 2 batch: the tensor-core schedule on the byte copy
+(the default; x_read_bytes 1), the tensor-core schedule on the fp16 copy
+(UML_B200_COMPACT_ROWS=2 with UML_B200_LINEAR_TC=1, which fails unless a tensor-core schedule runs) and the CUDA-core
+fp16 schedule (UML_B200_LINEAR_TC=0).
 
     python tools/ab_linear_tc.py [--warmup 5] [--launches 30]
 
-Stages the cfg 2 batch and the golden digits model once, alternates the two schedules one launch at a time (the EXACT,
+Stages the cfg 2 batch and the golden digits model once, alternates the three schedules one launch at a time (the EXACT,
 uint8-label predict_peers step bench.py times, bracketed by CUDA events), and prints one JSON object: per schedule the
 median and min-max time and n_flagged, whether the labels are byte-equal, the card's name, power limit and SM clock,
 and how many rows tier 1 leaves to the fp32 replay.  That count is estimated from float64 scores: rows whose exact
@@ -60,16 +62,22 @@ def main():
     X = eng.pinned_empty((n, F), np.float32)
     digits_rows(0, n, X)
     batch = eng.stage(X)
-    routes = ("tc", "cuda_core")
+    routes = ("tc_bytes", "tc", "cuda_core")
+    env = {"tc_bytes": {"UML_B200_LINEAR_TC": "1"},
+           "tc": {"UML_B200_COMPACT_ROWS": "2", "UML_B200_LINEAR_TC": "1"},
+           "cuda_core": {"UML_B200_LINEAR_TC": "0"}}
     labels = {r: torch.empty(n, dtype=torch.uint8, device="cuda") for r in routes}
 
     def step(route, want_stats=False):
-        os.environ["UML_B200_LINEAR_TC"] = "1" if route == "tc" else "0"
+        for k in ("UML_B200_COMPACT_ROWS", "UML_B200_LINEAR_TC"):
+            os.environ.pop(k, None)
+        os.environ.update(env[route])
         return eng.predict_peers(model, batch, [labels[route].data_ptr()], 0, exact=True, want_stats=want_stats,
                                  label_bytes=1)
 
     stats = {r: step(r, want_stats=True) for r in routes}
-    equal = bool(torch.equal(labels["tc"], labels["cuda_core"]))
+    assert [stats[r]["x_read_bytes"] for r in routes] == [1, 2, 2], stats
+    equal = bool(torch.equal(labels["tc"], labels["cuda_core"]) and torch.equal(labels["tc_bytes"], labels["tc"]))
     before = card()
     for _ in range(args.warmup):
         for r in routes:
@@ -84,7 +92,8 @@ def main():
             ev[1].synchronize()
             ms[r].append(ev[0].elapsed_time(ev[1]))
     after = card()
-    os.environ.pop("UML_B200_LINEAR_TC", None)
+    for k in ("UML_B200_COMPACT_ROWS", "UML_B200_LINEAR_TC"):
+        os.environ.pop(k, None)
 
     # float64 margins and A of every row, on the GPU in 1M-row chunks
     W = torch.tensor(np.asarray(arrs["coef"], dtype=np.float64), device="cuda")
@@ -107,6 +116,7 @@ def main():
         out["routes"][r] = {"ms_median": statistics.median(ms[r]), "ms_min": min(ms[r]), "ms_max": max(ms[r]),
                             "n_flagged": stats[r]["n_flagged"]}
     out["speedup_median"] = out["routes"]["cuda_core"]["ms_median"] / out["routes"]["tc"]["ms_median"]
+    out["bytes_speedup_median"] = out["routes"]["tc"]["ms_median"] / out["routes"]["tc_bytes"]["ms_median"]
     print(json.dumps(out))
 
 

@@ -90,7 +90,7 @@ def main():
     # every route reads the fp32 rows except the labels, which read the batch's fp16 copy when staging kept one
     _, st = eng.predict(m, b, exact=True, out_device_ptr=labels.data_ptr(), want_stats=True)
     read = {k: 4 * F for k in routes}
-    read["labels_exact"] = (st.get("x_elem_bytes") or 4) * F
+    read["labels_exact"] = (st.get("x_read_bytes") or 4) * F
     kern = {k: [] for k in routes}
     call = {k: [] for k in routes}
     for name, fn in routes.items():  # warm every route (module load, shared-memory attribute, scratch buffers)

@@ -1,12 +1,15 @@
-// Where the time of the linear tile kernel goes, on 10M x 64 fp32 rows (2.56 GB, the cfg2 shape) and on their compact
-// fp16 copy (1.28 GB), against the card's own read ceiling.  Built nine times by tools/linear_probe.sh from
-// linear_kernels.cu itself:
-//   plain                   read ceiling (streaming 16-byte non-allocating loads) over 2.56 GB and over 1.28 GB + the
-//                           tile kernel, all three schedules
+// Where the time of the linear tile kernel goes, on 10M x 64 fp32 rows (2.56 GB, the cfg2 shape), on their compact
+// fp16 copy (1.28 GB) and on their byte copy (0.64 GB), against the card's own read ceiling.  Built nine times by
+// tools/linear_probe.sh from linear_kernels.cu itself:
+//   plain                   read ceiling (streaming 16-byte non-allocating loads) over 2.56 GB, 1.28 GB and 0.64 GB +
+//                           the tile kernel, the three CUDA-core schedules and both tensor-core ones (kHalfMma on the
+//                           fp16 rows, kByteMma on the byte rows; B operand and kappa from build_tc_operands)
 //   -DUML_PROBE_FEED_ONLY   the same producer, ring, order and barriers with consumers that skip the math, under
-//                           L2_PROMOTION_256B (what the library encodes) and L2_PROMOTION_NONE
+//                           L2_PROMOTION_256B (what the library encodes) and L2_PROMOTION_NONE; also the byte
+//                           schedule's ring of 16 KiB {64 bytes, 256 rows} stages
 //   -DUML_PROBE_WAIT_CLOCKS the tile kernel with clock64() totals around the producer's `empty` and the scoring
-//                           warps' `full` waits, and over the time the scoring warps hold a landed stage
+//                           warps' `full` waits, over the time the scoring warps hold a landed stage, and over the time
+//                           the re-score warp spends on rows from the queue (its busy fraction); every schedule
 //   -DUML_PROBE_TIMELINE    the tile kernel with %globaltimer stamps per CTA (entry, first issue, first landing, last
 //                           release, exit) over two back-to-back launches: ramp, exit spread, launch gap
 //   -DUML_PROBE_NO_W, -DUML_PROBE_NO_X, both   the fp16 schedule without its W loads, without its x loads and
@@ -37,12 +40,13 @@ using namespace uml;
 static const long long kRows = 10000000;
 static const int kF = 64, kC = 10;
 
-__global__ void fill_kernel(float* x, __half* xh, long long n) {
+__global__ void fill_kernel(float* x, __half* xh, uint8_t* xb, long long n) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     unsigned h = static_cast<unsigned>(i) * 2654435761u;
     h ^= h >> 15;
     x[i] = static_cast<float>(h % 17u);  // digits-like pixel values 0..16
     xh[i] = __float2half_rn(x[i]);       // the same values, exactly (what the engine's pack kernel writes)
+    xb[i / kF * kByteRowBytes + linear_byte_pos(static_cast<int>(i % kF))] = static_cast<uint8_t>(h % 17u);
   }
 }
 
@@ -79,16 +83,19 @@ static PFN_cuTensorMapEncodeTiled_v12000 encoder() {
   return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
 }
 
-// fp32 rows: {32, box_rows} boxes; fp16 rows (half): {64, 128} boxes, as the engine encodes them
-static CUtensorMap make_map(const void* x, int box_rows, CUtensorMapL2promotion promo, bool half = false) {
+// fp32 rows: {32, box_rows} boxes; fp16 rows (elem 2): {64, 128} boxes; byte rows (elem 1): {64, 256} boxes without
+// swizzle, as the engine encodes them
+static CUtensorMap make_map(const void* x, int box_rows, CUtensorMapL2promotion promo, int elem = 4) {
   CUtensorMap map{};
   cuuint64_t gdim[2] = {(cuuint64_t)kF, (cuuint64_t)kRows};
-  cuuint64_t gstride[1] = {(cuuint64_t)kF * (half ? 2 : 4)};
-  cuuint32_t box[2] = {(cuuint32_t)(half ? kHalfBoxF : kChunkF), (cuuint32_t)box_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)kF * elem};
+  cuuint32_t box[2] = {(cuuint32_t)(elem == 4 ? kChunkF : kHalfBoxF), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = encoder()(&map, half ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)x,
-                         gdim, gstride, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = encoder()(&map, elem == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : elem == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                                                                     : CU_TENSOR_MAP_DATA_TYPE_UINT8,
+                         2, (void*)x, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         elem == 1 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, promo,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     fprintf(stderr, "cuTensorMapEncodeTiled: %d\n", (int)r);
     exit(1);
@@ -126,9 +133,11 @@ int main() {
   const double bytes = static_cast<double>(kRows) * kF * 4;
   float* x = nullptr;
   __half* xh = nullptr;
+  uint8_t* xb = nullptr;
   CK(cudaMalloc(&x, static_cast<size_t>(bytes)));
   CK(cudaMalloc(&xh, static_cast<size_t>(bytes / 2)));
-  fill_kernel<<<prop.multiProcessorCount * 8, 512>>>(x, xh, kRows * kF);
+  CK(cudaMalloc(&xb, static_cast<size_t>(bytes / 4)));
+  fill_kernel<<<prop.multiProcessorCount * 8, 512>>>(x, xh, xb, kRows * kF);
   CK(cudaDeviceSynchronize());
 
 #if defined(UML_PROBE_NO_W) || defined(UML_PROBE_NO_X)
@@ -158,9 +167,9 @@ int main() {
     CK(cudaMalloc(&sink, 4));
     CK(cudaMalloc(&cyc, 8));
     const int grid = prop.multiProcessorCount * 4;  // 2048 threads per SM resident, 64 KB of loads in flight per SM
-    // the fp16 copy's 1.28 GB first, then the fp32 rows' 2.56 GB: the last read_ceiling line is what
-    // MEASURED_PEAKS.json records
-    for (const double part : {0.5, 1.0}) {
+    // the byte copy's 0.64 GB and the fp16 copy's 1.28 GB first, then the fp32 rows' 2.56 GB: the last read_ceiling
+    // line is what MEASURED_PEAKS.json records
+    for (const double part : {0.25, 0.5, 1.0}) {
       const double b = bytes * part;
       const double ms = time_ms([&] {
         read_kernel<<<grid, 512>>>(reinterpret_cast<const uint4*>(x), static_cast<long long>(b) / 16, sink, cyc);
@@ -235,11 +244,29 @@ int main() {
 #endif
 
   // the EXACT + QUEUE kernel bench.py runs (uint8 labels to one target), in each schedule
+  // the tensor-core schedules' B operand and kappa, as the engine builds them at model load
+  std::vector<double> w_cf(static_cast<size_t>(kC) * kF), b_c(kC);
+  for (int c = 0; c < kC; ++c) {
+    b_c[c] = bias[c];
+    for (int f = 0; f < kF; ++f) w_cf[static_cast<size_t>(c) * kF + f] = wt[f * cp + c];
+  }
+  std::vector<uint8_t> tc_image;
+  float tc_kappa = 0.f;
+  if (!build_tc_operands(w_cf, b_c, wt, bias, kC, kF, kF, cp, 0.0, &tc_image, &tc_kappa)) {
+    fprintf(stderr, "build_tc_operands refused the probe's model\n");
+    exit(1);
+  }
+  void* d_tc = nullptr;
+  CK(cudaMalloc(&d_tc, tc_image.size()));
+  CK(cudaMemcpy(d_tc, tc_image.data(), tc_image.size(), cudaMemcpyHostToDevice));
   auto run = [&](LinearSched sched, CUtensorMapL2promotion promo, const char* promo_name) {
     const bool whole = sched == LinearSched::kWhole, half = sched == LinearSched::kHalf;
-    const int tile = whole ? kWholeTileRows : half ? kHalfTileRows : kTileRows;
-    const CUtensorMap map = half ? make_map(xh, kTileRows, promo, true) : make_map(x, tile, promo);
-    const double read_bytes = half ? bytes / 2 : bytes;
+    const bool byte = sched == LinearSched::kByteMma, tc = linear_tc_sched(sched);
+    const bool f16 = half || sched == LinearSched::kHalfMma;
+    const int tile = whole ? kWholeTileRows : f16 || byte ? kHalfTileRows : kTileRows;
+    const CUtensorMap map = byte ? make_map(xb, kHalfTileRows, promo, 1)
+                            : f16 ? make_map(xh, kTileRows, promo, 2) : make_map(x, tile, promo);
+    const double read_bytes = byte ? bytes / 4 : f16 ? bytes / 2 : bytes;
     TmaKernelParams p{};
     p.wt = m.wt;
     p.bias = m.bias;
@@ -250,7 +277,7 @@ int main() {
     p.num_tiles = (kRows + tile - 1) / tile;
     p.f_pad = kF;
     p.kc = kF / kChunkF;
-    const size_t fixed = tma_fixed_smem(m, half);
+    const size_t fixed = tma_fixed_smem(m, f16 || byte) + (tc ? linear_tc_b_bytes(kC) : 0);
     const int stage_bytes = linear_stage_bytes(sched);
     p.num_stages = std::min(64, static_cast<int>((kMaxSmemBytes - fixed) / stage_bytes));
     p.thr = static_cast<float>(2.0 * (kF + 4.0) * 5.9604644775390625e-08 * (1.0 + kF * 4.76837158203125e-07) * 1.0001);
@@ -264,6 +291,8 @@ int main() {
     p.fold_rel = m.fold_rel;  // 0: no affine fold
     p.binary = m.binary;      // 0: ten classes
     p.counters = counters;
+    p.tc_ops = d_tc;
+    p.tc_kappa = tc_kappa;
 #ifdef UML_PROBE_WAIT_CLOCKS
     p.probe_clocks = counters + 8;
 #endif
@@ -273,7 +302,9 @@ int main() {
     const size_t smem = fixed + static_cast<size_t>(p.num_stages) * stage_bytes;
     const int grid = prop.multiProcessorCount;
     auto launch = [&] {
-      const cudaError_t err = half    ? launch_one<kC, true, true, LinearSched::kHalf>(map, p, grid, smem, 0)
+      const cudaError_t err = byte    ? launch_one<kC, true, true, LinearSched::kByteMma>(map, p, grid, smem, 0)
+                              : tc    ? launch_one<kC, true, true, LinearSched::kHalfMma>(map, p, grid, smem, 0)
+                              : half  ? launch_one<kC, true, true, LinearSched::kHalf>(map, p, grid, smem, 0)
                               : whole ? launch_one<kC, true, true, LinearSched::kWhole>(map, p, grid, smem, 0)
                                       : launch_one<kC, true, true, LinearSched::kChunked>(map, p, grid, smem, 0);
       CK(err);
@@ -281,12 +312,15 @@ int main() {
     const double ms = time_ms(launch);
     printf("{\"probe\": \"tile_kernel\", \"build\": \"%s\", \"schedule\": \"%s\", \"l2_promotion\": \"%s\", \"stages\": %d, "
            "\"scoring_warps\": %d, \"rows_per_lane_per_pass\": %d, \"ms\": %.4f, \"bytes_read\": %.0f, \"gbs\": %.1f",
-           build, half ? "half_rows_256x64" : whole ? "whole_rows_64" : "chunked_128x32", promo_name, p.num_stages,
-           linear_consumer_warps(sched), half ? kHalfPassRows : tile / 32, ms, read_bytes,
+           build, byte ? "byte_rows_tc_256x64" : tc ? "half_rows_tc_256x64" : half ? "half_rows_256x64"
+                  : whole ? "whole_rows_64" : "chunked_128x32",
+           promo_name, p.num_stages, linear_consumer_warps(sched), half ? kHalfPassRows : tile / 32, ms, read_bytes,
            read_bytes / ms * 1e-6);
 #ifdef UML_PROBE_WAIT_CLOCKS
     // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time
-    CK(cudaMemset(counters + 8, 0, 5 * sizeof(unsigned long long)));
+    CK(cudaMemset(counters + 8, 0, 7 * sizeof(unsigned long long)));
+    unsigned long long flagged0 = 0, flagged1 = 0;
+    CK(cudaMemcpy(&flagged0, counters + kCounterFlagged, 8, cudaMemcpyDeviceToHost));
     cudaEvent_t a, b;
     CK(cudaEventCreate(&a));
     CK(cudaEventCreate(&b));
@@ -296,16 +330,20 @@ int main() {
     CK(cudaEventSynchronize(b));
     float one = 0.f;
     CK(cudaEventElapsedTime(&one, a, b));
-    unsigned long long c[5];
+    unsigned long long c[7];
     CK(cudaMemcpy(c, counters + 8, sizeof(c), cudaMemcpyDeviceToHost));
-    // mean stages per CTA landed and not yet released (one scoring warp per stage): the scoring warps' summed hold time
-    // over one warp's loop time, per CTA
+    CK(cudaMemcpy(&flagged1, counters + kCounterFlagged, 8, cudaMemcpyDeviceToHost));
+    // mean stages per CTA landed and not yet released (one scoring warp per stage, four in the tensor-core
+    // schedules): the scoring warps' summed hold time over one warp's loop time, per CTA
     const int scoring_warps = grid * linear_consumer_warps(sched);
-    const double held_stages = static_cast<double>(c[4]) / (static_cast<double>(c[3]) / scoring_warps) / grid;
+    const double held_stages =
+        static_cast<double>(c[4]) / (static_cast<double>(c[3]) / scoring_warps) / grid / (tc ? 4 : 1);
     printf(", \"producer_empty_wait_frac\": %.4f, \"consumer_full_wait_frac\": %.4f, \"held_stages\": %.3f, "
-           "\"ring_stages\": %d, \"sm_clock_mhz_under_load\": %.0f",
+           "\"ring_stages\": %d, \"sm_clock_mhz_under_load\": %.0f, \"rescore_warp_busy_frac\": %.4f, "
+           "\"rows_fp64_per_launch\": %llu",
            static_cast<double>(c[0]) / c[1], static_cast<double>(c[2]) / c[3], held_stages,
-           p.num_stages, static_cast<double>(c[1]) / grid / (one * 1e3));
+           p.num_stages, static_cast<double>(c[1]) / grid / (one * 1e3), c[6] ? static_cast<double>(c[5]) / c[6] : 0.0,
+           flagged1 - flagged0);
 #endif
 #ifdef UML_PROBE_TIMELINE
     // two launches back to back, each stamping its own [grid][5] block
@@ -369,6 +407,8 @@ int main() {
   run(LinearSched::kChunked, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
   run(LinearSched::kWhole, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
   run(LinearSched::kHalf, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
+  run(LinearSched::kHalfMma, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
+  run(LinearSched::kByteMma, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
 #ifdef UML_PROBE_FEED_ONLY
   run(LinearSched::kChunked, CU_TENSOR_MAP_L2_PROMOTION_NONE, "none");
   run(LinearSched::kWhole, CU_TENSOR_MAP_L2_PROMOTION_NONE, "none");

@@ -1,7 +1,8 @@
 #!/bin/bash
 # Read ceiling + feed-only + wait-clock + timeline breakdown of the linear tile kernel (tools/linear_probe.cu), on GPU 0,
 # for each schedule: chunked and whole fp32 rows, and the compact fp16 rows (whose feed-only and wait-clock lines say
-# whether that schedule is bound by its feed or by its scoring warps); then the fp16 schedule without its W loads,
+# whether that schedule is bound by its feed or by its scoring warps), and the feed of the byte rows' 16 KiB stages
+# against the read ceiling over their 0.64 GB; then the fp16 schedule without its W loads,
 # without its x loads, and with neither; then the fp16 schedule with 4 rows per lane per pass and with the library's 8,
 # alternating (both with four scoring warps and 256-row stages).
 # Writes MEASURED_PEAKS.json (the read ceiling bench.py's roofline divides by) and the probe's JSON lines to

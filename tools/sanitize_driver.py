@@ -92,6 +92,21 @@ for mm in (m, m16):
             assert eng.predict(mm, bb, exact=exact)[1]["x_elem_bytes"] == 2
         eng.predict_peers(mm, bb, [buf16.ptr], 1, exact=True, want_stats=True, label_bytes=1)
 del _os.environ["UML_B200_STAGES"]
+# byte rows: `b16` and `b200` hold integers 0..16, so staging also packed their byte copies and the EXACT predicts above
+# took the tensor-core schedule on them; here that schedule (x_read_bytes 1) at its 3-item ring floor and at full
+# depth, a ragged last item, 10 and 16 classes, uint8 peer stores at an odd offset, and the fp16 tensor-core schedule on
+# the same batches (UML_B200_COMPACT_ROWS=2, x_read_bytes 2)
+for stages in ("1", None):
+    if stages:
+        _os.environ["UML_B200_STAGES"] = stages
+    for env, read in (("1", 1), ("2", 2)):
+        _os.environ["UML_B200_COMPACT_ROWS"] = env
+        for mm in (m, m16):
+            for bb in (b16, b200):
+                assert eng.predict(mm, bb, exact=True)[1]["x_read_bytes"] == read
+                eng.predict_peers(mm, bb, [buf16.ptr], 1, exact=True, want_stats=True, label_bytes=1)
+    del _os.environ["UML_B200_COMPACT_ROWS"]
+    _os.environ.pop("UML_B200_STAGES", None)
 # float64 probabilities (the scores kernel's softmax / sigmoid epilogue): binary, C = 10 (one class group, in the strip),
 # C = 40 (grouped, normalised in global memory), F = 784 (W from global memory), host and resident, a device output
 # 8 bytes off 16-byte alignment

@@ -32,6 +32,7 @@ class Stats(C.Structure):
         ("kernel_launches", C.c_int32),
         ("path", C.c_int32),
         ("x_elem_bytes", C.c_int32),
+        ("x_read_bytes", C.c_int32),
     ]
 
     def as_dict(self) -> dict:

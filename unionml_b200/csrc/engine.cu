@@ -253,6 +253,11 @@ struct uml_batch {
   bool has_half = false;
   bool half_nonneg = false;  // the fp16 copy holds no value < 0 (the linear tile kernel's tensor-core schedule needs that)
   CUtensorMap half_map{};
+  // byte copy of the rows (batches with an fp16 copy whose every value is an integer in [0, 255]): what the tensor-core
+  // schedule reads instead of xh, through byte_map's {64 bytes, 256 rows} boxes (uml::linear_byte_pos order)
+  void* xb = nullptr;
+  bool has_bytes = false;
+  CUtensorMap byte_map{};
 };
 
 struct uml_mlp {
@@ -516,85 +521,6 @@ int uml_host_free(uml_engine* e, void* p) {
 // ---------------------------------------------------------------------------------------------------------------
 // model
 // ---------------------------------------------------------------------------------------------------------------
-// ---- tensor-core operands of the linear tile kernel (DESIGN.md 3.1, 3.2) ----
-// the fp16 value nearest to v (ties to even; up: the smallest fp16 value >= v), for |v| below 2^16
-static double f16_round(double v, bool up = false) {
-  if (v == 0.0) return v;
-  int e = 0;
-  std::frexp(std::fabs(v), &e);  // |v| in [2^(e-1), 2^e): 11 significant bits, or the subnormal spacing 2^-24
-  const int q = std::max(e - 11, -24);
-  const double m = std::ldexp(v, -q);
-  return std::ldexp(up ? std::ceil(m) : std::nearbyint(m), q);
-}
-// bit pattern of an fp16 value held exactly in v
-static uint16_t f16_bits(double v) {
-  const uint16_t sign = std::signbit(v) ? 0x8000u : 0u;
-  const double a = std::fabs(v);
-  if (a < 0x1p-14) return sign | (uint16_t)std::ldexp(a, 24);
-  int e = 0;
-  const double m = std::frexp(a, &e);  // a = m 2^e, m in [0.5, 1)
-  return sign | (uint16_t)((e + 14) << 10) | (uint16_t)std::ldexp(m * 2.0 - 1.0, 10);
-}
-// per-k16-step budget of the f16 wgmma accumulation, in u = 2^-24 of the running |.| sum (DESIGN.md 3.2): above the
-// 36u of a truncating aligner without guard bits over 16 products and the accumulator ((2 x 17 + 2) u, the model of
-// 3.3), and at least 4x the worst that tests/test_gpu_wgmma_f16_accum.py measures on the hardware
-constexpr double kTcStepBudget = 64.0;
-// The B operand image of LinearDeviceModel::tc_ops and the certification factor, or false when the model does not take
-// the tensor-core schedule: a folded affine map (its score error is bounded in the fp64 terms only), non-finite weights,
-// or magnitudes at which the scaled A of DESIGN.md 3.2 could leave the normal fp32 range.  wt / bias are the fp32
-// route's operands (its bound column and bias bound are what tier 1 must dominate).
-static bool build_tc_operands(const std::vector<double>& w, const std::vector<double>& b, const std::vector<float>& wt,
-                              const std::vector<float>& bias, int C, int F, int f_pad, int cp, double fold_rel,
-                              std::vector<uint8_t>* image, float* kappa) {
-  if (f_pad > uml::kHalfBoxF || fold_rel != 0.0) return false;
-  double wabs = 0.0;
-  for (double v : w) {
-    if (!std::isfinite(v)) return false;
-    wabs = std::max(wabs, std::fabs(v));
-  }
-  for (int c = 0; c < C; ++c)
-    if (!std::isfinite(b[c])) return false;
-  int ex = 0;
-  if (wabs > 0.0) std::frexp(wabs, &ex);  // wabs < 2^ex
-  const int sigma = 15 - ex;               // max |w| 2^sigma in [2^14, 2^15): every hi piece is a normal fp16 value
-  double wsum = 0.0;
-  for (int f = 0; f < F; ++f) wsum += wt[(size_t)f * cp + C];
-  const double a32 = (double)bias[C] + 65504.0 * wsum;  // the fp32 route's A of the largest fp16 row
-  if (!(std::ldexp(a32, std::max(sigma, 0)) < 0x1p100) || !(std::ldexp((double)bias[C], sigma) > 0x1p-100)) return false;
-  const int NH = uml::linear_tc_hi_cols(C), N = uml::linear_tc_cols(C);
-  std::vector<uint16_t> bt((size_t)N * uml::kHalfBoxF, 0);
-  // column n's 128-byte row, its 16-byte chunks XOR-swizzled by (n & 7): the SWIZZLE_128B K-major layout
-  auto put = [&](int n, int f, double v) { bt[(size_t)n * 64 + (((f / 8) ^ (n & 7)) * 8) + f % 8] = f16_bits(v); };
-  for (int f = 0; f < F; ++f) {
-    double wmax = std::ldexp((double)wt[(size_t)f * cp + C], sigma);
-    for (int c = 0; c < C; ++c) {
-      const double v = std::ldexp(w[(size_t)c * F + f], sigma);
-      const double hi = f16_round(v);
-      put(c, f, hi);
-      put(NH + c, f, f16_round(v - hi));
-      wmax = std::max(wmax, std::fabs(v));
-    }
-    // floored at 2^-3 so that 2^-22 of it covers the 2^-25 a subnormal piece errs by (hi + lo errs by <= 2^-21 of it).
-    // The fp32 route's FLT_MIN floor can scale past fp16 when every weight is below 2^-127: no route then.
-    const double wb = f16_round(std::max(wmax, 0.125), true);
-    if (!(wb <= 65504.0)) return false;
-    put(C, f, wb);
-  }
-  std::vector<float> tb(NH, 0.f);
-  for (int c = 0; c < C; ++c) tb[c] = (float)std::ldexp(b[c], sigma);
-  tb[C] = (float)std::ldexp((double)bias[C], sigma);  // exact: a power-of-two multiple of an fp32 value in range
-  image->assign((size_t)N * 128 + tb.size() * 4, 0);
-  std::memcpy(image->data(), bt.data(), (size_t)N * 128);
-  std::memcpy(image->data() + (size_t)N * 128, tb.data(), tb.size() * 4);
-  // tier 1 certifies iff margin > 2 Etc + 2.5 thr A32+ (DESIGN.md 3.2): Etc <= e_rel A, A <= Ahat / (1 - step)
-  const double u = uml::kU;
-  const double step = kTcStepBudget * u * (f_pad / 16);
-  const double e_rel = (0x1p-21 + step * (1.0 + 0x1p-10) + 4.0 * u) * (1.0 + 0x1p-10);
-  const double thr = uml::linear_margin_thr(F);
-  *kappa = (float)((2.0 * e_rel + 2.5 * thr * (1.0 + (F + 2.0) * u)) / (1.0 - step) * (1.0 + 0x1p-10));
-  return true;
-}
-
 // bmag[c] >= |b_c| is the bias magnitude both bounds use (|b_c| + sum_f |shift_f w'_cf| for a folded affine map) and
 // fold_rel the fp64 bound's extra relative term of such a map (DESIGN.md 3.2)
 static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& w, const std::vector<double>& b,
@@ -651,7 +577,7 @@ static int upload_model(uml_engine* e, uml_model* m, const std::vector<double>& 
   float kappa = 0.f;
   if (m->d_tc) cudaFree(m->d_tc);
   m->d_tc = nullptr;
-  if (build_tc_operands(w, b, wt, bias, C, F, f_pad, cp, fold_rel, &tc, &kappa)) {
+  if (uml::build_tc_operands(w, b, wt, bias, C, F, f_pad, cp, fold_rel, &tc, &kappa)) {
     UML_CUDA(e, cudaMalloc(&m->d_tc, tc.size()));
     UML_CUDA(e, cudaMemcpy(m->d_tc, tc.data(), tc.size(), cudaMemcpyHostToDevice));
   }
@@ -782,9 +708,32 @@ static int encode_batch_maps(uml_engine* e, uml_batch* b) {
   return rc;
 }
 
+// the byte copy of a batch whose fp16 pack found every value to be an integer in [0, 255] (stage.not_u8 == 0): one pack
+// kernel from the fp32 rows and its tensor map.  When there is no room for it the batch keeps the fp16 route.
+static int build_byte_copy(uml_engine* e, uml_batch* b) {
+  if (cudaMalloc(&b->xb, (size_t)b->n_rows * uml::kByteRowBytes) != cudaSuccess) {
+    (void)cudaGetLastError();
+    b->xb = nullptr;
+    return UML_OK;
+  }
+  UML_CUDA(e, uml::launch_pack_bytes(b->x, b->ld, b->n_rows, b->n_features, b->xb, e->stream));
+  cuuint64_t gdim[2] = {(cuuint64_t)uml::kByteRowBytes, (cuuint64_t)b->n_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)uml::kByteRowBytes};
+  cuuint32_t box[2] = {(cuuint32_t)uml::kByteRowBytes, (cuuint32_t)uml::kHalfTileRows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = e->encode(&b->byte_map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, b->xb, gdim, gstride, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) UML_FAIL(e, UML_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for the byte copy, %lld rows", (int)r,
+                                  (long long)b->n_rows);
+  UML_CUDA(e, cudaStreamSynchronize(e->stream));
+  b->has_bytes = true;
+  return UML_OK;
+}
+
 // the compact fp16 copy of a staged batch whose staging pass found every value to be an fp16 value (stage.not_f16 == 0):
-// one pack kernel from the fp32 rows and its tensor map.  The copy is an optimisation: when there is no room for it the
-// batch keeps the fp32 route, and the call still succeeds.
+// one pack kernel from the fp32 rows and its tensor map, then the byte copy when every value fits one.  Each copy is an
+// optimisation: when there is no room for it the batch keeps the wider route, and the call still succeeds.
 static int build_half_copy(uml_engine* e, uml_batch* b) {
   const int F = b->n_features;
   const int64_t ldh = uml::linear_half_ld(F);
@@ -794,9 +743,12 @@ static int build_half_copy(uml_engine* e, uml_batch* b) {
     return UML_OK;
   }
   b->ldh = ldh;
-  UML_CUDA(e, cudaMemsetAsync(&e->d_stage->negative, 0, sizeof(unsigned long long), e->stream));
-  UML_CUDA(e, uml::launch_pack_half(b->x, b->ld, b->n_rows, F, b->xh, ldh, &e->d_stage->negative, e->stream));
-  UML_CUDA(e, cudaMemcpyAsync(&e->h->stage.negative, &e->d_stage->negative, sizeof(unsigned long long),
+  // negative and not_u8 are adjacent: one memset, one copy back
+  static_assert(offsetof(StageResult, not_u8) == offsetof(StageResult, negative) + sizeof(unsigned long long), "");
+  UML_CUDA(e, cudaMemsetAsync(&e->d_stage->negative, 0, 2 * sizeof(unsigned long long), e->stream));
+  UML_CUDA(e, uml::launch_pack_half(b->x, b->ld, b->n_rows, F, b->xh, ldh, &e->d_stage->negative, &e->d_stage->not_u8,
+                                    e->stream));
+  UML_CUDA(e, cudaMemcpyAsync(&e->h->stage.negative, &e->d_stage->negative, 2 * sizeof(unsigned long long),
                               cudaMemcpyDeviceToHost, e->stream));
   cuuint64_t gdim[2] = {(cuuint64_t)F, (cuuint64_t)b->n_rows};
   cuuint64_t gstride[1] = {(cuuint64_t)ldh * 2};
@@ -810,14 +762,15 @@ static int build_half_copy(uml_engine* e, uml_batch* b) {
   UML_CUDA(e, cudaStreamSynchronize(e->stream));  // later calls may run on another stream (uml_engine_set_stream)
   b->has_half = true;
   b->half_nonneg = e->h->stage.negative == 0;
-  return UML_OK;
+  return e->h->stage.not_u8 == 0 ? build_byte_copy(e, b) : UML_OK;
 }
 
-// UML_B200_COMPACT_ROWS=0 makes the linear tile kernel read the fp32 rows of a batch that has an fp16 copy (test and A/B
-// hook, read per call)
-static bool compact_rows_enabled() {
+// the widest value, in bytes, of the rows the linear tile kernel may read (test and A/B hook, read per call):
+// UML_B200_COMPACT_ROWS unset (or any other value), the narrowest copy the batch has (1); =2, at most its fp16 copy;
+// =0, the fp32 rows (4).  uml_stats.x_read_bytes says which one a call read.
+static int compact_rows_max_bytes() {
   const char* env = getenv("UML_B200_COMPACT_ROWS");
-  return !(env && env[0] == '0');
+  return env && env[0] == '0' ? 4 : env && env[0] == '2' ? 2 : 1;
 }
 
 int uml_batch_from_device(uml_engine* e, uml_batch** out, const void* dev_ptr, int64_t n_rows, int n_features,
@@ -1112,6 +1065,7 @@ void uml_batch_free(uml_batch* b) {
   if (b->owns) cudaFree(b->x);
   cudaFree(b->x64);
   cudaFree(b->xh);
+  cudaFree(b->xb);
   delete b;
 }
 
@@ -1119,11 +1073,13 @@ void uml_batch_free(uml_batch* b) {
 // predict
 // ---------------------------------------------------------------------------------------------------------------
 // enqueue the scoring of one resident block of rows on e->stream; no host synchronisation.  timed: ev[2] ends the
-// scoring kernel (the caller brackets the step with ev[1] / ev[3]).  half_map (optional): the rows' compact fp16
-// copy, which the tile kernel then reads; *x_elem_bytes (optional) gets the bytes per feature it read (2 or 4).
+// scoring kernel (the caller brackets the step with ev[1] / ev[3]).  half_map, byte_map (optional): the rows' compact
+// fp16 and byte copies, which the tile kernel then reads; *x_elem_bytes (optional) gets the bytes per feature of the
+// values it multiplied (2 or 4), *x_read_bytes (optional) the bytes per feature it read (1, 2 or 4).
 static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch& l, const CUtensorMap* map,
                            const CUtensorMap* half_map, int mode, bool timed, int* launches, int* path,
-                           int* x_elem_bytes = nullptr, bool half_nonneg = false) {
+                           int* x_elem_bytes = nullptr, bool half_nonneg = false,
+                           const CUtensorMap* byte_map = nullptr, int* x_read_bytes = nullptr) {
   const FlagList fl = flag_list(e);
   const bool exact = mode == UML_PREDICT_EXACT;
   std::string why;
@@ -1132,13 +1088,16 @@ static int enqueue_predict(uml_engine* e, const uml_model* m, const LinearLaunch
     NvtxRange r_score("uml:score");
     std::string err;
     bool need_rescore = false;
-    if (half_map && !uml::linear_half_rows_ok(m->dm.f_pad)) half_map = nullptr;
-    cudaError_t ce = uml::launch_linear_tma(*map, half_map, m->dm, l, exact, fl, e->info.sm_count, e->stream, &err,
-                                            &need_rescore, half_nonneg);
+    if (half_map && !uml::linear_half_rows_ok(m->dm.f_pad)) half_map = byte_map = nullptr;
+    int elem_bytes = 4, read_bytes = 4;
+    cudaError_t ce = uml::launch_linear_tma(*map, half_map, half_map ? byte_map : nullptr, m->dm, l, exact, fl,
+                                            e->info.sm_count, e->stream, &err, &need_rescore, half_nonneg,
+                                            &elem_bytes, &read_bytes);
     if (ce != cudaSuccess) UML_FAIL(e, UML_ERR_CUDA, "linear_argmax_tma launch: %s %s", cudaGetErrorString(ce), err.c_str());
     *launches += 1;
     *path = 1;
-    if (x_elem_bytes) *x_elem_bytes = half_map ? 2 : 4;
+    if (x_elem_bytes) *x_elem_bytes = elem_bytes;
+    if (x_read_bytes) *x_read_bytes = read_bytes;
     if (timed) UML_CUDA(e, cudaEventRecord(e->ev[2], e->stream));
     if (need_rescore) {  // UML_B200_RESCORE_MODE=kernel; in queue mode flagged rows are re-scored by a warp of the tile kernel
       NvtxRange r_rescore("uml:rescore_f64");
@@ -1253,7 +1212,7 @@ struct ResidentCall {
 
 // One predict call on a resident batch: the checks, device setup, output scratch, events, counters, D2H and stats
 // that every such call shares.  prepare() makes the call's host-side checks and choices before the first timed stream
-// operation; score(out, timed, &launches, &path, &x_elem_bytes) enqueues its own step between ev[1] and ev[3], writing
+// operation; score(out, timed, &launches, &path, x_bytes) enqueues its own step between ev[1] and ev[3], writing
 // output i to out[i] (the caller's device memory, or scratch bound for host memory) and recording ev[2] after its
 // scoring kernel when timed.  An asynchronous call (device outputs, no stats) returns once the step is enqueued.
 extern "C++" {  // a template cannot have the C linkage of the ABI section around it
@@ -1289,8 +1248,9 @@ static int predict_resident(uml_engine* e, const uml_batch* b, const ResidentCal
   // The asynchronous step needs no memset at all: the flag list is handed back empty by the previous re-score kernel.
   if (sync_call) UML_CUDA(e, reset_counters(e, e->stream));
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[1], e->stream));
-  int launches = 0, path = 0, x_elem_bytes = 0;
-  if ((rc = score(out, timed, &launches, &path, &x_elem_bytes)) != UML_OK) return rc;
+  int launches = 0, path = 0;
+  int x_bytes[2] = {0, 0};  // uml_stats.x_elem_bytes, x_read_bytes
+  if ((rc = score(out, timed, &launches, &path, x_bytes)) != UML_OK) return rc;
   if (timed) UML_CUDA(e, cudaEventRecord(e->ev[3], e->stream));
   if (!sync_call) return UML_OK;
   for (int i = 0; i < 2; ++i)
@@ -1300,7 +1260,8 @@ static int predict_resident(uml_engine* e, const uml_batch* b, const ResidentCal
   rc = finish_stats(e, stats, b->n_rows, launches, path, timed);
   if (stats) {
     stats->d2h_bytes = d2h;
-    stats->x_elem_bytes = x_elem_bytes;
+    stats->x_elem_bytes = x_bytes[0];
+    stats->x_read_bytes = x_bytes[1];
   }
   return rc;
 }
@@ -1312,7 +1273,7 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
                                    int labels_on_device, void* const* peers, int n_peers, int64_t row_offset,
                                    int label_bytes, int mode, uml_stats* stats) {
   if (!m) return UML_ERR_INVALID;
-  auto score = [&](void* const* out, bool timed, int* launches, int* path, int* elem_bytes) {
+  auto score = [&](void* const* out, bool timed, int* launches, int* path, int* elem_bytes) -> int {
     LinearLaunch l{};
     l.x = b->x;
     l.x64 = b->x64;
@@ -1329,10 +1290,13 @@ static int linear_predict_resident(uml_engine* e, const uml_model* m, const uml_
     if (own) t.labels = static_cast<int32_t*>(peers[0]) + row_offset;
     t.n_peers = n_peers - own;
     for (int i = 0; i < t.n_peers; ++i) t.peers[i] = peers[own + i];
-    const CUtensorMap* half = b->has_half && compact_rows_enabled() ? &b->half_map : nullptr;
+    const int max_bytes = compact_rows_max_bytes();
+    const CUtensorMap* half = b->has_half && max_bytes <= 2 ? &b->half_map : nullptr;
+    const CUtensorMap* bytes = b->has_bytes && max_bytes <= 1 ? &b->byte_map : nullptr;
     *elem_bytes = 4;
+    elem_bytes[1] = 4;
     return enqueue_predict(e, m, l, b->has_map ? &b->lin_map : nullptr, half, mode, timed, launches, path, elem_bytes,
-                           b->half_nonneg);
+                           b->half_nonneg, bytes, &elem_bytes[1]);
   };
   ResidentCall c{m->dm.n_classes, m->n_features_in, "estimator", {labels_out, nullptr}, {4, 0}, labels_on_device, mode,
                  stats};
@@ -2392,7 +2356,7 @@ static int mlp_predict_resident(uml_engine* e, const uml_mlp* m, const uml_batch
     t.wire_u8 = n_peers > 0 && label_bytes == 1 ? 1 : 0;
     t.n_peers = n_peers;  // every peer vector, this rank's own included
     for (int i = 0; i < n_peers; ++i) t.peers[i] = peers[i];
-    *elem_bytes = 4;  // the MLP kernels read fp32 rows
+    elem_bytes[0] = elem_bytes[1] = 4;  // the MLP kernels read fp32 rows
     return enqueue_mlp(e, m->dm, b->map, b->x, b->ld, o, mode == UML_PREDICT_EXACT, route, timed, launches, path);
   };
   ResidentCall c{m->dm.n_classes, m->dm.n_in, "module", {labels_out, nullptr}, {4, 0}, labels_on_device, mode, stats};

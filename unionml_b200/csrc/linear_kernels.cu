@@ -18,7 +18,10 @@
 
 #include <algorithm>
 #include <cstdio>
+#include <cmath>
 #include <cstdlib>
+#include <cstring>
+#include <vector>
 
 #include "uml_common.cuh"
 #include "label_store.cuh"
@@ -153,12 +156,12 @@ struct TmaKernelParams {
   int binary;
   unsigned long long* counters;
 #ifdef UML_PROBE_WAIT_CLOCKS
-  unsigned long long* probe_clocks;  // [5], see the diagnostic builds below
+  unsigned long long* probe_clocks;  // [7], see the diagnostic builds below
 #endif
 #ifdef UML_PROBE_TIMELINE
   unsigned long long* probe_timeline;  // [gridDim.x][5], see the diagnostic builds below
 #endif
-  const void* tc_ops;  // kHalfMma: LinearDeviceModel::tc_ops
+  const void* tc_ops;  // tensor-core schedules: LinearDeviceModel::tc_ops
   float tc_kappa;
 };
 
@@ -188,7 +191,9 @@ constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this ma
 //                         ring (producer, order, barriers) delivers on its own
 //  UML_PROBE_WAIT_CLOCKS  clock64() totals added into p.probe_clocks: [0] the producer's `empty` waits, [1] its whole
 //                         loop, [2] the scoring warps' waits for their data, [3] their whole loops, [4] the time they
-//                         hold a landed stage (from the return of the `full` wait to the `empty` arrive)
+//                         hold a landed stage (from the return of the `full` wait to the `empty` arrive); QUEUE
+//                         kernels also [5] the re-score warp's time on rows it took from the queue (replay and fp64
+//                         re-score) and [6] its whole loop
 //  UML_PROBE_TIMELINE     %globaltimer per CTA into p.probe_timeline[blockIdx.x][5]: [0] entry, [1] the producer's first
 //                         issue, [2] the first stage landed (warp 0), [3] the last `empty` arrive, [4] exit
 //  UML_PROBE_NO_W         kHalf only, wrong scores: every feature's W^T row is one set of registers loaded once per warp,
@@ -251,20 +256,30 @@ __device__ __forceinline__ unsigned long long probe_globaltimer() {
 //            stages on the tensor cores (wgmma, f16 x f16 -> fp32, W^T as scaled hi | lo pieces); ring item n goes to
 //            warpgroup n % 2.  Rows the tensor-core guard does not certify go through the queue, where the re-score warp
 //            first replays the fp32 route on them (DESIGN.md 3.1, 3.2)
-// kWhole, kHalf and kHalfMma claim their tiles in groups of NCU (the units that take ring items: the scoring warps, or
-// kHalfMma's two warpgroups) from a global counter; ring item n goes to unit n % NCU.
-enum class LinearSched { kChunked, kWhole, kHalf, kHalfMma };
+//  kByteMma  (kHalfMma's conditions, the batch has a byte copy) kHalfMma on 16 KiB stages of one {64 bytes, 256 rows}
+//            box of the byte copy, with three warpgroups: a thread loads its A fragments of each m64 block with two
+//            LDS.128, widens the bytes to the same f16 values kHalfMma reads and issues wgmma with A from registers
+// kWhole, kHalf and the tensor-core schedules claim their tiles in groups of NCU (the units that take ring items: the
+// scoring warps, or the two warpgroups) from a global counter; ring item n goes to unit n % NCU.
+enum class LinearSched { kChunked, kWhole, kHalf, kHalfMma, kByteMma };
+__host__ __device__ constexpr bool linear_tc_sched(LinearSched s) { return s == LinearSched::kHalfMma || s == LinearSched::kByteMma; }
 
 // scoring warps of a schedule; the producer is warp NCW and the QUEUE kernels' re-score warp NCW + 1
-__host__ __device__ constexpr int linear_consumer_warps(LinearSched s) { return s == LinearSched::kHalf ? kHalfConsumerWarps : kConsumerWarps; }
-// units that take ring items (and the ring's floor): warps, or kHalfMma's warpgroups
-__host__ __device__ constexpr int linear_ring_units(LinearSched s) { return s == LinearSched::kHalfMma ? kConsumerWarps / 4 : linear_consumer_warps(s); }
+// kByteMma: three warpgroups.  Its feed takes half of kHalfMma's time, so the warpgroups' own time per item (the
+// epilogue's shuffle chains, stores and queue hand-off) is the limit; a third one hides more of that latency
+// (23.9 against 19.8 G rows/s with two at cfg 2, DESIGN.md 5.1), within the 128 registers that 14 warps leave.
+constexpr int kByteWarpgroups = 3;
+__host__ __device__ constexpr int linear_consumer_warps(LinearSched s) {
+  return s == LinearSched::kHalf ? kHalfConsumerWarps : s == LinearSched::kByteMma ? 4 * kByteWarpgroups : kConsumerWarps;
+}
+// units that take ring items (and the ring's floor): warps, or the tensor-core schedules' warpgroups
+__host__ __device__ constexpr int linear_ring_units(LinearSched s) { return linear_tc_sched(s) ? linear_consumer_warps(s) / 4 : linear_consumer_warps(s); }
 __host__ __device__ constexpr int linear_threads(LinearSched s, bool queue) { return (linear_consumer_warps(s) + (queue ? 2 : 1)) * 32; }
 // bytes of one ring stage: in kHalf and kHalfMma two 16 KiB fp16 boxes
 __host__ __device__ constexpr int linear_stage_bytes(LinearSched s) {
   return s == LinearSched::kHalf || s == LinearSched::kHalfMma ? 2 * kStageBytes : kStageBytes;
 }
-// kHalfMma: bytes of the B operand in shared memory (rounded up to the 1 KiB that keeps what follows aligned)
+// tensor-core schedules: bytes of the B operand in shared memory (rounded up to the 1 KiB that keeps what follows aligned)
 __host__ __device__ constexpr int linear_tc_b_bytes(int C) { return (linear_tc_cols(C) * 128 + 1023) / 1024 * 1024; }
 
 // kHalfMma's tier 2 (DESIGN.md 3.2): the fp32 route's scores of one row, replayed bit for bit by one warp: lane c <= C
@@ -336,13 +351,14 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr int NW4 = (NCOL + 3) / 4;        // float4 loads of W per feature
   constexpr bool WHOLE = SCHED == LinearSched::kWhole;
   constexpr bool HALF = SCHED == LinearSched::kHalf;
-  constexpr bool MMA = SCHED == LinearSched::kHalfMma;
-  constexpr bool F16 = HALF || MMA;                          // 256-row stages of the compact fp16 rows
-  constexpr bool CLAIMED = WHOLE || F16;                     // tiles claimed from kCounterTileClaim, one tile per stage
+  constexpr bool MMA = linear_tc_sched(SCHED);               // kHalfMma or kByteMma
+  constexpr bool BYTES = SCHED == LinearSched::kByteMma;    // 256-row stages of the byte rows, one box
+  constexpr bool F16 = HALF || SCHED == LinearSched::kHalfMma;  // 256-row stages of the compact fp16 rows, two boxes
+  constexpr bool CLAIMED = WHOLE || F16 || BYTES;            // tiles claimed from kCounterTileClaim, one tile per stage
   constexpr int NCW = linear_consumer_warps(SCHED);
   constexpr int NCU = linear_ring_units(SCHED);
   static_assert(!MMA || (EXACT && QUEUE), "the tensor-core schedule certifies rows through the queue's replay");
-  constexpr int TILE = F16 ? kHalfTileRows : WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = per ring stage
+  constexpr int TILE = F16 || BYTES ? kHalfTileRows : WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = per ring stage
   // free queue slots a scoring warp wants before it publishes: every scoring warp may publish a whole tile at once
   // (kHalfMma: the 64 rows of the tile a warp stores)
   constexpr int HEADROOM = HALF ? NCW * TILE : MMA ? NCW * 64 : kQueueHeadroom;
@@ -351,11 +367,12 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr int R = HALF ? kHalfPassRows : TILE / 32;
   constexpr int NPASS = TILE / 32 / R;
   static_assert(NPASS * R * 32 == TILE && (!HALF || R % 4 == 0), "a pass is whole 128-row boxes");
-  // one box: 8 KiB (two per kWhole stage) or 16 KiB (two per kHalf stage)
-  constexpr int BOX_BYTES = (F16 ? kTileRows : TILE) * kChunkF * 4;
+  // one box: 8 KiB (two per kWhole stage) or 16 KiB (two per kHalf stage, one per kByteMma stage)
+  constexpr int BOX_BYTES = BYTES ? kHalfTileRows * kByteRowBytes : (F16 ? kTileRows : TILE) * kChunkF * 4;
   constexpr int STAGE_BYTES = linear_stage_bytes(SCHED);
   static_assert(!F16 || (BOX_BYTES == kTileRows * kHalfBoxF * 2 && STAGE_BYTES == 2 * BOX_BYTES),
                 "an fp16 stage is two boxes");
+  static_assert(!BYTES || STAGE_BYTES == BOX_BYTES, "a byte stage is one box");
   // fp32x2 accumulator pairs (see the accumulator comment below).  Not in the fp16 schedule: fma2 is two fmaf, so the
   // scores are the same bits, and without the 64-bit register pairs ptxas schedules its 128 registers better
   // (0.534 -> 0.523 ms at cfg 2, DESIGN.md 5.1)
@@ -365,7 +382,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // SWIZZLE_128B wants 1 KiB alignment
 
   const int S = p.num_stages;
-  // kHalfMma: the B operand (1 KiB aligned, as SWIZZLE_128B wants) between the ring and W^T
+  // tensor-core schedules: the B operand (1 KiB aligned, as SWIZZLE_128B wants) between the ring and W^T
   float* wt_s = reinterpret_cast<float*>(smem + static_cast<size_t>(S) * STAGE_BYTES + (MMA ? linear_tc_b_bytes(C) : 0));
   float* bias_s = wt_s + p.f_pad * CP;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + CP);
@@ -403,7 +420,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], MMA ? 4 : 1);  // kHalfMma: every warp of the warpgroup hands the stage back
+      mbar_init(&empty_bar[s], MMA ? 4 : 1);  // tensor cores: every warp of the warpgroup hands the stage back
     }
     fence_barrier_init();
   }
@@ -461,6 +478,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
                 tma_load_2d(dst, &xmap, &full_bar[stage], 0, row, policy);
                 if (second) tma_load_2d(dst + BOX_BYTES, &xmap, &full_bar[stage], 0, row + kTileRows, policy);
               } else {
+                // (kByteMma: one {64, 256} box; rows past the batch are filled with zeros and never stored)
                 mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
                 uint8_t* dst = smem + static_cast<size_t>(stage) * kStageBytes;
                 const int row = static_cast<int>(tile * TILE);
@@ -767,11 +785,11 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     };
 
     if constexpr (MMA) {
-      // ===== kHalfMma: warpgroup wg = warp / 4 takes ring items wg, wg + 2, ...; per item four m64 blocks of 64 rows x
-      // NT columns, f_pad / 16 k16 steps each, one commit group; the stage goes back after the wait, the epilogue runs
-      // from registers.  Fragment (WgmmaTf32's layout): thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 and the
-      // row 8 below of each block, columns 8 i + 2 (l % 4) + {0, 1}: class c's hi piece at c, its lo piece at NH + c,
-      // the bound column at C - all of a row in one quad ----
+      // ===== kHalfMma, kByteMma: warpgroup wg = warp / 4 takes ring items wg, wg + NCU, ...; per item four m64 blocks of
+      // 64 rows x NT columns, f_pad / 16 k16 steps each, one commit group (kByteMma: one per block); the stage goes back
+      // after the wait, the epilogue runs from registers.  Fragment (WgmmaTf32's layout): thread (warp w, lane l) holds
+      // rows 16 (w % 4) + l / 4 and the row 8 below of each block, columns 8 i + 2 (l % 4) + {0, 1}: class c's hi piece
+      // at c, its lo piece at NH + c, the bound column at C - all of a row in one quad ----
       constexpr int NH = linear_tc_hi_cols(C), NT = linear_tc_cols(C), NL = NT - NH;
       const int q = lane & 3;
       const long long row_in = 16 * (warp & 3) + (lane >> 2);  // row of fragment row-half 0 in block 0
@@ -887,7 +905,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         const bool scored = !kFeedOnly && tile >= 0 && tile < num_tiles;
         float d[4][NT / 2];
         if (scored) {
-          const uint32_t a_base = smem_u32(smem + static_cast<size_t>(stage) * STAGE_BYTES);
+          [[maybe_unused]] const uint32_t a_base = smem_u32(smem + static_cast<size_t>(stage) * STAGE_BYTES);
 #pragma unroll
           for (int b = 0; b < 4; ++b)
 #pragma unroll
@@ -895,18 +913,64 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
               d[b][r] = 0.f;
               wgmma_fence_operand(d[b][r]);
             }
-          wgmma_fence();
+          if constexpr (BYTES) {
+            // one commit group per m64 block, its A fragments (f16 values equal to the bytes) loaded and converted just
+            // before it; a block's registers are free once its group is done, so at most two blocks' A fragments are
+            // live (all four would be 64 registers more than the 128 of three warpgroups)
+            uint32_t a[4][kHalfBoxF / 16][4];
+            const uint8_t* xs = smem + static_cast<size_t>(stage) * STAGE_BYTES + row_in * kByteRowBytes + 16 * q;
+            // (at NT = 40, C = 16, two blocks' fragments beside 80 accumulators made ptxas serialize the wgmma chain)
+            constexpr int INFLIGHT = NT >= 40 ? 1 : 2;
 #pragma unroll
-          for (int k = 0; k < kHalfBoxF / 16; ++k) {
-            if (k < nk) {  // f_pad 32: the box's zero columns 32-63 are not multiplied
-              const uint64_t bd = wgmma_desc_k_sw128(b_base + 32 * k);
+            for (int b = 0; b < 4; ++b) {
+              if (b >= INFLIGHT) {
+                wgmma_wait<INFLIGHT - 1>();
 #pragma unroll
-              for (int b = 0; b < 4; ++b)
-                WgmmaF16<NT>::mma(d[b], wgmma_desc_k_sw128(a_base + b * 64 * 128 + 32 * k), bd, k != 0 ? 1u : 0u);
+                for (int k = 0; k < kHalfBoxF / 16; ++k)
+#pragma unroll
+                  for (int i = 0; i < 4; ++i) wgmma_fence_operand(a[b - INFLIGHT][k][i]);
+              }
+              // the 16 bytes at 16 q of rows row_in and row_in + 8 of the block, one LDS.128 each (the eight lanes of a
+              // phase read two whole 64-byte rows: conflict-free)
+              const uint4 x0 = *reinterpret_cast<const uint4*>(xs + b * 64 * kByteRowBytes);
+              const uint4 x1 = *reinterpret_cast<const uint4*>(xs + (b * 64 + 8) * kByteRowBytes);
+#pragma unroll
+              for (int k = 0; k < kHalfBoxF / 16; ++k) {
+                const uint32_t w0 = k == 0 ? x0.x : k == 1 ? x0.y : k == 2 ? x0.z : x0.w;
+                const uint32_t w1 = k == 0 ? x1.x : k == 1 ? x1.y : k == 2 ? x1.z : x1.w;
+                a[b][k][0] = bytes_to_half2(w0, 0);
+                a[b][k][1] = bytes_to_half2(w1, 0);
+                a[b][k][2] = bytes_to_half2(w0, 1);
+                a[b][k][3] = bytes_to_half2(w1, 1);
+              }
+              wgmma_fence();
+#pragma unroll
+              for (int k = 0; k < kHalfBoxF / 16; ++k) {
+                if (k < nk) WgmmaF16<NT>::mma_ra(d[b], a[b][k], wgmma_desc_k_sw128(b_base + 32 * k), k != 0 ? 1u : 0u);
+              }
+              wgmma_commit();
             }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int b = 4 - INFLIGHT; b < 4; ++b)
+#pragma unroll
+              for (int k = 0; k < kHalfBoxF / 16; ++k)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) wgmma_fence_operand(a[b][k][i]);
+          } else {
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kHalfBoxF / 16; ++k) {
+              if (k < nk) {  // f_pad 32: the box's zero columns 32-63 are not multiplied
+                const uint64_t bd = wgmma_desc_k_sw128(b_base + 32 * k);
+#pragma unroll
+                for (int b = 0; b < 4; ++b)
+                  WgmmaF16<NT>::mma(d[b], wgmma_desc_k_sw128(a_base + b * 64 * 128 + 32 * k), bd, k != 0 ? 1u : 0u);
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
           }
-          wgmma_commit();
-          wgmma_wait<0>();
 #pragma unroll
           for (int b = 0; b < 4; ++b)
 #pragma unroll
@@ -1019,6 +1083,9 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       // that has finished its tiles joins in, so a long tail of flagged rows (wide rows, many near-ties) is shared
       // by all ten warps instead of waiting for one =====================
       int n_done = 0;
+#ifdef UML_PROBE_WAIT_CLOCKS
+      long long probe_busy = 0;
+#endif
       for (;;) {
         // claim the next ticket, then wait until its slot is published (lane 0 polls and broadcasts: the lanes of a
         // warp need not run in lockstep)
@@ -1046,6 +1113,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           atomicAdd(&q_ctl[3], 1);
         }
         const long long row = static_cast<long long>(v) - 1;
+        UML_PROBE_CLOCK(probe_row);
         if constexpr (MMA) {
           // tier 2: the fp32 route's own decision first; only the rows it would flag go to fp64 (and are counted)
           n_done += settle_row_tc(p, wt_s, bias_s, CP, row, lane);
@@ -1054,7 +1122,14 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           if (lane == 0) store_label(p.targets, row, idx64);
           ++n_done;
         }
+        UML_PROBE_SINCE(probe_busy, probe_row);
       }
+#ifdef UML_PROBE_WAIT_CLOCKS
+      if (warp == NCW + 1 && lane == 0) {
+        atomicAdd(&p.probe_clocks[5], static_cast<unsigned long long>(probe_busy));
+        atomicAdd(&p.probe_clocks[6], static_cast<unsigned long long>(clock64() - probe_start));
+      }
+#endif
       if (lane == 0 && n_done > 0) atomicAdd(&p.counters[kCounterFlagged], static_cast<unsigned long long>(n_done));
     }
   }
@@ -1294,6 +1369,86 @@ cudaError_t launch_linear_proba(const LinearDeviceModel& m, const float* x, int6
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
+// ---- tensor-core operands of the linear tile kernel (DESIGN.md 3.1, 3.2) ----
+// the fp16 value nearest to v (ties to even; up: the smallest fp16 value >= v), for |v| below 2^16
+static double f16_round(double v, bool up = false) {
+  if (v == 0.0) return v;
+  int e = 0;
+  std::frexp(std::fabs(v), &e);  // |v| in [2^(e-1), 2^e): 11 significant bits, or the subnormal spacing 2^-24
+  const int q = std::max(e - 11, -24);
+  const double m = std::ldexp(v, -q);
+  return std::ldexp(up ? std::ceil(m) : std::nearbyint(m), q);
+}
+// bit pattern of an fp16 value held exactly in v
+static uint16_t f16_bits(double v) {
+  const uint16_t sign = std::signbit(v) ? 0x8000u : 0u;
+  const double a = std::fabs(v);
+  if (a < 0x1p-14) return sign | (uint16_t)std::ldexp(a, 24);
+  int e = 0;
+  const double m = std::frexp(a, &e);  // a = m 2^e, m in [0.5, 1)
+  return sign | (uint16_t)((e + 14) << 10) | (uint16_t)std::ldexp(m * 2.0 - 1.0, 10);
+}
+// per-k16-step budget of the f16 wgmma accumulation, in u = 2^-24 of the running |.| sum (DESIGN.md 3.2): above the
+// 36u of a truncating aligner without guard bits over 16 products and the accumulator ((2 x 17 + 2) u, the model of
+// 3.3), and at least 4x the worst that tests/test_gpu_wgmma_f16_accum.py measures on the hardware
+constexpr double kTcStepBudget = 64.0;
+// The B operand image of LinearDeviceModel::tc_ops and the certification factor, or false when the model does not take
+// the tensor-core schedule: a folded affine map (its score error is bounded in the fp64 terms only), non-finite weights,
+// or magnitudes at which the scaled A of DESIGN.md 3.2 could leave the normal fp32 range.  wt / bias are the fp32
+// route's operands (its bound column and bias bound are what tier 1 must dominate).
+bool build_tc_operands(const std::vector<double>& w, const std::vector<double>& b, const std::vector<float>& wt,
+                              const std::vector<float>& bias, int C, int F, int f_pad, int cp, double fold_rel,
+                              std::vector<uint8_t>* image, float* kappa) {
+  if (f_pad > uml::kHalfBoxF || fold_rel != 0.0) return false;
+  double wabs = 0.0;
+  for (double v : w) {
+    if (!std::isfinite(v)) return false;
+    wabs = std::max(wabs, std::fabs(v));
+  }
+  for (int c = 0; c < C; ++c)
+    if (!std::isfinite(b[c])) return false;
+  int ex = 0;
+  if (wabs > 0.0) std::frexp(wabs, &ex);  // wabs < 2^ex
+  const int sigma = 15 - ex;               // max |w| 2^sigma in [2^14, 2^15): every hi piece is a normal fp16 value
+  double wsum = 0.0;
+  for (int f = 0; f < F; ++f) wsum += wt[(size_t)f * cp + C];
+  const double a32 = (double)bias[C] + 65504.0 * wsum;  // the fp32 route's A of the largest fp16 row
+  if (!(std::ldexp(a32, std::max(sigma, 0)) < 0x1p100) || !(std::ldexp((double)bias[C], sigma) > 0x1p-100)) return false;
+  const int NH = uml::linear_tc_hi_cols(C), N = uml::linear_tc_cols(C);
+  std::vector<uint16_t> bt((size_t)N * uml::kHalfBoxF, 0);
+  // column n's 128-byte row, its 16-byte chunks XOR-swizzled by (n & 7): the SWIZZLE_128B K-major layout
+  auto put = [&](int n, int f, double v) { bt[(size_t)n * 64 + (((f / 8) ^ (n & 7)) * 8) + f % 8] = f16_bits(v); };
+  for (int f = 0; f < F; ++f) {
+    double wmax = std::ldexp((double)wt[(size_t)f * cp + C], sigma);
+    for (int c = 0; c < C; ++c) {
+      const double v = std::ldexp(w[(size_t)c * F + f], sigma);
+      const double hi = f16_round(v);
+      put(c, f, hi);
+      put(NH + c, f, f16_round(v - hi));
+      wmax = std::max(wmax, std::fabs(v));
+    }
+    // floored at 2^-3 so that 2^-22 of it covers the 2^-25 a subnormal piece errs by (hi + lo errs by <= 2^-21 of it).
+    // The fp32 route's FLT_MIN floor can scale past fp16 when every weight is below 2^-127: no route then.
+    const double wb = f16_round(std::max(wmax, 0.125), true);
+    if (!(wb <= 65504.0)) return false;
+    put(C, f, wb);
+  }
+  std::vector<float> tb(NH, 0.f);
+  for (int c = 0; c < C; ++c) tb[c] = (float)std::ldexp(b[c], sigma);
+  tb[C] = (float)std::ldexp((double)bias[C], sigma);  // exact: a power-of-two multiple of an fp32 value in range
+  image->assign((size_t)N * 128 + tb.size() * 4, 0);
+  std::memcpy(image->data(), bt.data(), (size_t)N * 128);
+  std::memcpy(image->data() + (size_t)N * 128, tb.data(), tb.size() * 4);
+  // tier 1 certifies iff margin > 2 Etc + 2.5 thr A32+ (DESIGN.md 3.2): Etc <= e_rel A, A <= Ahat / (1 - step)
+  const double u = uml::kU;
+  const double step = kTcStepBudget * u * (f_pad / 16);
+  const double e_rel = (0x1p-21 + step * (1.0 + 0x1p-10) + 4.0 * u) * (1.0 + 0x1p-10);
+  const double thr = uml::linear_margin_thr(F);
+  *kappa = (float)((2.0 * e_rel + 2.5 * thr * (1.0 + (F + 2.0) * u)) / (1.0 - step) * (1.0 + 0x1p-10));
+  return true;
+}
+
+
 static size_t tma_fixed_smem(const LinearDeviceModel& m, bool claimed = false) {
   // alignment slack + W^T + bias + barriers (64 stages max) + the flagged-row queue of the QUEUE kernels (+ the tile
   // index of each stage, claimed schedules)
@@ -1360,9 +1515,10 @@ bool linear_queue_rescore() {
   return mode == 1;
 }
 
-cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const LinearDeviceModel& m,
-                              const LinearLaunch& l, bool exact, const FlagList& flags, int sm_count,
-                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed, bool half_nonneg) {
+cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const CUtensorMap* byte_map,
+                              const LinearDeviceModel& m, const LinearLaunch& l, bool exact, const FlagList& flags,
+                              int sm_count, cudaStream_t stream, std::string* err, bool* rescore_kernel_needed,
+                              bool half_nonneg, int* x_elem_bytes, int* x_read_bytes) {
   // the in-kernel queue re-scores rows with W in global memory / L2: fine for a 5 KB model, not for 62 KB of fp64
   // weights per row (cfg 3) - wide models take the re-score kernel, which stages W in shared memory
   const bool small_model = static_cast<size_t>(m.w64_stride) * m.n_features * sizeof(double) <= 16 * 1024;
@@ -1390,7 +1546,10 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
     if (err) *err = "UML_B200_LINEAR_TC=1, but the batch or the model does not take the tensor-core schedule";
     return cudaErrorInvalidValue;
   }
-  const LinearSched sched = tc     ? LinearSched::kHalfMma
+  // a batch with a byte copy reads it on the tensor cores (a quarter of the fp32 rows' bytes)
+  const bool bytes = tc && byte_map != nullptr;
+  const LinearSched sched = bytes  ? LinearSched::kByteMma
+                            : tc   ? LinearSched::kHalfMma
                             : half ? LinearSched::kHalf
                             : linear_whole_rows(m.f_pad) ? LinearSched::kWhole
                                                          : LinearSched::kChunked;
@@ -1429,7 +1588,10 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   const size_t smem = fixed + static_cast<size_t>(stages) * stage_bytes;
   const long long slots = (p.num_tiles + warps - 1) / warps;
   const int grid = static_cast<int>(std::min<long long>(sm_count, std::max<long long>(1, slots)));
+  if (x_elem_bytes) *x_elem_bytes = half ? 2 : 4;  // (kByteMma multiplies the fp16 values kHalfMma reads)
+  if (x_read_bytes) *x_read_bytes = bytes ? 1 : half ? 2 : 4;
   using S = LinearSched;
+  if (sched == S::kByteMma) return dispatch_classes<true, true, S::kByteMma>(m.n_classes, *byte_map, p, grid, smem, stream);
   if (sched == S::kHalfMma) return dispatch_classes<true, true, S::kHalfMma>(m.n_classes, *half_map, p, grid, smem, stream);
   if (sched == S::kHalf) {
     const CUtensorMap& hmap = *half_map;

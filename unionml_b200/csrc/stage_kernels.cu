@@ -26,6 +26,9 @@ __device__ __forceinline__ bool f16_exact(float f) {
   return isfinite(f) && __float_as_uint(__half2float(__float2half_rn(f))) == __float_as_uint(f);
 }
 
+// the fp32 value is an integer in [0, 255] (-0.0 included, NaN not): it fits one unsigned byte exactly
+__device__ __forceinline__ bool is_byte_value(float f) { return f >= 0.f && f <= 255.f && truncf(f) == f; }
+
 // flag bits accumulated per thread: 1 = NaN/Inf; in `lossy`: 1 = fp32 copy differs from the source value, 2 = fp32
 // value is not a tf32 value (low 13 mantissa bits set), 4 = fp32 value is not a finite fp16 value
 template <typename T>
@@ -273,12 +276,14 @@ cudaError_t launch_stage_convert(const void* src, int src_dtype, bool feature_ma
 // compact fp16 copy of resident rows (read by the linear tile kernel's fp16 schedule): one thread per 8 features of a
 // row, two 16-byte loads, one 16-byte store.  fp32 -> fp16 is exact for the values the staging pass let through
 // (not_f16 == 0); columns F..ldh-1 are written as zero, whatever the fp32 rows hold there.  A warp that saw a value < 0
-// raises *negative (the tensor-core schedule takes only batches without one).
+// raises *negative (the tensor-core schedule takes only batches without one), one that saw a value other than an
+// integer in [0, 255] raises *not_u8 (the byte copy takes only batches without one).
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) pack_half_kernel(const float* __restrict__ x, long long ld, long long rows, int F,
                                                         uint4* __restrict__ xh, long long ldh,
-                                                        unsigned long long* __restrict__ negative) {
-  bool neg = false;
+                                                        unsigned long long* __restrict__ negative,
+                                                        unsigned long long* __restrict__ not_u8) {
+  bool neg = false, wide = false;
   const long long groups = ldh / 8;
   const long long total = rows * groups;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
@@ -295,20 +300,56 @@ __global__ void __launch_bounds__(256) pack_half_kernel(const float* __restrict_
     for (int k = 0; k < 4; ++k) {
       const float lo = f0 + 2 * k < F ? v[2 * k] : 0.f, hi = f0 + 2 * k + 1 < F ? v[2 * k + 1] : 0.f;
       neg |= lo < 0.f || hi < 0.f;
+      wide |= !is_byte_value(lo) || !is_byte_value(hi);
       const __half2 h = __floats2half2_rn(lo, hi);
       w[k] = *reinterpret_cast<const uint32_t*>(&h);
     }
     xh[i] = make_uint4(w[0], w[1], w[2], w[3]);
   }
   if (__any_sync(0xffffffffu, neg) && (threadIdx.x & 31) == 0) atomicAdd(negative, 1ull);
+  if (__any_sync(0xffffffffu, wide) && (threadIdx.x & 31) == 0) atomicAdd(not_u8, 1ull);
 }
 
 cudaError_t launch_pack_half(const float* x, int64_t ld, int64_t rows, int n_features, void* xh, int64_t ldh,
-                             unsigned long long* negative, cudaStream_t stream) {
+                             unsigned long long* negative, unsigned long long* not_u8, cudaStream_t stream) {
   if (rows <= 0) return cudaSuccess;
   const long long want = (rows * (ldh / 8) + 255) / 256;
   const int grid = static_cast<int>(want < 132 * 16 ? want : 132 * 16);
-  pack_half_kernel<<<grid, 256, 0, stream>>>(x, ld, rows, n_features, static_cast<uint4*>(xh), ldh, negative);
+  pack_half_kernel<<<grid, 256, 0, stream>>>(x, ld, rows, n_features, static_cast<uint4*>(xh), ldh, negative, not_u8);
+  return cudaGetLastError();
+}
+
+// byte copy of resident rows (read by the linear tile kernel's tensor-core byte schedule): one thread per 16 bytes of a
+// row, column group t = i % 4 of linear_byte_pos's order.  Exact when launch_pack_half found not_u8 == 0.
+__global__ void __launch_bounds__(256) pack_bytes_kernel(const float* __restrict__ x, long long ld, long long rows,
+                                                         int F, uint4* __restrict__ xb) {
+  const long long total = rows * (kByteRowBytes / 16);
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long r = i / (kByteRowBytes / 16);
+    const int t = static_cast<int>(i % (kByteRowBytes / 16));
+    const float* xr = x + r * ld;
+    uint32_t w[4];
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      w[s] = 0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int f = 16 * s + 2 * t + (j & 1) + 8 * (j >> 1);
+        // (-0 converts to 0)
+        const uint32_t v = f < F ? static_cast<uint32_t>(__ldg(xr + f)) : 0u;
+        w[s] |= v << (8 * j);
+      }
+    }
+    xb[i] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+cudaError_t launch_pack_bytes(const float* x, int64_t ld, int64_t rows, int n_features, void* xb, cudaStream_t stream) {
+  if (rows <= 0) return cudaSuccess;
+  const long long want = (rows * (kByteRowBytes / 16) + 255) / 256;
+  const int grid = static_cast<int>(want < 132 * 16 ? want : 132 * 16);
+  pack_bytes_kernel<<<grid, 256, 0, stream>>>(x, ld, rows, n_features, static_cast<uint4*>(xb));
   return cudaGetLastError();
 }
 

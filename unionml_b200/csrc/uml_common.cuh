@@ -43,6 +43,14 @@ constexpr int kHalfTileRows = 2 * kTileRows;
 // Scoring warps of the fp16 schedule: one per SM sub-partition, with up to 255 registers for its 8 rows of
 // accumulators and the operands of the next feature.  The ring must hold at least this many items.
 constexpr int kHalfConsumerWarps = 4;
+// Byte rows (F <= 64, every value an integer in [0, 255]): 64 bytes per row, zeros past F, one {64, 256} uint8 box =
+// one 256-row ring item of kStageBytes.  The bytes of a row are stored in the order of the f16 A fragment of wgmma
+// m64nNk16 (PTX ISA, "Register fragments, A, .f16"): the thread of column group t = lane % 4 loads the 16 bytes at
+// 16 t, and their word s holds the four features it owns in k16 step s, 16 s + {2t, 2t+1, 2t+8, 2t+9}.
+constexpr int kByteRowBytes = 64;
+__host__ __device__ inline int linear_byte_pos(int f) {
+  return 16 * ((f & 7) >> 1) + 4 * (f >> 4) + 2 * ((f >> 3) & 1) + (f & 1);
+}
 
 struct LinearDeviceModel {
   // fp32 operands of the tile kernel: wt[f][cp] (feature-major, classes padded to cp = 4*ceil((C+1)/4), column C holds
@@ -191,12 +199,20 @@ inline cudaError_t launch_dependent(void (*kern)(Params), int grid, int block, s
 // *rescore_kernel_needed: exact mode with the inline re-score switched off -> the caller launches launch_rescore_f64
 // xmap: the rows as a 2-D map {F, n_rows} with {kChunkF, linear_box_rows(m.f_pad)} boxes, SWIZZLE_128B.
 // half_map (optional): the batch's compact fp16 copy of the same rows, {kHalfBoxF, kTileRows} boxes, SWIZZLE_128B;
-// when given and linear_half_rows_ok(m.f_pad), the kernel reads it instead of xmap (same labels, half the bytes)
-cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const LinearDeviceModel& m,
-                              const LinearLaunch& l, bool exact, const FlagList& flags, int sm_count,
-                              cudaStream_t stream, std::string* err, bool* rescore_kernel_needed,
-                              bool half_nonneg = false);
+// when given and linear_half_rows_ok(m.f_pad), the kernel reads it instead of xmap (same labels, half the bytes).
+// byte_map (optional, with half_map): the batch's byte copy, {kByteRowBytes, kHalfTileRows} boxes, no swizzle; the
+// tensor-core schedule reads it instead of half_map.  *x_elem_bytes: the bytes per feature of the values the kernel
+// multiplies (uml_stats.x_elem_bytes: 2 on either copy, 4); *x_read_bytes: the bytes per feature it reads (1, 2, 4).
+cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_map, const CUtensorMap* byte_map,
+                              const LinearDeviceModel& m, const LinearLaunch& l, bool exact, const FlagList& flags,
+                              int sm_count, cudaStream_t stream, std::string* err, bool* rescore_kernel_needed,
+                              bool half_nonneg, int* x_elem_bytes, int* x_read_bytes);
 bool linear_tma_supported(const LinearDeviceModel& m, std::string* why);
+// the tensor-core schedules' B operand image (LinearDeviceModel::tc_ops) and certification factor kappa of a model with
+// fp64 weights w [C][F] and biases b, and its fp32 operands wt / bias; false when the model does not take them
+bool build_tc_operands(const std::vector<double>& w, const std::vector<double>& b, const std::vector<float>& wt,
+                       const std::vector<float>& bias, int C, int F, int f_pad, int cp, double fold_rel,
+                       std::vector<uint8_t>* image, float* kappa);
 cudaError_t launch_rescore_f64(const LinearDeviceModel& m, const LinearLaunch& l, const FlagList& flags, bool all_rows,
                                int sm_count, cudaStream_t stream);
 // small-batch kernel of the online path (/predict, B <= 64): warp per row, fp64 straight from the raw source view
@@ -308,14 +324,19 @@ struct StageResult {  // device-side counters
   unsigned long long not_tf32;  // fp32 values with any of the low 13 mantissa bits set (tensor-core path needs none)
   unsigned long long not_f16;   // fp32 values that are not finite fp16 values (the compact fp16 copy needs none)
   unsigned long long negative;  // values < 0 in the compact fp16 copy (written by launch_pack_half; -0 is not one)
+  unsigned long long not_u8;    // values that are not integers in [0, 255] (launch_pack_half; -0 is one, NaN is not)
 };
 cudaError_t launch_stage_convert(const void* src, int src_dtype, bool feature_major, int64_t src_pitch_elems,
                                  int64_t rows, int n_features, float* dst, int64_t ld, double* dst64, int64_t ld64,
                                  StageResult* result, bool check_finite, cudaStream_t stream);
 // fp32 rows [rows][ld] -> fp16 rows [rows][ldh] (ldh = linear_half_ld(F), columns >= F zero); exact when the staging
 // pass found not_f16 == 0
-// (*negative is raised when any value is < 0: the tensor-core schedule needs none)
+// (*negative is raised when any value is < 0: the tensor-core schedule needs none; *not_u8 when any value is not an
+// integer in [0, 255]: the byte copy needs none)
 cudaError_t launch_pack_half(const float* x, int64_t ld, int64_t rows, int n_features, void* xh, int64_t ldh,
-                             unsigned long long* negative, cudaStream_t stream);
+                             unsigned long long* negative, unsigned long long* not_u8, cudaStream_t stream);
+// fp32 rows [rows][ld] -> byte rows [rows][kByteRowBytes], feature f at byte linear_byte_pos(f), zeros past F; exact
+// when launch_pack_half found not_u8 == 0 (-0 becomes byte 0)
+cudaError_t launch_pack_bytes(const float* x, int64_t ld, int64_t rows, int n_features, void* xb, cudaStream_t stream);
 
 }  // namespace uml

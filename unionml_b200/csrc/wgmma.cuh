@@ -75,11 +75,15 @@ struct WgmmaTf32<32> {
 
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, f16 x f16 -> fp32, one K = 16 step (32 bytes of f16 per row), both operands
 // K-major (transpose immediates 0, 0); scale_d = 0 overwrites D.  Same fragment layout as WgmmaTf32.  N: the widths the
-// linear tile kernel's tensor-core schedule uses (linear_tc_cols).
+// linear tile kernel's tensor-core schedules use (linear_tc_cols).
+// mma_ra: the same with A from registers (f16 A fragment of the PTX ISA): thread t of the warpgroup holds row
+// r = 16 (t / 32) + (t % 32) / 4 and column group q = t % 4 as a[0] = (r, 2q..2q+1), a[1] = (r + 8, 2q..2q+1),
+// a[2] = (r, 2q+8..2q+9), a[3] = (r + 8, 2q+8..2q+9), each an f16x2 with the lower column in the low half.  The
+// registers are read asynchronously: the caller keeps them unchanged until the wgmma_wait that covers the MMA.
 template <int N>
 struct WgmmaF16;
 
-#define UML_WGMMA_F16(N, REGS, NA, NB, NS, ...)                                                               \
+#define UML_WGMMA_F16(N, REGS, NA, NB, NS, RA, RB, RS, ...)                                                   \
   template <>                                                                                                 \
   struct WgmmaF16<N> {                                                                                        \
     static __device__ __forceinline__ void mma(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc,           \
@@ -91,16 +95,39 @@ struct WgmmaF16;
                    : "l"(a_desc), "l"(b_desc), "r"(scale_d)                                                   \
                    : "memory");                                                                               \
     }                                                                                                         \
+    static __device__ __forceinline__ void mma_ra(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b_desc, \
+                                                  uint32_t scale_d) {                                         \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" RS ", 0;\n\t"                                     \
+                   "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 {" REGS "}, {" RA "}, %" RB        \
+                   ", p, 1, 1, 0;\n\t}"                                                                       \
+                   : __VA_ARGS__                                                                              \
+                   : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d)                    \
+                   : "memory");                                                                               \
+    }                                                                                                         \
   };
 #define UML_R4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
-UML_WGMMA_F16(16, "%0, %1, %2, %3, %4, %5, %6, %7", "8", "9", "10", UML_R4(0), UML_R4(4))
-UML_WGMMA_F16(24, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11", "12", "13", "14", UML_R4(0), UML_R4(4), UML_R4(8))
-UML_WGMMA_F16(32, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15", "16", "17", "18", UML_R4(0),
-              UML_R4(4), UML_R4(8), UML_R4(12))
+UML_WGMMA_F16(16, "%0, %1, %2, %3, %4, %5, %6, %7", "8", "9", "10", "%8, %9, %10, %11", "12", "13", UML_R4(0),
+              UML_R4(4))
+UML_WGMMA_F16(24, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11", "12", "13", "14", "%12, %13, %14, %15", "16",
+              "17", UML_R4(0), UML_R4(4), UML_R4(8))
+UML_WGMMA_F16(32, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15", "16", "17", "18",
+              "%16, %17, %18, %19", "20", "21", UML_R4(0), UML_R4(4), UML_R4(8), UML_R4(12))
 UML_WGMMA_F16(40, "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19", "20",
-              "21", "22", UML_R4(0), UML_R4(4), UML_R4(8), UML_R4(12), UML_R4(16))
+              "21", "22", "%20, %21, %22, %23", "24", "25", UML_R4(0), UML_R4(4), UML_R4(8), UML_R4(12), UML_R4(16))
 #undef UML_R4
 #undef UML_WGMMA_F16
+
+// keeps the compiler from reusing an A register of a register-A wgmma before the wgmma_wait that covers it
+__device__ __forceinline__ void wgmma_fence_operand(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+
+// two bytes of w (bytes 2i, 2i + 1) -> f16x2 with the lower byte in the low half, exactly: PRMT places each byte under
+// an exponent byte 0x64 (the f16 value 1024 + byte), HADD2 subtracts 1024
+__device__ __forceinline__ uint32_t bytes_to_half2(uint32_t w, int i) {
+  uint32_t h, r;
+  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(h) : "r"(w), "r"(0x64646464u), "r"(i == 0 ? 0x4140u : 0x4342u));
+  asm("add.rn.f16x2 %0, %1, %2;" : "=r"(r) : "r"(h), "r"(0xe400e400u));
+  return r;
+}
 
 // generic-proxy writes to shared memory (st.shared) -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
