@@ -9,9 +9,11 @@ fp16 schedule (UML_B200_LINEAR_TC=0).
 Stages the cfg 2 batch and the golden digits model once, alternates the three schedules one launch at a time (the EXACT,
 uint8-label predict_peers step bench.py times, bracketed by CUDA events), and prints one JSON object: per schedule the
 median and min-max time and n_flagged, whether the labels are byte-equal, the card's name, power limit and SM clock,
-and how many rows tier 1 leaves to the fp32 replay.  That count is estimated from float64 scores: rows whose exact
-top-2 margin is at most kappa A (the tensor-core guard's threshold; kappa as build_tc_operands computes it) or at most
-thr A (the fp32 route's; these are the rows it flags, up to its rounding).
+and how many rows tier 1 leaves to the fp32 replay.  That count is measured by one untimed call with
+UML_B200_TC_REPLAY=0 (every row tier 1 leaves then goes to float64 and counts in n_flagged), and estimated beside it
+from float64 scores as a cross-check: rows whose exact top-2 margin is at most kappa A (the tensor-core guard's
+threshold; kappa as build_tc_operands computes it) or at most thr A (the fp32 route's; these are the rows it flags, up
+to its rounding).
 """
 import argparse
 import json
@@ -76,6 +78,9 @@ def main():
                                  label_bytes=1)
 
     stats = {r: step(r, want_stats=True) for r in routes}
+    os.environ["UML_B200_TC_REPLAY"] = "0"
+    tier1 = {r: step(r, want_stats=True)["n_flagged"] for r in ("tc_bytes", "tc")}
+    os.environ.pop("UML_B200_TC_REPLAY")
     assert [stats[r]["x_read_bytes"] for r in routes] == [1, 2, 2], stats
     equal = bool(torch.equal(labels["tc"], labels["cuda_core"]) and torch.equal(labels["tc_bytes"], labels["tc"]))
     before = card()
@@ -111,7 +116,8 @@ def main():
 
     out = {"rows": n, "features": F, "launches_per_route": args.launches, "warmup_pairs": args.warmup,
            "labels_byte_equal": equal, "card_before": before, "card_after": after, "thr": thr, "kappa": kappa,
-           "rows_margin_le_kappa_A": n_kappa, "rows_margin_le_thr_A": n_thr, "routes": {}}
+           "tier1_left_measured": tier1, "rows_margin_le_kappa_A": n_kappa, "rows_margin_le_thr_A": n_thr,
+           "routes": {}}
     for r in routes:
         out["routes"][r] = {"ms_median": statistics.median(ms[r]), "ms_min": min(ms[r]), "ms_max": max(ms[r]),
                             "n_flagged": stats[r]["n_flagged"]}

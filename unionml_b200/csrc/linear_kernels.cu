@@ -1569,6 +1569,11 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   p.num_stages = stages;
   // margin > 2 err guarantees the fp32 argmax is the exact argmax; err <= (F+4) 2^-24 A (1 + F 2^-21), see DESIGN.md
   p.thr = linear_margin_thr(m.n_features);
+  // UML_B200_TC_REPLAY=0 (read per call; a test hook): in the tensor-core schedules p.thr is read only by tier 2's
+  // replay, which then certifies no row, so every row tier 1 leaves goes to fp64 and n_flagged counts exactly those
+  // rows (DESIGN.md 3.2).  The kernels are unchanged.
+  const char* replay_env = getenv("UML_B200_TC_REPLAY");
+  if (tc && replay_env && replay_env[0] == '0') p.thr = INFINITY;
   p.flag_count = flags.count;
   p.flag_rows = flags.rows;
   p.flag_cap = flags.capacity;
