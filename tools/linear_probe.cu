@@ -1,5 +1,5 @@
 // Where the time of the linear tile kernel goes, on 10M x 64 fp32 rows (2.56 GB, the cfg2 shape), on their compact
-// fp16 copy (1.28 GB) and on their byte copy (0.64 GB), against the card's own read ceiling.  Built nine times by
+// fp16 copy (1.28 GB) and on their byte copy (0.64 GB), against the card's own read ceiling.  Built eleven times by
 // tools/linear_probe.sh from linear_kernels.cu itself:
 //   plain                   read ceiling (streaming 16-byte non-allocating loads) over 2.56 GB, 1.28 GB and 0.64 GB +
 //                           the tile kernel, the three CUDA-core schedules and both tensor-core ones (kHalfMma on the
@@ -15,6 +15,8 @@
 //   -DUML_PROBE_NO_W, -DUML_PROBE_NO_X, both   the fp16 schedule without its W loads, without its x loads and
 //                           conversions, and with neither (the FMAs and the epilogue alone): which of the scoring
 //                           warps' operands the time above the feed pays for.  Wrong scores by design.
+//   -DUML_PROBE_NO_EPILOGUE, -DUML_PROBE_NO_HANDOFF   the byte schedule alone, without its per-item epilogue (wgmma
+//                           and stage release only) and with tier 1's verdict forced to "certified" (no queue hand-off)
 //   -DUML_PROBE_HALF_ONLY   the fp16 schedule alone, and once more with -DUML_PROBE_HALF_PASS_ROWS=4 (256-row stages
 //                           scored in two passes of 4 rows per lane by the same four warps): the script runs the two
 //                           alternately, which separates the W reuse of 8 rows per lane from the warp count
@@ -149,6 +151,10 @@ int main() {
   const char* build = "no_w_loads";
 #elif defined(UML_PROBE_NO_X)
   const char* build = "no_x_loads";
+#elif defined(UML_PROBE_NO_EPILOGUE)
+  const char* build = "no_epilogue";
+#elif defined(UML_PROBE_NO_HANDOFF)
+  const char* build = "no_handoff";
 #elif defined(UML_PROBE_FEED_ONLY)
   const char* build = "feed_only";
 #elif defined(UML_PROBE_WAIT_CLOCKS)
@@ -277,7 +283,7 @@ int main() {
     p.num_tiles = (kRows + tile - 1) / tile;
     p.f_pad = kF;
     p.kc = kF / kChunkF;
-    const size_t fixed = tma_fixed_smem(m, f16 || byte) + (tc ? linear_tc_b_bytes(kC) : 0);
+    const size_t fixed = tma_fixed_smem(m, f16 || byte) + (tc ? linear_tc_b_bytes(kC) : 0) + linear_epi_bytes(sched, kC);
     const int stage_bytes = linear_stage_bytes(sched);
     p.num_stages = std::min(64, static_cast<int>((kMaxSmemBytes - fixed) / stage_bytes));
     p.thr = static_cast<float>(2.0 * (kF + 4.0) * 5.9604644775390625e-08 * (1.0 + kF * 4.76837158203125e-07) * 1.0001);
@@ -402,6 +408,10 @@ int main() {
   };
 #ifdef UML_PROBE_HALF_ONLY
   run(LinearSched::kHalf, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
+  return 0;
+#endif
+#if defined(UML_PROBE_NO_EPILOGUE) || defined(UML_PROBE_NO_HANDOFF)
+  run(LinearSched::kByteMma, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");
   return 0;
 #endif
   run(LinearSched::kChunked, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "256B");

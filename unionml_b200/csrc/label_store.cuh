@@ -30,17 +30,19 @@ __device__ __forceinline__ void store_label_i32(const LabelTargets& t, long long
 // differently.
 
 // byte labels of rows row4 .. row4 + 3 (row row4 + b in byte b of `word`) into every peer of p.targets, from the lanes
-// that hold a word (`active`): one aligned 4-byte store when all four rows are in the batch and the destination is word
-// aligned, else one byte per row in the batch
+// that hold a word (`active`): one aligned 4-byte store when all four rows are in the batch, all four are kept and the
+// destination is word aligned, else one byte per kept row in the batch.  `keep` bit b clear: row row4 + b has another
+// writer (a row the linear tensor-core schedule queued for its re-score warp), so its byte is not touched.
 template <class P>
-__device__ __forceinline__ void store_label_word_u8(const P& p, long long row4, uint32_t word, bool active) {
+__device__ __forceinline__ void store_label_word_u8(const P& p, long long row4, uint32_t word, bool active,
+                                                    unsigned keep = 0xfu) {
   const long long at = p.targets.row_offset + row4;
   if (active) {
-    if (row4 + 3 < p.n_rows && (at & 3) == 0) {
+    if (keep == 0xfu && row4 + 3 < p.n_rows && (at & 3) == 0) {
       for (int i = 0; i < p.targets.n_peers; ++i) *reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(p.targets.peers[i]) + at) = word;
     } else {
       for (int b = 0; b < 4; ++b)
-        if (row4 + b < p.n_rows)
+        if (((keep >> b) & 1u) && row4 + b < p.n_rows)
           for (int i = 0; i < p.targets.n_peers; ++i)
             static_cast<uint8_t*>(p.targets.peers[i])[at + b] = static_cast<uint8_t>((word >> (8 * b)) & 0xffu);
     }

@@ -200,6 +200,20 @@ constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this ma
 //                         so the scoring loop issues no W loads
 //  UML_PROBE_NO_X         kHalf only, wrong scores: every feature of a row is one register set once per warp, so the
 //                         scoring loop issues no x loads and no fp16 conversions (both defines: the FMAs alone)
+//  UML_PROBE_NO_EPILOGUE  kByteMma only, no labels: the warpgroups issue their wgmma and hand the stages back, and skip
+//                         the score write-out, the top-2, the label stores and the queue hand-off
+//  UML_PROBE_NO_HANDOFF   kByteMma only, wrong labels for near-ties: tier 1's verdict is forced to "certified", so no
+//                         row goes through the queue
+#ifdef UML_PROBE_NO_EPILOGUE
+constexpr bool kProbeNoEpilogue = true;
+#else
+constexpr bool kProbeNoEpilogue = false;
+#endif
+#ifdef UML_PROBE_NO_HANDOFF
+constexpr bool kProbeNoHandoff = true;
+#else
+constexpr bool kProbeNoHandoff = false;
+#endif
 #ifdef UML_PROBE_NO_W
 constexpr bool kProbeNoW = true;
 #else
@@ -281,6 +295,12 @@ __host__ __device__ constexpr int linear_stage_bytes(LinearSched s) {
 }
 // tensor-core schedules: bytes of the B operand in shared memory (rounded up to the 1 KiB that keeps what follows aligned)
 __host__ __device__ constexpr int linear_tc_b_bytes(int C) { return (linear_tc_cols(C) * 128 + 1023) / 1024 * 1024; }
+// kByteMma: each scoring warp's score buffer, the C + 1 folded columns (classes, bound) of its 64 rows, column-major
+// with a pitch of kEpiPitch floats (the bank argument is at the write-out in the kernel)
+constexpr int kEpiPitch = 68;
+__host__ __device__ constexpr int linear_epi_bytes(LinearSched s, int C) {
+  return s == LinearSched::kByteMma ? linear_consumer_warps(s) * (C + 1) * kEpiPitch * 4 : 0;
+}
 
 // kHalfMma's tier 2 (DESIGN.md 3.2): the fp32 route's scores of one row, replayed bit for bit by one warp: lane c <= C
 // runs column c's FMA chain in feature order from bias_s[c] over the caller's fp32 row (zeros past F, as the fp32 route's
@@ -395,6 +415,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   // CLAIMED: the tile each stage holds, written by the producer before the stage's `full` arrive (whose release makes it
   // visible to the waiters); kTileSentinel ends a scoring warp's loop
   int* tile_slot = q_ctl + 4;
+  // kByteMma: the scoring warps' score buffers (linear_epi_bytes), behind the 64 tile slots the host reserves
+  [[maybe_unused]] float* epi_buf = reinterpret_cast<float*>(tile_slot + 64);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -786,13 +808,11 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
 
     if constexpr (MMA) {
       // ===== kHalfMma, kByteMma: warpgroup wg = warp / 4 takes ring items wg, wg + NCU, ...; per item four m64 blocks of
-      // 64 rows x NT columns, f_pad / 16 k16 steps each, one commit group (kByteMma: one per block); the stage goes back
-      // after the wait, the epilogue runs from registers.  Fragment (WgmmaTf32's layout): thread (warp w, lane l) holds
-      // rows 16 (w % 4) + l / 4 and the row 8 below of each block, columns 8 i + 2 (l % 4) + {0, 1}: class c's hi piece
-      // at c, its lo piece at NH + c, the bound column at C - all of a row in one quad ----
+      // 64 rows x NT columns, f_pad / 16 k16 steps each.  Fragment (WgmmaTf32's layout): thread (warp w, lane l) holds
+      // fragment rows 16 (w % 4) + l / 4 and the row 8 below of each block, columns 8 i + 2 (l % 4) + {0, 1}: class c's
+      // hi piece at c, its lo piece at NH + c, the bound column at C - all of a row in one quad ----
       constexpr int NH = linear_tc_hi_cols(C), NT = linear_tc_cols(C), NL = NT - NH;
       const int q = lane & 3;
-      const long long row_in = 16 * (warp & 3) + (lane >> 2);  // row of fragment row-half 0 in block 0
       const float* tcb = reinterpret_cast<const float*>(static_cast<const uint8_t*>(p.tc_ops) + NT * 128);
       float bz[NH / 8][2];
 #pragma unroll
@@ -803,137 +823,165 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       const uint32_t b_base = smem_u32(smem + static_cast<size_t>(S) * STAGE_BYTES);
       const int nk = p.f_pad / 16;
       const float kappa = p.tc_kappa;
-      // scores, top-2 and the tier-1 guard of the 8 rows whose columns this thread's quad holds; quad lane q then stores
-      // and (if not certified) publishes the two rows of block q, so every row leaves once
-      auto finish_mma = [&](float (&d)[4][NT / 2], long long row0) {
-        int lab[4][2];
-        bool flg[4][2];
+      if constexpr (BYTES) {
+        // ----- kByteMma.  A comes from registers, so the kernel picks the tile row of each fragment row: warp w's
+        // fragment rows of block b are tile rows 64 (w % 4) + 16 b + {l / 4, l / 4 + 8}, and every warp owns 64
+        // consecutive rows of the tile.  Per block (one commit group) a thread loads its two fragment rows with one
+        // LDS.128 each (the eight lanes of a phase read two whole 64-byte rows: conflict-free), widens the bytes to the
+        // f16 values kHalfMma reads and issues the block's wgmma.  The stage goes back as soon as the last block's A
+        // fragments are in registers (B lives outside the ring).  Once a block's group is done its scores are folded
+        // as finish_mma folds them, (hi + lo) + bz, into the warp's own buffer, which frees the accumulators; then lane
+        // l scores rows l and l + 32 of the warp from the buffer with the fp32 route's sequential top-2: the same
+        // values and comparisons as finish_mma's quad merge, so labels and tier-1 verdicts are the same bit for bit.
+        float* eb = epi_buf + warp * (C + 1) * kEpiPitch;  // column c of the warp's row r at eb[c * kEpiPitch + r]
+        const int rw = 64 * (warp & 3);                     // the warp's first row in the tile
+        // Bank of the write of (block b, half h, column 8 i + 2 q + e) by lane l = 4 t + q: (8 i + 2 q + e) * 68 + 16 b +
+        // 8 h + t = 8 q + t + (32 i + 4 e + 16 b + 8 h) mod 32, so the warp's 32 lanes (t < 8, q < 4) hit 32 banks.  The
+        // reads (column c of rows l and l + 32) are 32 consecutive words.
+        static_assert(kEpiPitch % 32 == 4 && kEpiPitch >= 64, "conflict-free write-out and reads");
+        auto write_out = [&](float (&db)[NT / 2], int b) {
+          if constexpr (kProbeNoEpilogue) return;
 #pragma unroll
-        for (int b = 0; b < 4; ++b) {
+          for (int h = 0; h < 2; ++h)
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float best = -INFINITY, second = -INFINITY, bound = 0.f;
-            int bi = C;  // a thread without classes loses every tie
-#pragma unroll
-            for (int i = 0; i < NH / 8; ++i) {
+            for (int i = 0; i < NH / 8; ++i)
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const int c = 8 * i + 2 * q + e;
-                const float lo = i < NL / 8 ? d[b][4 * (NH / 8 + i) + 2 * h + e] : 0.f;
-                const float v = (d[b][4 * i + 2 * h + e] + lo) + bz[i][e];
-                if (c < C) {
-                  if (v > best) {
-                    second = best;
-                    best = v;
-                    bi = c;
-                  } else {
-                    second = fmaxf(second, v);
-                  }
-                } else if (c == C) {
-                  bound = v;
-                }
+                const float lo = i < NL / 8 ? db[4 * (NH / 8 + i) + 2 * h + e] : 0.f;
+                if (c <= C) eb[c * kEpiPitch + 16 * b + 8 * h + (lane >> 2)] = (db[4 * i + 2 * h + e] + lo) + bz[i][e];
               }
-            }
-            // merge over the quad: the larger score wins, the lower class on a tie (first maximum, like np.argmax)
+        };
+        // top-2 and tier 1 of rows row0 + l and row0 + l + 32 (the warp's rows), their label stores and the queue
+        // hand-off.  Every row has one writer: certified rows are stored here, queued rows only by the re-score warp
+        // (settle_row_tc stores every target).  So a queued row carries no provisional label that the re-score warp's
+        // store must be ordered after, and publication needs no device-scope fence: the slot's shared-memory atomic
+        // carries the row index, and nothing this warp wrote to global memory is read or overwritten by the drain.  The
+        // byte words of peers leave out queued rows' bytes (store_label_word_u8's `keep`), so a peer's byte has one
+        // writer as well.
+        auto score_rows = [&](long long row0) {
+          if constexpr (kProbeNoEpilogue) return;
+          __syncwarp();  // the warp's write-out is visible to every lane
+          int lab[2];
+          bool flg[2];
 #pragma unroll
-            for (int off = 1; off <= 2; off <<= 1) {
-              const float ob = __shfl_xor_sync(0xffffffffu, best, off);
-              const float os = __shfl_xor_sync(0xffffffffu, second, off);
-              const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-              if (ob > best || (ob == best && oi < bi)) {
-                second = fmaxf(best, os);
-                best = ob;
-                bi = oi;
+          for (int j = 0; j < 2; ++j) {
+            const float* col = eb + lane + 32 * j;
+            float best = col[0], second = -INFINITY;
+            int bi = 0;
+#pragma unroll
+            for (int c = 1; c < C; ++c) {
+              const float v = col[c * kEpiPitch];
+              if (v > best) {
+                second = best;
+                best = v;
+                bi = c;
               } else {
-                second = fmaxf(second, ob);
+                second = fmaxf(second, v);
               }
             }
-            const float a = __shfl_sync(0xffffffffu, bound, (lane & ~3) | ((C % 8) / 2));
-            const long long row = row0 + b * 64 + row_in + 8 * h;
-            lab[b][h] = bi;
+            const float a = col[C * kEpiPitch];
+            lab[j] = bi;
             // tier 1: certain iff margin > kappa A; NaN / Inf anywhere makes the comparison false
-            flg[b][h] = row < p.n_rows && !((best - second) > kappa * a);
+            flg[j] = !kProbeNoHandoff && row0 + lane + 32 * j < p.n_rows && !((best - second) > kappa * a);
           }
-        }
-        unsigned masks[2];
-        int total = 0;
+          __syncwarp();  // every lane has read the buffer before the next item's write-out
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int idx = q == 0 ? lab[0][h] : q == 1 ? lab[1][h] : q == 2 ? lab[2][h] : lab[3][h];
-          const bool flag = q == 0 ? flg[0][h] : q == 1 ? flg[1][h] : q == 2 ? flg[2][h] : flg[3][h];
-          const long long row = row0 + q * 64 + row_in + 8 * h;
-          if (row < p.n_rows) store_label(p.targets, row, idx);
-          masks[h] = __ballot_sync(0xffffffffu, flag);
-          total += __popc(masks[h]);
-        }
-        if (total == 0) return;
-        // the (few) uncertified rows go to the re-score warp, as in finish_rows: the labels above are provisional.  When
-        // the queue is backed up (most rows near-ties) the warp waits for room instead of settling its rows itself: a
-        // call from this loop made ptxas save the loop's live registers around it, spill stores and loads in the hot
-        // path at every class count (-Xptxas -v).  The drain never waits for a scoring warp, so the wait ends.
-        auto row_of = [&](int l, int h) { return row0 + (l & 3) * 64 + 16 * (warp & 3) + (l >> 2) + 8 * h; };
-        __threadfence();
-        int base = -1;
-        if (lane == 0) {
-          for (;;) {
-            const int tail = atomicAdd(&q_ctl[0], 0);
-            const int consumed = atomicAdd(&q_ctl[3], 0);
-            if (tail - consumed <= kQueueCap - HEADROOM) break;
-            __nanosleep(500);
+          for (int j = 0; j < 2; ++j) {
+            const long long row = row0 + lane + 32 * j;
+            if (row < p.n_rows && !flg[j]) store_label_i32(p.targets, row, lab[j]);
           }
-          base = atomicAdd(&q_ctl[0], total);
-        }
-        base = __shfl_sync(0xffffffffu, base, 0);
-        int off = base;
+          if (p.targets.wire_u8 && p.targets.n_peers > 0) {
+            // lane l < 16 gathers rows 4 l .. 4 l + 3 (row 4 l + t sits in lane (4 l + t) % 32, half l / 8) into one word,
+            // and the bits of the queued ones into `keep`
+            const uint32_t packed = static_cast<uint32_t>(lab[0]) | static_cast<uint32_t>(lab[1]) << 8 |
+                                    (flg[0] ? 1u << 16 : 0u) | (flg[1] ? 1u << 17 : 0u);
+            uint32_t word = 0;
+            unsigned keep = 0;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if ((masks[h] >> lane) & 1u) {
-            const int slot = (off + __popc(masks[h] & ((1u << lane) - 1u))) & (kQueueCap - 1);
-            while (atomicAdd(&q_slots[slot], 0) != 0) {
+            for (int t = 0; t < 4; ++t) {
+              const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
+              word |= ((w >> (8 * (lane >> 3))) & 0xffu) << (8 * t);
+              keep |= ((w >> (16 + (lane >> 3))) & 1u) ? 0u : 1u << t;
             }
-            atomicExch(&q_slots[slot], static_cast<int>(row_of(lane, h)) + 1);
+            store_label_word_u8(p, row0 + 4 * lane, word, lane < 16, keep);
           }
-          off += __popc(masks[h]);
-        }
-      };
-      uint32_t stage = static_cast<uint32_t>(warp >> 2), phase = 0;
-      for (bool first = true; scoring_warp; first = false) {
-        UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
-        UML_PROBE_CLOCK(probe_landed);
-        UML_PROBE_LANDED(first);
-        const int tile = tile_slot[stage];
-        const bool scored = !kFeedOnly && tile >= 0 && tile < num_tiles;
-        float d[4][NT / 2];
-        if (scored) {
-          [[maybe_unused]] const uint32_t a_base = smem_u32(smem + static_cast<size_t>(stage) * STAGE_BYTES);
+          unsigned masks[2];
+          int total = 0;
 #pragma unroll
-          for (int b = 0; b < 4; ++b)
-#pragma unroll
-            for (int r = 0; r < NT / 2; ++r) {
-              d[b][r] = 0.f;
-              wgmma_fence_operand(d[b][r]);
+          for (int j = 0; j < 2; ++j) {
+            masks[j] = __ballot_sync(0xffffffffu, flg[j]);
+            total += __popc(masks[j]);
+          }
+          if (total == 0) return;
+          // When the queue is backed up (most rows near-ties) the warp waits for room: the drain never waits for a
+          // scoring warp, so the wait ends
+          int base = -1;
+          if (lane == 0) {
+            for (;;) {
+              const int tail = atomicAdd(&q_ctl[0], 0);
+              const int consumed = atomicAdd(&q_ctl[3], 0);
+              if (tail - consumed <= kQueueCap - HEADROOM) break;
+              __nanosleep(500);
             }
-          if constexpr (BYTES) {
-            // one commit group per m64 block, its A fragments (f16 values equal to the bytes) loaded and converted just
-            // before it; a block's registers are free once its group is done, so at most two blocks' A fragments are
-            // live (all four would be 64 registers more than the 128 of three warpgroups)
+            base = atomicAdd(&q_ctl[0], total);
+          }
+          int off = __shfl_sync(0xffffffffu, base, 0);
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            if (flg[j]) {
+              const int slot = (off + __popc(masks[j] & ((1u << lane) - 1u))) & (kQueueCap - 1);
+              while (atomicAdd(&q_slots[slot], 0) != 0) {  // only if the slot's previous ticket is claimed but not read yet
+              }
+              atomicExch(&q_slots[slot], static_cast<int>(row0 + lane + 32 * j) + 1);
+            }
+            off += __popc(masks[j]);
+          }
+        };
+        // (at NT = 40, C = 16, two blocks' fragments beside 80 accumulators made ptxas serialize the wgmma chain)
+        constexpr int INFLIGHT = NT >= 40 ? 1 : 2;
+        uint32_t stage = static_cast<uint32_t>(warp >> 2), phase = 0;
+        for (bool first = true; scoring_warp; first = false) {
+          UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
+          UML_PROBE_CLOCK(probe_landed);
+          UML_PROBE_LANDED(first);
+          const int tile = tile_slot[stage];
+          const bool scored = !kFeedOnly && tile >= 0 && tile < num_tiles;
+          auto release = [&] {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);  // the fourth warp's arrive hands the stage back
+            UML_PROBE_SINCE(probe_hold, probe_landed);
+            UML_PROBE_RELEASED();
+          };
+          if (scored) {
+            float d[4][NT / 2];
             uint32_t a[4][kHalfBoxF / 16][4];
-            const uint8_t* xs = smem + static_cast<size_t>(stage) * STAGE_BYTES + row_in * kByteRowBytes + 16 * q;
-            // (at NT = 40, C = 16, two blocks' fragments beside 80 accumulators made ptxas serialize the wgmma chain)
-            constexpr int INFLIGHT = NT >= 40 ? 1 : 2;
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+              for (int r = 0; r < NT / 2; ++r) {
+                d[b][r] = 0.f;
+                wgmma_fence_operand(d[b][r]);
+              }
+            const uint8_t* xs = smem + static_cast<size_t>(stage) * STAGE_BYTES + (rw + (lane >> 2)) * kByteRowBytes + 16 * q;
+            // block b's group is done: its A registers may be reused, its scores go to the buffer
+            auto retire = [&](int b) {
+#pragma unroll
+              for (int k = 0; k < kHalfBoxF / 16; ++k)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) wgmma_fence_operand(a[b][k][i]);
+#pragma unroll
+              for (int r = 0; r < NT / 2; ++r) wgmma_fence_operand(d[b][r]);
+              write_out(d[b], b);
+            };
 #pragma unroll
             for (int b = 0; b < 4; ++b) {
               if (b >= INFLIGHT) {
                 wgmma_wait<INFLIGHT - 1>();
-#pragma unroll
-                for (int k = 0; k < kHalfBoxF / 16; ++k)
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) wgmma_fence_operand(a[b - INFLIGHT][k][i]);
+                retire(b - INFLIGHT);
               }
-              // the 16 bytes at 16 q of rows row_in and row_in + 8 of the block, one LDS.128 each (the eight lanes of a
-              // phase read two whole 64-byte rows: conflict-free)
-              const uint4 x0 = *reinterpret_cast<const uint4*>(xs + b * 64 * kByteRowBytes);
-              const uint4 x1 = *reinterpret_cast<const uint4*>(xs + (b * 64 + 8) * kByteRowBytes);
+              const uint4 x0 = *reinterpret_cast<const uint4*>(xs + 16 * b * kByteRowBytes);
+              const uint4 x1 = *reinterpret_cast<const uint4*>(xs + (16 * b + 8) * kByteRowBytes);
 #pragma unroll
               for (int k = 0; k < kHalfBoxF / 16; ++k) {
                 const uint32_t w0 = k == 0 ? x0.x : k == 1 ? x0.y : k == 2 ? x0.z : x0.w;
@@ -943,6 +991,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
                 a[b][k][2] = bytes_to_half2(w0, 1);
                 a[b][k][3] = bytes_to_half2(w1, 1);
               }
+              if (b == 3) release();
               wgmma_fence();
 #pragma unroll
               for (int k = 0; k < kHalfBoxF / 16; ++k) {
@@ -952,12 +1001,131 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             }
             wgmma_wait<0>();
 #pragma unroll
-            for (int b = 4 - INFLIGHT; b < 4; ++b)
-#pragma unroll
-              for (int k = 0; k < kHalfBoxF / 16; ++k)
-#pragma unroll
-                for (int i = 0; i < 4; ++i) wgmma_fence_operand(a[b][k][i]);
+            for (int b = 4 - INFLIGHT; b < 4; ++b) retire(b);
           } else {
+            release();
+          }
+          if (tile == kTileSentinel) break;
+          stage += NCU;
+          if (stage >= static_cast<uint32_t>(S)) {
+            stage -= S;
+            phase ^= 1u;
+          }
+          if (scored) score_rows(static_cast<long long>(tile) * TILE + rw);
+        }
+      } else {
+        // ----- kHalfMma: one commit group per item; the stage goes back after the wait, the epilogue runs from registers
+        const long long row_in = 16 * (warp & 3) + (lane >> 2);  // row of fragment row-half 0 in block 0
+        // scores, top-2 and the tier-1 guard of the 8 rows whose columns this thread's quad holds; quad lane q then stores
+        // and (if not certified) publishes the two rows of block q, so every row leaves once
+        auto finish_mma = [&](float (&d)[4][NT / 2], long long row0) {
+          int lab[4][2];
+          bool flg[4][2];
+#pragma unroll
+          for (int b = 0; b < 4; ++b) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float best = -INFINITY, second = -INFINITY, bound = 0.f;
+              int bi = C;  // a thread without classes loses every tie
+#pragma unroll
+              for (int i = 0; i < NH / 8; ++i) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int c = 8 * i + 2 * q + e;
+                  const float lo = i < NL / 8 ? d[b][4 * (NH / 8 + i) + 2 * h + e] : 0.f;
+                  const float v = (d[b][4 * i + 2 * h + e] + lo) + bz[i][e];
+                  if (c < C) {
+                    if (v > best) {
+                      second = best;
+                      best = v;
+                      bi = c;
+                    } else {
+                      second = fmaxf(second, v);
+                    }
+                  } else if (c == C) {
+                    bound = v;
+                  }
+                }
+              }
+              // merge over the quad: the larger score wins, the lower class on a tie (first maximum, like np.argmax)
+#pragma unroll
+              for (int off = 1; off <= 2; off <<= 1) {
+                const float ob = __shfl_xor_sync(0xffffffffu, best, off);
+                const float os = __shfl_xor_sync(0xffffffffu, second, off);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+                if (ob > best || (ob == best && oi < bi)) {
+                  second = fmaxf(best, os);
+                  best = ob;
+                  bi = oi;
+                } else {
+                  second = fmaxf(second, ob);
+                }
+              }
+              const float a = __shfl_sync(0xffffffffu, bound, (lane & ~3) | ((C % 8) / 2));
+              const long long row = row0 + b * 64 + row_in + 8 * h;
+              lab[b][h] = bi;
+              // tier 1: certain iff margin > kappa A; NaN / Inf anywhere makes the comparison false
+              flg[b][h] = row < p.n_rows && !((best - second) > kappa * a);
+            }
+          }
+          unsigned masks[2];
+          int total = 0;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int idx = q == 0 ? lab[0][h] : q == 1 ? lab[1][h] : q == 2 ? lab[2][h] : lab[3][h];
+            const bool flag = q == 0 ? flg[0][h] : q == 1 ? flg[1][h] : q == 2 ? flg[2][h] : flg[3][h];
+            const long long row = row0 + q * 64 + row_in + 8 * h;
+            if (row < p.n_rows) store_label(p.targets, row, idx);
+            masks[h] = __ballot_sync(0xffffffffu, flag);
+            total += __popc(masks[h]);
+          }
+          if (total == 0) return;
+          // the (few) uncertified rows go to the re-score warp, as in finish_rows: the labels above are provisional.  When
+          // the queue is backed up (most rows near-ties) the warp waits for room instead of settling its rows itself: a
+          // call from this loop made ptxas save the loop's live registers around it, spill stores and loads in the hot
+          // path at every class count (-Xptxas -v).  The drain never waits for a scoring warp, so the wait ends.
+          auto row_of = [&](int l, int h) { return row0 + (l & 3) * 64 + 16 * (warp & 3) + (l >> 2) + 8 * h; };
+          __threadfence();
+          int base = -1;
+          if (lane == 0) {
+            for (;;) {
+              const int tail = atomicAdd(&q_ctl[0], 0);
+              const int consumed = atomicAdd(&q_ctl[3], 0);
+              if (tail - consumed <= kQueueCap - HEADROOM) break;
+              __nanosleep(500);
+            }
+            base = atomicAdd(&q_ctl[0], total);
+          }
+          base = __shfl_sync(0xffffffffu, base, 0);
+          int off = base;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if ((masks[h] >> lane) & 1u) {
+              const int slot = (off + __popc(masks[h] & ((1u << lane) - 1u))) & (kQueueCap - 1);
+              while (atomicAdd(&q_slots[slot], 0) != 0) {
+              }
+              atomicExch(&q_slots[slot], static_cast<int>(row_of(lane, h)) + 1);
+            }
+            off += __popc(masks[h]);
+          }
+        };
+        uint32_t stage = static_cast<uint32_t>(warp >> 2), phase = 0;
+        for (bool first = true; scoring_warp; first = false) {
+          UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
+          UML_PROBE_CLOCK(probe_landed);
+          UML_PROBE_LANDED(first);
+          const int tile = tile_slot[stage];
+          const bool scored = !kFeedOnly && tile >= 0 && tile < num_tiles;
+          float d[4][NT / 2];
+          if (scored) {
+            [[maybe_unused]] const uint32_t a_base = smem_u32(smem + static_cast<size_t>(stage) * STAGE_BYTES);
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+              for (int r = 0; r < NT / 2; ++r) {
+                d[b][r] = 0.f;
+                wgmma_fence_operand(d[b][r]);
+              }
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < kHalfBoxF / 16; ++k) {
@@ -970,23 +1138,23 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
             }
             wgmma_commit();
             wgmma_wait<0>();
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+              for (int r = 0; r < NT / 2; ++r) wgmma_fence_operand(d[b][r]);
           }
-#pragma unroll
-          for (int b = 0; b < 4; ++b)
-#pragma unroll
-            for (int r = 0; r < NT / 2; ++r) wgmma_fence_operand(d[b][r]);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);  // the fourth warp's arrive hands the stage back
+          UML_PROBE_SINCE(probe_hold, probe_landed);
+          UML_PROBE_RELEASED();
+          if (tile == kTileSentinel) break;
+          stage += NCU;
+          if (stage >= static_cast<uint32_t>(S)) {
+            stage -= S;
+            phase ^= 1u;
+          }
+          if (scored) finish_mma(d, static_cast<long long>(tile) * TILE);
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);  // the fourth warp's arrive hands the stage back
-        UML_PROBE_SINCE(probe_hold, probe_landed);
-        UML_PROBE_RELEASED();
-        if (tile == kTileSentinel) break;
-        stage += NCU;
-        if (stage >= static_cast<uint32_t>(S)) {
-          stage -= S;
-          phase ^= 1u;
-        }
-        if (scored) finish_mma(d, static_cast<long long>(tile) * TILE);
       }
     } else if constexpr (CLAIMED) {
       // this warp's ring items are n = warp, warp + NCW, ... (stage n % S, phase (n / S) & 1); S >= NCW lets stage and
@@ -1559,7 +1727,8 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
   p.kc = m.f_pad / kChunkF;
   p.tc_ops = m.tc_ops;
   p.tc_kappa = m.tc_kappa;
-  const size_t fixed = tma_fixed_smem(m, half) + (tc ? linear_tc_b_bytes(m.n_classes) : 0);
+  const size_t fixed =
+      tma_fixed_smem(m, half) + (tc ? linear_tc_b_bytes(m.n_classes) : 0) + linear_epi_bytes(sched, m.n_classes);
   const int stage_bytes = linear_stage_bytes(sched);
   int stages = static_cast<int>((static_cast<size_t>(kMaxSmemBytes) - fixed) / stage_bytes);
   stages = std::min(stages, 64);
