@@ -240,8 +240,8 @@ int main() {
   uint8_t* labels = nullptr;
   unsigned long long* counters = nullptr;
   CK(cudaMalloc(&labels, kRows));
-  CK(cudaMalloc(&counters, 16 * sizeof(unsigned long long)));
-  CK(cudaMemset(counters, 0, 16 * sizeof(unsigned long long)));
+  CK(cudaMalloc(&counters, 24 * sizeof(unsigned long long)));  // the kernel's slots, then probe_clocks from 8
+  CK(cudaMemset(counters, 0, 24 * sizeof(unsigned long long)));
 #ifdef UML_PROBE_TIMELINE
   unsigned long long* timeline = nullptr;  // [2 launches][grid][5]
   const size_t timeline_words = 2 * static_cast<size_t>(prop.multiProcessorCount) * 5;
@@ -324,7 +324,7 @@ int main() {
            read_bytes / ms * 1e-6);
 #ifdef UML_PROBE_WAIT_CLOCKS
     // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time
-    CK(cudaMemset(counters + 8, 0, 7 * sizeof(unsigned long long)));
+    CK(cudaMemset(counters + 8, 0, 10 * sizeof(unsigned long long)));
     unsigned long long flagged0 = 0, flagged1 = 0;
     CK(cudaMemcpy(&flagged0, counters + kCounterFlagged, 8, cudaMemcpyDeviceToHost));
     cudaEvent_t a, b;
@@ -336,12 +336,13 @@ int main() {
     CK(cudaEventSynchronize(b));
     float one = 0.f;
     CK(cudaEventElapsedTime(&one, a, b));
-    unsigned long long c[7];
+    unsigned long long c[10];
     CK(cudaMemcpy(c, counters + 8, sizeof(c), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(&flagged1, counters + kCounterFlagged, 8, cudaMemcpyDeviceToHost));
     // mean stages per CTA landed and not yet released (one scoring warp per stage, four in the tensor-core
     // schedules): the scoring warps' summed hold time over one warp's loop time, per CTA
-    const int scoring_warps = grid * linear_consumer_warps(sched);
+    // (kByteMma: the MMA warps; its epilogue warps report in [8] and [9])
+    const int scoring_warps = grid * (tc ? 4 * linear_ring_units(sched) : linear_consumer_warps(sched));
     const double held_stages =
         static_cast<double>(c[4]) / (static_cast<double>(c[3]) / scoring_warps) / grid / (tc ? 4 : 1);
     printf(", \"producer_empty_wait_frac\": %.4f, \"consumer_full_wait_frac\": %.4f, \"held_stages\": %.3f, "
@@ -350,6 +351,9 @@ int main() {
            static_cast<double>(c[0]) / c[1], static_cast<double>(c[2]) / c[3], held_stages,
            p.num_stages, static_cast<double>(c[1]) / grid / (one * 1e3), c[6] ? static_cast<double>(c[5]) / c[6] : 0.0,
            flagged1 - flagged0);
+    if (byte)  // MMA warps' waits for a free score slot over their loop; epilogue warps' waits for a full one over theirs
+      printf(", \"mma_slot_wait_frac\": %.4f, \"epilogue_full_wait_frac\": %.4f", static_cast<double>(c[7]) / c[3],
+             c[9] ? static_cast<double>(c[8]) / c[9] : 0.0);
 #endif
 #ifdef UML_PROBE_TIMELINE
     // two launches back to back, each stamping its own [grid][5] block

@@ -4,8 +4,8 @@
 # whether that schedule is bound by its feed or by its scoring warps), and the feed of the byte rows' 16 KiB stages
 # against the read ceiling over their 0.64 GB; then the fp16 schedule without its W loads,
 # without its x loads, and with neither; then the fp16 schedule with 4 rows per lane per pass and with the library's 8,
-# alternating (both with four scoring warps and 256-row stages); then the byte schedule without its per-item epilogue
-# and without its queue hand-off.
+# alternating (both with four scoring warps and 256-row stages); then the byte schedule without its per-row epilogue
+# (its epilogue warps hand every score slot back unread) and without its queue hand-off.
 # Writes MEASURED_PEAKS.json (the read ceiling bench.py's roofline divides by) and the probe's JSON lines to
 # ${1:-build/probe}/linear_probe.jsonl.  Binaries go to build/probe/.
 set -euo pipefail

@@ -156,7 +156,7 @@ struct TmaKernelParams {
   int binary;
   unsigned long long* counters;
 #ifdef UML_PROBE_WAIT_CLOCKS
-  unsigned long long* probe_clocks;  // [7], see the diagnostic builds below
+  unsigned long long* probe_clocks;  // [10], see the diagnostic builds below
 #endif
 #ifdef UML_PROBE_TIMELINE
   unsigned long long* probe_timeline;  // [gridDim.x][5], see the diagnostic builds below
@@ -193,15 +193,17 @@ constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this ma
 //                         loop, [2] the scoring warps' waits for their data, [3] their whole loops, [4] the time they
 //                         hold a landed stage (from the return of the `full` wait to the `empty` arrive); QUEUE
 //                         kernels also [5] the re-score warp's time on rows it took from the queue (replay and fp64
-//                         re-score) and [6] its whole loop
+//                         re-score) and [6] its whole loop; kByteMma also [7] the MMA warps' waits for a free score
+//                         slot, [8] the epilogue warps' waits for a full one and [9] their whole loops ([2]-[4] count
+//                         the MMA warps only)
 //  UML_PROBE_TIMELINE     %globaltimer per CTA into p.probe_timeline[blockIdx.x][5]: [0] entry, [1] the producer's first
 //                         issue, [2] the first stage landed (warp 0), [3] the last `empty` arrive, [4] exit
 //  UML_PROBE_NO_W         kHalf only, wrong scores: every feature's W^T row is one set of registers loaded once per warp,
 //                         so the scoring loop issues no W loads
 //  UML_PROBE_NO_X         kHalf only, wrong scores: every feature of a row is one register set once per warp, so the
 //                         scoring loop issues no x loads and no fp16 conversions (both defines: the FMAs alone)
-//  UML_PROBE_NO_EPILOGUE  kByteMma only, no labels: the warpgroups issue their wgmma and hand the stages back, and skip
-//                         the score write-out, the top-2, the label stores and the queue hand-off
+//  UML_PROBE_NO_EPILOGUE  kByteMma only, no labels: the epilogue warps hand every score slot back unread, and skip the
+//                         top-2, the label stores and the queue hand-off (the MMA warpgroups and the slots as they are)
 //  UML_PROBE_NO_HANDOFF   kByteMma only, wrong labels for near-ties: tier 1's verdict is forced to "certified", so no
 //                         row goes through the queue
 #ifdef UML_PROBE_NO_EPILOGUE
@@ -271,23 +273,28 @@ __device__ __forceinline__ unsigned long long probe_globaltimer() {
 //            warpgroup n % 2.  Rows the tensor-core guard does not certify go through the queue, where the re-score warp
 //            first replays the fp32 route on them (DESIGN.md 3.1, 3.2)
 //  kByteMma  (kHalfMma's conditions, the batch has a byte copy) kHalfMma on 16 KiB stages of one {64 bytes, 256 rows}
-//            box of the byte copy, with three warpgroups: a thread loads its A fragments of each m64 block with two
-//            LDS.128, widens the bytes to the same f16 values kHalfMma reads and issues wgmma with A from registers
+//            box of the byte copy: a thread loads its A fragments of each m64 block with two LDS.128, widens the
+//            bytes to the same f16 values kHalfMma reads and issues wgmma with A from registers; epilogue warps of their
+//            own score the rows
 // kWhole, kHalf and the tensor-core schedules claim their tiles in groups of NCU (the units that take ring items: the
 // scoring warps, or the two warpgroups) from a global counter; ring item n goes to unit n % NCU.
 enum class LinearSched { kChunked, kWhole, kHalf, kHalfMma, kByteMma };
 __host__ __device__ constexpr bool linear_tc_sched(LinearSched s) { return s == LinearSched::kHalfMma || s == LinearSched::kByteMma; }
 
 // scoring warps of a schedule; the producer is warp NCW and the QUEUE kernels' re-score warp NCW + 1
-// kByteMma: three warpgroups.  Its feed takes half of kHalfMma's time, so the warpgroups' own time per item (the
-// epilogue's shuffle chains, stores and queue hand-off) is the limit; a third one hides more of that latency
-// (23.9 against 19.8 G rows/s with two at cfg 2, DESIGN.md 5.1), within the 128 registers that 14 warps leave.
-constexpr int kByteWarpgroups = 3;
+// kByteMma: two MMA warpgroups (warps 0-7) and a pair of epilogue warps per warpgroup (8-11).  Its feed takes half of
+// kHalfMma's time, so the time per item outside the tensor cores is the limit: the epilogue warps take the per-row tail
+// (top-2, tier 1, label stores, queue hand-off) off the warpgroups, which then keep up with the feed in two.  Two
+// epilogue warps for three warpgroups (16 warps) could not: 0.349 against 0.280 ms (DESIGN.md 5.1).
+constexpr int kByteWarpgroups = 2;
+constexpr int kByteEpiWarps = 2 * kByteWarpgroups;
 __host__ __device__ constexpr int linear_consumer_warps(LinearSched s) {
-  return s == LinearSched::kHalf ? kHalfConsumerWarps : s == LinearSched::kByteMma ? 4 * kByteWarpgroups : kConsumerWarps;
+  return s == LinearSched::kHalf ? kHalfConsumerWarps : s == LinearSched::kByteMma ? 4 * kByteWarpgroups + kByteEpiWarps : kConsumerWarps;
 }
 // units that take ring items (and the ring's floor): warps, or the tensor-core schedules' warpgroups
-__host__ __device__ constexpr int linear_ring_units(LinearSched s) { return linear_tc_sched(s) ? linear_consumer_warps(s) / 4 : linear_consumer_warps(s); }
+__host__ __device__ constexpr int linear_ring_units(LinearSched s) {
+  return s == LinearSched::kByteMma ? kByteWarpgroups : linear_tc_sched(s) ? linear_consumer_warps(s) / 4 : linear_consumer_warps(s);
+}
 __host__ __device__ constexpr int linear_threads(LinearSched s, bool queue) { return (linear_consumer_warps(s) + (queue ? 2 : 1)) * 32; }
 // bytes of one ring stage: in kHalf and kHalfMma two 16 KiB fp16 boxes
 __host__ __device__ constexpr int linear_stage_bytes(LinearSched s) {
@@ -295,11 +302,15 @@ __host__ __device__ constexpr int linear_stage_bytes(LinearSched s) {
 }
 // tensor-core schedules: bytes of the B operand in shared memory (rounded up to the 1 KiB that keeps what follows aligned)
 __host__ __device__ constexpr int linear_tc_b_bytes(int C) { return (linear_tc_cols(C) * 128 + 1023) / 1024 * 1024; }
-// kByteMma: each scoring warp's score buffer, the C + 1 folded columns (classes, bound) of its 64 rows, column-major
-// with a pitch of kEpiPitch floats (the bank argument is at the write-out in the kernel)
+// kByteMma: the score slots between the MMA warpgroups and the epilogue warps, kEpiSlots per warpgroup.  A slot holds
+// one item: per MMA warp the C + 1 folded columns (classes, bound) of its 64 rows, column-major with a pitch of
+// kEpiPitch floats (the bank argument is at the write-out in the kernel).  In front of the slots: their `full` and
+// `empty` mbarriers and tile indices (kEpiCtlBytes).
 constexpr int kEpiPitch = 68;
+constexpr int kEpiSlots = 2;
+constexpr int kEpiCtlBytes = 128;
 __host__ __device__ constexpr int linear_epi_bytes(LinearSched s, int C) {
-  return s == LinearSched::kByteMma ? linear_consumer_warps(s) * (C + 1) * kEpiPitch * 4 : 0;
+  return s == LinearSched::kByteMma ? kEpiCtlBytes + kByteWarpgroups * kEpiSlots * 4 * (C + 1) * kEpiPitch * 4 : 0;
 }
 
 // kHalfMma's tier 2 (DESIGN.md 3.2): the fp32 route's scores of one row, replayed bit for bit by one warp: lane c <= C
@@ -379,9 +390,13 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   constexpr int NCU = linear_ring_units(SCHED);
   static_assert(!MMA || (EXACT && QUEUE), "the tensor-core schedule certifies rows through the queue's replay");
   constexpr int TILE = F16 || BYTES ? kHalfTileRows : WHOLE ? kWholeTileRows : kTileRows;  // rows per tile = per ring stage
-  // free queue slots a scoring warp wants before it publishes: every scoring warp may publish a whole tile at once
-  // (kHalfMma: the 64 rows of the tile a warp stores)
-  constexpr int HEADROOM = HALF ? NCW * TILE : MMA ? NCW * 64 : kQueueHeadroom;
+  // warps that publish to the queue (kByteMma: the epilogue warps, warps NMW .. NCW - 1)
+  constexpr int NMW = BYTES ? 4 * kByteWarpgroups : NCW;
+  constexpr int NPUB = BYTES ? kByteEpiWarps : NCW;
+  static_assert(!BYTES || NMW + NPUB == NCW, "warps NMW .. NCW - 1 are the epilogue warps");
+  // free queue slots a publishing warp wants before it publishes: every one may publish all its rows of a tile at once
+  // (kHalfMma: the 64 rows of the tile a warp stores; kByteMma: an epilogue warp's 128, half a tile)
+  constexpr int HEADROOM = HALF ? NCW * TILE : BYTES ? NPUB * TILE / 2 : MMA ? NCW * 64 : kQueueHeadroom;
   static_assert(HEADROOM <= kQueueCap, "the queue holds one tile of every scoring warp");
   // rows per lane held in registers at once (kHalf: one pass, NPASS passes per tile)
   constexpr int R = HALF ? kHalfPassRows : TILE / 32;
@@ -408,15 +423,21 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + CP);
   uint64_t* empty_bar = full_bar + S;
   // QUEUE kernels: rows flagged by the scoring warps travel through this shared-memory queue to the re-score warp
-  // (slot value = row + 1, 0 = empty); ctl[0] = tail (reserved), ctl[1] = head (tickets claimed), ctl[2] = scoring
-  // warps done, ctl[3] = slots consumed
+  // (slot value = row + 1, 0 = empty); ctl[0] = tail (reserved), ctl[1] = head (tickets claimed), ctl[2] = publishing
+  // warps done (NPUB), ctl[3] = slots consumed
   int* q_slots = reinterpret_cast<int*>(empty_bar + S);
   int* q_ctl = q_slots + kQueueCap;
   // CLAIMED: the tile each stage holds, written by the producer before the stage's `full` arrive (whose release makes it
   // visible to the waiters); kTileSentinel ends a scoring warp's loop
   int* tile_slot = q_ctl + 4;
-  // kByteMma: the scoring warps' score buffers (linear_epi_bytes), behind the 64 tile slots the host reserves
-  [[maybe_unused]] float* epi_buf = reinterpret_cast<float*>(tile_slot + 64);
+  // kByteMma: the score slots (linear_epi_bytes), behind the 64 tile slots the host reserves; slot s of warpgroup g is
+  // epi_full / epi_empty / epi_tile [g * kEpiSlots + s] and its MMA warp w's rows at epi_buf + ((g * kEpiSlots + s) * 4
+  // + w % 4) * (C + 1) * kEpiPitch
+  [[maybe_unused]] uint64_t* epi_full = reinterpret_cast<uint64_t*>(tile_slot + 64);
+  [[maybe_unused]] uint64_t* epi_empty = epi_full + kByteWarpgroups * kEpiSlots;
+  [[maybe_unused]] int* epi_tile = reinterpret_cast<int*>(epi_empty + kByteWarpgroups * kEpiSlots);
+  static_assert(2 * kByteWarpgroups * kEpiSlots * 8 + kByteWarpgroups * kEpiSlots * 4 <= kEpiCtlBytes, "slot control");
+  [[maybe_unused]] float* epi_buf = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(epi_full) + kEpiCtlBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -443,6 +464,12 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], MMA ? 4 : 1);  // tensor cores: every warp of the warpgroup hands the stage back
+    }
+    if constexpr (BYTES) {
+      for (int s = 0; s < kByteWarpgroups * kEpiSlots; ++s) {
+        mbar_init(&epi_full[s], 4);   // the four warps of the warpgroup post the item
+        mbar_init(&epi_empty[s], 2);  // both epilogue warps of the warpgroup hand the slot back
+      }
     }
     fence_barrier_init();
   }
@@ -553,7 +580,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     }
   } else {
     // ===================== consumers: one tile per warp at a time (warp 9 of the QUEUE kernels: re-score) ==========
-    const bool scoring_warp = warp < NCW;
+    const bool scoring_warp = warp < NMW;  // (kByteMma: the MMA warps)
     // lane l owns rows l, l+32, ... of the tile.  In every box row r sits at byte r*128 with its 16-byte chunks
     // XOR-swizzled by (r & 7); r & 7 == l & 7 for all of a lane's rows, so one swizzle term serves them all and the
     // eight lanes of every LDS.128 phase (lanes 8i..8i+7: l & 7 = 0..7) hit eight distinct bank groups.  The whole-row
@@ -830,188 +857,254 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         // LDS.128 each (the eight lanes of a phase read two whole 64-byte rows: conflict-free), widens the bytes to the
         // f16 values kHalfMma reads and issues the block's wgmma.  The stage goes back as soon as the last block's A
         // fragments are in registers (B lives outside the ring).  Once a block's group is done its scores are folded
-        // as finish_mma folds them, (hi + lo) + bz, into the warp's own buffer, which frees the accumulators; then lane
-        // l scores rows l and l + 32 of the warp from the buffer with the fp32 route's sequential top-2: the same
-        // values and comparisons as finish_mma's quad merge, so labels and tier-1 verdicts are the same bit for bit.
-        float* eb = epi_buf + warp * (C + 1) * kEpiPitch;  // column c of the warp's row r at eb[c * kEpiPitch + r]
-        const int rw = 64 * (warp & 3);                     // the warp's first row in the tile
-        // Bank of the write of (block b, half h, column 8 i + 2 q + e) by lane l = 4 t + q: (8 i + 2 q + e) * 68 + 16 b +
-        // 8 h + t = 8 q + t + (32 i + 4 e + 16 b + 8 h) mod 32, so the warp's 32 lanes (t < 8, q < 4) hit 32 banks.  The
-        // reads (column c of rows l and l + 32) are 32 consecutive words.
+        // as finish_mma folds them, (hi + lo) + bz, into the warp's part of a score slot, which frees the accumulators.
+        // The warpgroup then posts the item and takes its next stage.  Its two epilogue warps score the posted rows
+        // with the fp32 route's sequential top-2: the same values and comparisons as finish_mma's quad merge, so labels
+        // and tier-1 verdicts are the same bit for bit.
+        // Slots: warpgroup g's k-th item goes to slot (g, k % kEpiSlots), and g's epilogue warps walk the same
+        // sequence.  Every item is posted; an unscored one (past the batch, or the sentinel) carries only its tile
+        // index, and the sentinel ends both sides' loops.
         static_assert(kEpiPitch % 32 == 4 && kEpiPitch >= 64, "conflict-free write-out and reads");
-        auto write_out = [&](float (&db)[NT / 2], int b) {
-          if constexpr (kProbeNoEpilogue) return;
+        constexpr int WARP_FLOATS = (C + 1) * kEpiPitch;  // one MMA warp's part of a slot
+        if (warp < NMW) {
+          const int g = warp >> 2;
+          // Bank of the write of (block b, half h, column 8 i + 2 q + e) by lane l = 4 t + q: (8 i + 2 q + e) * 68 + 16 b
+          // + 8 h + t = 8 q + t + (32 i + 4 e + 16 b + 8 h) mod 32, so the warp's 32 lanes (t < 8, q < 4) hit 32 banks.
+          auto write_out = [&](float* eb, float (&db)[NT / 2], int b) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int i = 0; i < NH / 8; ++i)
+              for (int i = 0; i < NH / 8; ++i)
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int c = 8 * i + 2 * q + e;
-                const float lo = i < NL / 8 ? db[4 * (NH / 8 + i) + 2 * h + e] : 0.f;
-                if (c <= C) eb[c * kEpiPitch + 16 * b + 8 * h + (lane >> 2)] = (db[4 * i + 2 * h + e] + lo) + bz[i][e];
-              }
-        };
-        // top-2 and tier 1 of rows row0 + l and row0 + l + 32 (the warp's rows), their label stores and the queue
-        // hand-off.  Every row has one writer: certified rows are stored here, queued rows only by the re-score warp
-        // (settle_row_tc stores every target).  So a queued row carries no provisional label that the re-score warp's
-        // store must be ordered after, and publication needs no device-scope fence: the slot's shared-memory atomic
-        // carries the row index, and nothing this warp wrote to global memory is read or overwritten by the drain.  The
-        // byte words of peers leave out queued rows' bytes (store_label_word_u8's `keep`), so a peer's byte has one
-        // writer as well.
-        auto score_rows = [&](long long row0) {
-          if constexpr (kProbeNoEpilogue) return;
-          __syncwarp();  // the warp's write-out is visible to every lane
-          int lab[2];
-          bool flg[2];
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const float* col = eb + lane + 32 * j;
-            float best = col[0], second = -INFINITY;
-            int bi = 0;
-#pragma unroll
-            for (int c = 1; c < C; ++c) {
-              const float v = col[c * kEpiPitch];
-              if (v > best) {
-                second = best;
-                best = v;
-                bi = c;
-              } else {
-                second = fmaxf(second, v);
-              }
-            }
-            const float a = col[C * kEpiPitch];
-            lab[j] = bi;
-            // tier 1: certain iff margin > kappa A; NaN / Inf anywhere makes the comparison false
-            flg[j] = !kProbeNoHandoff && row0 + lane + 32 * j < p.n_rows && !((best - second) > kappa * a);
-          }
-          __syncwarp();  // every lane has read the buffer before the next item's write-out
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const long long row = row0 + lane + 32 * j;
-            if (row < p.n_rows && !flg[j]) store_label_i32(p.targets, row, lab[j]);
-          }
-          if (p.targets.wire_u8 && p.targets.n_peers > 0) {
-            // lane l < 16 gathers rows 4 l .. 4 l + 3 (row 4 l + t sits in lane (4 l + t) % 32, half l / 8) into one word,
-            // and the bits of the queued ones into `keep`
-            const uint32_t packed = static_cast<uint32_t>(lab[0]) | static_cast<uint32_t>(lab[1]) << 8 |
-                                    (flg[0] ? 1u << 16 : 0u) | (flg[1] ? 1u << 17 : 0u);
-            uint32_t word = 0;
-            unsigned keep = 0;
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
-              word |= ((w >> (8 * (lane >> 3))) & 0xffu) << (8 * t);
-              keep |= ((w >> (16 + (lane >> 3))) & 1u) ? 0u : 1u << t;
-            }
-            store_label_word_u8(p, row0 + 4 * lane, word, lane < 16, keep);
-          }
-          unsigned masks[2];
-          int total = 0;
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            masks[j] = __ballot_sync(0xffffffffu, flg[j]);
-            total += __popc(masks[j]);
-          }
-          if (total == 0) return;
-          // When the queue is backed up (most rows near-ties) the warp waits for room: the drain never waits for a
-          // scoring warp, so the wait ends
-          int base = -1;
-          if (lane == 0) {
-            for (;;) {
-              const int tail = atomicAdd(&q_ctl[0], 0);
-              const int consumed = atomicAdd(&q_ctl[3], 0);
-              if (tail - consumed <= kQueueCap - HEADROOM) break;
-              __nanosleep(500);
-            }
-            base = atomicAdd(&q_ctl[0], total);
-          }
-          int off = __shfl_sync(0xffffffffu, base, 0);
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            if (flg[j]) {
-              const int slot = (off + __popc(masks[j] & ((1u << lane) - 1u))) & (kQueueCap - 1);
-              while (atomicAdd(&q_slots[slot], 0) != 0) {  // only if the slot's previous ticket is claimed but not read yet
-              }
-              atomicExch(&q_slots[slot], static_cast<int>(row0 + lane + 32 * j) + 1);
-            }
-            off += __popc(masks[j]);
-          }
-        };
-        // (at NT = 40, C = 16, two blocks' fragments beside 80 accumulators made ptxas serialize the wgmma chain)
-        constexpr int INFLIGHT = NT >= 40 ? 1 : 2;
-        uint32_t stage = static_cast<uint32_t>(warp >> 2), phase = 0;
-        for (bool first = true; scoring_warp; first = false) {
-          UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
-          UML_PROBE_CLOCK(probe_landed);
-          UML_PROBE_LANDED(first);
-          const int tile = tile_slot[stage];
-          const bool scored = !kFeedOnly && tile >= 0 && tile < num_tiles;
-          auto release = [&] {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[stage]);  // the fourth warp's arrive hands the stage back
-            UML_PROBE_SINCE(probe_hold, probe_landed);
-            UML_PROBE_RELEASED();
+                for (int e = 0; e < 2; ++e) {
+                  const int c = 8 * i + 2 * q + e;
+                  const float lo = i < NL / 8 ? db[4 * (NH / 8 + i) + 2 * h + e] : 0.f;
+                  if (c <= C) eb[c * kEpiPitch + 16 * b + 8 * h + (lane >> 2)] = (db[4 * i + 2 * h + e] + lo) + bz[i][e];
+                }
           };
-          if (scored) {
-            float d[4][NT / 2];
-            uint32_t a[4][kHalfBoxF / 16][4];
-#pragma unroll
-            for (int b = 0; b < 4; ++b)
-#pragma unroll
-              for (int r = 0; r < NT / 2; ++r) {
-                d[b][r] = 0.f;
-                wgmma_fence_operand(d[b][r]);
-              }
-            const uint8_t* xs = smem + static_cast<size_t>(stage) * STAGE_BYTES + (rw + (lane >> 2)) * kByteRowBytes + 16 * q;
-            // block b's group is done: its A registers may be reused, its scores go to the buffer
-            auto retire = [&](int b) {
-#pragma unroll
-              for (int k = 0; k < kHalfBoxF / 16; ++k)
-#pragma unroll
-                for (int i = 0; i < 4; ++i) wgmma_fence_operand(a[b][k][i]);
-#pragma unroll
-              for (int r = 0; r < NT / 2; ++r) wgmma_fence_operand(d[b][r]);
-              write_out(d[b], b);
+          // (at NT = 40, C = 16, two blocks' fragments beside 80 accumulators made ptxas serialize the wgmma chain)
+          constexpr int INFLIGHT = NT >= 40 ? 1 : 2;
+          uint32_t stage = static_cast<uint32_t>(g), phase = 0;
+          int slot = 0;
+          uint32_t slot_phase = 0;
+#ifdef UML_PROBE_WAIT_CLOCKS
+          long long probe_slot_wait = 0;
+#endif
+          for (bool first = true;; first = false) {
+            UML_PROBE_TIMED(probe_wait, mbar_wait(&empty_bar[stage], phase ^ 1u); mbar_wait(&full_bar[stage], phase));
+            UML_PROBE_CLOCK(probe_landed);
+            UML_PROBE_LANDED(first);
+            const int tile = tile_slot[stage];
+            const bool scored = !kFeedOnly && tile >= 0 && tile < num_tiles;
+            const int es = g * kEpiSlots + slot;
+            auto release = [&] {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&empty_bar[stage]);  // the fourth warp's arrive hands the stage back
+              UML_PROBE_SINCE(probe_hold, probe_landed);
+              UML_PROBE_RELEASED();
             };
+            // both epilogue warps have read the slot's previous item
+            auto wait_slot = [&] { UML_PROBE_TIMED(probe_slot_wait, mbar_wait(&epi_empty[es], slot_phase ^ 1u)); };
+            if (scored) {
+              float* eb = epi_buf + (es * 4 + (warp & 3)) * WARP_FLOATS;  // column c of the warp's row r at eb[c * kEpiPitch + r]
+              float d[4][NT / 2];
+              uint32_t a[4][kHalfBoxF / 16][4];
 #pragma unroll
-            for (int b = 0; b < 4; ++b) {
-              if (b >= INFLIGHT) {
-                wgmma_wait<INFLIGHT - 1>();
-                retire(b - INFLIGHT);
-              }
-              const uint4 x0 = *reinterpret_cast<const uint4*>(xs + 16 * b * kByteRowBytes);
-              const uint4 x1 = *reinterpret_cast<const uint4*>(xs + (16 * b + 8) * kByteRowBytes);
+              for (int b = 0; b < 4; ++b)
 #pragma unroll
-              for (int k = 0; k < kHalfBoxF / 16; ++k) {
-                const uint32_t w0 = k == 0 ? x0.x : k == 1 ? x0.y : k == 2 ? x0.z : x0.w;
-                const uint32_t w1 = k == 0 ? x1.x : k == 1 ? x1.y : k == 2 ? x1.z : x1.w;
-                a[b][k][0] = bytes_to_half2(w0, 0);
-                a[b][k][1] = bytes_to_half2(w1, 0);
-                a[b][k][2] = bytes_to_half2(w0, 1);
-                a[b][k][3] = bytes_to_half2(w1, 1);
-              }
-              if (b == 3) release();
-              wgmma_fence();
+                for (int r = 0; r < NT / 2; ++r) {
+                  d[b][r] = 0.f;
+                  wgmma_fence_operand(d[b][r]);
+                }
+              const uint8_t* xs = smem + static_cast<size_t>(stage) * STAGE_BYTES + (64 * (warp & 3) + (lane >> 2)) * kByteRowBytes + 16 * q;
+              // block b's group is done: its A registers may be reused, its scores go to the slot
+              auto retire = [&](int b) {
 #pragma unroll
-              for (int k = 0; k < kHalfBoxF / 16; ++k) {
-                if (k < nk) WgmmaF16<NT>::mma_ra(d[b], a[b][k], wgmma_desc_k_sw128(b_base + 32 * k), k != 0 ? 1u : 0u);
+                for (int k = 0; k < kHalfBoxF / 16; ++k)
+#pragma unroll
+                  for (int i = 0; i < 4; ++i) wgmma_fence_operand(a[b][k][i]);
+#pragma unroll
+                for (int r = 0; r < NT / 2; ++r) wgmma_fence_operand(d[b][r]);
+                write_out(eb, d[b], b);
+              };
+#pragma unroll
+              for (int b = 0; b < 4; ++b) {
+                if (b >= INFLIGHT) {
+                  wgmma_wait<INFLIGHT - 1>();
+                  if (b == INFLIGHT) wait_slot();  // (under the wgmma of the blocks in flight)
+                  retire(b - INFLIGHT);
+                }
+                const uint4 x0 = *reinterpret_cast<const uint4*>(xs + 16 * b * kByteRowBytes);
+                const uint4 x1 = *reinterpret_cast<const uint4*>(xs + (16 * b + 8) * kByteRowBytes);
+#pragma unroll
+                for (int k = 0; k < kHalfBoxF / 16; ++k) {
+                  const uint32_t w0 = k == 0 ? x0.x : k == 1 ? x0.y : k == 2 ? x0.z : x0.w;
+                  const uint32_t w1 = k == 0 ? x1.x : k == 1 ? x1.y : k == 2 ? x1.z : x1.w;
+                  a[b][k][0] = bytes_to_half2(w0, 0);
+                  a[b][k][1] = bytes_to_half2(w1, 0);
+                  a[b][k][2] = bytes_to_half2(w0, 1);
+                  a[b][k][3] = bytes_to_half2(w1, 1);
+                }
+                if (b == 3) release();
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kHalfBoxF / 16; ++k) {
+                  if (k < nk) WgmmaF16<NT>::mma_ra(d[b], a[b][k], wgmma_desc_k_sw128(b_base + 32 * k), k != 0 ? 1u : 0u);
+                }
+                wgmma_commit();
               }
-              wgmma_commit();
+              wgmma_wait<0>();
+#pragma unroll
+              for (int b = 4 - INFLIGHT; b < 4; ++b) retire(b);
+            } else {
+              release();
+              wait_slot();
             }
-            wgmma_wait<0>();
+            // post the item: warp 0 of the group writes the tile index, and the slot is full once all four warps'
+            // scores are in (each warp's __syncwarp orders its lanes' writes before its arrive)
+            if ((warp & 3) == 0 && lane == 0) epi_tile[es] = tile;
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&epi_full[es]);
+            if (tile == kTileSentinel) break;
+            stage += NCU;
+            if (stage >= static_cast<uint32_t>(S)) {
+              stage -= S;
+              phase ^= 1u;
+            }
+            if (++slot == kEpiSlots) {
+              slot = 0;
+              slot_phase ^= 1u;
+            }
+          }
+#ifdef UML_PROBE_WAIT_CLOCKS
+          if (lane == 0) atomicAdd(&p.probe_clocks[7], static_cast<unsigned long long>(probe_slot_wait));
+#endif
+        } else if (warp < NCW) {
+          // ===== epilogue warp e = warp - NMW serves warpgroup e / 2: rows 128 h .. 128 h + 127 (h = e % 2) of each of
+          // its items, lane l rows 128 h + 32 j + l (j < 4) from the parts of MMA warps 2 h (j < 2) and 2 h + 1; the reads
+          // of column c are 32 consecutive words.
+          // Every row has one writer: certified rows are stored here, queued rows only by the re-score warp
+          // (settle_row_tc stores every target).  So a queued row carries no provisional label that the re-score warp's
+          // store must be ordered after, and publication needs no device-scope fence: the slot's shared-memory atomic
+          // carries the row index, and nothing this warp wrote to global memory is read or overwritten by the drain.
+          // The byte words of peers leave out queued rows' bytes (store_label_word_u8's `keep`), so a peer's byte has
+          // one writer as well.
+          static_assert(C <= 16, "a label takes 4 bits of the byte-word gather");
+          const int g = (warp - NMW) >> 1, h = (warp - NMW) & 1;
+#ifdef UML_PROBE_WAIT_CLOCKS
+          long long probe_epi_wait = 0;
+#endif
+          auto score_rows = [&](int es, long long row0) {
+            auto hand_back = [&] {
+              __syncwarp();  // every lane has read the slot
+              if (lane == 0) mbar_arrive(&epi_empty[es]);
+            };
+            if constexpr (kProbeNoEpilogue) {
+              hand_back();
+              return;
+            }
+            const float* eb = epi_buf + (es * 4 + 2 * h) * WARP_FLOATS + lane;
+            int lab[4];
+            bool flg[4];
 #pragma unroll
-            for (int b = 4 - INFLIGHT; b < 4; ++b) retire(b);
-          } else {
-            release();
+            for (int j = 0; j < 4; ++j) {
+              const float* col = eb + (j >> 1) * WARP_FLOATS + 32 * (j & 1);
+              float best = col[0], second = -INFINITY;
+              int bi = 0;
+#pragma unroll
+              for (int c = 1; c < C; ++c) {
+                const float v = col[c * kEpiPitch];
+                if (v > best) {
+                  second = best;
+                  best = v;
+                  bi = c;
+                } else {
+                  second = fmaxf(second, v);
+                }
+              }
+              const float a = col[C * kEpiPitch];
+              lab[j] = bi;
+              // tier 1: certain iff margin > kappa A; NaN / Inf anywhere makes the comparison false
+              flg[j] = !kProbeNoHandoff && row0 + 32 * j + lane < p.n_rows && !((best - second) > kappa * a);
+            }
+            hand_back();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const long long row = row0 + 32 * j + lane;
+              if (row < p.n_rows && !flg[j]) store_label_i32(p.targets, row, lab[j]);
+            }
+            if (p.targets.wire_u8 && p.targets.n_peers > 0) {
+              // lane l gathers rows 4 l .. 4 l + 3 (row 4 l + t sits in lane (4 l + t) % 32, j = l / 8) into one word,
+              // and the bits of the queued ones into `keep`
+              uint32_t packed = 0;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) packed |= static_cast<uint32_t>(lab[j]) << (4 * j) | (flg[j] ? 1u << (16 + j) : 0u);
+              uint32_t word = 0;
+              unsigned keep = 0;
+#pragma unroll
+              for (int t = 0; t < 4; ++t) {
+                const uint32_t w = __shfl_sync(0xffffffffu, packed, (4 * lane + t) & 31);
+                word |= ((w >> (4 * (lane >> 3))) & 0xfu) << (8 * t);
+                keep |= ((w >> (16 + (lane >> 3))) & 1u) ? 0u : 1u << t;
+              }
+              store_label_word_u8(p, row0 + 4 * lane, word, true, keep);
+            }
+            unsigned masks[4];
+            int total = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              masks[j] = __ballot_sync(0xffffffffu, flg[j]);
+              total += __popc(masks[j]);
+            }
+            if (total == 0) return;
+            // When the queue is backed up (most rows near-ties) the warp waits for room: the drain never waits for an
+            // epilogue warp, so the wait ends
+            int base = -1;
+            if (lane == 0) {
+              for (;;) {
+                const int tail = atomicAdd(&q_ctl[0], 0);
+                const int consumed = atomicAdd(&q_ctl[3], 0);
+                if (tail - consumed <= kQueueCap - HEADROOM) break;
+                __nanosleep(500);
+              }
+              base = atomicAdd(&q_ctl[0], total);
+            }
+            int off = __shfl_sync(0xffffffffu, base, 0);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              if (flg[j]) {
+                const int slot = (off + __popc(masks[j] & ((1u << lane) - 1u))) & (kQueueCap - 1);
+                while (atomicAdd(&q_slots[slot], 0) != 0) {  // only if the slot's previous ticket is claimed but not read yet
+                }
+                atomicExch(&q_slots[slot], static_cast<int>(row0 + 32 * j + lane) + 1);
+              }
+              off += __popc(masks[j]);
+            }
+          };
+          int slot = 0;
+          uint32_t slot_phase = 0;
+          for (;;) {
+            const int es = g * kEpiSlots + slot;
+            UML_PROBE_TIMED(probe_epi_wait, mbar_wait(&epi_full[es], slot_phase));
+            const int tile = epi_tile[es];
+            if (tile == kTileSentinel) break;
+            if (!kFeedOnly && tile < num_tiles) {
+              score_rows(es, static_cast<long long>(tile) * TILE + 128 * h);
+            } else {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&epi_empty[es]);
+            }
+            if (++slot == kEpiSlots) {
+              slot = 0;
+              slot_phase ^= 1u;
+            }
           }
-          if (tile == kTileSentinel) break;
-          stage += NCU;
-          if (stage >= static_cast<uint32_t>(S)) {
-            stage -= S;
-            phase ^= 1u;
+#ifdef UML_PROBE_WAIT_CLOCKS
+          if (lane == 0) {
+            atomicAdd(&p.probe_clocks[8], static_cast<unsigned long long>(probe_epi_wait));
+            atomicAdd(&p.probe_clocks[9], static_cast<unsigned long long>(clock64() - probe_start));
           }
-          if (scored) score_rows(static_cast<long long>(tile) * TILE + rw);
+#endif
         }
       } else {
         // ----- kHalfMma: one commit group per item; the stage goes back after the wait, the epilogue runs from registers
@@ -1240,11 +1333,11 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     }
 #endif
     if constexpr (EXACT && QUEUE) {
-      if (warp < NCW) {
+      if (BYTES ? warp >= NMW && warp < NCW : warp < NCW) {
         __syncwarp();
         if (lane == 0) {
           __threadfence_block();
-          atomicAdd(&q_ctl[2], 1);  // this scoring warp has published everything it will ever publish
+          atomicAdd(&q_ctl[2], 1);  // this warp has published everything it will ever publish
         }
       }
       // ===================== fp64 re-score: warp 9 drains the queue while the scoring warps stream; a scoring warp
@@ -1265,7 +1358,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           int state = 0;  // 1: nothing will ever be published for this ticket
           if (lane == 0) {
             v = atomicAdd(&q_slots[t & (kQueueCap - 1)], 0);
-            if (v == 0 && atomicAdd(&q_ctl[2], 0) == NCW) {
+            if (v == 0 && atomicAdd(&q_ctl[2], 0) == NPUB) {
               __threadfence_block();
               if (t >= atomicAdd(&q_ctl[0], 0)) state = 1;
             }
