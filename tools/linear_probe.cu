@@ -9,7 +9,8 @@
 //                           schedule's ring of 16 KiB {64 bytes, 256 rows} stages
 //   -DUML_PROBE_WAIT_CLOCKS the tile kernel with clock64() totals around the producer's `empty` and the scoring
 //                           warps' `full` waits, over the time the scoring warps hold a landed stage, and over the time
-//                           the re-score warp spends on rows from the queue (its busy fraction); every schedule
+//                           the re-score warp spends on rows from the queue (its busy fraction, split into the fp32
+//                           replay and the fp64 re-score), and the rows tier 1 queued per launch; every schedule
 //   -DUML_PROBE_TIMELINE    the tile kernel with %globaltimer stamps per CTA (entry, first issue, first landing, last
 //                           release, exit) over two back-to-back launches: ramp, exit spread, launch gap
 //   -DUML_PROBE_NO_W, -DUML_PROBE_NO_X, both   the fp16 schedule without its W loads, without its x loads and
@@ -324,7 +325,7 @@ int main() {
            read_bytes / ms * 1e-6);
 #ifdef UML_PROBE_WAIT_CLOCKS
     // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time
-    CK(cudaMemset(counters + 8, 0, 10 * sizeof(unsigned long long)));
+    CK(cudaMemset(counters + 8, 0, 12 * sizeof(unsigned long long)));
     unsigned long long flagged0 = 0, flagged1 = 0;
     CK(cudaMemcpy(&flagged0, counters + kCounterFlagged, 8, cudaMemcpyDeviceToHost));
     cudaEvent_t a, b;
@@ -336,7 +337,7 @@ int main() {
     CK(cudaEventSynchronize(b));
     float one = 0.f;
     CK(cudaEventElapsedTime(&one, a, b));
-    unsigned long long c[10];
+    unsigned long long c[12];
     CK(cudaMemcpy(c, counters + 8, sizeof(c), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(&flagged1, counters + kCounterFlagged, 8, cudaMemcpyDeviceToHost));
     // mean stages per CTA landed and not yet released (one scoring warp per stage, four in the tensor-core
@@ -347,9 +348,11 @@ int main() {
         static_cast<double>(c[4]) / (static_cast<double>(c[3]) / scoring_warps) / grid / (tc ? 4 : 1);
     printf(", \"producer_empty_wait_frac\": %.4f, \"consumer_full_wait_frac\": %.4f, \"held_stages\": %.3f, "
            "\"ring_stages\": %d, \"sm_clock_mhz_under_load\": %.0f, \"rescore_warp_busy_frac\": %.4f, "
+           "\"rescore_warp_replay_frac\": %.4f, \"rescore_warp_fp64_frac\": %.4f, \"rows_queued_per_launch\": %llu, "
            "\"rows_fp64_per_launch\": %llu",
            static_cast<double>(c[0]) / c[1], static_cast<double>(c[2]) / c[3], held_stages,
            p.num_stages, static_cast<double>(c[1]) / grid / (one * 1e3), c[6] ? static_cast<double>(c[5]) / c[6] : 0.0,
+           c[6] ? static_cast<double>(c[5] - c[10]) / c[6] : 0.0, c[6] ? static_cast<double>(c[10]) / c[6] : 0.0, c[11],
            flagged1 - flagged0);
     if (byte)  // MMA warps' waits for a free score slot over their loop; epilogue warps' waits for a full one over theirs
       printf(", \"mma_slot_wait_frac\": %.4f, \"epilogue_full_wait_frac\": %.4f", static_cast<double>(c[7]) / c[3],
@@ -387,10 +390,12 @@ int main() {
       const double x0 = *std::min_element(ex.begin(), ex.end()), x1 = *std::max_element(ex.begin(), ex.end());
       printf(", \"launch%d\": {\"span_us\": %.2f, \"entry_spread_us\": %.2f, \"first_issue_us_median\": %.2f, "
              "\"ramp_us_median\": %.2f, \"ramp_us_max\": %.2f, \"exit_spread_us_max\": %.2f, "
-             "\"exit_spread_us_median\": %.2f, \"last_release_to_exit_us_max\": %.2f}",
+             "\"exit_spread_us_median\": %.2f, \"last_release_to_exit_us_median\": %.2f, "
+             "\"last_release_to_exit_us_max\": %.2f}",
              k, (x1 - e0) * 1e-3, (*std::max_element(entry.begin(), entry.end()) - e0) * 1e-3,
              median(first_issue) * 1e-3, median(ramp) * 1e-3, *std::max_element(ramp.begin(), ramp.end()) * 1e-3,
-             (x1 - x0) * 1e-3, (median(ex) - x0) * 1e-3, *std::max_element(tail.begin(), tail.end()) * 1e-3);
+             (x1 - x0) * 1e-3, (median(ex) - x0) * 1e-3, median(tail) * 1e-3,
+             *std::max_element(tail.begin(), tail.end()) * 1e-3);
     }
     {
       const std::vector<double> ex0 = col(0, 4), entry1 = col(1, 0);

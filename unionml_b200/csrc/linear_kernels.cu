@@ -156,7 +156,7 @@ struct TmaKernelParams {
   int binary;
   unsigned long long* counters;
 #ifdef UML_PROBE_WAIT_CLOCKS
-  unsigned long long* probe_clocks;  // [10], see the diagnostic builds below
+  unsigned long long* probe_clocks;  // [12], see the diagnostic builds below
 #endif
 #ifdef UML_PROBE_TIMELINE
   unsigned long long* probe_timeline;  // [gridDim.x][5], see the diagnostic builds below
@@ -193,9 +193,10 @@ constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this ma
 //                         loop, [2] the scoring warps' waits for their data, [3] their whole loops, [4] the time they
 //                         hold a landed stage (from the return of the `full` wait to the `empty` arrive); QUEUE
 //                         kernels also [5] the re-score warp's time on rows it took from the queue (replay and fp64
-//                         re-score) and [6] its whole loop; kByteMma also [7] the MMA warps' waits for a free score
-//                         slot, [8] the epilogue warps' waits for a full one and [9] their whole loops ([2]-[4] count
-//                         the MMA warps only)
+//                         re-score), [6] its whole loop, [10] the fp64 part of [5] and [11] the rows every warp took
+//                         from the queue; kByteMma also [7] the MMA warps' waits for a free score slot, [8] the
+//                         epilogue warps' waits for a full one and [9] their whole loops ([2]-[4] count the MMA warps
+//                         only)
 //  UML_PROBE_TIMELINE     %globaltimer per CTA into p.probe_timeline[blockIdx.x][5]: [0] entry, [1] the producer's first
 //                         issue, [2] the first stage landed (warp 0), [3] the last `empty` arrive, [4] exit
 //  UML_PROBE_NO_W         kHalf only, wrong scores: every feature's W^T row is one set of registers loaded once per warp,
@@ -313,55 +314,66 @@ __host__ __device__ constexpr int linear_epi_bytes(LinearSched s, int C) {
   return s == LinearSched::kByteMma ? kEpiCtlBytes + kByteWarpgroups * kEpiSlots * 4 * (C + 1) * kEpiPitch * 4 : 0;
 }
 
-// kHalfMma's tier 2 (DESIGN.md 3.2): the fp32 route's scores of one row, replayed bit for bit by one warp: lane c <= C
-// runs column c's FMA chain in feature order from bias_s[c] over the caller's fp32 row (zeros past F, as the fp32 route's
-// boxes hold), the bound column on |x|; lane 0's sequential best / second loop of finish_rows on the gathered C + 1
-// values and the same p.thr comparison.  True: that route certifies the row, *idx is its label.
-__device__ __noinline__ bool replay_fp32_row(const TmaKernelParams& p, const float* wt_s, const float* bias_s, int cp,
-                                             long long row, int lane, int* idx) {
-  const int C = p.n_classes, F = p.n_features;
-  const float* xr = p.x + row * p.ld;
-  const float x0 = lane < F ? xr[lane] : 0.f, x1 = lane + 32 < F ? xr[lane + 32] : 0.f;
-  const int col = lane <= C ? lane : C;
-  float acc = bias_s[col];
-  // unrolled so that the W loads and shuffles of later features issue ahead of the FMA chain, which alone is serial
-#pragma unroll 16
-  for (int f = 0; f < p.f_pad; ++f) {
-    const float xf = __shfl_sync(0xffffffffu, f < 32 ? x0 : x1, f & 31);
-    const float wv = wt_s[f * cp + col];
-    acc = lane < C ? fmaf(xf, wv, acc) : fmaf(fabsf(xf), wv, acc);
-  }
-  float best = __shfl_sync(0xffffffffu, acc, 0);
-  float second = -INFINITY;
-  int bi = 0;
-  for (int c = 1; c < C; ++c) {
-    const float v = __shfl_sync(0xffffffffu, acc, c);
-    if (v > best) {
-      second = best;
-      best = v;
-      bi = c;
+// The tensor-core schedules' tier 2 (DESIGN.md 3.2): the fp32 route's scores of up to 32 queued rows, one row per lane
+// (row < 0: the lane has none), replayed bit for bit: columns c < C run their FMA chains in feature order from bias_s[c]
+// over the lane's fp32 row (zeros past F up to f_pad, as the fp32 route's boxes hold), column C (the bound) on |x|; then
+// finish_rows' sequential best / second loop and the same p.thr comparison.  A lane whose row that route certifies
+// stores its label and returns true; the caller sends the others to fp64.  W^T reads are warp-uniform (broadcast LDS).
+// Out of line, so that the MMA and epilogue loops keep their register allocation.
+template <int C>
+__device__ __noinline__ bool replay_fp32_rows(const TmaKernelParams& p, const float* wt_s, const float* bias_s,
+                                              long long row) {
+  constexpr int CP = (C + 1 + 3) / 4 * 4;
+  const int F = p.n_features;
+  const bool has = row >= 0;
+  const float* xr = p.x + (has ? row : 0) * p.ld;
+  const bool vec = ((reinterpret_cast<uintptr_t>(p.x) | static_cast<uintptr_t>(p.ld) * 4u) & 15u) == 0;
+  float acc[C + 1];
+#pragma unroll
+  for (int c = 0; c <= C; ++c) acc[c] = bias_s[c];
+  // the whole row (f_pad <= 64) is loaded before the first FMA: one round trip to memory per batch
+  float xv[64];
+#pragma unroll
+  for (int g = 0; g < 16; ++g) {
+    const int f = 4 * g;
+    if (vec && has && f + 4 <= F) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(xr + f));
+      xv[4 * g] = v.x;
+      xv[4 * g + 1] = v.y;
+      xv[4 * g + 2] = v.z;
+      xv[4 * g + 3] = v.w;
     } else {
-      second = fmaxf(second, v);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) xv[4 * g + k] = has && f + k < F ? __ldg(xr + f + k) : 0.f;
     }
   }
-  const float bound = __shfl_sync(0xffffffffu, acc, C);
-  *idx = bi;
-  return (best - second) > p.thr * bound;
-}
-
-// tier 2 of one row the tensor-core guard left, by the whole warp: the fp32 route's decision first, fp64 only where that
-// route would flag the row; stores the final label.  Returns 1 when the row went to fp64 (it counts in n_flagged).
-// The scoring warps' only call site in the tensor-core schedule, so their registers are not saved around two calls.
-__device__ __noinline__ int settle_row_tc(const TmaKernelParams& p, const float* wt_s, const float* bias_s, int cp,
-                                          long long row, int lane) {
-  int idx = 0;
-  int f64 = 0;
-  if (!replay_fp32_row(p, wt_s, bias_s, cp, row, lane, &idx)) {
-    idx = rescore_row_inline(p, row, lane);
-    f64 = 1;
+#pragma unroll
+  for (int f0 = 0; f0 < 64; f0 += 32) {
+    if (f0 < p.f_pad) {
+#pragma unroll
+      for (int k = 0; k < 32; ++k) {
+        const float* w = wt_s + (f0 + k) * CP;
+#pragma unroll
+        for (int c = 0; c < C; ++c) acc[c] = fmaf(xv[f0 + k], w[c], acc[c]);
+        acc[C] = fmaf(fabsf(xv[f0 + k]), w[C], acc[C]);
+      }
+    }
   }
-  if (lane == 0) store_label(p.targets, row, idx);
-  return f64;
+  float best = acc[0], second = -INFINITY;
+  int bi = 0;
+#pragma unroll
+  for (int c = 1; c < C; ++c) {
+    if (acc[c] > best) {
+      second = best;
+      best = acc[c];
+      bi = c;
+    } else {
+      second = fmaxf(second, acc[c]);
+    }
+  }
+  const bool certified = has && (best - second) > p.thr * acc[C];
+  if (certified) store_label(p.targets, row, bi);
+  return certified;
 }
 
 // kHalf: rows per lane scored in one pass over a 256-row stage (NPASS = 8 / this passes).  All 8 rows of a lane at
@@ -983,8 +995,8 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           // ===== epilogue warp e = warp - NMW serves warpgroup e / 2: rows 128 h .. 128 h + 127 (h = e % 2) of each of
           // its items, lane l rows 128 h + 32 j + l (j < 4) from the parts of MMA warps 2 h (j < 2) and 2 h + 1; the reads
           // of column c are 32 consecutive words.
-          // Every row has one writer: certified rows are stored here, queued rows only by the re-score warp
-          // (settle_row_tc stores every target).  So a queued row carries no provisional label that the re-score warp's
+          // Every row has one writer: certified rows are stored here, queued rows only by the drain (which stores
+          // every target of a row it takes).  So a queued row carries no provisional label that the drain's
           // store must be ordered after, and publication needs no device-scope fence: the slot's shared-memory atomic
           // carries the row index, and nothing this warp wrote to global memory is read or overwritten by the drain.
           // The byte words of peers leave out queued rows' bytes (store_label_word_u8's `keep`), so a peer's byte has
@@ -1345,51 +1357,112 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       // by all ten warps instead of waiting for one =====================
       int n_done = 0;
 #ifdef UML_PROBE_WAIT_CLOCKS
-      long long probe_busy = 0;
+      long long probe_busy = 0, probe_f64 = 0, probe_rows = 0;
 #endif
-      for (;;) {
-        // claim the next ticket, then wait until its slot is published (lane 0 polls and broadcasts: the lanes of a
-        // warp need not run in lockstep)
-        int t = 0;
-        if (lane == 0) t = atomicAdd(&q_ctl[1], 1);
-        t = __shfl_sync(0xffffffffu, t, 0);
-        int v = 0;
+      if constexpr (MMA) {
+        // tier 2 in batches of 32 rows, one per lane.  While publishers are still running a batch starts only when 32
+        // tickets are reserved (at about one row every few thousand cycles, smaller batches would mostly hold one row);
+        // once all have published, what is left is split evenly over the NCW + 1 warps that drain, so that the float64
+        // rows of the CTA's last batch do not run one after another in one warp.  Labels are due at the end of the grid
+        // only, and the queue holds 2048 rows against ~100 per CTA, so the wait costs nothing.  Tickets are claimed
+        // with a CAS on the head, so every claimed ticket is reserved and its row is being published.
         for (;;) {
-          int state = 0;  // 1: nothing will ever be published for this ticket
+          int t0 = 0, n = 0;
           if (lane == 0) {
-            v = atomicAdd(&q_slots[t & (kQueueCap - 1)], 0);
-            if (v == 0 && atomicAdd(&q_ctl[2], 0) == NPUB) {
-              __threadfence_block();
-              if (t >= atomicAdd(&q_ctl[0], 0)) state = 1;
+            for (;;) {
+              const bool done = atomicAdd(&q_ctl[2], 0) == NPUB;
+              __threadfence_block();  // the tail read below is final once `done` is seen
+              const int head = atomicAdd(&q_ctl[1], 0);
+              const int avail = atomicAdd(&q_ctl[0], 0) - head;
+              if (done && avail <= 0) break;
+              if (done || avail >= 32) {
+                n = done ? min((avail + NCW) / (NCW + 1), 32) : 32;
+                if (atomicCAS(&q_ctl[1], head, head + n) == head) {
+                  t0 = head;
+                  break;
+                }
+                n = 0;
+                continue;
+              }
+              __nanosleep(200);
             }
           }
-          v = __shfl_sync(0xffffffffu, v, 0);
-          state = __shfl_sync(0xffffffffu, state, 0);
-          if (v != 0 || state == 1) break;
-          __nanosleep(200);
+          n = __shfl_sync(0xffffffffu, n, 0);
+          t0 = __shfl_sync(0xffffffffu, t0, 0);
+          if (n == 0) break;
+          UML_PROBE_CLOCK(probe_batch);
+          // lane i takes ticket t0 + i: its publisher has reserved it, so the slot is written soon
+          long long row = -1;
+          if (lane < n) {
+            int* slot = &q_slots[(t0 + lane) & (kQueueCap - 1)];
+            int v;
+            while ((v = atomicAdd(slot, 0)) == 0) {
+            }
+            atomicExch(slot, 0);
+            row = static_cast<long long>(v) - 1;
+          }
+          __syncwarp();
+          if (lane == 0) atomicAdd(&q_ctl[3], n);
+          const bool certified = replay_fp32_rows<C>(p, wt_s, bias_s, row);
+          // the rows the fp32 route would flag go to fp64 one at a time, by the whole warp (they count in n_flagged)
+          UML_PROBE_CLOCK(probe_f64_start);
+          for (unsigned todo = __ballot_sync(0xffffffffu, row >= 0 && !certified); todo != 0; todo &= todo - 1) {
+            const long long r = __shfl_sync(0xffffffffu, row, __ffs(todo) - 1);
+            const int idx64 = rescore_row_inline(p, r, lane);
+            if (lane == 0) store_label(p.targets, r, idx64);
+            ++n_done;
+          }
+          UML_PROBE_SINCE(probe_f64, probe_f64_start);
+          UML_PROBE_SINCE(probe_busy, probe_batch);
+#ifdef UML_PROBE_WAIT_CLOCKS
+          probe_rows += n;
+#endif
         }
-        if (v == 0) break;
-        if (lane == 0) {
-          atomicExch(&q_slots[t & (kQueueCap - 1)], 0);
-          atomicAdd(&q_ctl[3], 1);
-        }
-        const long long row = static_cast<long long>(v) - 1;
-        UML_PROBE_CLOCK(probe_row);
-        if constexpr (MMA) {
-          // tier 2: the fp32 route's own decision first; only the rows it would flag go to fp64 (and are counted)
-          n_done += settle_row_tc(p, wt_s, bias_s, CP, row, lane);
-        } else {
+      } else {
+        for (;;) {
+          // claim the next ticket, then wait until its slot is published (lane 0 polls and broadcasts: the lanes of a
+          // warp need not run in lockstep)
+          int t = 0;
+          if (lane == 0) t = atomicAdd(&q_ctl[1], 1);
+          t = __shfl_sync(0xffffffffu, t, 0);
+          int v = 0;
+          for (;;) {
+            int state = 0;  // 1: nothing will ever be published for this ticket
+            if (lane == 0) {
+              v = atomicAdd(&q_slots[t & (kQueueCap - 1)], 0);
+              if (v == 0 && atomicAdd(&q_ctl[2], 0) == NPUB) {
+                __threadfence_block();
+                if (t >= atomicAdd(&q_ctl[0], 0)) state = 1;
+              }
+            }
+            v = __shfl_sync(0xffffffffu, v, 0);
+            state = __shfl_sync(0xffffffffu, state, 0);
+            if (v != 0 || state == 1) break;
+            __nanosleep(200);
+          }
+          if (v == 0) break;
+          if (lane == 0) {
+            atomicExch(&q_slots[t & (kQueueCap - 1)], 0);
+            atomicAdd(&q_ctl[3], 1);
+          }
+          const long long row = static_cast<long long>(v) - 1;
+          UML_PROBE_CLOCK(probe_row);
           const int idx64 = rescore_row_inline(p, row, lane);
           if (lane == 0) store_label(p.targets, row, idx64);
           ++n_done;
+          UML_PROBE_SINCE(probe_busy, probe_row);
+#ifdef UML_PROBE_WAIT_CLOCKS
+          ++probe_rows;
+#endif
         }
-        UML_PROBE_SINCE(probe_busy, probe_row);
       }
 #ifdef UML_PROBE_WAIT_CLOCKS
       if (warp == NCW + 1 && lane == 0) {
         atomicAdd(&p.probe_clocks[5], static_cast<unsigned long long>(probe_busy));
         atomicAdd(&p.probe_clocks[6], static_cast<unsigned long long>(clock64() - probe_start));
+        atomicAdd(&p.probe_clocks[10], static_cast<unsigned long long>(MMA ? probe_f64 : probe_busy));
       }
+      if (lane == 0 && probe_rows > 0) atomicAdd(&p.probe_clocks[11], static_cast<unsigned long long>(probe_rows));
 #endif
       if (lane == 0 && n_done > 0) atomicAdd(&p.counters[kCounterFlagged], static_cast<unsigned long long>(n_done));
     }
