@@ -12,7 +12,9 @@
 //                           the re-score warp spends on rows from the queue (its busy fraction, split into the fp32
 //                           replay and the fp64 re-score), and the rows tier 1 queued per launch; every schedule
 //   -DUML_PROBE_TIMELINE    the tile kernel with %globaltimer stamps per CTA (entry, first issue, first landing, last
-//                           release, exit) over two back-to-back launches: ramp, exit spread, launch gap
+//                           release, exit; in the tensor-core schedules also the first drain warp to see every
+//                           publisher done, the last batch claimed, the last replay and the last fp64 row finished) over
+//                           two back-to-back launches: ramp, exit spread, launch gap, and where the tail goes
 //   -DUML_PROBE_NO_W, -DUML_PROBE_NO_X, both   the fp16 schedule without its W loads, without its x loads and
 //                           conversions, and with neither (the FMAs and the epilogue alone): which of the scoring
 //                           warps' operands the time above the feed pays for.  Wrong scores by design.
@@ -244,10 +246,16 @@ int main() {
   CK(cudaMalloc(&counters, 24 * sizeof(unsigned long long)));  // the kernel's slots, then probe_clocks from 8
   CK(cudaMemset(counters, 0, 24 * sizeof(unsigned long long)));
 #ifdef UML_PROBE_TIMELINE
-  unsigned long long* timeline = nullptr;  // [2 launches][grid][5]
-  const size_t timeline_words = 2 * static_cast<size_t>(prop.multiProcessorCount) * 5;
+  unsigned long long* timeline = nullptr;  // [2 launches][grid][kProbeStamps]
+  const size_t timeline_words = 2 * static_cast<size_t>(prop.multiProcessorCount) * kProbeStamps;
   CK(cudaMalloc(&timeline, timeline_words * sizeof(unsigned long long)));
-  CK(cudaMemset(timeline, 0, timeline_words * sizeof(unsigned long long)));
+  // stamp 5 is a minimum over the drain warps, the others are stores or maxima
+  std::vector<unsigned long long> timeline_init(timeline_words, 0ull);
+  for (size_t i = 5; i < timeline_words; i += kProbeStamps) timeline_init[i] = ~0ull;
+  auto reset_timeline = [&] {
+    CK(cudaMemcpy(timeline, timeline_init.data(), timeline_words * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+  };
+  reset_timeline();
 #endif
 
   // the EXACT + QUEUE kernel bench.py runs (uint8 labels to one target), in each schedule
@@ -359,11 +367,11 @@ int main() {
              c[9] ? static_cast<double>(c[8]) / c[9] : 0.0);
 #endif
 #ifdef UML_PROBE_TIMELINE
-    // two launches back to back, each stamping its own [grid][5] block
-    CK(cudaMemset(timeline, 0, timeline_words * sizeof(unsigned long long)));
+    // two launches back to back, each stamping its own [grid][kProbeStamps] block
+    reset_timeline();
     CK(cudaDeviceSynchronize());
     launch();
-    p.probe_timeline = timeline + static_cast<size_t>(grid) * 5;
+    p.probe_timeline = timeline + static_cast<size_t>(grid) * kProbeStamps;
     launch();
     p.probe_timeline = timeline;
     CK(cudaDeviceSynchronize());
@@ -371,7 +379,7 @@ int main() {
     CK(cudaMemcpy(t.data(), timeline, timeline_words * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     auto col = [&](int launch_k, int slot) {
       std::vector<double> v(grid);
-      for (int b = 0; b < grid; ++b) v[b] = static_cast<double>(t[(static_cast<size_t>(launch_k) * grid + b) * 5 + slot]);
+      for (int b = 0; b < grid; ++b) v[b] = static_cast<double>(t[(static_cast<size_t>(launch_k) * grid + b) * kProbeStamps + slot]);
       return v;
     };
     auto median = [](std::vector<double> v) {
@@ -396,12 +404,40 @@ int main() {
              median(first_issue) * 1e-3, median(ramp) * 1e-3, *std::max_element(ramp.begin(), ramp.end()) * 1e-3,
              (x1 - x0) * 1e-3, (median(ex) - x0) * 1e-3, median(tail) * 1e-3,
              *std::max_element(tail.begin(), tail.end()) * 1e-3);
+      if (tc) {
+        // the tail after the last release, stamp by stamp: median and maximum over the CTAs that have the stamp
+        // (a CTA whose drain took no batch has no claim, replay or fp64 stamp)
+        const std::vector<double> done = col(k, 5), claim = col(k, 6), replay = col(k, 7), f64 = col(k, 8);
+        auto after = [&](const std::vector<double>& v, const char* key) {
+          std::vector<double> d;
+          for (int b = 0; b < grid; ++b)
+            if (v[b] > 0.0 && v[b] < 1.8e19) d.push_back(v[b] - rel[b]);
+          if (d.empty()) return;
+          printf(", \"%s_us_median\": %.2f, \"%s_us_max\": %.2f, \"%s_ctas\": %zu", key, median(d) * 1e-3, key,
+                 *std::max_element(d.begin(), d.end()) * 1e-3, key, d.size());
+        };
+        printf(", \"launch%d_tail\": {\"last_release_to_exit_us_median\": %.2f", k, median(tail) * 1e-3);
+        after(done, "all_published");
+        after(claim, "last_claim");
+        after(replay, "last_replay_done");
+        after(f64, "last_fp64_done");
+        std::vector<double> work_end(grid);  // the drain's last work (replay or fp64) to exit
+        std::vector<double> d;
+        for (int b = 0; b < grid; ++b) {
+          const double w = std::max(replay[b], f64[b]);
+          if (w > 0.0) d.push_back(ex[b] - w);
+        }
+        if (!d.empty())
+          printf(", \"drain_end_to_exit_us_median\": %.2f, \"drain_end_to_exit_us_max\": %.2f", median(d) * 1e-3,
+                 *std::max_element(d.begin(), d.end()) * 1e-3);
+        printf("}");
+      }
     }
     {
       const std::vector<double> ex0 = col(0, 4), entry1 = col(1, 0);
       std::vector<double> all;
       for (int k = 0; k < 2; ++k)
-        for (int s = 0; s < 5; ++s)
+        for (int s = 0; s < 5; ++s)  // (the drain stamps are absent in the CUDA-core schedules)
           for (double v : col(k, s)) all.push_back(v);
       std::sort(all.begin(), all.end());
       double quantum = 0.0;  // the smallest step between distinct stamps: the timer's resolution, or finer

@@ -43,14 +43,17 @@ struct RowScore {
 };
 
 // float64 scores of one row by one warp, first maximum wins like np.argmax.  Lanes split the features; classes are
-// scored sixteen at a time (32 independent fp64 chains per lane), the sixteen sums are reduced with warp_reduce16 and
-// the arg-max / runner-up found by a butterfly over the lanes.  LOAD(f) yields feature f of the row as double.
+// scored CB at a time (at most sixteen: 2 CB independent fp64 chains per lane), the sums are reduced with warp_reduce16
+// and the arg-max / runner-up found by a butterfly over the lanes.  LOAD(f) yields feature f of the row as double.
+// Callers that know the class count at compile time pass CB = C, KNOWN_C and C itself: one round, whose accumulators
+// ptxas keeps in registers (warp_reduce16<true>); the generic callers take CB = 16 and loop over the rounds.  For
+// C <= 16 both do the same operations in the same order.
 // w64 is feature-major, w64[f * S + c]: a lane fetches the classes of its feature with 16-byte loads off ONE address
 // (immediate offsets) - the class-major table this replaces cost a 64-bit multiply-add per weight, half of the kernel's
 // instructions at F = 784.  b64 holds 2C doubles: the biases, then each class's bias magnitude for the bound (|b_c|, or
 // |b_c| + sum_f |shift_f w'_cf| for a folded affine map); fold_rel is the bound's extra relative term of a folded map
 // (0 otherwise) and `binary` selects sklearn's `score > 0` rule for the expanded binary layout [0, s] (DESIGN.md 3.2).
-template <typename LOAD>
+template <int CB = 16, bool KNOWN_C = false, typename LOAD>
 __device__ __forceinline__ RowScore score_row_f64(LOAD load, const double* __restrict__ w64, int S,
                                                   const double* __restrict__ b64, int F, int C, double fold_rel,
                                                   bool binary, int lane) {
@@ -59,8 +62,9 @@ __device__ __forceinline__ RowScore score_row_f64(LOAD load, const double* __res
   bool bad = false;
   double best = 0.0, second = -INFINITY, amax = 0.0;
   int idx = 0;
-  for (int c0 = 0; c0 < C; c0 += 16) {
-    const int pairs = min(8, (C - c0 + 1) / 2);  // 16-byte loads per feature this round (an odd C ends in a zero pad)
+  static_assert(KNOWN_C ? CB >= 1 && CB <= 16 : CB == 16, "rounds of sixteen classes, or one round of the known C");
+  for (int c0 = 0; c0 < (KNOWN_C ? CB : C); c0 += CB) {
+    const int pairs = KNOWN_C ? (CB + 1) / 2 : min((CB + 1) / 2, (C - c0 + 1) / 2);  // 16-byte loads per feature this round (an odd C ends in a zero pad)
     double s[16], a[16];
 #pragma unroll
     for (int q = 0; q < 16; ++q) s[q] = a[q] = 0.0;
@@ -92,7 +96,7 @@ __device__ __forceinline__ RowScore score_row_f64(LOAD load, const double* __res
         }
       }
     }
-    const double sv = warp_reduce16(s, lane), av = warp_reduce16(a, lane);
+    const double sv = warp_reduce16<KNOWN_C>(s, lane), av = warp_reduce16<KNOWN_C>(a, lane);
     const int cl = c0 + (lane >> 1);  // the class this lane pair now holds
     const bool valid = cl < C;
     Top2 t;
@@ -159,7 +163,7 @@ struct TmaKernelParams {
   unsigned long long* probe_clocks;  // [12], see the diagnostic builds below
 #endif
 #ifdef UML_PROBE_TIMELINE
-  unsigned long long* probe_timeline;  // [gridDim.x][5], see the diagnostic builds below
+  unsigned long long* probe_timeline;  // [gridDim.x][kProbeStamps], see the diagnostic builds below
 #endif
   const void* tc_ops;  // tensor-core schedules: LinearDeviceModel::tc_ops
   float tc_kappa;
@@ -182,6 +186,20 @@ __device__ __noinline__ int rescore_row_inline(const TmaKernelParams& p, long lo
   return r.idx;
 }
 
+// The tensor-core schedules' fp64 scores of one row, from the batch's float64 copy when it keeps one (its fp32 rows are
+// not the caller's values) and from the fp32 rows otherwise; no source view reaches these schedules (launch_linear_tma's
+// dispatch).  C is known, so this is one copy of score_row_f64 with its 2 C accumulators in registers, instead of
+// rescore_row_inline's three copies with sixteen of each in local memory.
+template <int C>
+__device__ __noinline__ int rescore_row_tc(const TmaKernelParams& p, long long row, int lane) {
+  const float* xr = p.x + row * p.ld;
+  const double* xr64 = p.x64 ? p.x64 + row * p.ld64 : nullptr;
+  const RowScore r = score_row_f64<C, true>([&](int f) { return xr64 ? xr64[f] : static_cast<double>(xr[f]); }, p.w64,
+                                            p.w64_stride, p.b64, p.n_features, C, p.fold_rel, p.binary != 0, lane);
+  if (lane == 0) count_rescored_row(p, r.bad, r.ambiguous);
+  return r.idx;
+}
+
 constexpr int kTileSentinel = -1;        // claimed schedules: ring item that ends a scoring warp's loop
 constexpr int kQueueCap = 2048;           // flagged-row queue of the QUEUE kernels (power of two)
 constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this many slots are free (8 warps x 128 rows)
@@ -197,8 +215,10 @@ constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this ma
 //                         from the queue; kByteMma also [7] the MMA warps' waits for a free score slot, [8] the
 //                         epilogue warps' waits for a full one and [9] their whole loops ([2]-[4] count the MMA warps
 //                         only)
-//  UML_PROBE_TIMELINE     %globaltimer per CTA into p.probe_timeline[blockIdx.x][5]: [0] entry, [1] the producer's first
-//                         issue, [2] the first stage landed (warp 0), [3] the last `empty` arrive, [4] exit
+//  UML_PROBE_TIMELINE     %globaltimer per CTA into p.probe_timeline[blockIdx.x][kProbeStamps]: [0] entry, [1] the
+//                         producer's first issue, [2] the first stage landed (warp 0), [3] the last `empty` arrive,
+//                         [4] exit; tensor-core schedules also [5] the first drain warp to see every publisher done,
+//                         [6] the last batch claimed, [7] the last replay finished, [8] the last fp64 row finished
 //  UML_PROBE_NO_W         kHalf only, wrong scores: every feature's W^T row is one set of registers loaded once per warp,
 //                         so the scoring loop issues no W loads
 //  UML_PROBE_NO_X         kHalf only, wrong scores: every feature of a row is one register set once per warp, so the
@@ -207,6 +227,7 @@ constexpr int kQueueHeadroom = 1024;      // a warp publishes only while this ma
 //                         top-2, the label stores and the queue hand-off (the MMA warpgroups and the slots as they are)
 //  UML_PROBE_NO_HANDOFF   kByteMma only, wrong labels for near-ties: tier 1's verdict is forced to "certified", so no
 //                         row goes through the queue
+constexpr int kProbeStamps = 9;  // UML_PROBE_TIMELINE's stamps per CTA
 #ifdef UML_PROBE_NO_EPILOGUE
 constexpr bool kProbeNoEpilogue = true;
 #else
@@ -252,12 +273,16 @@ __device__ __forceinline__ unsigned long long probe_globaltimer() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-#define UML_PROBE_STAMP(slot) (p.probe_timeline[blockIdx.x * 5 + (slot)] = probe_globaltimer())
+#define UML_PROBE_STAMP(slot) (p.probe_timeline[blockIdx.x * kProbeStamps + (slot)] = probe_globaltimer())
+#define UML_PROBE_STAMP_MIN(slot) atomicMin(&p.probe_timeline[blockIdx.x * kProbeStamps + (slot)], probe_globaltimer())
+#define UML_PROBE_STAMP_MAX(slot) atomicMax(&p.probe_timeline[blockIdx.x * kProbeStamps + (slot)], probe_globaltimer())
 #define UML_PROBE_LANDED(first) \
   if ((first) && warp == 0 && lane == 0) UML_PROBE_STAMP(2)
 #define UML_PROBE_RELEASED() probe_last_release = probe_globaltimer()
 #else
 #define UML_PROBE_STAMP(slot)
+#define UML_PROBE_STAMP_MIN(slot)
+#define UML_PROBE_STAMP_MAX(slot)
 #define UML_PROBE_LANDED(first)
 #define UML_PROBE_RELEASED()
 #endif
@@ -318,8 +343,10 @@ __host__ __device__ constexpr int linear_epi_bytes(LinearSched s, int C) {
 // (row < 0: the lane has none), replayed bit for bit: columns c < C run their FMA chains in feature order from bias_s[c]
 // over the lane's fp32 row (zeros past F up to f_pad, as the fp32 route's boxes hold), column C (the bound) on |x|; then
 // finish_rows' sequential best / second loop and the same p.thr comparison.  A lane whose row that route certifies
-// stores its label and returns true; the caller sends the others to fp64.  W^T reads are warp-uniform (broadcast LDS).
-// Out of line, so that the MMA and epilogue loops keep their register allocation.
+// stores its label and returns true; the caller sends the others to fp64.  W^T rows are read as warp-uniform LDS.128
+// (broadcast; CP % 4 == 0).  Out of line, so that the MMA and epilogue loops keep their register allocation, and small:
+// it runs a few times per CTA per launch, from a cold instruction cache, so the FMAs of one 32-feature half are
+// unrolled and the two halves are one rolled loop (the second half's values move down between the passes).
 template <int C>
 __device__ __noinline__ bool replay_fp32_rows(const TmaKernelParams& p, const float* wt_s, const float* bias_s,
                                               long long row) {
@@ -327,37 +354,46 @@ __device__ __noinline__ bool replay_fp32_rows(const TmaKernelParams& p, const fl
   const int F = p.n_features;
   const bool has = row >= 0;
   const float* xr = p.x + (has ? row : 0) * p.ld;
-  const bool vec = ((reinterpret_cast<uintptr_t>(p.x) | static_cast<uintptr_t>(p.ld) * 4u) & 15u) == 0;
   float acc[C + 1];
 #pragma unroll
   for (int c = 0; c <= C; ++c) acc[c] = bias_s[c];
-  // the whole row (f_pad <= 64) is loaded before the first FMA: one round trip to memory per batch
-  float xv[64];
+  // one feature x with its W^T row wf: every column's next FMA, in the fp32 route's order
+  auto fma_feature = [&](float x, const float* wf) {
 #pragma unroll
-  for (int g = 0; g < 16; ++g) {
-    const int f = 4 * g;
-    if (vec && has && f + 4 <= F) {
-      const float4 v = __ldg(reinterpret_cast<const float4*>(xr + f));
-      xv[4 * g] = v.x;
-      xv[4 * g + 1] = v.y;
-      xv[4 * g + 2] = v.z;
-      xv[4 * g + 3] = v.w;
-    } else {
+    for (int m = 0; m < CP / 4; ++m) {
+      const float4 w = *reinterpret_cast<const float4*>(wf + 4 * m);
+      const float wv[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
-      for (int k = 0; k < 4; ++k) xv[4 * g + k] = has && f + k < F ? __ldg(xr + f + k) : 0.f;
-    }
-  }
-#pragma unroll
-  for (int f0 = 0; f0 < 64; f0 += 32) {
-    if (f0 < p.f_pad) {
-#pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        const float* w = wt_s + (f0 + k) * CP;
-#pragma unroll
-        for (int c = 0; c < C; ++c) acc[c] = fmaf(xv[f0 + k], w[c], acc[c]);
-        acc[C] = fmaf(fabsf(xv[f0 + k]), w[C], acc[C]);
+      for (int e = 0; e < 4; ++e) {
+        const int c = 4 * m + e;
+        if (c < C) acc[c] = fmaf(x, wv[e], acc[c]);
+        if (c == C) acc[C] = fmaf(fabsf(x), wv[e], acc[C]);
       }
     }
+  };
+  if (((reinterpret_cast<uintptr_t>(p.x) | static_cast<uintptr_t>(p.ld) * 4u) & 15u) == 0) {
+    // 16-byte loads of the whole row (f_pad <= 64) before the first FMA: one round trip to memory per batch.  ld is a
+    // multiple of 4 >= F, so the last group's load stays inside the row; its values past F are replaced by zeros.
+    float xv[64];
+#pragma unroll
+    for (int g = 0; g < 16; ++g) {
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (has && 4 * g < F) v = __ldg(reinterpret_cast<const float4*>(xr + 4 * g));
+      xv[4 * g] = v.x;
+      xv[4 * g + 1] = 4 * g + 1 < F ? v.y : 0.f;
+      xv[4 * g + 2] = 4 * g + 2 < F ? v.z : 0.f;
+      xv[4 * g + 3] = 4 * g + 3 < F ? v.w : 0.f;
+    }
+#pragma unroll 1
+    for (int f0 = 0; f0 < p.f_pad; f0 += 32) {
+#pragma unroll
+      for (int k = 0; k < 32; ++k) fma_feature(xv[k], wt_s + (f0 + k) * CP);
+#pragma unroll
+      for (int k = 0; k < 32; ++k) xv[k] = xv[32 + k];
+    }
+  } else {
+#pragma unroll 1
+    for (int f = 0; f < p.f_pad; ++f) fma_feature(has && f < F ? __ldg(xr + f) : 0.f, wt_s + f * CP);
   }
   float best = acc[0], second = -INFINITY;
   int bi = 0;
@@ -1335,7 +1371,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
       }
     }
 #ifdef UML_PROBE_TIMELINE
-    if (scoring_warp && lane == 0 && probe_last_release != 0) atomicMax(&p.probe_timeline[blockIdx.x * 5 + 3], probe_last_release);
+    if (scoring_warp && lane == 0 && probe_last_release != 0) atomicMax(&p.probe_timeline[blockIdx.x * kProbeStamps + 3], probe_last_release);
 #endif
 #ifdef UML_PROBE_WAIT_CLOCKS
     if (scoring_warp && lane == 0) {
@@ -1366,12 +1402,19 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
         // rows of the CTA's last batch do not run one after another in one warp.  Labels are due at the end of the grid
         // only, and the queue holds 2048 rows against ~100 per CTA, so the wait costs nothing.  Tickets are claimed
         // with a CAS on the head, so every claimed ticket is reserved and its row is being published.
+#ifdef UML_PROBE_TIMELINE
+        bool probe_saw_done = false;
+#endif
         for (;;) {
           int t0 = 0, n = 0;
           if (lane == 0) {
             for (;;) {
               const bool done = atomicAdd(&q_ctl[2], 0) == NPUB;
               __threadfence_block();  // the tail read below is final once `done` is seen
+#ifdef UML_PROBE_TIMELINE
+              if (done && !probe_saw_done) UML_PROBE_STAMP_MIN(5);
+              probe_saw_done = done;
+#endif
               const int head = atomicAdd(&q_ctl[1], 0);
               const int avail = atomicAdd(&q_ctl[0], 0) - head;
               if (done && avail <= 0) break;
@@ -1379,6 +1422,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
                 n = done ? min((avail + NCW) / (NCW + 1), 32) : 32;
                 if (atomicCAS(&q_ctl[1], head, head + n) == head) {
                   t0 = head;
+                  UML_PROBE_STAMP_MAX(6);
                   break;
                 }
                 n = 0;
@@ -1404,12 +1448,16 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
           __syncwarp();
           if (lane == 0) atomicAdd(&q_ctl[3], n);
           const bool certified = replay_fp32_rows<C>(p, wt_s, bias_s, row);
+          if (lane == 0) UML_PROBE_STAMP_MAX(7);
           // the rows the fp32 route would flag go to fp64 one at a time, by the whole warp (they count in n_flagged)
           UML_PROBE_CLOCK(probe_f64_start);
           for (unsigned todo = __ballot_sync(0xffffffffu, row >= 0 && !certified); todo != 0; todo &= todo - 1) {
             const long long r = __shfl_sync(0xffffffffu, row, __ffs(todo) - 1);
-            const int idx64 = rescore_row_inline(p, r, lane);
-            if (lane == 0) store_label(p.targets, r, idx64);
+            const int idx64 = rescore_row_tc<C>(p, r, lane);
+            if (lane == 0) {
+              store_label(p.targets, r, idx64);
+              UML_PROBE_STAMP_MAX(8);
+            }
             ++n_done;
           }
           UML_PROBE_SINCE(probe_f64, probe_f64_start);
@@ -1468,7 +1516,7 @@ linear_argmax_tma_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_
     }
   }
 #ifdef UML_PROBE_TIMELINE
-  if (lane == 0) atomicMax(&p.probe_timeline[blockIdx.x * 5 + 4], probe_globaltimer());
+  if (lane == 0) atomicMax(&p.probe_timeline[blockIdx.x * kProbeStamps + 4], probe_globaltimer());
 #endif
 }
 
@@ -1871,10 +1919,12 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
                 "kHalfConsumerWarps stages do not fit");
   const bool half = half_map != nullptr && linear_half_rows_ok(m.f_pad);
   // the tensor-core schedule: EXACT with the queue (its uncertified rows are replayed there), a model with tc_ops, an
-  // fp16 copy without negative values (its bound column is a product with x, not |x|).  UML_B200_LINEAR_TC=0 (read per
-  // call) keeps such a batch on kHalf: a test and A/B hook.
+  // fp16 copy without negative values (its bound column is a product with x, not |x|), and no source view (its drain
+  // re-scores in fp64 from the float64 copy or the fp32 rows only, rescore_row_tc; resident batches, the only ones with
+  // an fp16 copy, have no view).  UML_B200_LINEAR_TC=0 (read per call) keeps such a batch on kHalf: a test and A/B hook.
   const char* tc_env = getenv("UML_B200_LINEAR_TC");
-  const bool tc = half && half_nonneg && inline_rescore && m.tc_ops != nullptr && l.x != nullptr && !(tc_env && tc_env[0] == '0');
+  const bool tc = half && half_nonneg && inline_rescore && m.tc_ops != nullptr && l.x != nullptr && l.src.base == nullptr &&
+                  !(tc_env && tc_env[0] == '0');
   // UML_B200_LINEAR_TC=1: the call fails unless it takes the tensor-core schedule (tests assert the dispatch with it)
   if (tc_env && tc_env[0] == '1' && !tc) {
     if (err) *err = "UML_B200_LINEAR_TC=1, but the batch or the model does not take the tensor-core schedule";

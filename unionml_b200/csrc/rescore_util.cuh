@@ -7,19 +7,49 @@
 
 namespace uml {
 
+// c ? a : b as one selp on values already in registers (the compiler cannot turn it into a select of addresses)
+__device__ __forceinline__ double select_reg(bool c, double a, double b) {
+  double r;
+  asm("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %3, 0;\n\tselp.f64 %0, %1, %2, p;\n\t}" : "=d"(r) : "d"(a), "d"(b), "r"((unsigned)c));
+  return r;
+}
+
+// one butterfly step of warp_reduce16<true>: lanes with bit 2 M set keep the upper M of their 2 M values
+template <int M>
+__device__ __forceinline__ void reduce16_step(double (&v)[16], int lane) {
+  const bool upper = (lane & (2 * M)) != 0;
+#pragma unroll
+  for (int i = 0; i < M; ++i) {
+    const double send = select_reg(upper, v[i], v[i + M]);
+    const double keep = select_reg(upper, v[i + M], v[i]);
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 2 * M);
+  }
+}
+
 // Sum 16 per-lane values across the warp with 16 shuffles instead of 16 x 5: every butterfly step halves the number
 // of values a lane is still responsible for (lanes with the offset bit set keep the upper half).  On return lane l
-// holds the complete sum of value (l >> 1); the two lanes of a pair hold the same one.
+// holds the complete sum of value (l >> 1); the two lanes of a pair hold the same one.  REGS: the same additions of the
+// same values, with every step's trip count a constant and the lane-dependent choice of the half made on values
+// (select_reg), so that v can live in registers.  (The loop nest below leaves each step's trip count to the outer loop
+// and chooses between addresses: v is kept in local memory.)
+template <bool REGS = false>
 __device__ __forceinline__ double warp_reduce16(double (&v)[16], int lane) {
+  if constexpr (REGS) {
+    reduce16_step<8>(v, lane);
+    reduce16_step<4>(v, lane);
+    reduce16_step<2>(v, lane);
+    reduce16_step<1>(v, lane);
+  } else {
 #pragma unroll
-  for (int m = 8; m >= 1; m >>= 1) {
-    const int o = 2 * m;  // 16, 8, 4, 2
-    const bool upper = (lane & o) != 0;
+    for (int m = 8; m >= 1; m >>= 1) {
+      const int o = 2 * m;  // 16, 8, 4, 2
+      const bool upper = (lane & o) != 0;
 #pragma unroll
-    for (int i = 0; i < m; ++i) {
-      const double send = upper ? v[i] : v[i + m];
-      const double keep = upper ? v[i + m] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+      for (int i = 0; i < m; ++i) {
+        const double send = upper ? v[i] : v[i + m];
+        const double keep = upper ? v[i + m] : v[i];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+      }
     }
   }
   return v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
