@@ -1,7 +1,7 @@
 // Test-only probe of the Hopper f16 wgmma accumulation that the tensor-core schedule of the linear tile kernel relies on
 // (DESIGN.md 3.2).  It runs the product's own WgmmaF16<N>::mma and wgmma_desc_k_sw128 on chosen operands:
 // D[64 x N] = sum over n_steps accumulating k16 steps of A[64 x 16 n_steps] . B[N x 16 n_steps]^T, as
-// linear_argmax_tma_kernel<..., kHalfMma> issues them (first step scale_d = 0, one commit group, wait 0), and returns D
+// linear_argmax_tc_kernel<..., kHalfMma> issues them (first step scale_d = 0, one commit group, wait 0), and returns D
 // row-major.  tests/test_gpu_wgmma_f16_accum.py compares D with exact sums.  Built by
 // unionml_b200/_build.py:build_test_probes into build/tests/; the product never loads it.
 #include <cuda_fp16.h>

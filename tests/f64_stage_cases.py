@@ -2,7 +2,7 @@
 
 The stage's contract: a row's label is the argmax of its exact scores (numpy's first-maximum rule), or the row is
 counted in ``n_ambiguous``.  Rows are planted at exact margins measured against the stage's own bound beta (twice the
-per-score error bound of ``score_row_f64`` in linear_kernels.cu, or of ``mlp_rs_rows`` in mlp_rescore.cuh), and split
+per-score error bound of ``score_row_f64`` in linear_tile.cuh, or of ``mlp_rs_rows`` in mlp_rescore.cuh), and split
 into batches by that margin: certain (>= 4 beta), inside (<= beta / 4, exact ties included) and straddle (between).
 """
 from __future__ import annotations

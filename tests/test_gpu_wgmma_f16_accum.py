@@ -1,7 +1,7 @@
 """Measured error of the Hopper f16 wgmma accumulation against the budget of the linear tile kernel's tensor-core guard.
 
-`linear_argmax_tma_kernel<..., kHalfMma>` certifies a row on its tensor-core margin with a bound that budgets
-kTcStepBudget = 64u (u = 2^-24) of the running absolute sum per accumulating m64nNk16 step (engine.cu, DESIGN.md 3.2).
+`linear_argmax_tc_kernel<..., kHalfMma>` certifies a row on its tensor-core margin with a bound that budgets
+kTcStepBudget = 64u (u = 2^-24) of the running absolute sum per accumulating m64nNk16 step (linear_tc_kernels.cu, DESIGN.md 3.2).
 Here the product's own `WgmmaF16<N>::mma` runs on chosen fp16 operands (tests/cuda/wgmma_f16_accum_probe.cu, a
 test-only library built by `build()`), and every element of D is compared with the exact sum: f16 x f16 products are
 exact in float64, and `math.fsum` rounds their sum once.  For each element the error is divided by u * sum_s S_s, where
@@ -24,7 +24,7 @@ if not torch.cuda.is_available():
 
 PROBE = ROOT / "build" / "tests" / "libwgmma_f16_accum_probe.so"
 U = 2.0**-24
-BUDGET_PER_STEP = 64  # engine.cu: kTcStepBudget
+BUDGET_PER_STEP = 64  # linear_tc_kernels.cu: kTcStepBudget
 STEPS = 4  # k16 steps of a 64-feature row
 
 

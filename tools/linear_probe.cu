@@ -1,6 +1,6 @@
 // Where the time of the linear tile kernel goes, on 10M x 64 fp32 rows (2.56 GB, the cfg2 shape), on their compact
 // fp16 copy (1.28 GB) and on their byte copy (0.64 GB), against the card's own read ceiling.  Built eleven times by
-// tools/linear_probe.sh from linear_kernels.cu itself:
+// tools/linear_probe.sh from linear_kernels.cu and linear_tc_kernels.cu themselves:
 //   plain                   read ceiling (streaming 16-byte non-allocating loads) over 2.56 GB, 1.28 GB and 0.64 GB +
 //                           the tile kernel, the three CUDA-core schedules and both tensor-core ones (kHalfMma on the
 //                           fp16 rows, kByteMma on the byte rows; B operand and kappa from build_tc_operands)
@@ -23,8 +23,11 @@
 //   -DUML_PROBE_HALF_ONLY   the fp16 schedule alone, and once more with -DUML_PROBE_HALF_PASS_ROWS=4 (256-row stages
 //                           scored in two passes of 4 rows per lane by the same four warps): the script runs the two
 //                           alternately, which separates the W reuse of 8 rows per lane from the warp count
+// Tile rows, ring depth and shared memory of each schedule come from linear_geometry, as in the library, so
+// UML_B200_STAGES caps the ring here too.
 // Every figure is CUDA-event time over >= 0.5 s of back-to-back launches.  Prints one JSON object per line.
 #include "../unionml_b200/csrc/linear_kernels.cu"
+#include "../unionml_b200/csrc/linear_tc_kernels.cu"
 
 #include <cudaTypedefs.h>
 
@@ -278,9 +281,10 @@ int main() {
     const bool whole = sched == LinearSched::kWhole, half = sched == LinearSched::kHalf;
     const bool byte = sched == LinearSched::kByteMma, tc = linear_tc_sched(sched);
     const bool f16 = half || sched == LinearSched::kHalfMma;
-    const int tile = whole ? kWholeTileRows : f16 || byte ? kHalfTileRows : kTileRows;
+    const int grid = prop.multiProcessorCount;
+    const LinearGeometry g = linear_geometry(m, sched, kRows, grid);
     const CUtensorMap map = byte ? make_map(xb, kHalfTileRows, promo, 1)
-                            : f16 ? make_map(xh, kTileRows, promo, 2) : make_map(x, tile, promo);
+                            : f16 ? make_map(xh, kTileRows, promo, 2) : make_map(x, g.tile_rows, promo);
     const double read_bytes = byte ? bytes / 4 : f16 ? bytes / 2 : bytes;
     TmaKernelParams p{};
     p.wt = m.wt;
@@ -289,12 +293,10 @@ int main() {
     p.targets.n_peers = 1;
     p.targets.wire_u8 = 1;
     p.n_rows = kRows;
-    p.num_tiles = (kRows + tile - 1) / tile;
+    p.num_tiles = g.num_tiles;
     p.f_pad = kF;
     p.kc = kF / kChunkF;
-    const size_t fixed = tma_fixed_smem(m, f16 || byte) + (tc ? linear_tc_b_bytes(kC) : 0) + linear_epi_bytes(sched, kC);
-    const int stage_bytes = linear_stage_bytes(sched);
-    p.num_stages = std::min(64, static_cast<int>((kMaxSmemBytes - fixed) / stage_bytes));
+    p.num_stages = g.stages;
     p.thr = static_cast<float>(2.0 * (kF + 4.0) * 5.9604644775390625e-08 * (1.0 + kF * 4.76837158203125e-07) * 1.0001);
     p.x = x;
     p.ld = kF;
@@ -314,11 +316,10 @@ int main() {
 #ifdef UML_PROBE_TIMELINE
     p.probe_timeline = timeline;
 #endif
-    const size_t smem = fixed + static_cast<size_t>(p.num_stages) * stage_bytes;
-    const int grid = prop.multiProcessorCount;
+    const size_t smem = g.smem;
     auto launch = [&] {
-      const cudaError_t err = byte    ? launch_one<kC, true, true, LinearSched::kByteMma>(map, p, grid, smem, 0)
-                              : tc    ? launch_one<kC, true, true, LinearSched::kHalfMma>(map, p, grid, smem, 0)
+      const cudaError_t err = byte    ? launch_tc<kC, LinearSched::kByteMma>(map, p, grid, smem, 0)
+                              : tc    ? launch_tc<kC, LinearSched::kHalfMma>(map, p, grid, smem, 0)
                               : half  ? launch_one<kC, true, true, LinearSched::kHalf>(map, p, grid, smem, 0)
                               : whole ? launch_one<kC, true, true, LinearSched::kWhole>(map, p, grid, smem, 0)
                                       : launch_one<kC, true, true, LinearSched::kChunked>(map, p, grid, smem, 0);
@@ -329,7 +330,8 @@ int main() {
            "\"scoring_warps\": %d, \"rows_per_lane_per_pass\": %d, \"ms\": %.4f, \"bytes_read\": %.0f, \"gbs\": %.1f",
            build, byte ? "byte_rows_tc_256x64" : tc ? "half_rows_tc_256x64" : half ? "half_rows_256x64"
                   : whole ? "whole_rows_64" : "chunked_128x32",
-           promo_name, p.num_stages, linear_consumer_warps(sched), half ? kHalfPassRows : tile / 32, ms, read_bytes,
+           promo_name, p.num_stages, tc ? linear_tc_warps(sched) : linear_consumer_warps(sched),
+           half ? kHalfPassRows : g.tile_rows / 32, ms, read_bytes,
            read_bytes / ms * 1e-6);
 #ifdef UML_PROBE_WAIT_CLOCKS
     // one more launch with the totals cleared: fractions of the producer's / scoring warps' own loop time

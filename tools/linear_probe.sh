@@ -22,6 +22,7 @@ variants=(plain feed_only wait_clocks timeline no_w_loads no_x_loads math_only h
 for v in "${variants[@]}"; do
   bin=build/probe/linear_probe_$v
   if [ ! -x "$bin" ] || [ tools/linear_probe.cu -nt "$bin" ] || [ unionml_b200/csrc/linear_kernels.cu -nt "$bin" ] ||
+     [ unionml_b200/csrc/linear_tc_kernels.cu -nt "$bin" ] || [ unionml_b200/csrc/linear_tile.cuh -nt "$bin" ] ||
      [ unionml_b200/csrc/uml_common.cuh -nt "$bin" ] || [ unionml_b200/csrc/label_store.cuh -nt "$bin" ]; then
     "$nvcc" "${flags[@]}" ${defs[$v]} tools/linear_probe.cu -o "$bin" &
   fi

@@ -4,9 +4,10 @@ their SASS instruction by instruction, and their ptxas registers / stack / spill
     nvcc -Xptxas=-v <the flags of unionml_b200/_build.py> -c X.cu -o OLD/X.o 2> OLD/X.ptxas.txt    # every .cu, both trees
     python tools/sass_diff.py OLD NEW [--skip REGEX] [--sub REGEX REPL]
 
---skip drops old kernels whose name matches (instantiations the change deletes); --sub rewrites the remaining old names
-(e.g. a template argument the change removes) so that they pair with the new ones.  Instructions are compared without
-their /*addr*/ and encoding comments.  A kernel that differs only in constant-bank offsets (a parameter struct that
+Kernels are paired by mangled name across all objects of each directory, so a kernel that moved to another source
+file pairs with its old self.  --skip drops old kernels whose name matches (instantiations the change deletes); --sub
+rewrites the remaining old names (e.g. a template argument the change removes) so that they pair with the new ones.
+Instructions are compared without their /*addr*/ and encoding comments.  A kernel that differs only in constant-bank offsets (a parameter struct that
 lost fields) is reported as such.  Exit status 1 if anything else differs or a kernel has no partner.
 
     python tools/sass_diff.py --sizes DIR [--match REGEX]
@@ -90,12 +91,37 @@ def resources(log):  # ptxas -v: entry function -> its stack / spill and registe
     return out
 
 
-def paired(old, new, args):
-    renamed = {}
+def ptxas(obj):
+    return resources(obj.with_suffix(".ptxas.txt"))
+
+
+def build(directory, read):  # kernel -> (object stem, read(object)[kernel]) over every object of a build directory
+    copies = {}
+    for obj in sorted(directory.glob("*.o")):
+        for name, v in read(obj).items():
+            copies.setdefault(name, []).append((obj.stem, v))
+    # a name that more than one object emits keeps every copy, keyed by its object, so that each copy pairs with the
+    # same object's copy on the other side (or is reported as unpaired) instead of one copy hiding the others
+    out = {}
+    for name, found in copies.items():
+        for stem, v in found:
+            out[name if len(found) == 1 else f"{name} [{stem}]"] = (stem, v)
+    return out
+
+
+def where(kernels, name):
+    return f"{kernels[name][0]}: {name}"
+
+
+def paired(old, new, args):  # (old names after --skip / --sub, new, old names that --sub mapped onto one name)
+    renamed, clashes = {}, []
     for name, v in old.items():
         if not (args.skip and re.search(args.skip, name)):
-            renamed[re.sub(args.sub[0], args.sub[1], name) if args.sub else name] = v
-    return renamed, new
+            key = re.sub(args.sub[0], args.sub[1], name) if args.sub else name
+            if key in renamed:
+                clashes.append(key)
+            renamed[key] = v
+    return renamed, new, clashes
 
 
 def main():
@@ -112,28 +138,33 @@ def main():
     if args.new is None:
         ap.error("two build directories are compared (or one with --sizes)")
     bad = same = offsets_only = 0
-    for obj in sorted(args.old.glob("*.o")):
-        old, new = paired(sass(obj), sass(args.new / obj.name), args)
-        for name in sorted(set(old) | set(new)):
-            if name not in old or name not in new:
-                print(f"{obj.stem}: only in {'new' if name in new else 'old'}: {name}")
-                bad += 1
-            elif old[name] == new[name]:
-                same += 1
+    old, new, clashes = paired(build(args.old, sass), build(args.new, sass), args)
+    for name in clashes:
+        print(f"--sub maps several old kernels onto {name}")
+        bad += 1
+    for name in sorted(set(old) | set(new)):
+        if name not in old or name not in new:
+            side = new if name in new else old
+            print(f"{side[name][0]}: only in {'new' if name in new else 'old'}: {name}")
+            bad += 1
+        elif old[name][1] == new[name][1]:
+            same += 1
+        else:
+            (ostem, o), (nstem, n) = old[name], new[name]
+            label = where(old, name) if ostem == nstem else f"{ostem} -> {nstem}: {name}"
+            diffs = [(x, y) for x, y in zip(o, n) if x != y]
+            if len(o) == len(n) and all(CBANK.sub("c[]", x) == CBANK.sub("c[]", y) for x, y in diffs):
+                moved = sorted({(CBANK.findall(x)[0], CBANK.findall(y)[0]) for x, y in diffs})
+                print(f"{label}: constant-bank offsets only {moved}")
+                offsets_only += 1
             else:
-                diffs = [(x, y) for x, y in zip(old[name], new[name]) if x != y]
-                if len(old[name]) == len(new[name]) and all(CBANK.sub("c[]", x) == CBANK.sub("c[]", y) for x, y in diffs):
-                    moved = sorted({(CBANK.findall(x)[0], CBANK.findall(y)[0]) for x, y in diffs})
-                    print(f"{obj.stem}: {name}: constant-bank offsets only {moved}")
-                    offsets_only += 1
-                else:
-                    print(f"{obj.stem}: {name}: {len(diffs)} of {len(old[name])} instructions differ")
-                    bad += 1
-        old, new = paired(resources(obj.with_suffix(".ptxas.txt")), resources(args.new / (obj.stem + ".ptxas.txt")), args)
-        for name in sorted(set(old) & set(new)):
-            if old[name] != new[name]:
-                print(f"{obj.stem}: {name}: ptxas {old[name]} -> {new[name]}")
+                print(f"{label}: {len(diffs)} of {len(o)} instructions differ")
                 bad += 1
+    old, new, _ = paired(build(args.old, ptxas), build(args.new, ptxas), args)
+    for name in sorted(set(old) & set(new)):
+        if old[name][1] != new[name][1]:
+            print(f"{where(old, name)}: ptxas {old[name][1]} -> {new[name][1]}")
+            bad += 1
     print(f"{same} kernels identical, {offsets_only} differ in constant-bank offsets only, {bad} other differences")
     return 1 if bad else 0
 

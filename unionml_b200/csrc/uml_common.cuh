@@ -208,7 +208,7 @@ cudaError_t launch_linear_tma(const CUtensorMap& xmap, const CUtensorMap* half_m
                               int sm_count, cudaStream_t stream, std::string* err, bool* rescore_kernel_needed,
                               bool half_nonneg, int* x_elem_bytes, int* x_read_bytes);
 bool linear_tma_supported(const LinearDeviceModel& m, std::string* why);
-// the tensor-core schedules' B operand image (LinearDeviceModel::tc_ops) and certification factor kappa of a model with
+// (linear_tc_kernels.cu) the tensor-core schedules' B operand image (LinearDeviceModel::tc_ops) and certification factor kappa of a model with
 // fp64 weights w [C][F] and biases b, and its fp32 operands wt / bias; false when the model does not take them
 bool build_tc_operands(const std::vector<double>& w, const std::vector<double>& b, const std::vector<float>& wt,
                        const std::vector<float>& bias, int C, int F, int f_pad, int cp, double fold_rel,
